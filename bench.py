@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py — headline benchmark of the Lasso prover hot path on B200 (contract in the task prompt).
+"""bench.py — headline benchmark of the Lasso prover hot path on H100.
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload prove|msm] [--log-s 20]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic lookups:
     DensifiedRepresentation::from_lookup_indices -> commit -> SparsePolynomialEvaluationProof::prove
@@ -23,17 +24,31 @@ no data-path collective — proofs of different lookup batches are independent o
 --impl reference: the reference's own CPU implementation of the path = the oracle port (the Rust crate cannot
 be built in this image: no cargo/rustc, crates not vendored), all host threads, rank 0 only, the SAME 2^20 workload.
 --workload msm: BASELINE.json configs[4], the VariableBaseMSM-only sweep (tools/msm_bench.py holds the details).
+--dump-outputs DIR: after the timed steps, rank 0 writes what the last timed step returned as DIR/<name>.npy, so that
+two builds can be compared output for output on the same inputs: the commitment bytes, proof bytes and Fiat-Shamir
+challenges (prove, --impl reference), or the result point of every MSM of the sweep (--workload msm).
+--steps / --warmup set the timed and untimed runs of every mode (the GPU prove mode warms up at least 3 times); the
+`configs` rows time min(steps, 3) runs of each large configuration and report the count as `timed_runs`.
+
+Nothing is written inside the repository: the oracle's generator cache goes to a temporary directory.
 """
 import argparse
+import atexit
 import hashlib
 import json
 import os
+import shutil
 import subprocess
 import sys
+import tempfile
 import threading
 import time
 
+sys.dont_write_bytecode = True  # the tree may be read-only, and a benchmark leaves it as it found it
 ROOT = os.path.dirname(os.path.abspath(__file__))
+if "LASSO_ORACLE_CACHE" not in os.environ:
+    os.environ["LASSO_ORACLE_CACHE"] = tempfile.mkdtemp(prefix="lasso_bench_")
+    atexit.register(shutil.rmtree, os.environ["LASSO_ORACLE_CACHE"], True)
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
@@ -53,7 +68,7 @@ def golden_cases():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region (read-only queries)."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -69,6 +84,7 @@ class ClockSampler:
             self.proc = subprocess.Popen(["nvidia-smi", "-i", str(self.idx), "--query-gpu=" + self.Q,
                                           "--format=csv,noheader,nounits", "-lms", "100"],
                                          stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True)
+            atexit.register(self.proc.kill)  # never outlive the benchmark, whatever ends it
             self.t = threading.Thread(target=self._read, daemon=True)
             self.t.start()
         except Exception:
@@ -110,11 +126,7 @@ class ClockSampler:
                 "reasons": sorted(reasons), "samples": len(sm)}
 
 
-def measured_peak_hbm():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3, 700 W part): an upper bound, not a measured rate
 
 
 def generator_stream(lb, need):
@@ -176,14 +188,15 @@ def run_reference(args):
     nthreads, ncpu = best_threads()
     ol, idx, r, seed, gens = cpu_workload(log_s, C, log_m)
     cores = ol.lib().orc_num_threads()
-    res = None
-    for _ in range(max(1, args.warmup)):
-        res = ol.prove(KIND_XOR, C, log_m, 0, idx, r, gens, seed, flags=0)
+    for _ in range(args.warmup):
+        ol.prove(KIND_XOR, C, log_m, 0, idx, r, gens, seed, flags=0)
     t0 = time.perf_counter()
     for _ in range(args.steps):
         res = ol.prove(KIND_XOR, C, log_m, 0, idx, r, gens, seed, flags=0)
         assert res["rc"] == 0
     dt = time.perf_counter() - t0
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res["commitment"], res["proof"], res["challenges"])
     val = args.steps * (1 << log_s) / dt
     sha = hashlib.sha256(res["proof"]).hexdigest()
     gold = golden_cases().get("xor_c4_s20", {}) if log_s == 20 else {}
@@ -233,13 +246,33 @@ def prove_config(lb, ctx, name, steps, stream_cache, sync=lambda: None):
         if it >= 1 and (best is None or cur["commit_ms"] + cur["prove_ms"] < best["commit_ms"] + best["prove_ms"]):
             best = cur
     del gens
-    out = {"name": name, "lookups": s, "setup_ms": round(setup_ms, 1)}
+    out = {"name": name, "lookups": s, "setup_ms": round(setup_ms, 1), "timed_runs": steps, "stat": "best timed run"}
     out.update({k: round(v, 3) for k, v in best.items()})
     out["ms_per_proof"] = round(best["commit_ms"] + best["prove_ms"], 3)  # device-resident: commit + prove
     out["e2e_ms_per_proof"] = round(best["densify_ms"] + best["commit_ms"] + best["prove_ms"], 3)
     out["proof_sha256"] = hashlib.sha256(proof.bytes).hexdigest()
     out["commitment_sha256"] = hashlib.sha256(com).hexdigest()
     return out
+
+
+def dump_outputs(d, com, proof, challenges):
+    """What a caller of commit + prove receives, as float arrays with every value exact: the commitment and proof
+    bytes (0..255 in float32) and the Fiat-Shamir challenges (Montgomery limbs as 8 x u32 in float64)."""
+    os.makedirs(d, exist_ok=True)
+    np.save(os.path.join(d, "commitment.npy"), np.frombuffer(com, dtype=np.uint8).astype(np.float32))
+    np.save(os.path.join(d, "proof.npy"), np.frombuffer(proof, dtype=np.uint8).astype(np.float32))
+    chal = np.ascontiguousarray(challenges, dtype=np.uint64).view(np.uint32).reshape(-1, 8)
+    np.save(os.path.join(d, "challenges.npy"), chal.astype(np.float64))
+
+
+def gpu_info():
+    """Name and power limit of the card the numbers were taken on (they belong to the numbers)."""
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", os.environ.get("LOCAL_RANK", "0"), "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader"], capture_output=True, text=True, timeout=30).stdout.strip()
+        return out or None
+    except Exception:
+        return None
 
 
 def run_msm(args):
@@ -254,7 +287,7 @@ def main():
     ap.add_argument("--gpus", type=int, default=1)
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--impl", default="b200")
+    ap.add_argument("--impl", default="cuda")
     ap.add_argument("--workload", default="prove", choices=["prove", "msm"])
     ap.add_argument("--log-s", type=int, default=20)
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -265,7 +298,12 @@ def main():
     ap.add_argument("--no-batched", action="store_true")
     ap.add_argument("--no-numa-bind", action="store_true", help="N > 1: do not pin the host threads to the GPU's NUMA node")
     ap.add_argument("--no-sampler", action="store_true", help="diagnosis: no nvidia-smi clock sampler during the run")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.warmup < 0:
+        ap.error("--warmup must be >= 0")
     if args.workload == "msm":
         run_msm(args)
         return
@@ -347,7 +385,7 @@ def main():
     ev0.record()
     t0 = time.perf_counter()
     for _ in range(args.steps):
-        step_resident(dense)
+        last = step_resident(dense)
     ev1.record()
     barrier()
     wall = time.perf_counter() - t0
@@ -440,13 +478,15 @@ def main():
         except Exception as e:
             batched = {"error": repr(e)}
 
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last[0], last[1].bytes, last[1].challenges)
+
     # ---- roofline of the bind kernel (K1), timed alone with CUDA events on the library's stream:
-    # 5 polynomials x 2^22 elements (640 MiB > 126 MB L2), 96 algorithmic bytes per output element
+    # 5 polynomials x 2^22 elements (640 MiB > 50 MB L2), 96 algorithmic bytes per output element
     bind_len, bind_np = 1 << 22, 5
     ms = ctx.bench_bind(bind_len, bind_np, 20)
     alg_bytes = 96.0 * (bind_len // 2) * bind_np
     achieved = alg_bytes / (ms * 1e-3) / 1e9
-    peak, peak_src = measured_peak_hbm()
 
     # ---- BASELINE configs 2-4, ONE proof each: single GPU at N = 1, the SAME proof sharded over the N GPUs otherwise
     gold = golden_cases()
@@ -510,12 +550,9 @@ def main():
                     "densify_ms_per_step": dens_ms / args.steps},
             "gpu_launches": launches,
             "clocks": clocks,
-            "roofline": {"kernel": "bind_top2_kernel (K1: bound_poly_var_top, two outputs per thread)", "bound": "hbm", "achieved": achieved, "peak": peak,
-                         "unit": "GB/s", "frac": achieved / peak,
-                         # dram__bytes_read.sum + dram__bytes_write.sum per launch of this exact shape, from the
-                         # ncu --set full capture in profiles/r02_bind_top2_kernel_ncu_full.txt (671.1 MB + 294.3 MB)
-                         "traffic": 965458176,
-                         "peak_source": peak_src, "ms_per_launch": ms,
+            "roofline": {"kernel": "bind_top_kernel (K1: bound_poly_var_top, one output per thread)", "bound": "hbm", "achieved": achieved,
+                         "peak": HBM_PEAK_GBS, "unit": "GB/s", "frac": achieved / HBM_PEAK_GBS, "traffic": None,
+                         "peak_source": "H100 SXM data sheet (3.35 TB/s HBM3)", "gpu": gpu_info(), "ms_per_launch": ms,
                          "alg_bytes_per_launch": alg_bytes},
             "throughput_batched": batched,
             "configs": config_rows,

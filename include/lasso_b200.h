@@ -1,4 +1,4 @@
-/* lasso_b200 — C ABI of the B200-native Lasso prover hot path.
+/* lasso_b200 — C ABI of the H100-native Lasso prover hot path.
  *
  * This is the drop-in boundary for a16z/Lasso's
  *   DensifiedRepresentation::from_lookup_indices -> commit -> SparsePolynomialEvaluationProof::prove

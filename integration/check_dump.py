@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Check the vectors dumped by the reference itself (integration/rust/reference_patch/, run on any machine with
 cargo) against this repository: the CPU oracle must reproduce the Rust commitment and proof bytes from the same
-explicit inputs, and — with --gpu on a B200 — so must liblasso_b200.so.  A PASS pins everything the repository calls
+explicit inputs, and — with --gpu on an H100 — so must liblasso_b200.so.  A PASS pins everything the repository calls
 "bit-exact" to the real Rust binary (SURVEY.md §8c, DESIGN.md §5).
 
     python integration/check_dump.py /tmp/lasso_vectors [--gpu]

@@ -1,4 +1,4 @@
-"""lasso_b200 — B200-native (sm_100a) accelerator for the a16z/Lasso prover hot path.
+"""lasso_b200 — H100-native (sm_90a) accelerator for the a16z/Lasso prover hot path.
 
 Host-side mirror of the reference's surface for that path (names follow the Rust items):
 

@@ -31,7 +31,7 @@ def lib():
         p = library_path()
         if not os.path.exists(p):
             raise RuntimeError("liblasso_b200.so is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                               "(nvcc, sm_100a).  lasso_b200 has no CPU fallback.")
+                               "(nvcc, sm_90a).  lasso_b200 has no CPU fallback.")
         L = C.CDLL(p)
         L.lasso_last_error.restype = C.c_char_p
         L.lasso_gens_points_needed.restype = C.c_size_t

@@ -1,4 +1,4 @@
-// lasso_b200 — shared device helpers: 256-bit global loads/stores of field elements,
+// lasso_b200 — shared device helpers: 32-byte global loads/stores of field elements,
 // warp-shuffle + shared-memory reductions of Fr partial sums, error checking.
 #pragma once
 #include <cuda_runtime.h>
@@ -24,46 +24,49 @@ namespace lb {
 // fails synchronously and must not go unnoticed
 #define LB_LAUNCH_CHECK() LB_CUDA_CHECK(cudaGetLastError())
 
-static constexpr int kNumSMs = 148;  // B200
+static constexpr int kNumSMs = 132;  // H100 SXM
 
 #if defined(__CUDACC__)
-// One 32-byte element per thread per instruction: LDG.E.ENL2.256 / STG.E.ENL2.256 on sm_100a,
-// so a warp moves 1 KiB fully coalesced.
+// One 32-byte element per thread as two 128-bit accesses (the widest global access sm_90 has). The first
+// instruction of a warp touches every 32-byte sector the warp needs; the second is expected to hit those sectors in
+// L1, so DRAM should still see each element once (not profiled; the bind kernel's measured bandwidth, DESIGN.md §7,
+// is consistent with it).
+__device__ __forceinline__ void ld_u32x8(uint32_t (&v)[8], const void* p) {
+  asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "l"(p));
+  asm volatile("ld.global.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
+               : "l"((const char*)p + 16));
+}
+__device__ __forceinline__ void st_u32x8(void* p, const uint32_t (&v)[8]) {
+  asm volatile("st.global.v4.u32 [%4], {%0,%1,%2,%3};" ::"r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "l"(p) : "memory");
+  asm volatile("st.global.v4.u32 [%4], {%0,%1,%2,%3};" ::"r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
+               "l"((char*)p + 16)
+               : "memory");
+}
 __device__ __forceinline__ fr_t ld_fr(const fr_t* p) {
   fr_t r;
-  asm volatile("ld.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]),
-                 "=r"(r.v[7])
-               : "l"(p));
+  ld_u32x8(r.v, p);
   return r;
 }
-// streaming variant for data read exactly once per kernel
+// streaming variant for data read exactly once per kernel: first in line for eviction from L1, rather than not
+// allocated there, so that the second half of the element can still hit
 __device__ __forceinline__ fr_t ld_fr_stream(const fr_t* p) {
   fr_t r;
-  asm volatile("ld.global.L1::no_allocate.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]),
-                 "=r"(r.v[7])
+  asm volatile("ld.global.L1::evict_first.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3])
                : "l"(p));
+  asm volatile("ld.global.L1::evict_first.v4.u32 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]), "=r"(r.v[7])
+               : "l"((const char*)p + 16));
   return r;
 }
-__device__ __forceinline__ void st_fr(fr_t* p, const fr_t& r) {
-  asm volatile("st.global.v8.u32 [%8], {%0,%1,%2,%3,%4,%5,%6,%7};" ::"r"(r.v[0]), "r"(r.v[1]), "r"(r.v[2]),
-               "r"(r.v[3]), "r"(r.v[4]), "r"(r.v[5]), "r"(r.v[6]), "r"(r.v[7]), "l"(p)
-               : "memory");
-}
+__device__ __forceinline__ void st_fr(fr_t* p, const fr_t& r) { st_u32x8(p, r.v); }
 __device__ __forceinline__ fq_t ld_fq(const fq_t* p) {
   fq_t r;
-  asm volatile("ld.global.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r.v[0]), "=r"(r.v[1]), "=r"(r.v[2]), "=r"(r.v[3]), "=r"(r.v[4]), "=r"(r.v[5]), "=r"(r.v[6]),
-                 "=r"(r.v[7])
-               : "l"(p));
+  ld_u32x8(r.v, p);
   return r;
 }
-__device__ __forceinline__ void st_fq(fq_t* p, const fq_t& r) {
-  asm volatile("st.global.v8.u32 [%8], {%0,%1,%2,%3,%4,%5,%6,%7};" ::"r"(r.v[0]), "r"(r.v[1]), "r"(r.v[2]),
-               "r"(r.v[3]), "r"(r.v[4]), "r"(r.v[5]), "r"(r.v[6]), "r"(r.v[7]), "l"(p)
-               : "memory");
-}
+__device__ __forceinline__ void st_fq(fq_t* p, const fq_t& r) { st_u32x8(p, r.v); }
 
 __device__ __forceinline__ fr_t shfl_down_fr(const fr_t& a, int delta) {
   fr_t r;

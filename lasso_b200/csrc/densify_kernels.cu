@@ -16,8 +16,8 @@
 //   scan_*_kernel    start[a] from the counts; final_ts (this rank's shard) = the counts
 //   read_kernel      read[k] = p - start[a] for this rank's k
 // Integer, order-preserving, bit-identical to the sequential scan for every input (skew included: nothing here depends
-// on how the addresses are distributed).  A few launches of ~10-40 us for 2^20 accesses x 4 dimensions where the host
-// scan needs ~3 ms on C threads; no 2^log_m table in shared memory, so any log_m <= 31.
+// on how the addresses are distributed).  A few parallel launches where the host scan is a sequential pass per
+// dimension on C threads; no 2^log_m table in shared memory, so any log_m <= 31.
 #include "kernels.cuh"
 
 namespace lb {

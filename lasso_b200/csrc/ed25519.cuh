@@ -1,4 +1,4 @@
-// lasso_b200 — twisted-Edwards group of curve25519 (-x^2 + y^2 = 1 + d x^2 y^2) on sm_100a.
+// lasso_b200 — twisted-Edwards group of curve25519 (-x^2 + y^2 = 1 + d x^2 y^2) on sm_90a.
 //
 // Replaces ark-ec's `twisted_edwards::{Affine, Projective}` under the reference's MSM
 // (src/msm/mod.rs:127-163: `buckets[..] += base`, running sums, window doublings) and

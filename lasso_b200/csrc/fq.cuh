@@ -1,4 +1,4 @@
-// lasso_b200 — curve25519 base field Fq = GF(2^255 - 19) on sm_100a.
+// lasso_b200 — curve25519 base field Fq = GF(2^255 - 19) on sm_90a.
 //
 // Replaces what the reference gets from ark-ff (generic 4x64 Montgomery Fq) underneath
 // ark-ec's twisted-Edwards group in src/msm/mod.rs:127-163 and src/poly/commitments.rs:84-93.

@@ -1,4 +1,4 @@
-// lasso_b200 — curve25519 scalar field Fr on sm_100a (and on the host, for the prover's
+// lasso_b200 — curve25519 scalar field Fr on sm_90a (and on the host, for the prover's
 // Fiat–Shamir / interpolation glue).
 //
 // Replaces what the reference gets from ark-ff's `Fp<MontBackend<_,4>,4>` under

@@ -1,6 +1,6 @@
 // lasso_b200 — host-side Fq = GF(2^255 - 19) on 4 x 64-bit limbs (unsigned __int128), used only to
 // normalise / compress the one or two group elements a Bulletproofs round sends to the transcript:
-// a single Fq inversion is ~2 us on a CPU core (binary GCD) and ~100 us on one GPU thread (a 265-step serial chain).
+// a single Fq inversion is ~2 us on a CPU core (binary GCD) against a 265-step serial chain on one GPU thread.
 // Values are plain (non-Montgomery) integers, loosely reduced below 2^256 like the device code (fq.cuh).
 #pragma once
 #include <cstdint>

@@ -83,7 +83,7 @@ int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* c
                      uint32_t* out_raw, cudaStream_t st);
 // msm_final.cu: A = nw x nlev level sums; lgL[k] = log2 of level k's group size
 void launch_msm_final(const pt_ext* A, int nlev, const int* lgL, int nw, int c, fq_t* out_ext, uint32_t* out_raw, cudaStream_t st);
-// independent evaluation for the parity tests: per-term double-and-add + tree sum (partial: 148 * 8 points of scratch)
+// independent evaluation for the parity tests: per-term double-and-add + tree sum (partial: kNumSMs * 8 points of scratch)
 void launch_msm_naive(const fq_t* bases_ark, const fr_t* scalars_mont, size_t n, size_t n_pool, pt_ext* partial, fq_t* out_ext,
                       cudaStream_t st);
 

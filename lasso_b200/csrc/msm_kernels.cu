@@ -1,4 +1,4 @@
-// lasso_b200 — K6: Pippenger bucket MSM over curve25519 on sm_100a, row-batched with shared
+// lasso_b200 — K6: Pippenger bucket MSM over curve25519 on sm_90a, row-batched with shared
 // bases.  Replaces src/msm/mod.rs:91-164 (msm_bigint_wnaf) and its callers
 // src/poly/commitments.rs:84-93 (batch_commit) / src/poly/dense_mlpoly.rs:109-128 (commit_inner:
 // L_size independent row MSMs over the same R_size generators).
@@ -509,8 +509,8 @@ __global__ void __launch_bounds__(1024)
 
 // ---------------------------------------------------------------- bucket-free MSM over a multiples table
 // The MSMs of the opening proofs are short (two rows of ~1-8 K terms) and sit on the critical path ~50 times
-// per proof: the bucket method spends most of its ~100 us on the fixed 14-step weighted bucket sum.  180 GB of
-// HBM buy a shortcut: for the first `npts` generators (the ones the openings use) keep every digit multiple
+// per proof: the bucket method spends most of its time on the fixed 14-step weighted bucket sum.  Memory buys a
+// shortcut: for the first `npts` generators (the ones the openings use) keep every digit multiple
 //   M[w][j][d-1] = d * 2^(8w) * G_j,  d = 1..128, affine-niels (96 B): 32 * npts * 128 * 96 B (0.8 GB at
 //   npts = 2050, the 2^20-lookup configuration),
 // so a term is ONE table entry per window and the MSM is a plain sum of (terms x 32) points: quads of lanes
@@ -958,7 +958,7 @@ __global__ void __launch_bounds__(MSM_T)
   }
   if (tid == 0) partials[row] = M16 ? pt_add(acc, ld_pt(K16)) : acc;
 }
-// One THREAD per row: normalise (one Fq inversion = a 265-step dependent chain, ~80 us whatever the row count)
+// One THREAD per row: normalise (one Fq inversion = a 265-step dependent chain whatever the row count)
 // and emit.  32 rows per CTA so that the chains of a commitment spread over all SMs.
 __global__ void __launch_bounds__(32)
     normalize_rows_kernel(const pt_ext* pts, int nrows, fq_t* out_ext, uint32_t* out_comp) {

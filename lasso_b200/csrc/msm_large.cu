@@ -22,7 +22,7 @@
 //   7. msm_final_kernel    per window W = A_0 + 16 (A_1 + 16 (...)), then the window combination sum_w 2^(c w) W_w
 //                          (msm/mod.rs:150-163: c doublings per window, ~250 dependent doublings) by Horner on one QUAD
 //                          of lanes (quad.cuh), then normalisation.
-// Integer-ALU bound: reported as mixed additions/s against the 7.2 G/s the row-commitment kernel reaches.
+// Integer-ALU bound: reported as mixed additions/s.
 // Same group element as msm_bigint_wnaf for every input; outputs are compared after affine normalisation.
 #if defined(__CUDACC__)
 #define LB_FQ_MUL_ATTR static __host__ __device__ __noinline__
@@ -457,7 +457,7 @@ __global__ void __launch_bounds__(128) msm_naive_sum_kernel(const pt_ext* partia
     out_ext[3] = fq_to_ark(fq_one());
   }
 }
-void launch_msm_naive(const fq_t* bases_ark, const fr_t* scalars_mont, size_t n, size_t n_pool, pt_ext* partial /* 1184 */,
+void launch_msm_naive(const fq_t* bases_ark, const fr_t* scalars_mont, size_t n, size_t n_pool, pt_ext* partial /* kNumSMs * 8 */,
                       fq_t* out_ext, cudaStream_t st) {
   const int blocks = kNumSMs * 8;
   msm_naive_terms_kernel<<<blocks, 128, 0, st>>>(bases_ark, scalars_mont, n, n_pool, partial);

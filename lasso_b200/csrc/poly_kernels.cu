@@ -1,10 +1,10 @@
-// lasso_b200 — CUDA kernels (sm_100a) for the multilinear-polynomial side of the Lasso prover
+// lasso_b200 — CUDA kernels (sm_90a) for the multilinear-polynomial side of the Lasso prover
 // hot path: bind (K1), sumcheck round evaluation (K2, K3), eq evals (K4), subtable
 // materialisation + gather (K5), and the supporting reductions (K7).  SURVEY.md §2.2.
 //
 // All of these are streaming integer kernels over 32-byte field elements: one element per
-// thread per 256-bit load (a warp covers 1 KiB contiguous), grid sized as a multiple of the
-// 148 SMs, grid-stride loops, warp-shuffle + shared-memory reductions for partial sums.
+// thread per pair of 128-bit loads (a warp covers 1 KiB contiguous), grid sized as a multiple of the
+// 132 SMs, grid-stride loops, warp-shuffle + shared-memory reductions for partial sums.
 // No tensor cores: this is 256-bit modular integer arithmetic, not a dense contraction.
 #include "kernels.cuh"
 
@@ -12,10 +12,11 @@ namespace lb {
 
 static constexpr int kThreads = 256;
 static constexpr int kBlocksPerSM = 4;
-static constexpr int kMaxBlocks = kNumSMs * kBlocksPerSM;  // 592
-// bind_top launch shape, measured with tools/bind_sweep.py on 5 x 2^22 elements (GB/s of the 96 B per output):
-// CTAs/SM x outputs per thread: 4x1 5340, 4x2 5514, 5x1 5496, 5x2 5661, 6x1 5655, 6x2 5582
-static constexpr int kBindBlocksPerSM = 5, kBindIlp = 2;
+static constexpr int kMaxBlocks = kNumSMs * kBlocksPerSM;  // 528
+// bind_top launch shape, measured with tools/bind_sweep.py on 5 x 2^22 elements (GB/s of the 96 B per output), one
+// H100 80GB HBM3 SXM at a 400 W power limit, CTAs per SM: 4: 2681, 5: 2617, 6: 2415.  A variant with two outputs
+// per thread measured 2599 / 2302 / 2419 at the same CTA counts and was dropped.
+static constexpr int kBindBlocksPerSM = 4;
 
 static inline int grid_for(size_t n, int threads = kThreads, int max_blocks = kMaxBlocks) {
   size_t b = (n + threads - 1) / threads;
@@ -48,37 +49,18 @@ __global__ void __launch_bounds__(kThreads) bind_bot_kernel(const fr_t* Z, fr_t*
     st_fr(out + i, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
   }
 }
-// two outputs per thread and iteration: four independent 32-byte loads in flight before the first multiplication
-__global__ void __launch_bounds__(kThreads) bind_top2_kernel(fr_t* base, size_t stride, size_t half, fr_t r) {
-  fr_t* Z = base + (size_t)blockIdx.y * stride;
-  const size_t step = (size_t)gridDim.x * blockDim.x;
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  for (; i + step < half; i += 2 * step) {
-    const fr_t lo0 = ld_fr_stream(Z + i), hi0 = ld_fr_stream(Z + half + i);
-    const fr_t lo1 = ld_fr_stream(Z + i + step), hi1 = ld_fr_stream(Z + half + i + step);
-    st_fr(Z + i, fr_add(lo0, fr_mul(r, fr_sub(hi0, lo0))));
-    st_fr(Z + i + step, fr_add(lo1, fr_mul(r, fr_sub(hi1, lo1))));
-  }
-  if (i < half) {
-    const fr_t lo = ld_fr_stream(Z + i), hi = ld_fr_stream(Z + half + i);
-    st_fr(Z + i, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
-  }
-}
-// experiment knobs (tools/bind_sweep.py): resident CTAs per SM the grid is sized for, outputs per thread and iteration
+// experiment knob (tools/bind_sweep.py): resident CTAs per SM the grid is sized for
 static int bind_env(const char* name, int dflt) {
   const char* e = getenv(name);
   return e ? atoi(e) : dflt;
 }
 void launch_bind_top(fr_t* base, size_t stride, int npolys, size_t half, const fr_t& r, cudaStream_t st) {
   if (half == 0 || npolys == 0) return;
-  static const int bps = bind_env("LASSO_B200_BIND_BLOCKS", kBindBlocksPerSM), ilp = bind_env("LASSO_B200_BIND_ILP", kBindIlp);
+  static const int bps = bind_env("LASSO_B200_BIND_BLOCKS", kBindBlocksPerSM);
   int per = kNumSMs * bps / npolys;
   if (per < kNumSMs / 4) per = kNumSMs / 4;
   dim3 grid(grid_for(half, kThreads, per), npolys);
-  if (ilp == 2)
-    bind_top2_kernel<<<grid, kThreads, 0, st>>>(base, stride, half, r);
-  else
-    bind_top_kernel<<<grid, kThreads, 0, st>>>(base, stride, half, r);
+  bind_top_kernel<<<grid, kThreads, 0, st>>>(base, stride, half, r);
   LB_LAUNCH_CHECK();
 }
 void launch_bind_top_ptrs(fr_t* const* d_ptrs, int npolys, size_t half, const fr_t& r, cudaStream_t st) {
@@ -461,9 +443,9 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
 }
 // bind with r (length 4q -> 2q) then evaluate the round over the bound polynomials, one launch; only the strategies
 // with a linear g have a fused kernel (false: the caller binds and evaluates separately)
-// Measured (tools/ab_primary.py, XOR C=4): at 2^24 lookups the fused rounds take 5 % off Sumcheck.prove; below
-// q = 2^15 a round is a latency chain and the longer per-thread chain of the fused kernel costs ~0.7 us more than
-// the two short launches it replaces — those rounds stay unfused (min_q = 0: that default; 1: always fuse).
+// Fusing pays on the large rounds; below q = 2^15 a round is a latency chain and the longer per-thread chain of the
+// fused kernel can cost more than the two short launches it replaces — those rounds stay unfused (min_q = 0: that
+// default; 1: always fuse).  tools/ab_primary.py compares the two in one process.
 bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t stride, size_t q, const fr_t& r,
                                          const Finalize& fin, size_t min_q, cudaStream_t st) {
   static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
@@ -639,7 +621,7 @@ __global__ void __launch_bounds__(kThreads)
 }
 // Latency-oriented variant of the two kernels above for the small and medium rounds (most of the ~300 rounds of
 // a grand-product argument move a few KB: what the host waits for is the dependent chain inside one thread,
-// 12 field multiplications ~ 4.5 us on a lone warp).  FOUR lanes per (circuit k, pair index i):
+// 12 field multiplications).  FOUR lanes per (circuit k, pair index i):
 //   lane 0 / 1 / 2 binds its side (A_k / B_k / eq) at i and i+q (2 multiplications, do_bind != 0) and forms
 //   the side's values at t = 0, 2, 3; three quad shuffles hand lane t the three factors of its evaluation
 //   point, which it multiplies (2 multiplications): 4 dependent multiplications instead of 12.

@@ -198,7 +198,7 @@ Ctx* ctx_create(int device) {
   int count = 0;
   cudaError_t e = cudaGetDeviceCount(&count);
   if (e != cudaSuccess || count == 0)
-    throw std::runtime_error("lasso_b200 needs a CUDA device (sm_100a); there is no CPU fallback");
+    throw std::runtime_error("lasso_b200 needs a CUDA device (sm_90a); there is no CPU fallback");
   if (device < 0 || device >= count) throw std::runtime_error("invalid device id");
   LB_CUDA_CHECK(cudaSetDevice(device));
   {
@@ -433,7 +433,8 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
     } else {
       c->d2h(xyzt, raw.p, (size_t)nrows * 128);
     }
-    // a couple of points per Bulletproofs round: invert on the host (3 us vs ~100 us on one GPU thread)
+    // a couple of points per Bulletproofs round: invert on the host (binary GCD) rather than as a 265-step dependent
+    // chain on one GPU thread
     for (int i = 0; i < nrows; i++) h64::compress_xyz(xyzt + 32 * i, out.data() + 32 * i);
     return out;
   }
@@ -522,8 +523,7 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
     const char* hd = getenv("LASSO_B200_HOST_DENSIFY");
     const char* gd = getenv("LASSO_B200_GPU_DENSIFY");
     // The device path (a stable radix sort by address, densify_kernels.cu) replaces the C host threads of the
-    // sequential scan: ~0.5 ms of kernels instead of ~3 ms of host time at 2^20 lookups, and nothing that slows
-    // down when several processes share the host (one process per GPU).  Tiny inputs stay on the host (the ~20
+    // sequential scan with parallel kernels, and nothing that slows down when several processes share the host (one process per GPU).  Tiny inputs stay on the host (the ~20
     // launches cost more than the scan).
     const bool want_gpu = (gd && gd[0] == '1') || s >= ((size_t)1 << 15) || G > 1;
     if (densify_gpu_supported(s, log_m) && want_gpu && !(hd && hd[0] == '1')) {

@@ -52,8 +52,8 @@ struct Ctx {
 
   void sync() { LB_CUDA_CHECK(cudaStreamSynchronize(st)); }
   // Small results (<= 4 KiB) that are not round messages: a one-warp kernel copies the result into mapped pinned
-  // host memory and then raises a sequence flag (system-scope fence); the host spins on the flag.  ~10-15 us
-  // cheaper than cudaMemcpyAsync + cudaStreamSynchronize.
+  // host memory and then raises a sequence flag (system-scope fence); the host spins on the flag instead of paying
+  // for cudaMemcpyAsync + cudaStreamSynchronize.
   uint32_t* h_mapped = nullptr;  // [0..1024) payload words, [1024] flag
   uint32_t* d_mapped = nullptr;
   uint32_t mapped_seq = 0;

@@ -10,8 +10,7 @@
 namespace lb {
 
 // ---------------------------------------------------------------- quad-lane point addition
-// The latency of one extended addition on one thread is 9 dependent Fq multiplications (~2.6 us on a lone
-// warp); the short MSMs of the opening proofs (two rows, a few thousand terms) are nothing but a chain of
+// The latency of one extended addition on one thread is 9 dependent Fq multiplications; the short MSMs of the opening proofs (two rows, a few thousand terms) are nothing but a chain of
 // ~30 of them.  Here the FOUR lanes of a quad hold X, Y, Z, T of the accumulator (role = lane & 3) and run
 // the 4-way parallel form of add-2008-hwcd-3 (Hisil et al. sect. 4.2): A, B, D, C side by side, then
 // E*F, G*H, F*G, E*H side by side -> 2 multiplication levels (+1 on the T lane for 2d*T2), the coordinates

@@ -6,7 +6,7 @@ Runs the CPU oracle (oracle/: the restatement of the reference prover AND verifi
 own known-answer tests by tests/test_oracle_kats.py) on the seeded workloads of tests/workloads.py — minutes to
 tens of minutes of CPU and tens of GB of RAM for the large ones, which is why only the SHA-256 of the commitment
 and proof bytes is committed.  The oracle's verifier must accept every proof it hashes.  The GPU tests
-(tests/test_gpu_big_configs.py) and bench.py compare the bytes produced on the B200 with these hashes."""
+(tests/test_gpu_big_configs.py) and bench.py compare the bytes produced on the GPU with these hashes."""
 import hashlib
 import json
 import os

@@ -112,7 +112,8 @@ def generators(count, label=b"gens_sparse_poly"):
     have = _gens_cache.get(key)
     if have is not None and have.shape[0] >= count:
         return have[:count]
-    cache = os.path.join(ROOT, "oracle", "_build", "gens_%s_%d.npy" % (label.decode(), count))
+    cache = os.path.join(os.environ.get("LASSO_ORACLE_CACHE", os.path.join(ROOT, "oracle", "_build")),
+                         "gens_%s_%d.npy" % (label.decode(), count))
     if os.path.exists(cache):
         g = np.load(cache)
     else:

@@ -1,4 +1,4 @@
-"""BASELINE.json configs 2-4 AT SIZE on one B200: the commitment and proof bytes must hash to the golden values the
+"""BASELINE.json configs 2-4 AT SIZE on one H100: the commitment and proof bytes must hash to the golden values the
 CPU oracle produced offline (tests/golden/big_proofs.json, tests/golden/make_golden_big.py; the oracle's verifier
 accepted every one of them).  Mirrors the reference's end-to-end tests (src/e2e_test.rs:64-99,
 src/subtables/range_check.rs:101-128) at the benchmark sizes."""

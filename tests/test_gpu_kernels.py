@@ -94,8 +94,6 @@ def test_sumcheck_bind_round_arbitrary(ctx, kind, C, log_m, log_r, log_len):
     import lasso_b200 as lb
 
     S = lb.Strategy(kind, C, log_m, log_r)
-    if log_len == 17 and S.num_memories > 8:
-        pytest.skip("covered at 2^14")
     rng = np.random.default_rng(kind * 1000 + C * 10 + log_len)
     n = 1 << log_len
     np_ = S.num_memories + 1

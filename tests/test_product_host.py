@@ -291,7 +291,7 @@ def test_portable_build_of_the_host_code():
 
 
 def test_host_microbenchmark_builds():
-    """tools/hostbench/host_bench.cpp (the source of profiles/r02_host_microbench.txt) keeps compiling from the headers."""
+    """tools/hostbench/host_bench.cpp (the host-side microbenchmark) keeps compiling from the headers."""
     with tempfile.TemporaryDirectory() as d:
         exe = os.path.join(d, "hb")
         subprocess.check_call(["g++", "-O1", "-std=c++17", "-Wno-psabi", "-I", CSRC,

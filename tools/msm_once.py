@@ -1,4 +1,4 @@
-"""One warm-up + one measured large MSM per size (the command profiled with ncu for profiles/)."""
+"""One warm-up + one measured large MSM per size (a short command to put under a profiler)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))

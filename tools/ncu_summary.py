@@ -1,4 +1,4 @@
-"""Summarise an .ncu-rep (read here, without a GPU) into the few metrics DESIGN.md / profiles/ quote."""
+"""Summarise an .ncu-rep (read here, without a GPU) into a few headline metrics per kernel."""
 import csv, subprocess, sys
 rep = sys.argv[1]
 out = subprocess.run(["ncu", "-i", rep, "--page", "raw", "--csv"], capture_output=True, text=True).stdout

@@ -1,5 +1,5 @@
-"""One warm-up + one measured pass of the hot path (XOR C=4 M=2^16, 2^LOG_S lookups) — the command profiled
-with ncu for profiles/ (launch list and --set full captures)."""
+"""One warm-up + one measured pass of the hot path (XOR C=4 M=2^16, 2^LOG_S lookups) — a short command to put
+under a profiler (launch list, per-kernel captures)."""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
