@@ -147,11 +147,10 @@ int lasso_sumcheck_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M,
   DBuf<fr_t> d(c, (size_t)np * len);
   for (int k = 0; k < np; k++)
     LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
-  Finalize f = c->fin_begin();
-  f.pub.ndst = 0;  // plain device result + copy on this entry point
+  const Finalize f = c->fin_begin();
   launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
   g_launches += 1;
-  c->d2h(evals_out, c->d_small, (size_t)npts * 32);
+  c->fin_wait(f, (fr_t*)evals_out, npts);
   return 0;
   LB_CATCH
 }
@@ -168,15 +167,14 @@ int lasso_sumcheck_bind_round_arbitrary(lasso_ctx* h, int strategy, int C, int l
     LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
   fr_t rr;
   memcpy(&rr, r, 32);
-  Finalize f = c->fin_begin();
-  f.pub.ndst = 0;  // plain device result + copy on this entry point
+  const Finalize f = c->fin_begin();
   if (!launch_sumcheck_bind_eval_arbitrary(S, d.p, len, len / 4, rr, f, 1, c->st)) {
     launch_bind_top(d.p, len, np, len / 2, rr, c->st);
     launch_sumcheck_eval_arbitrary(S, d.p, len, len / 4, f, c->st);
     g_launches += 1;
   }
   g_launches += 1;
-  c->d2h(evals_out, c->d_small, (size_t)npts * 32);
+  c->fin_wait(f, (fr_t*)evals_out, npts);
   for (int k = 0; k < np; k++) c->d2h(polys[k], d.p + (size_t)k * len, (len / 2) * 32);
   return 0;
   LB_CATCH
@@ -199,11 +197,16 @@ int lasso_sumcheck_round_cubic(lasso_ctx* h, int n_circuits, const uint64_t* con
   LB_CUDA_CHECK(cudaMemcpyAsync(dC.p, Ceq, len * 32, cudaMemcpyHostToDevice, c->st));
   LB_CUDA_CHECK(cudaMemcpyAsync(pA.p, hA.data(), n_circuits * sizeof(fr_t*), cudaMemcpyHostToDevice, c->st));
   LB_CUDA_CHECK(cudaMemcpyAsync(pB.p, hB.data(), n_circuits * sizeof(fr_t*), cudaMemcpyHostToDevice, c->st));
-  Finalize f = c->fin_begin();
-  f.pub.ndst = 0;
-  launch_sumcheck_eval_cubic(pA.p, pB.p, dC.p, n_circuits, len / 2, f, c->st);
-  g_launches += 1;
-  c->d2h(out, c->d_small, (size_t)n_circuits * 3 * 32);
+  // one circuit at a time through the prover's batched kernels: with scale = 0 no coefficient is applied, so the 3
+  // values of a batch of one are that circuit's (e0, e2, e3).  Each message is read before the next launch, so the
+  // ring of publication regions never wraps.
+  const CubicCoeffs cf = {};
+  for (int k = 0; k < n_circuits; k++) {
+    const Finalize f = c->fin_begin();
+    launch_sumcheck_eval_cubic_comb(pA.p + k, pB.p + k, dC.p, 1, len / 2, cf, 0, f, c->st);
+    g_launches += 1;
+    c->fin_wait(f, (fr_t*)out + 3 * (size_t)k, 3);
+  }
   return 0;
   LB_CATCH
 }

@@ -156,16 +156,11 @@ void comm_init(Ctx* c, const uint8_t id_bytes[128], int rank, int world) {
   c->lg_world = 0;
   while ((1 << c->lg_world) < world) c->lg_world++;
   if (world == 1) return;
-  if (!c->h_pub) throw std::runtime_error("a sharded proof needs the mapped publication buffers (unset LASSO_B200_NO_MAPPED)");
   std::unique_ptr<Xchg> x(new Xchg());
   try {
     comm_init_impl(c, x.get(), id_bytes, rank, world);
   } catch (...) {  // a failed or timed-out rendezvous must not leave mappings, registrations or a shm name behind
     xchg_release(x.get());
-    if (!c->h_pub_owned) {  // the publication buffer had already moved into the (now unmapped) segment
-      c->h_pub = nullptr;
-      for (int r = 0; r < kPubMaxReaders; r++) c->d_pub_reader[r] = nullptr;
-    }
     if (c->d_gather) cudaFree(c->d_gather);
     c->d_gather = nullptr;
     c->world = 1;
@@ -263,18 +258,21 @@ static void comm_init_impl(Ctx* c, Xchg* x, const uint8_t id_bytes[128], int ran
     memcpy(&id, id_bytes, 128);
     LB_NCCL_CHECK(nccl().CommInitRank(&x->nccl_comm, world, id, rank));
   }
-  // publication: this process now receives in its shared segment and sees every reader's segment
-  if (c->h_pub_owned) cudaFreeHost(c->h_pub);
-  c->h_pub_owned = false;
-  c->h_pub = (unsigned long long*)((uint8_t*)x->seg[rank] + kSegHeaderBytes);
+  c->gather_elems = 1 << 16;
+  LB_CUDA_CHECK(cudaMalloc((void**)&c->d_gather, c->gather_elems * sizeof(fr_t)));
+  unsigned long long* readers[kPubMaxReaders] = {};
   for (int r = 0; r < world; r++) {
     void* dp = nullptr;
     LB_CUDA_CHECK(cudaHostGetDevicePointer(&dp, x->seg[r], 0));
-    c->d_pub_reader[r] = (unsigned long long*)((uint8_t*)dp + kSegHeaderBytes);
+    readers[r] = (unsigned long long*)((uint8_t*)dp + kSegHeaderBytes);
   }
+  // publication: this process now receives in its shared segment and sees every reader's segment.  Nothing below
+  // can fail: a failed initialisation leaves the context with its own publication buffer.
+  if (c->h_pub_owned) cudaFreeHost(c->h_pub);
+  c->h_pub_owned = false;
+  c->h_pub = (unsigned long long*)((uint8_t*)x->seg[rank] + kSegHeaderBytes);
+  for (int r = 0; r < world; r++) c->d_pub_reader[r] = readers[r];
   c->pub_seq = 0;
-  c->gather_elems = 1 << 16;
-  LB_CUDA_CHECK(cudaMalloc((void**)&c->d_gather, c->gather_elems * sizeof(fr_t)));
 }
 
 void comm_destroy(Ctx* c) {

@@ -103,8 +103,7 @@ __device__ __forceinline__ void block_sum_fr(fr_t (&v)[NV], fr_t* scratch) {
 
 // ---- single-launch reduction + publication of a round message ---------------------------------------------
 // Every CTA stores its partial sums, takes a ticket, and the LAST CTA to finish adds the partials of all
-// values, writes the results to device memory and (optionally) straight into mapped pinned host memory the
-// host is spinning on.  One kernel per sumcheck round instead of eval + reduce + copy: the rounds of the
+// values and writes the results straight into mapped pinned host memory the host is spinning on.  One kernel per sumcheck round instead of eval + reduce + copy: the rounds of the
 // grand-product ladder are pure launch/sync latency.
 //
 // Publication needs no flag and no system-scope fence (each costs microseconds per round) and makes NO
@@ -124,7 +123,7 @@ static constexpr int kPubElems = 512;         // elements per region (largest me
 static constexpr uint32_t kPubTagMod = 8191;  // tags 1..8191 (13 bits, 0 = empty)
 struct PubDst {
   unsigned long long* dst[kPubMaxReaders];  // device pointers: (this writer, region) inside reader p's buffer
-  int ndst;                                 // 0: no publication
+  int ndst;
   uint32_t tag;
   // host-side bookkeeping of the wait (ignored by kernels)
   int region, all;
@@ -144,8 +143,7 @@ __device__ __forceinline__ void pub_store(const PubDst& p, int v, const uint32_t
 struct Finalize {
   fr_t* partial;      // scratch: [nvals][blocks_per_val]
   unsigned* counter;  // device ticket counter: 0 on entry, reset to 0 by the last CTA
-  fr_t* out_dev;      // nvals results (always written, untagged)
-  PubDst pub;         // optional publication to mapped host memory
+  PubDst pub;         // publication of the nvals results to mapped host memory
 };
 __device__ __forceinline__ fr_t ld_fr_cg(const fr_t* p) {  // bypass L1: written by other CTAs of this launch
   fr_t r;
@@ -155,11 +153,8 @@ __device__ __forceinline__ fr_t ld_fr_cg(const fr_t* p) {  // bypass L1: written
                : "l"((const char*)p + 16));
   return r;
 }
-// result v of a round: device copy + tagged host copy
-__device__ __forceinline__ void finalize_publish(const Finalize& f, int v, const fr_t& val) {
-  f.out_dev[v] = val;
-  if (f.pub.ndst) pub_store(f.pub, v, val.v);
-}
+// result v of a round: tagged host copy
+__device__ __forceinline__ void finalize_publish(const Finalize& f, int v, const fr_t& val) { pub_store(f.pub, v, val.v); }
 // the LAST CTA of a launch (all threads): add the partials of every value and publish
 __device__ __forceinline__ void finalize_last_stage(const Finalize& f, int blocks_per_val, int nvals_total) {
   __threadfence();

@@ -65,13 +65,10 @@ bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t s
 int sumcheck_max_blocks();
 
 // ---- K3: batched cubic round evaluation (sumcheck.rs:49-93) ----
-// A, B: ncirc device pointers each to 2*half elements; Ceq: 2*half elements. out = ncirc x 3 (e0,e2,e3).
-void launch_sumcheck_eval_cubic(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Ceq, int ncirc, size_t half,
-                                const Finalize& fin, cudaStream_t st);
-
-// What the prover runs (poly_kernels.cu): the same rounds with the batching coefficients of sumcheck.rs:95-97 folded
-// in — out = 3 elements  sum_k coeff_k (e0, e2, e3)_k.  scale != 0: the arrays A_k are still unscaled in memory (the
-// first evaluation and the first bind of a layer); the first bind stores coeff_k * A_k and later rounds use scale = 0.
+// A, B: ncirc device pointers each to 2*half elements; Ceq: 2*half elements.  The batching coefficients of
+// sumcheck.rs:95-97 are folded in (poly_kernels.cu): out = 3 elements  sum_k coeff_k (e0, e2, e3)_k.  scale != 0: the
+// arrays A_k are still unscaled in memory (the first evaluation and the first bind of a layer); the first bind stores
+// coeff_k * A_k and later rounds use scale = 0.
 struct CubicCoeffs {
   fr_t v[32];
 };
@@ -94,19 +91,15 @@ void launch_from_u32(const uint32_t* in, fr_t* out, size_t n, cudaStream_t st);
 void launch_fill_zero(fr_t* out, size_t n, cudaStream_t st);
 
 // ---- K7: supporting reductions ----
-// out[k] = <P_k, eq>, P_k = base + k*stride, k < npolys, n elements each
-void launch_multi_dot(const fr_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial,
-                      fr_t* out, cudaStream_t st);
 // sum_k eq[k] * g(E_1[k..]) (subtables/mod.rs:186-216)
 void launch_sumcheck_claim(const Strategy& S, const fr_t* base, size_t stride, size_t n, fr_t* partial, fr_t* out,
                            cudaStream_t st);
+// Over the u32 mirror of an INTEGER-valued polynomial (dim, read, final, E): 8 IMAD per term instead of a Montgomery
+// product, 4 B read per element instead of 32 B, one reduction at the end.
 // LZ[i] = sum_j L[j] Z[j*R_size + i] (dense_mlpoly.rs:183-207); partial: chunks x R_size scratch
-void launch_bound(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out,
-                  cudaStream_t st);
-int bound_max_chunks();
-// the same two reductions over the u32 mirror of an INTEGER-valued polynomial (dim, read, final, E): 8 IMAD per term
-// instead of a Montgomery product, 4 B read per element instead of 32 B, one reduction at the end
 void launch_bound_u32(const uint32_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out, cudaStream_t st);
+int bound_max_chunks();
+// out[k] = <z_k, eq>, z_k = base + k*stride, k < npolys, n elements each
 void launch_multi_dot_u32(const uint32_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
                           cudaStream_t st);
 // Reed-Solomon fingerprints (memory_checking.rs:236-310).  init/final over M cells, read/write over s ops.
@@ -116,9 +109,7 @@ void launch_gp_fingerprints_mem(const fr_t* table, const fr_t* final_fr, size_t 
 void launch_gp_fingerprints_ops(const fr_t* dim_fr, const fr_t* E_fr, const fr_t* read_fr, size_t s,
                                 const fr_t& gamma, const fr_t& tau, fr_t* out_read, fr_t* out_write,
                                 cudaStream_t st);
-// product-tree layer (grand_product.rs:20-36): out[i] = in[i] * in[i + n_out], i < n_out
-void launch_product_layer(const fr_t* in, fr_t* out, size_t n_out, cudaStream_t st);
-// every product tree of one size N (contiguous layers, see poly_kernels.cu) + tagged publication of the two
+// every product tree of one size N (grand_product.rs:20-58; contiguous layers, see poly_kernels.cu) + tagged publication of the two
 // top-layer elements of tree t as values 2*(slot0 + t) + {0, 1}
 struct TreePtrs {
   fr_t* p[32];
@@ -135,10 +126,6 @@ void launch_fold_ab(fr_t* a, fr_t* b, size_t h, const fr_t& u, const fr_t& uinv,
 void launch_cross_inner_products(const fr_t* a, const fr_t* b, size_t h, fr_t* partial, fr_t* out, cudaStream_t st);
 // w'[2t] = w[t]*uinv, w'[2t+1] = w[t]*u  (weights of the unfolded generators, see msm_kernels.cu)
 void launch_expand_weights(const fr_t* w, fr_t* w_out, size_t n_in, const fr_t& u, const fr_t& uinv, cudaStream_t st);
-// scalars for the L / R MSMs over the ORIGINAL generators: see prover.cu
-void launch_bullet_round(const fr_t* a_in, const fr_t* b_in, const fr_t* w_in, fr_t* a_out, fr_t* b_out, fr_t* w_out, size_t n,
-                         size_t m, int fold, const fr_t& u, const fr_t& uinv, const fr_t& blind_L, const fr_t& blind_R,
-                         fr_t* s_out, uint32_t* cols_out, fr_t* partial, unsigned* counter, cudaStream_t st);
 void launch_two_row_scalars(const fr_t* v, int scale, const fr_t& k, const fr_t& t00, const fr_t& t01, const fr_t& t10,
                             const fr_t& t11, size_t n, fr_t* out, cudaStream_t st);
 void launch_bullet_scalars(const fr_t* a, const fr_t* w, size_t n_loc, size_t m, int G, int g, int a_rep, fr_t* sL,

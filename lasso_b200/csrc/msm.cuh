@@ -29,14 +29,14 @@ void launch_sum_raw_points(const uint32_t* raw, int nsrc, int nrows, uint32_t* o
                            cudaStream_t st);
 // multiples table M[w][j][d-1] = d * 2^(8w) * G_j (d = 1..128) of the first npts generators, from the window table T
 void launch_build_multiples(const pt_niels* T, size_t table_stride, size_t npts, int nwindows, pt_niels* M, cudaStream_t st);
-// bucket-free MSM of nrows <= 8 short rows over M (msm_kernels.cu): scalars = nrows x len canonical integers,
-// cols = generator index per term (null: term k uses generator k); heavy_rows = how many of the rows carry
-// non-zero scalars (the CTAs per row are sized for those); partials: nrows x msm_direct_chunks(len, heavy_rows);
+// CTAs per row of a bucket-free MSM over M with len terms per row when heavy_rows of the rows carry non-zero scalars
+int msm_direct_chunks(int len, int heavy_rows);
+// bucket-free MSM of two short rows over M (msm_kernels.cu): scalars = 2 x len canonical integers, term k of a row
+// uses generator k; the CTAs per row are sized for one row carrying the terms; partials: 2 x msm_direct_chunks(len, 1);
 // pub: tagged publication to mapped pinned host memory (common.cuh PubDst) — element 3*row + {0,1,2} = canonical
 // X, Y, Z; the host waits for the message and clears it (Ctx::wait_points)
-int msm_direct_chunks(int len, int heavy_rows);
-void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, const uint32_t* cols, int nrows, int len,
-                       int heavy_rows, pt_ext* partials, uint32_t* out_raw, const PubDst& pub, cudaStream_t st);
+void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, pt_ext* partials, const PubDst& pub,
+                       cudaStream_t st);
 // One Bulletproofs round (bullet.rs:73-134, unfolded generators) in ONE launch over the multiples table: scalars from
 // the (folded) a, b, w vectors, both rows L / R summed, tail terms c * Q + blind * h, publication of the two points.
 // a_in / b_in: 2m elements when fold != 0 (folded with u / uinv into a_out / b_out, m elements), else m;

@@ -467,7 +467,7 @@ __global__ void __launch_bounds__(256)
 // The result (X, Y, Z canonical) goes to mapped host memory as a tagged message (common.cuh PubDst): no flag,
 // no system fence.
 __global__ void __launch_bounds__(1024)
-    msm_finish_quad_kernel(const pt_ext* partials, int nrows, int P, uint32_t* out_raw, PubDst pub) {
+    msm_finish_quad_kernel(const pt_ext* partials, int nrows, int P, PubDst pub) {
   __shared__ fq_t sm_pt[8 * 32 * 4];
   const int tid = threadIdx.x, lane = tid & 31, role = tid & 3;
   const int row = tid >> 7, qr = (tid & 127) >> 2;  // blockDim = 128 * nrows
@@ -495,15 +495,9 @@ __global__ void __launch_bounds__(1024)
     }
     __syncthreads();
   }
-  if (qr == 0 && role < 3) {
-    if (out_raw) {
-#pragma unroll
-      for (int l = 0; l < 8; l++) out_raw[(size_t)row * 32 + role * 8 + l] = mine.v[l];
-    }
-    if (pub.ndst) {  // canonical coordinate < 2^255: element 3*row + {0, 1, 2} of the tagged message
-      const fq_t c = fq_canonical(mine);
-      pub_store(pub, row * 3 + role, c.v);
-    }
+  if (qr == 0 && role < 3) {  // canonical coordinate < 2^255: element 3*row + {0, 1, 2} of the tagged message
+    const fq_t c = fq_canonical(mine);
+    pub_store(pub, row * 3 + role, c.v);
   }
 }
 
@@ -581,17 +575,16 @@ void launch_build_multiples16(const pt_niels* T, const pt_niels* M, size_t npts8
 }
 
 static constexpr int MSMD_T = 512;  // 128 quads
-// scalars: nrows x len canonical 256-bit integers; cols (may be null = identity): generator index of each term.
+// scalars: nrows x len canonical 256-bit integers; term k uses generator k.
 // CTA (chunk, row) takes the terms k = chunk (mod nchunks): an odd nchunks spreads any power-of-two pattern of
 // zero scalars evenly.  Quad (w, sub): window w of the terms chunk + nchunks * (sub + 4 i).
 __global__ void __launch_bounds__(MSMD_T)
-    msm_direct_kernel(const pt_niels* M, size_t npts, const uint32_t* scalars, const uint32_t* cols, int len, pt_ext* partials) {
+    msm_direct_kernel(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, pt_ext* partials) {
   __shared__ fq_t sm_pt[128 * 4];
   const int tid = threadIdx.x, lane = tid & 31, role = tid & 3, quad = tid >> 2;
   const int w = quad & 31, sub = quad >> 5;
   const int chunk = blockIdx.x, nchunks = gridDim.x, row = blockIdx.y;
   const uint32_t* srow = scalars + (size_t)row * len * 8;
-  const uint32_t* crow = cols ? cols + (size_t)row * len : nullptr;
   fq_t mine = (role == 1 || role == 2) ? fq_one() : fq_zero();  // identity (0, 1, 1, 0)
   // operand of an entry for this lane; digit 0 -> the identity entry (1, 1, 0): the control flow stays uniform
   auto fetch = [&](int k, fq_t& op) -> bool {
@@ -611,8 +604,7 @@ __global__ void __launch_bounds__(MSMD_T)
     const int ad = d < 0 ? -d : d;
     op = role == 3 ? fq_zero() : fq_one();
     if (ad != 0 && role != 2) {
-      const size_t col = crow ? crow[k] : (size_t)k;
-      const pt_niels* e = M + ((size_t)w * npts + col) * 128 + (ad - 1);
+      const pt_niels* e = M + ((size_t)w * npts + k) * 128 + (ad - 1);
       const bool neg = d < 0;
       if (role == 0) op = ld_fq(neg ? &e->yplusx : &e->yminusx);
       else if (role == 1) op = ld_fq(neg ? &e->yminusx : &e->yplusx);
@@ -655,9 +647,8 @@ __global__ void __launch_bounds__(MSMD_T)
   }
 }
 // ---------------------------------------------------------------- one Bulletproofs round in ONE launch
-// bullet.rs:73-134 with unfolded generators (prover.cu file header).  Replaces bullet_round_kernel (scalars) +
-// msm_direct_kernel (both rows) + msm_finish_quad_kernel (sum + publication): three dependent launches on the
-// critical path of each of the ~43 rounds of a proof.
+// bullet.rs:73-134 with unfolded generators (prover.cu file header).  The scalars, the sums of both rows and their
+// publication in one launch instead of three dependent ones on the critical path of each of the ~43 rounds of a proof.
 //   grid (nchunks, 2): row 0 = L, row 1 = R.  CTA (chunk, row) owns the main terms k = chunk + nchunks * q of its row:
 //     k = t * h + p (h = m / 2, t < n / m):   L: generator t*m + h + p, scalar a'[p]     * w'[t]
 //                                             R: generator t*m + p,     scalar a'[p + h] * w'[t]
@@ -872,7 +863,7 @@ void launch_bullet_fused(const pt_niels* M, size_t npts, const fr_t* a_in, const
   LB_LAUNCH_CHECK();
 }
 
-// nrows (<= 8) short MSMs over the multiples table; the points go to mapped host memory (msm_finish_quad_kernel)
+// two short MSMs over the multiples table; the points go to mapped host memory (msm_finish_quad_kernel)
 int msm_direct_chunks(int len, int heavy_rows) {
   int c = (len * kMsmFullWindows + 128 * 4 - 1) / (128 * 4);  // ~4 entries per quad
   if (heavy_rows < 1) heavy_rows = 1;
@@ -881,14 +872,13 @@ int msm_direct_chunks(int len, int heavy_rows) {
   if (c < 1) c = 1;
   return c | 1;
 }
-void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, const uint32_t* cols, int nrows, int len,
-                       int heavy_rows, pt_ext* partials, uint32_t* out_raw, const PubDst& pub, cudaStream_t st) {
-  if (nrows < 1 || nrows > 8) throw std::runtime_error("msm_direct: 1..8 rows");
-  const int nchunks = msm_direct_chunks(len, heavy_rows);
+void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, pt_ext* partials, const PubDst& pub,
+                       cudaStream_t st) {
+  const int nrows = 2, nchunks = msm_direct_chunks(len, 1);
   dim3 grid(nchunks, nrows);
-  msm_direct_kernel<<<grid, MSMD_T, 0, st>>>(M, npts, scalars, cols, len, partials);
+  msm_direct_kernel<<<grid, MSMD_T, 0, st>>>(M, npts, scalars, len, partials);
   LB_LAUNCH_CHECK();
-  msm_finish_quad_kernel<<<1, 128 * nrows, 0, st>>>(partials, nrows, nchunks, out_raw, pub);
+  msm_finish_quad_kernel<<<1, 128 * nrows, 0, st>>>(partials, nrows, nchunks, pub);
   LB_LAUNCH_CHECK();
 }
 

@@ -186,8 +186,8 @@ __global__ void __launch_bounds__(kThreads)
 // over the polynomials: thread i owns the four elements i, i+q, i+2q, i+3q of every polynomial (q = a quarter of
 // the length before the bind), folds them to the two elements i, i+q of the bound polynomial, stores those in place
 // and feeds them to round j's sums.  192 B per poly per i instead of 96 + 96 (bind) + 64 + 64 (evaluation).
-template <int MINB>
-__global__ void __launch_bounds__(kThreads, MINB)
+// Compiled for 2 resident CTAs per SM (128 registers); the grid is one wave of those.
+__global__ void __launch_bounds__(kThreads, 2)
     sc_bind_eval_linear_kernel(fr_t* base, size_t stride, int alpha, size_t q, fr_t r, int inc, Finalize fin) {
   __shared__ fr_t scratch[3 * kThreads / 32];
   fr_t acc[3] = {fr_zero(), fr_zero(), fr_zero()};
@@ -450,14 +450,8 @@ bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t s
                                          const Finalize& fin, size_t min_q, cudaStream_t st) {
   static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
   if (S.kind == STRAT_LT || q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
-  // resident CTAs per SM the kernel is compiled for: 2 (128 registers) or 3 (80 registers, a few spilled words);
-  // the grid is one wave of those
-  static const int minb = bind_env("LASSO_B200_FUSED_MINB", 2);
-  const int alpha = S.num_memories(), inc = linear_inc(S);
-  if (minb == 3)
-    sc_bind_eval_linear_kernel<3><<<grid_for(q, kThreads, kNumSMs * 3), kThreads, 0, st>>>(base, stride, alpha, q, r, inc, fin);
-  else
-    sc_bind_eval_linear_kernel<2><<<grid_for(q, kThreads, kNumSMs * 2), kThreads, 0, st>>>(base, stride, alpha, q, r, inc, fin);
+  sc_bind_eval_linear_kernel<<<grid_for(q, kThreads, kNumSMs * 2), kThreads, 0, st>>>(base, stride, S.num_memories(), q, r,
+                                                                                       linear_inc(S), fin);
   LB_LAUNCH_CHECK();
   return true;
 }
@@ -505,29 +499,7 @@ void launch_sumcheck_claim(const Strategy& S, const fr_t* base, size_t stride, s
 }
 
 // ------------------------------------------------------------------------------------ K3
-// sumcheck.rs:49-93: per circuit (e0, e2, e3) = sum_i A B C at t = 0, 2, 3.
-__global__ void __launch_bounds__(kThreads)
-    sc_eval_cubic_kernel(fr_t* const* A, fr_t* const* B, const fr_t* Ceq, size_t half, Finalize fin) {
-  __shared__ fr_t scratch[3 * kThreads / 32];
-  const fr_t* a = A[blockIdx.y];
-  const fr_t* b = B[blockIdx.y];
-  fr_t acc[3] = {fr_zero(), fr_zero(), fr_zero()};
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
-    fr_t a0 = ld_fr_stream(a + i), a1 = ld_fr_stream(a + half + i);
-    fr_t b0 = ld_fr_stream(b + i), b1 = ld_fr_stream(b + half + i);
-    fr_t c0 = ld_fr(Ceq + i), c1 = ld_fr(Ceq + half + i);
-    acc[0] = fr_add(acc[0], fr_mul(fr_mul(a0, b0), c0));
-    fr_t da = fr_sub(a1, a0), db = fr_sub(b1, b0), dc = fr_sub(c1, c0);
-    fr_t a2 = fr_add(a1, da), b2 = fr_add(b1, db), c2 = fr_add(c1, dc);
-    acc[1] = fr_add(acc[1], fr_mul(fr_mul(a2, b2), c2));
-    fr_t a3 = fr_add(a2, da), b3 = fr_add(b2, db), c3 = fr_add(c2, dc);
-    acc[2] = fr_add(acc[2], fr_mul(fr_mul(a3, b3), c3));
-  }
-  block_sum_fr<3>(acc, scratch);
-  // value index = circuit*3 + t
-  finalize_block<3>(fin, acc, blockIdx.y * 3, blockIdx.x, gridDim.x, 3 * gridDim.y, gridDim.x * gridDim.y);
-}
-// ---- the same rounds with the batching coefficients folded in (what the prover runs) --------------------------
+// sumcheck.rs:49-93: per circuit (e0, e2, e3) = sum_i A B C at t = 0, 2, 3, with the batching coefficients folded in.
 // prove_cubic_batched only ever uses  sum_k coeff_k * (e0, e2, e3)_k  (sumcheck.rs:95-104), and everything in a
 // round is linear in A_k.  So the FIRST bind of a layer stores coeff_k * A_k, every later round works on the
 // scaled arrays, and a round evaluates  sum_i C_i(t) * sum_k A'_k,i(t) B_k,i(t):  per element pair 7
@@ -631,10 +603,10 @@ __global__ void __launch_bounds__(kThreads)
 //   do_bind = 0: arrays hold 2q elements, evaluated as (i, i+q)               (q a power of two)
 __global__ void __launch_bounds__(1024)
     sc_cubic_quad_kernel(fr_t* const* A, fr_t* const* B, const fr_t* Cin, fr_t* Cout, size_t q, int lg_q, int do_bind,
-                         fr_t r, int ncirc, CubicCoeffs cf, int scale, int comb, Finalize fin) {
-  // cf / scale / comb: see the combined kernels above — scale: lane 0 multiplies its side by coeff_k (stored when
-  // binding); comb: the CTA yields 3 values (summed over all its circuits) instead of 3 per circuit
-  __shared__ fr_t s_part[256 * 3];
+                         fr_t r, int ncirc, CubicCoeffs cf, int scale, Finalize fin) {
+  // cf / scale: see the kernels above — scale: lane 0 multiplies its side by coeff_k (stored when binding); the CTA
+  // yields 3 values, summed over all its circuits
+  __shared__ fr_t s_part[32 * 3];  // per warp
   __shared__ int s_last;
   const int tid = threadIdx.x, role = tid & 3, lane = tid & 31;
   const int upb = blockDim.x >> 2;  // (circuit, pair) units per CTA
@@ -683,66 +655,50 @@ __global__ void __launch_bounds__(1024)
     P = j == 0 ? got : fr_mul(P, got);
   }
   if (!valid || role == 3) P = fr_zero();
-  // sum over the pair indices of a circuit: gq = min(q, 8) consecutive units of a warp belong to one circuit
-  // (combined: all 8 units of the warp, whatever their circuit)
-  const int gq = comb ? 8 : (q < 8 ? (int)q : 8);
-  for (int off = 1; off < gq; off <<= 1) {
+  // sum over the 8 units of the warp, whatever their circuit
+  for (int off = 1; off < 8; off <<= 1) {
     fr_t o;
 #pragma unroll
     for (int l = 0; l < 8; l++) o.v[l] = __shfl_xor_sync(0xffffffffu, P.v[l], off * 4);
     P = fr_add(P, o);
   }
   const int unit = tid >> 2;
-  if ((unit & (gq - 1)) == 0 && role < 3) s_part[(unit / gq) * 3 + role] = P;
+  if ((unit & 7) == 0 && role < 3) s_part[(unit / 8) * 3 + role] = P;
   __syncthreads();
-  // block outputs: cpb circuits x 3 values, each the sum of gpc group partials (combined: 3 values, all warps)
-  const int cpb = q >= (size_t)upb ? 1 : upb >> lg_q;
-  const int gpc = (int)((q >= (size_t)upb ? (size_t)upb : q) / gq);
-  const int bpv = comb ? (int)gridDim.x : (q >= (size_t)upb ? (int)(q / upb) : 1);  // CTAs per value
-  int v = -1;
+  // block outputs: 3 values, each the sum over all warps
   fr_t val = fr_zero();
-  if (comb) {
-    if (tid < 3) {
-      const int nw = blockDim.x >> 5;
-      for (int w = 0; w < nw; w++) val = fr_add(val, s_part[w * 3 + tid]);
-      v = tid;
-    }
-  } else if (tid < cpb * 3) {
-    const int cl = tid / 3, t = tid - 3 * cl;
-    const int kk = q >= (size_t)upb ? (int)(blockIdx.x / bpv) : (int)blockIdx.x * cpb + cl;
-    if (kk < ncirc) {
-      for (int w = 0; w < gpc; w++) val = fr_add(val, s_part[(cl * gpc + w) * 3 + t]);
-      v = kk * 3 + t;
-    }
+  if (tid < 3) {
+    const int nw = blockDim.x >> 5;
+    for (int w = 0; w < nw; w++) val = fr_add(val, s_part[w * 3 + tid]);
   }
   if (gridDim.x == 1) {
-    if (v >= 0) finalize_publish(fin, v, val);
+    if (tid < 3) finalize_publish(fin, tid, val);
     return;
   }
-  if (v >= 0) {
-    fin.partial[(size_t)v * bpv + (blockIdx.x % bpv)] = val;
+  if (tid < 3) {
+    fin.partial[(size_t)tid * gridDim.x + blockIdx.x] = val;
     __threadfence();
   }
   __syncthreads();
   if (tid == 0) s_last = (atomicAdd(fin.counter, 1u) == gridDim.x - 1);
   __syncthreads();
   if (!s_last) return;
-  finalize_last_stage(fin, bpv, comb ? 3 : 3 * ncirc);
+  finalize_last_stage(fin, gridDim.x, 3);
 }
 static constexpr size_t kQuadMaxQ = 2048;  // beyond this the rounds are throughput-bound: thread-per-pair kernels
 static void launch_cubic_quad(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Cin, fr_t* Cout, int ncirc, size_t q,
-                              int do_bind, const fr_t& r, const CubicCoeffs& cf, int scale, int comb, const Finalize& fin,
+                              int do_bind, const fr_t& r, const CubicCoeffs& cf, int scale, const Finalize& fin,
                               cudaStream_t st) {
   int lg_q = 0;
   while (((size_t)1 << lg_q) < q) lg_q++;
   const size_t threads = 4 * (size_t)ncirc * q;
   if (threads <= 1024) {
     unsigned t = (unsigned)((threads + 31) / 32 * 32);
-    sc_cubic_quad_kernel<<<1, t, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, comb, fin);
+    sc_cubic_quad_kernel<<<1, t, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
     LB_LAUNCH_CHECK();
   } else {
     unsigned blocks = (unsigned)(((size_t)ncirc * q + 63) / 64);
-    sc_cubic_quad_kernel<<<blocks, 256, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, comb, fin);
+    sc_cubic_quad_kernel<<<blocks, 256, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
     LB_LAUNCH_CHECK();
   }
 }
@@ -757,29 +713,15 @@ static dim3 comb_grid(size_t pairs, int ncirc) {
 void launch_sumcheck_bind_eval_cubic_comb(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Cin, fr_t* Cout, int ncirc, size_t h,
                                           const fr_t& r, const CubicCoeffs& cf, int scale, const Finalize& fin, cudaStream_t st) {
   size_t q = h / 2;
-  if (q <= kQuadMaxQ && (q & (q - 1)) == 0) return launch_cubic_quad(d_A, d_B, Cin, Cout, ncirc, q, 1, r, cf, scale, 1, fin, st);
+  if (q <= kQuadMaxQ && (q & (q - 1)) == 0) return launch_cubic_quad(d_A, d_B, Cin, Cout, ncirc, q, 1, r, cf, scale, fin, st);
   sc_bind_eval_cubic_comb_kernel<<<comb_grid(q, ncirc), kThreads, 0, st>>>(d_A, d_B, Cin, Cout, h, r, ncirc, cf, scale, fin);
   LB_LAUNCH_CHECK();
 }
 void launch_sumcheck_eval_cubic_comb(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Ceq, int ncirc, size_t half,
                                      const CubicCoeffs& cf, int scale, const Finalize& fin, cudaStream_t st) {
   if (half <= kQuadMaxQ && (half & (half - 1)) == 0)
-    return launch_cubic_quad(d_A, d_B, Ceq, nullptr, ncirc, half, 0, fr_zero(), cf, scale, 1, fin, st);
+    return launch_cubic_quad(d_A, d_B, Ceq, nullptr, ncirc, half, 0, fr_zero(), cf, scale, fin, st);
   sc_eval_cubic_comb_kernel<<<comb_grid(half, ncirc), kThreads, 0, st>>>(d_A, d_B, Ceq, half, ncirc, cf, scale, fin);
-  LB_LAUNCH_CHECK();
-}
-// per-circuit outputs (e0, e2, e3)_k, no batching coefficients: the per-loop C-ABI entry lasso_sumcheck_round_cubic
-void launch_sumcheck_eval_cubic(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Ceq, int ncirc, size_t half,
-                                const Finalize& fin, cudaStream_t st) {
-  if (half <= kQuadMaxQ && (half & (half - 1)) == 0) {
-    CubicCoeffs none;
-    return launch_cubic_quad(d_A, d_B, Ceq, nullptr, ncirc, half, 0, fr_zero(), none, 0, 0, fin, st);
-  }
-  int per = kMaxBlocks / ncirc;
-  if (per < 1) per = 1;
-  int bx = grid_for(half, kThreads, per);
-  dim3 grid(bx, ncirc);
-  sc_eval_cubic_kernel<<<grid, kThreads, 0, st>>>(d_A, d_B, Ceq, half, fin);
   LB_LAUNCH_CHECK();
 }
 
@@ -854,62 +796,8 @@ void launch_fill_zero(fr_t* out, size_t n, cudaStream_t st) {
 }
 
 // ------------------------------------------------------------------------------------ K7
-// dense_mlpoly.rs:228-235 + utils/mod.rs:63-73 with the eq table shared by all polynomials
-__global__ void __launch_bounds__(kThreads)
-    multi_dot_kernel(const fr_t* base, size_t stride, const fr_t* eq, size_t n, fr_t* partial) {
-  __shared__ fr_t scratch[kThreads / 32];
-  const fr_t* P = base + (size_t)blockIdx.y * stride;
-  fr_t acc[1] = {fr_zero()};
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
-    acc[0] = fr_add(acc[0], fr_mul(ld_fr_stream(P + i), ld_fr(eq + i)));
-  block_sum_fr<1>(acc, scratch);
-  if (threadIdx.x == 0) partial[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = acc[0];
-}
-void launch_multi_dot(const fr_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial,
-                      fr_t* out, cudaStream_t st) {
-  int per = kMaxBlocks / npolys;
-  if (per < 1) per = 1;
-  int bx = grid_for(n, kThreads, per);
-  dim3 grid(bx, npolys);
-  multi_dot_kernel<<<grid, kThreads, 0, st>>>(base, stride, eq, n, partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
-  LB_LAUNCH_CHECK();
-}
-
-// dense_mlpoly.rs:183-207: LZ[i] = sum_j L[j] Z[j*R + i].  Thread = column (coalesced across the
-// warp), rows split into chunks over blockIdx.y, second pass sums the chunk partials.
-static constexpr int kBoundChunks = 64;
-int bound_max_chunks() { return kBoundChunks; }
-__global__ void __launch_bounds__(kThreads)
-    bound_kernel(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, size_t rows_per_chunk, fr_t* partial) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= R_size) return;
-  size_t j0 = (size_t)blockIdx.y * rows_per_chunk, j1 = j0 + rows_per_chunk;
-  if (j1 > L_size) j1 = L_size;
-  fr_t acc = fr_zero();
-  for (size_t j = j0; j < j1; j++) acc = fr_add(acc, fr_mul(L[j], ld_fr_stream(Z + j * R_size + i)));
-  st_fr(partial + (size_t)blockIdx.y * R_size + i, acc);
-}
-__global__ void __launch_bounds__(kThreads) bound_reduce_kernel(const fr_t* partial, int chunks, size_t R_size, fr_t* out) {
-  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= R_size) return;
-  fr_t acc = fr_zero();
-  for (int c = 0; c < chunks; c++) acc = fr_add(acc, ld_fr(partial + (size_t)c * R_size + i));
-  st_fr(out + i, acc);
-}
-void launch_bound(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out,
-                  cudaStream_t st) {
-  int chunks = (int)(L_size < (size_t)kBoundChunks ? L_size : (size_t)kBoundChunks);
-  size_t rows_per_chunk = (L_size + chunks - 1) / chunks;
-  dim3 grid((unsigned)((R_size + kThreads - 1) / kThreads), chunks);
-  bound_kernel<<<grid, kThreads, 0, st>>>(Z, L, L_size, R_size, rows_per_chunk, partial);
-  LB_LAUNCH_CHECK();
-  bound_reduce_kernel<<<(unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st>>>(partial, chunks, R_size, out);
-  LB_LAUNCH_CHECK();
-}
-
-// ---- the same two reductions for INTEGER-valued polynomials (dim, read, final, E: everything the prover commits to and
+// dense_mlpoly.rs:183-207 (bound) and dense_mlpoly.rs:228-235 + utils/mod.rs:63-73 (dot products with one eq table)
+// for INTEGER-valued polynomials (dim, read, final, E: everything the prover commits to and
 // opens is an index, a counter or a table value < 2^32, kept as a u32 mirror next to the field form).  A field element
 // times a 32-bit integer is 8 IMAD.WIDE instead of a ~235-instruction Montgomery product, and the sum can be carried
 // as a plain 320-bit integer (X = sum_j L_j * z_j < 2^288 * #terms) and reduced ONCE: L_j is stored as L_j*R mod l, so
@@ -942,7 +830,10 @@ __device__ __forceinline__ fr_t wide_reduce(const wide_t& a) {
   const fr_t lo_mod = fr_to_canonical(fr_from_raw_int(lo));
   return fr_add(lo_mod, fr_from_u64((uint64_t)a.v[8] | ((uint64_t)a.v[9] << 32)));
 }
-// LZ[i] = sum_j L[j] z[j*R + i]: thread = column, rows split into chunks over blockIdx.y (<= 2^20 rows per chunk)
+// LZ[i] = sum_j L[j] z[j*R + i]: thread = column (coalesced across the warp), rows split into chunks over blockIdx.y
+// (<= 2^20 rows per chunk), a second pass sums the chunk partials
+static constexpr int kBoundChunks = 64;
+int bound_max_chunks() { return kBoundChunks; }
 __global__ void __launch_bounds__(kThreads)
     bound_u32_kernel(const uint32_t* Z, const fr_t* L, size_t L_size, size_t R_size, size_t rows_per_chunk, fr_t* partial) {
   __shared__ fr_t sL[64];
@@ -961,6 +852,13 @@ __global__ void __launch_bounds__(kThreads)
       for (size_t j = jb; j < je; j++) wide_mad(acc, sL[j - jb], Z[j * R_size + i]);
   }
   if (i < R_size) st_fr(partial + (size_t)blockIdx.y * R_size + i, wide_reduce(acc));
+}
+__global__ void __launch_bounds__(kThreads) bound_reduce_kernel(const fr_t* partial, int chunks, size_t R_size, fr_t* out) {
+  size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R_size) return;
+  fr_t acc = fr_zero();
+  for (int c = 0; c < chunks; c++) acc = fr_add(acc, ld_fr(partial + (size_t)c * R_size + i));
+  st_fr(out + i, acc);
 }
 void launch_bound_u32(const uint32_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out, cudaStream_t st) {
   int chunks = (int)(L_size < (size_t)kBoundChunks ? L_size : (size_t)kBoundChunks);
@@ -1032,17 +930,8 @@ void launch_gp_fingerprints_ops(const fr_t* dim_fr, const fr_t* E_fr, const fr_t
                                                   out_write);
   LB_LAUNCH_CHECK();
 }
-// grand_product.rs:20-36 with the layer stored contiguously as [left | right]
-__global__ void __launch_bounds__(kThreads) product_layer_kernel(const fr_t* in, fr_t* out, size_t n_out) {
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n_out; i += (size_t)gridDim.x * blockDim.x)
-    st_fr(out + i, fr_mul(ld_fr_stream(in + i), ld_fr_stream(in + n_out + i)));
-}
-void launch_product_layer(const fr_t* in, fr_t* out, size_t n_out, cudaStream_t st) {
-  product_layer_kernel<<<grid_for(n_out), kThreads, 0, st>>>(in, out, n_out);
-  LB_LAUNCH_CHECK();
-}
 
-// All product trees of one size at once (single GPU).  A tree is one contiguous array: layer 0 (N elements),
+// grand_product.rs:20-58, all product trees of one size at once (single GPU).  A tree is one contiguous array: layer 0 (N elements),
 // then layer 1 (N/2), ...; layer k+1[i] = layer k[i] * layer k[i + len/2].  One launch per layer for every
 // tree (blockIdx.y) while the layers are large, then ONE CTA per tree walks the remaining small layers with
 // a barrier in between and publishes the two elements of the top layer (grand_product.rs:60-65 `evaluate`)
@@ -1176,91 +1065,6 @@ __global__ void __launch_bounds__(kThreads)
 void launch_bullet_scalars(const fr_t* a, const fr_t* w, size_t n_loc, size_t m, int G, int g, int a_rep, fr_t* sL,
                            fr_t* sR, cudaStream_t st) {
   bullet_scalars_kernel<<<grid_for(n_loc), kThreads, 0, st>>>(a, w, n_loc, m, G, g, a_rep, sL, sR);
-  LB_LAUNCH_CHECK();
-}
-// One Bulletproofs round's scalar side in ONE launch (single GPU): fold a, b with the previous round's
-// challenge (bullet.rs:127-130), expand the generator weights, form the L / R scalars of the unfolded
-// generators in canonical form, and (last CTA, Finalize ticket) the cross inner products c_L, c_R
-// (bullet.rs:78-79) + blinds as the two tail columns (Q, h).  Replaces fold_ab + expand_weights + cross_ip +
-// reduce + bullet_scalars + set_tail + canonicalize: seven launches of a few microseconds each on the
-// critical path of every round.
-//   a_in, b_in : length 2m when fold != 0 (folded here into a_out, b_out of length m), else length m
-//   w_in       : n/(2m) weights when fold != 0 (expanded into w_out, n/m weights), else n/m weights
-//   s_out      : 2 rows x (n/2 + 2) canonical scalars, row 0 = L, row 1 = R, with the generator index of every
-//                term in cols_out (same shape): each generator is in exactly one of L, R, so the rows are
-//                stored compacted; the last two terms of a row are (c, blind) on the generators n (Q), n+1 (h)
-// Thread j <-> generator column j = t*m + pos.  h = m/2:  L gets a'[pos-h] w'[t] G_j for pos >= h (term t*h +
-// pos-h), R gets a'[pos+h] w'[t] G_j for pos < h (term t*h + pos).  Threads j < h also own the pair (pos, pos+h)
-// of a', b'.
-__global__ void __launch_bounds__(kThreads)
-    bullet_round_kernel(const fr_t* a_in, const fr_t* b_in, const fr_t* w_in, fr_t* a_out, fr_t* b_out, fr_t* w_out,
-                        size_t n, size_t m, int fold, fr_t u, fr_t uinv, fr_t blind_L, fr_t blind_R, fr_t* s_out,
-                        uint32_t* cols_out, fr_t* partial, unsigned* counter) {
-  __shared__ fr_t scratch[2 * kThreads / 32];
-  __shared__ int s_last;
-  const size_t h = m / 2, stride = n / 2 + 2;
-  const int lg_m = 63 - __clzll((long long)m);
-  fr_t acc[2] = {fr_zero(), fr_zero()};
-  auto folded_a = [&](size_t i) {
-    return fold ? fr_add(fr_mul(ld_fr(a_in + i), u), fr_mul(uinv, ld_fr(a_in + m + i))) : ld_fr(a_in + i);
-  };
-  auto folded_b = [&](size_t i) {
-    return fold ? fr_add(fr_mul(ld_fr(b_in + i), uinv), fr_mul(u, ld_fr(b_in + m + i))) : ld_fr(b_in + i);
-  };
-  const size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (j < n) {
-    const size_t t = j >> lg_m, pos = j & (m - 1);  // m is a power of two
-    fr_t wt = fold ? fr_mul(ld_fr(w_in + (t >> 1)), (t & 1) ? u : uinv) : ld_fr(w_in + t);
-    if (pos == 0 && fold) st_fr(w_out + t, wt);
-    const bool is_l = pos >= h;
-    const size_t idx = is_l ? pos - h : pos + h;
-    const fr_t ai = folded_a(idx);
-    const fr_t sc = fr_to_canonical(fr_mul(ai, wt));
-    const size_t term = (is_l ? 0 : stride) + t * h + (is_l ? pos - h : pos);
-    st_fr(s_out + term, sc);
-    cols_out[term] = (uint32_t)j;
-    if (t == 0 && pos < h) {  // owner of the pair (pos, pos + h): ai = a'[pos + h]
-      const fr_t alo = folded_a(pos), blo = folded_b(pos), bhi = folded_b(idx);
-      if (fold) {
-        st_fr(a_out + pos, alo);
-        st_fr(a_out + idx, ai);
-        st_fr(b_out + pos, blo);
-        st_fr(b_out + idx, bhi);
-      }
-      acc[0] = fr_mul(alo, bhi);  // c_L = <a_lo, b_hi>
-      acc[1] = fr_mul(ai, blo);   // c_R = <a_hi, b_lo>
-    }
-  }
-  block_sum_fr<2>(acc, scratch);
-  if (threadIdx.x == 0) {
-    partial[blockIdx.x] = acc[0];
-    partial[gridDim.x + blockIdx.x] = acc[1];
-    __threadfence();
-    s_last = (atomicAdd(counter, 1u) == gridDim.x - 1);
-  }
-  __syncthreads();
-  if (!s_last) return;
-  __threadfence();
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  if (warp < 2) {
-    fr_t v = fr_zero();
-    for (unsigned i = lane; i < gridDim.x; i += 32) v = fr_add(v, ld_fr_cg(partial + (size_t)warp * gridDim.x + i));
-    v = warp_sum_fr(v);
-    if (lane == 0) {
-      st_fr(s_out + (size_t)warp * stride + n / 2, fr_to_canonical(v));
-      st_fr(s_out + (size_t)warp * stride + n / 2 + 1, fr_to_canonical(warp == 0 ? blind_L : blind_R));
-      cols_out[(size_t)warp * stride + n / 2] = (uint32_t)n;
-      cols_out[(size_t)warp * stride + n / 2 + 1] = (uint32_t)(n + 1);
-    }
-  }
-  if (threadIdx.x == 0) *counter = 0;
-}
-void launch_bullet_round(const fr_t* a_in, const fr_t* b_in, const fr_t* w_in, fr_t* a_out, fr_t* b_out, fr_t* w_out, size_t n,
-                         size_t m, int fold, const fr_t& u, const fr_t& uinv, const fr_t& blind_L, const fr_t& blind_R,
-                         fr_t* s_out, uint32_t* cols_out, fr_t* partial, unsigned* counter, cudaStream_t st) {
-  unsigned blocks = (unsigned)((n + kThreads - 1) / kThreads);
-  bullet_round_kernel<<<blocks, kThreads, 0, st>>>(a_in, b_in, w_in, a_out, b_out, w_out, n, m, fold, u, uinv, blind_L,
-                                                   blind_R, s_out, cols_out, partial, counter);
   LB_LAUNCH_CHECK();
 }
 // Two MSM rows over the n + 2 generators (G_0..G_{n-1}, Q, h) in canonical form:

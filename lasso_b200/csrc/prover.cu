@@ -223,18 +223,13 @@ Ctx* ctx_create(int device) {
   LB_CUDA_CHECK(cudaMalloc((void**)&c->d_eq_scratch, (size_t)(4096 + (1 << 17) + 4096) * sizeof(fr_t)));
   LB_CUDA_CHECK(cudaMalloc((void**)&c->d_flag, 64));
   LB_CUDA_CHECK(cudaMemset(c->d_flag, 0, 64));
-  {
-    const char* nm = getenv("LASSO_B200_NO_MAPPED");
-    if (!(nm && nm[0] == '1')) {
-      LB_CUDA_CHECK(cudaHostAlloc((void**)&c->h_mapped, Ctx::kMappedBytes, cudaHostAllocMapped));
-      memset(c->h_mapped, 0, Ctx::kMappedBytes);
-      LB_CUDA_CHECK(cudaHostGetDevicePointer((void**)&c->d_mapped, c->h_mapped, 0));
-      LB_CUDA_CHECK(cudaHostAlloc((void**)&c->h_pub, Ctx::kPubBytes, cudaHostAllocMapped));
-      memset(c->h_pub, 0, Ctx::kPubBytes);
-      c->h_pub_owned = true;
-      LB_CUDA_CHECK(cudaHostGetDevicePointer((void**)&c->d_pub_reader[0], c->h_pub, 0));
-    }
-  }
+  LB_CUDA_CHECK(cudaHostAlloc((void**)&c->h_mapped, Ctx::kMappedBytes, cudaHostAllocMapped));
+  memset(c->h_mapped, 0, Ctx::kMappedBytes);
+  LB_CUDA_CHECK(cudaHostGetDevicePointer((void**)&c->d_mapped, c->h_mapped, 0));
+  LB_CUDA_CHECK(cudaHostAlloc((void**)&c->h_pub, Ctx::kPubBytes, cudaHostAllocMapped));
+  memset(c->h_pub, 0, Ctx::kPubBytes);
+  c->h_pub_owned = true;
+  LB_CUDA_CHECK(cudaHostGetDevicePointer((void**)&c->d_pub_reader[0], c->h_pub, 0));
   msm_init_device();      // per-device function attributes (dynamic shared memory opt-in)
   msm_large_init_device();
   densify_init_device();
@@ -355,31 +350,17 @@ __global__ void publish_fr_kernel(const fr_t* src, int count, PubDst pub) {
     pub_store(pub, v, x.v);
   }
 }
-// In two halves so that host work can sit between the launch and the wait; `f.pub.ndst == 0` after _begin: no
-// publication buffers, _end copies synchronously.
-static Finalize reduce_to_host_begin(Ctx* c, fr_t* d_buf, int count) {
-  if (!c->h_pub || count > kPubElems) {
-    if (c->world > 1) throw std::runtime_error("sharded proof without publication buffers");
-    Finalize f{};
-    f.pub.ndst = 0;
-    return f;
-  }
+// In two halves so that host work can sit between the launch and the wait.
+static Finalize reduce_to_host_begin(Ctx* c, const fr_t* d_buf, int count) {
+  if (count > kPubElems) throw std::runtime_error("message larger than a publication region");
   Finalize f = c->fin_begin(true);
   publish_fr_kernel<<<1, 128, 0, c->st>>>(d_buf, count, f.pub);
   LB_LAUNCH_CHECK();
   g_launches += 1;
   return f;
 }
-static void reduce_to_host_end(Ctx* c, const Finalize& f, fr_t* d_buf, int count, fr_t* h_out) {
-  if (f.pub.ndst == 0) {
-    c->d2h(h_out, d_buf, (size_t)count * sizeof(fr_t));
-    return;
-  }
-  c->fin_wait(f, h_out, count);
-}
-static void reduce_to_host(Ctx* c, fr_t* d_buf, int count, fr_t* h_out) {
-  const Finalize f = reduce_to_host_begin(c, d_buf, count);
-  reduce_to_host_end(c, f, d_buf, count, h_out);
+static void reduce_to_host(Ctx* c, const fr_t* d_buf, int count, fr_t* h_out) {
+  c->fin_wait(reduce_to_host_begin(c, d_buf, count), h_out, count);
 }
 // this rank's shard of eq(r[off .. off+ell)) (eq_poly.rs:21-38): eq[i*G + g] = eq_hi[i] * eq_lo[g] where
 // eq_lo is the table of the LAST log2(G) coordinates (they bind the low index bits: r[0] <-> MSB)
@@ -820,10 +801,7 @@ static SumcheckProof prove_arbitrary(Ctx* c, const Strategy& S, fr_t* base, size
         flush_bind();
         launch_sumcheck_eval_arbitrary(S, base, stride, half, f, c->st);
       }
-      if (f.pub.ndst)
-        c->fin_wait(f, evals.data(), npts);
-      else
-        c->d2h(evals.data(), c->d_small, (size_t)npts * sizeof(fr_t));
+      c->fin_wait(f, evals.data(), npts);
     }
     g_launches += 1;
     std::vector<fr_t> coeffs = unipoly_from_evals(evals);
@@ -878,12 +856,6 @@ static void circuit_alloc(Ctx* c, Circuit& ci, size_t N, fr_t* rtree_slot) {
   if (ci.G > 1) {
     ci.k_rep = ci.num_layers - (size_t)c->lg_world;
     ci.rtree = rtree_slot;
-  }
-}
-static void build_tree(Ctx* c, Circuit& ci) {  // grand_product.rs:38-58 (layer 0 already filled); single GPU, tree by tree
-  for (size_t k = 0; k + 1 < ci.num_layers; k++) {
-    launch_product_layer(ci.layer_local(k), ci.layer_local(k + 1), ci.layer_len_global(k + 1), c->st);
-    g_launches += 1;
   }
 }
 // All product trees, size by size, layer by layer in batched launches (poly_kernels.cu).  groups[i] = trees of one
@@ -1053,10 +1025,7 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
       }
       size_t half = cur / 2;
       auto tp0 = std::chrono::steady_clock::now();
-      if (fz.pub.ndst)  // sharded: the three sums of every rank, added here
-        c->fin_wait(fz, ev.data(), 3);
-      else
-        c->d2h(ev.data(), c->d_small, ev.size() * sizeof(fr_t));
+      c->fin_wait(fz, ev.data(), 3);  // sharded: the three sums of every rank, added here
       auto tp1 = std::chrono::steady_clock::now();
       const fr_t c0 = ev[0], c2 = ev[1], c3 = ev[2];  // already combined over the circuits (sumcheck.rs:95-97)
       std::vector<fr_t> evals = {c0, fr_sub(e, c0), c2, c3};  // eval(1) = e - eval(0), sumcheck.rs:99-104
@@ -1073,7 +1042,7 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
         g_launches += 1;
         std::swap(Ccur, Cnext);
         have_evals = true;
-      } else if (!sharded && fz.pub.ndst) {
+      } else if (!sharded) {
         // last round: bind the 2*ncirc heads and publish them (the layer's claims); eq is not needed any more
         fz = c->fin_begin();
         launch_bind_heads(dAB, 2 * ncirc, r_j, fz, c->st);
@@ -1162,13 +1131,13 @@ __global__ void set_elems_kernel(fr_t* dst, fr_t a, fr_t b) {
 }
 
 // PolyEvalProof::prove (dense_mlpoly.rs:301-359) -> DotProductProofLog::prove (dot_product.rs:166-249)
-// -> BulletReductionProof::prove (bullet.rs:40-154).  Z: this rank's shard of a polynomial of 2^nv elements,
-// i.e. for every one of the L rows the R/G columns congruent to the rank.
+// -> BulletReductionProof::prove (bullet.rs:40-154).  Z_u32: this rank's shard of an integer-valued polynomial of
+// 2^nv elements, i.e. for every one of the L rows the R/G columns congruent to the rank.
 // One proof sharded over G GPUs: LZ = L . Z is computed on the column shards and all-gathered (R elements); from
 // there on the opening runs REPLICATED on every rank — its vectors are only R = 2^(nv - nv/2) long and every round
 // is latency-bound, so splitting its two-row MSMs would add an exchange per round and save nothing.  Every rank
 // computes the same points and the same transcript.
-static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t* Z, const uint32_t* Z_u32, size_t nv,
+static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const uint32_t* Z_u32, size_t nv,
                                                const std::vector<fr_t>& r, const fr_t& Zr, Transcript& transcript,
                                                RandomTape& tape) {
   SpanTimer sp(c, "DensePolyEval.prove");
@@ -1185,11 +1154,8 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
   eq_evals_dev(c, r, 0, lv, Lvec.p);  // rows are not sharded: L is replicated
   eq_evals_dev(c, r, lv, rv, b.p);    // a_vec of the dot product proof = R
   if ((size_t)bound_max_chunks() * n_loc > c->partial_elems) throw std::runtime_error("bound scratch too small");
-  // x_vec = LZ (this rank's columns); the opened polynomials are integer-valued: over their u32 mirror when there is one
-  if (Z_u32)
-    launch_bound_u32(Z_u32, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
-  else
-    launch_bound(Z, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
+  // x_vec = LZ (this rank's columns) over the u32 mirror of the polynomial
+  launch_bound_u32(Z_u32, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
   g_launches += 2;
   if (G > 1) comm_gather_vector(c, a_loc.p, n_loc, a_gath.p, a.p);
 
@@ -1203,7 +1169,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
   std::vector<fr_t> v2 = tape.random_vector("blinds_vec_2", 2 * lg_n);
   DotProductProofLogBytes out;
   // table pipeline below: needs the multiples table of the generators 0 .. n+1
-  const bool fast = c->h_pub != nullptr && n * 32 <= c->h_pin_bytes && g.d_multiples.p && n + 2 <= g.n_direct;
+  const bool fast = n * 32 <= c->h_pin_bytes && g.d_multiples.p && n + 2 <= g.n_direct;
   // ---- BulletReductionProof::prove with unfolded generators (see file header)
   fr_t blind_fin = fr_zero();  // blind_Gamma = blind_x + blind_y = 0
   DBuf<fr_t> W0(c, n), W1(c, n), sLR(c, 2 * (n + 2));
@@ -1218,11 +1184,12 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
   fr_t* bv = b.p;
   DBuf<fr_t> a_alt, b_alt;
   if (fast) {
-    // Per message ONE scalar kernel + the two MSM kernels, the finish kernel publishing straight to mapped host
-    // memory; the host part of a message (compression, Fiat-Shamir) overlaps the device work of the next one
-    // wherever the transcript allows it.
-    //   (Cx, Cy): rows (x_vec, 0, 0) and (0.., y, 0) of one two-row MSM        (dot_product.rs:192-197)
-    //   round k : fold with u_{k-1}, weights, L/R scalars, c_L, c_R -> two-row MSM   (bullet.rs:73-134)
+    // Every point goes straight to mapped host memory; the host part of a message (compression, Fiat-Shamir)
+    // overlaps the device work of the next one wherever the transcript allows it.
+    //   (Cx, Cy): rows (x_vec, 0, 0) and (0.., y, 0) of one two-row MSM: a scalar kernel + the two MSM kernels
+    //             (dot_product.rs:192-197)
+    //   round k : fold with u_{k-1}, weights, L/R scalars, c_L, c_R and the two-row MSM in ONE launch
+    //             (bullet.rs:73-134)
     auto read_two_points = [&](const PubDst& pd, uint8_t* comp64) {
       uint32_t xyz[48];
       c->wait_points(pd, 2, xyz);
@@ -1233,18 +1200,10 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
     fr_t *an = a_alt.p, *bn = b_alt.p;
     DBuf<pt_ext> part(c, 2 * (size_t)msm_direct_chunks((int)(n + 2), 1));
     DBuf<fr_t> canon(c, n);
-    DBuf<uint32_t> cols(c, 2 * (n / 2 + 2));
-    // two short rows over the multiples table; len terms per row, generator index per term in cols (or identity)
-    // heavy = rows that carry the terms: both in a round (L, R), one for (Cx, Cy) — Cy is a single term
-    auto two_row_msm = [&](const uint32_t* d_cols, size_t len, int heavy) {
-      const PubDst pd = c->pub_begin(false);
-      launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, d_cols, 2, (int)len, heavy, part.p, nullptr, pd,
-                        c->st);
-      g_launches += 2;
-      return pd;
-    };
     launch_two_row_scalars(av, 0, fr_one(), fr_zero(), fr_zero(), Zr, fr_zero(), n, sLR.p, c->st);
-    const PubDst pd_c = two_row_msm(nullptr, n + 2, 1);
+    const PubDst pd_c = c->pub_begin(false);
+    launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd_c, c->st);
+    g_launches += 2;
     // a_vec of the transcript = canonical bytes of b; the copy is waited for only when it is appended
     launch_canonicalize(bv, canon.p, n, c->d_flag, c->st);
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, canon.p, n * 32, cudaMemcpyDeviceToHost, c->st));
@@ -1254,31 +1213,18 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
     int fold = 0;
     size_t m = n;  // vector length entering the round (after the fold with the previous challenge)
     PubDst pd_round;
-    static const bool unfused = [] {
-      const char* e = getenv("LASSO_B200_UNFUSED_ROUNDS");
-      return e && e[0] == '1';
-    }();
     DBuf<pt_ext> part_f(c, 2 * (size_t)bullet_fused_chunks((int)n));
     auto launch_round = [&](size_t round) {
-      if (!unfused) {
-        // the whole round in ONE launch: scalars, both rows over the multiples table, tail terms, publication
-        pd_round = c->pub_begin(false);
-        launch_bullet_fused(g.d_multiples.p, g.n_direct, av, bv, W, an, bn, Wn, n, m, fold, u, u_inv, v1[round], v2[round],
-                            part_f.p, c->d_partial, c->d_flag + 4, pd_round, c->st);
-        g_launches += 1;
-      } else {
-        launch_bullet_round(av, bv, W, an, bn, Wn, n, m, fold, u, u_inv, v1[round], v2[round], sLR.p, cols.p, c->d_partial,
-                            c->d_flag + 4, c->st);
-        g_launches += 1;
-      }
+      pd_round = c->pub_begin(false);
+      launch_bullet_fused(g.d_multiples.p, g.n_direct, av, bv, W, an, bn, Wn, n, m, fold, u, u_inv, v1[round], v2[round],
+                          part_f.p, c->d_partial, c->d_flag + 4, pd_round, c->st);
+      g_launches += 1;
       if (fold) {
         std::swap(av, an);
         std::swap(bv, bn);
         std::swap(W, Wn);
       }
-      if (unfused) pd_round = two_row_msm(cols.p, n / 2 + 2, 2);
     };
-    // NB: the (Cx, Cy) MSM reads sLR before round 0 overwrites it: same stream, so ordered
     uint8_t CxCy[64];
     read_two_points(pd_c, CxCy);
     if (m != 1) launch_round(0);  // round 0 needs no challenge: it runs while the host absorbs Cx, Cy, a
@@ -1308,8 +1254,8 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
       std::swap(W, Wn);
     }
   } else {
-    // no multiples table (LASSO_B200_NO_MULTIPLES=1 / not enough memory) or no mapped buffers: bucket MSMs over
-    // the window table, one kernel per step
+    // no multiples table (LASSO_B200_NO_MULTIPLES=1 / not enough memory): bucket MSMs over the window table, one
+    // kernel per step
     DBuf<fr_t> two(c, 4);
     {
       // Cx = batch_commit(x_vec, blind_x = 0) ; Cy = y*Q + 0*h
@@ -1364,8 +1310,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
     launch_two_row_scalars(W, 1, d, fr_zero(), r_delta, d, r_beta, n, sLR.p, c->st);
     DBuf<pt_ext> part(c, 2 * (size_t)msm_direct_chunks((int)(n + 2), 1));
     const PubDst pd = c->pub_begin(false);
-    launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, nullptr, 2, (int)(n + 2), 1, part.p, nullptr, pd,
-                      c->st);
+    launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd, c->st);
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, av, 32, cudaMemcpyDeviceToHost, c->st));
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 32, bv, 32, cudaMemcpyDeviceToHost, c->st));
     g_launches += 3;
@@ -1408,7 +1353,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const fr_t
 
 // CombinedTableEvalProof::prove (subtables/mod.rs:284-313 + prove_single 230-281) and the two analogous
 // n-to-1 reductions of HashLayerProof::prove: fold `evals` with bound_poly_var_bot in reverse challenge order.
-static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, const fr_t* Z, const uint32_t* Z_u32, size_t nv, std::vector<fr_t> evals,
+static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, const uint32_t* Z_u32, size_t nv, std::vector<fr_t> evals,
                                            bool pad_before_append, const char* evals_label, const char* chal_label,
                                            const char* joint_label, const std::vector<fr_t>& r,
                                            Transcript& transcript, RandomTape& tape) {
@@ -1428,7 +1373,7 @@ static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, const fr_t* Z,
   std::vector<fr_t> r_joint = challenges;
   r_joint.insert(r_joint.end(), r.begin(), r.end());
   transcript.append_scalar(joint_label, joint);
-  return prove_poly_eval(c, g, Z, Z_u32, nv, r_joint, joint, transcript, tape);
+  return prove_poly_eval(c, g, Z_u32, nv, r_joint, joint, transcript, tape);
 }
 
 // ---------------------------------------------------------------------------------------------- prove
@@ -1493,7 +1438,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     fr_t claimed_eval;
     const Finalize fclaim = reduce_to_host_begin(c, c->d_small, 1);
     absorb_comm_E();  // transcript order unchanged: the commitment, then the claim
-    reduce_to_host_end(c, fclaim, c->d_small, 1, &claimed_eval);
+    c->fin_wait(fclaim, &claimed_eval, 1);
     transcript.append_scalar("claim_eval_scalar_product", claimed_eval);
     SumcheckProof primary = prove_arbitrary(c, S, Wk.p, s_loc, s_loc, transcript, r_z);
     ser_sumcheck(w, primary);
@@ -1510,7 +1455,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     reduce_to_host(c, c->d_small, (int)alpha, eval_derefs.data());
     w.arr_fr(eval_derefs);
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
-    ser_dpl(w, prove_joint(c, g, E.p, E_u32.p, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
+    ser_dpl(w, prove_joint(c, g, E_u32.p, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
                            "joint_claim_eval", r_z, transcript, tape));
   }
   // ---- memory checking (surge.rs:186-198)
@@ -1541,10 +1486,9 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
                                  wr[i]->tree.p, c->st);
       g_launches += 2;
     }
-    // all trees of a size at once + the top layers straight to the host; without the mapped buffers: tree by tree
-    const bool batched = c->h_pub != nullptr;
+    // all trees of a size at once + the top layers straight to the host
     std::vector<std::vector<fr_t>> tops(2);  // [0]: init_i, final_i interleaved; [1]: read_i, write_i interleaved
-    if (batched) {
+    {
       std::vector<std::vector<Circuit*>> groups(2);
       for (size_t i = 0; i < alpha; i++) {
         groups[0].push_back(init[i].get());
@@ -1555,27 +1499,13 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
       build_trees(c, groups, {M, s}, tops, rtree_host, rtree_all.p);
       if (G > 1)  // pageable source: the copy is staged before the call returns
         LB_CUDA_CHECK(cudaMemcpyAsync(rtree_all.p, rtree_host.data(), rtree_host.size() * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
-    } else {
-      if (G > 1) throw std::runtime_error("sharded proof without publication buffers");
-      for (size_t i = 0; i < alpha; i++) {
-        build_tree(c, *init[i]);
-        build_tree(c, *fin[i]);
-        build_tree(c, *rd[i]);
-        build_tree(c, *wr[i]);
-      }
     }
     // ProductLayerProof::prove (memory_checking.rs:673-731)
     transcript.append_protocol_name("Lasso ProductLayerProof");
-    auto evaluate = [&](Circuit& ci, int grp, size_t t) {  // grand_product.rs:60-65
-      if (batched) return fr_mul(tops[grp][2 * t], tops[grp][2 * t + 1]);
-      fr_t top[2];
-      c->d2h(top, ci.layer_local(ci.num_layers - 1), 64);
-      return fr_mul(top[0], top[1]);
-    };
+    auto evaluate = [&](int grp, size_t t) { return fr_mul(tops[grp][2 * t], tops[grp][2 * t + 1]); };  // grand_product.rs:60-65
     std::vector<fr_t> claims_rw, claims_if;
     for (size_t i = 0; i < alpha; i++) {
-      fr_t hi = evaluate(*init[i], 0, 2 * i), hr = evaluate(*rd[i], 1, 2 * i), hw = evaluate(*wr[i], 1, 2 * i + 1),
-           hf = evaluate(*fin[i], 0, 2 * i + 1);
+      fr_t hi = evaluate(0, 2 * i), hr = evaluate(1, 2 * i), hw = evaluate(1, 2 * i + 1), hf = evaluate(0, 2 * i + 1);
       if (!fr_eq(fr_mul(hi, hw), fr_mul(hr, hf))) throw std::runtime_error("multiset hash check failed (memory_checking.rs:689)");
       transcript.append_scalar("claim_hash_init", hi);
       transcript.append_scalar("claim_hash_read", hr);
@@ -1622,7 +1552,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     }
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
     DotProductProofLogBytes proof_derefs =
-        prove_joint(c, g, E.p, E_u32.p, nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
+        prove_joint(c, g, E_u32.p, nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
                     "joint_claim_eval", rand_ops, transcript, tape);
     eq_evals_shard(c, rand_mem, 0, rand_mem.size(), eqtab.p);
     launch_multi_dot_u32(dense.d_m_u32.p, M_loc, (int)C, eqtab.p, M_loc, c->d_partial, c->d_small, c->st);
@@ -1631,11 +1561,11 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     std::vector<fr_t> evals_ops = eval_dim;
     evals_ops.insert(evals_ops.end(), eval_read.begin(), eval_read.end());
     DotProductProofLogBytes proof_ops =
-        prove_joint(c, g, dense.d_l_fr.p, dense.d_l_u32.p, dense.nv_l, evals_ops, true, "claim_evals_ops", "challenge_combine_n_to_one",
+        prove_joint(c, g, dense.d_l_u32.p, dense.nv_l, evals_ops, true, "claim_evals_ops", "challenge_combine_n_to_one",
                     "joint_claim_eval_ops", rand_ops, transcript, tape);
     // claim_evals_mem is appended UNPADDED and uses Math::log_2 (ceil) of C (memory_checking.rs:413-418)
     DotProductProofLogBytes proof_mem =
-        prove_joint(c, g, dense.d_m_fr.p, dense.d_m_u32.p, dense.nv_m, eval_final, false, "claim_evals_mem",
+        prove_joint(c, g, dense.d_m_u32.p, dense.nv_m, eval_final, false, "claim_evals_mem",
                     "challenge_combine_two_to_one", "joint_claim_eval_mem", rand_mem, transcript, tape);
     // field order (memory_checking.rs:313-329)
     w.arr_fr(eval_dim);

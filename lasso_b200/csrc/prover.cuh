@@ -85,7 +85,6 @@ struct Ctx {
     p.region = 0;
     p.all = 0;
     for (int i = 0; i < kPubMaxReaders; i++) p.dst[i] = nullptr;
-    if (!h_pub) return p;
     const uint32_t seq = pub_seq++;
     p.region = (int)(seq % kPubRegions);
     p.tag = 1 + seq % kPubTagMod;
@@ -100,13 +99,12 @@ struct Ctx {
   }
   // count elements of 8 x u32 words from one writer's region; blocks until every word carries the tag
   void pub_wait_raw(const PubDst& p, int writer, int count, uint32_t* out);  // prover.cu
-  // a round message produced by a single launch (common.cuh Finalize): results land in d_small and directly in
-  // the mapped host buffer(s); reduce = sum over the ranks of a sharded proof
+  // a round message produced by a single launch (common.cuh Finalize): results land directly in the mapped host
+  // buffer(s); reduce = sum over the ranks of a sharded proof
   Finalize fin_begin(bool reduce = false) {
     Finalize f;
     f.partial = d_partial;
     f.counter = d_flag + 4;
-    f.out_dev = d_small;
     f.pub = pub_begin(reduce);
     return f;
   }
@@ -115,7 +113,7 @@ struct Ctx {
   void wait_points(const PubDst& p, int npoints, uint32_t* xyz /* npoints x 24 words */);
   // device -> host through the pinned buffer (small) or directly (large)
   void d2h(void* dst, const void* src, size_t bytes) {
-    if (bytes <= 4096 && h_mapped) {
+    if (bytes <= 4096) {
       d2h_small(dst, src, bytes);
       return;
     }

@@ -3,8 +3,11 @@ Merlin transcript (host_transcript.hpp) against the published vector, the 64-bit
 32-bit carry-chain code that also runs on the device (fr.cuh / fq.cuh / host_fq64.hpp), the wire format of the
 tagged device -> host publication (pub_codec.hpp)."""
 import os
+import shutil
 import subprocess
 import tempfile
+
+import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "lasso_b200", "csrc")
@@ -297,3 +300,13 @@ def test_host_microbenchmark_builds():
         subprocess.check_call(["g++", "-O1", "-std=c++17", "-Wno-psabi", "-I", CSRC,
                                os.path.join(ROOT, "tools", "hostbench", "host_bench.cpp"), "-o", exe])
         assert os.path.exists(exe)
+
+
+def test_kernel_microbenchmark_builds():
+    """tools/ubench (the kernel microbenchmarks, linked against the library's kernel objects) keeps compiling against the
+    current launcher interfaces."""
+    objs = [os.path.join(ROOT, "lasso_b200", "_build", o) for o in ("poly_kernels.o", "msm_kernels.o")]
+    if shutil.which("nvcc") is None or not all(os.path.exists(o) for o in objs):
+        pytest.skip("needs nvcc and the library objects under lasso_b200/_build (run build() first)")
+    subprocess.check_call(["make", "-s", "-B", "-C", os.path.join(ROOT, "tools", "ubench")])
+    assert os.path.exists(os.path.join(ROOT, "tools", "ubench", "kbench"))

@@ -45,7 +45,7 @@ int main(int argc, char** argv) {
     fill_kernel<<<256, 256, 0, st>>>((uint32_t*)hA[k], maxlen * 8, 0x0fffffffu);
     fill_kernel<<<256, 256, 0, st>>>((uint32_t*)hB[k], maxlen * 8, 0x0fffffffu);
   }
-  fr_t **dA, **dB, *C0, *C1, *partial, *small;
+  fr_t **dA, **dB, *C0, *C1, *partial;
   cudaMalloc(&dA, ncirc * 8);
   cudaMalloc(&dB, ncirc * 8);
   cudaMemcpy(dA, hA.data(), ncirc * 8, cudaMemcpyHostToDevice);
@@ -54,50 +54,44 @@ int main(int argc, char** argv) {
   cudaMalloc(&C1, maxlen * 32);
   fill_kernel<<<256, 256, 0, st>>>((uint32_t*)C0, maxlen * 8, 0x0fffffffu);
   cudaMalloc(&partial, 1 << 22);
-  cudaMalloc(&small, 1 << 20);
   unsigned* counter;
   cudaMalloc(&counter, 64);
   cudaMemset(counter, 0, 64);
   uint32_t* small32;
   cudaMalloc(&small32, 4096);
-  uint32_t *h_mapped, *d_mapped;
-  cudaHostAlloc((void**)&h_mapped, 4096 + 64, cudaHostAllocMapped);
-  cudaHostGetDevicePointer((void**)&d_mapped, h_mapped, 0);
+  // one publication region in mapped pinned memory, as the prover's (nobody waits for the messages here)
+  const size_t pub_bytes = (size_t)kPubElems * kPubSlotWords * 8;
+  unsigned long long *h_pub, *d_pub;
+  cudaHostAlloc((void**)&h_pub, pub_bytes, cudaHostAllocMapped);
+  cudaHostGetDevicePointer((void**)&d_pub, h_pub, 0);
+  PubDst pub = {};
+  pub.dst[0] = d_pub;
+  pub.ndst = 1;
+  pub.tag = 1;
   fr_t r;
   for (int l = 0; l < 8; l++) r.v[l] = 0x01234567u * (l + 1) & 0x0fffffffu;
   Finalize fz;
   fz.partial = partial;
   fz.counter = counter;
-  fz.out_dev = small;
-  fz.mapped = d_mapped;
-  fz.tag = 1;
+  fz.pub = pub;
   CubicCoeffs cf;
   for (int k = 0; k < 32; k++) cf.v[k] = r;
   printf("%-52s %8.2f us\n", "empty kernel, back-to-back", time_us([&] { empty_kernel<<<1, 32, 0, st>>>(); }, 2000, st));
   for (size_t h : {2, 8, 32, 128, 512, 2048, 8192, 32768, 262144}) {
     char nm[96];
     snprintf(nm, sizeof nm, "sc_bind_eval_cubic ncirc=8 h=%zu (mapped)", h);
-    fz.mapped = d_mapped;
-    double a = time_us([&] { launch_sumcheck_bind_eval_cubic_comb(dA, dB, C0, C1, ncirc, h, r, cf, 0, fz, st); }, 500, st);
-    fz.mapped = nullptr;
-    double b = time_us([&] { launch_sumcheck_bind_eval_cubic_comb(dA, dB, C0, C1, ncirc, h, r, cf, 0, fz, st); }, 500, st);
-    printf("%-52s %8.2f us   (no mapped publish: %.2f us)\n", nm, a, b);
+    printf("%-52s %8.2f us\n", nm,
+           time_us([&] { launch_sumcheck_bind_eval_cubic_comb(dA, dB, C0, C1, ncirc, h, r, cf, 0, fz, st); }, 500, st));
   }
   for (size_t half : {1, 16, 256, 4096}) {
     char nm[96];
     snprintf(nm, sizeof nm, "sc_eval_cubic ncirc=8 half=%zu (mapped)", half);
-    fz.mapped = d_mapped;
     printf("%-52s %8.2f us\n", nm, time_us([&] { launch_sumcheck_eval_cubic_comb(dA, dB, C0, ncirc, half, cf, 1, fz, st); }, 500, st));
   }
   // Bulletproofs round pieces at n = 2048 (the 2^20-lookup openings)
   for (size_t n : {1024, 2048, 4096}) {
     fr_t *a0 = hA[0], *b0 = hB[0], *a1 = hA[1], *b1 = hB[1], *w0 = hA[2], *w1 = hA[3], *sLR = hA[4];
     char nm[96];
-    for (size_t m : {n / 2, (size_t)64, (size_t)2}) {
-      snprintf(nm, sizeof nm, "bullet_round n=%zu m=%zu fold=1", n, m);
-      printf("%-52s %8.2f us\n", nm,
-             time_us([&] { launch_bullet_round(a0, b0, w0, a1, b1, w1, n, m, 1, r, r, r, r, sLR, (uint32_t*)hB[5], partial, counter, st); }, 500, st));
-    }
     // table for n+2 generators: any niels-shaped data works for timing (field ops are data-independent)
     pt_niels* table;
     cudaMalloc(&table, (size_t)kMsmFullWindows * (n + 2) * sizeof(pt_niels));
@@ -127,13 +121,19 @@ int main(int argc, char** argv) {
         cudaEventElapsedTime(&ms, e0, e1);
         snprintf(nm, sizeof nm, "build multiples table, %zu generators (%.0f MB)", npts, kMsmFullWindows * npts * 128 * 96 / 1e6);
         printf("%-52s %8.2f ms\n", nm, ms);
-        // compact bullet-round shape: n/2 + 2 terms per row, all non-zero; identity columns
-        snprintf(nm, sizeof nm, "msm_direct 2 rows x %zu terms (direct+finish)", n / 2 + 2);
-        printf("%-52s %8.2f us\n", nm,
-               time_us([&] { launch_msm_direct(M, npts, (const uint32_t*)sLR, nullptr, 2, (int)(n / 2 + 2), 2, part, nullptr, d_mapped, st); }, 300, st));
+        // one whole Bulletproofs round: scalars, both rows, tail terms, publication
+        pt_ext* part_f;
+        cudaMalloc(&part_f, 2 * (size_t)bullet_fused_chunks((int)n) * sizeof(pt_ext));
+        for (size_t m : {n / 2, (size_t)64, (size_t)2}) {
+          snprintf(nm, sizeof nm, "bullet_fused n=%zu m=%zu fold=1", n, m);
+          printf("%-52s %8.2f us\n", nm,
+                 time_us([&] { launch_bullet_fused(M, npts, a0, b0, w0, a1, b1, w1, n, m, 1, r, r, r, r, part_f, partial, counter, pub, st); },
+                         500, st));
+        }
+        cudaFree(part_f);
         snprintf(nm, sizeof nm, "msm_direct 2 rows x %zu terms (direct+finish)", n + 2);
         printf("%-52s %8.2f us\n", nm,
-               time_us([&] { launch_msm_direct(M, npts, (const uint32_t*)sLR, nullptr, 2, (int)(n + 2), 1, part, nullptr, d_mapped, st); }, 300, st));
+               time_us([&] { launch_msm_direct(M, npts, (const uint32_t*)sLR, (int)(n + 2), part, pub, st); }, 300, st));
         cudaFree(M);
       }
     }
