@@ -169,6 +169,42 @@ int lasso_prove(lasso_ctx*, int strategy, int log_R, lasso_dense*, const uint64_
                 uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
                 size_t challenges_cap, size_t* n_challenges);
 
+/* ---------------------------------------------------------------- caller-defined strategies
+ *
+ * A SubtableStrategy (subtables/mod.rs:31-93) given as data instead of one of the built-in kinds above:
+ *  - C, log_m: the const generics, 1 <= C <= 16, 2 <= log_m <= 24 (log_m may be odd);
+ *  - tables[k], k < num_subtables: materialize_subtables() as M = 2^log_m u32 values each (entries must be integers
+ *    below 2^32: the commitments and openings run over them as integers);
+ *  - mem_to_subtable[i], mem_to_dimension[i], i < num_memories (alpha): memory_to_subtable_index /
+ *    memory_to_dimension_index; 1 <= num_subtables <= alpha <= 16 (2 alpha grand-product circuits in one batch);
+ *  - program (n_ops instructions of 3 int32 {op, a, b}): combine_lookups in SSA form.  Slots 0..alpha-1 hold the
+ *    memory values, instruction j writes slot alpha + j, the last instruction's slot is g.  Operands name earlier
+ *    slots; for MULK / ADDK b indexes `constants` (n_constants Fr, 4 Montgomery limbs each).  1 <= n_ops <= 128,
+ *    n_constants <= 64, at most 16 intermediate values live at once;
+ *  - g_degree: g_poly_degree(), 1..16, at least the program's degree (an input has degree 1, ADD / SUB / ADDK take the
+ *    larger operand degree, MUL the sum, MULK its operand's).  It sets the number of evaluation points, so proofs
+ *    match a Rust strategy that declares the same value.
+ * Any malformed part fails with LASSO_ERR_STRATEGY before a CUDA call.  The tables (u32 and Montgomery form) and the
+ * program are uploaded to the context's device once; destroy the strategy before its context.  On a sharded context
+ * every rank creates the same strategy (the tables are replicated). */
+typedef struct lasso_strategy lasso_strategy;
+enum { LASSO_OP_ADD = 0, LASSO_OP_SUB = 1, LASSO_OP_MUL = 2, LASSO_OP_MULK = 3, LASSO_OP_ADDK = 4 };
+int lasso_strategy_create(lasso_ctx*, int C, int log_m, int num_subtables, const uint32_t* const* tables,
+                          int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
+                          const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
+                          int g_degree, lasso_strategy** out);
+void lasso_strategy_destroy(lasso_strategy*);
+/* lasso_sumcheck_round_arbitrary for a custom strategy: polys = num_memories + 1 arrays of `len` elements (the last
+ * one eq); evals_out receives g_degree + 2 elements. */
+int lasso_sumcheck_round_custom(lasso_ctx*, const lasso_strategy*, const uint64_t* const* polys, size_t len,
+                                uint64_t* evals_out);
+/* lasso_prove with a custom strategy: the same semantics, outputs, errors and collectiveness.  LASSO_ERR_STRATEGY
+ * when the strategy's (C, log_m) differ from the densified representation's. */
+int lasso_prove_custom(lasso_ctx*, const lasso_strategy*, lasso_dense*, const uint64_t* r, size_t r_len,
+                       const lasso_gens*, const char* transcript_label, const char* tape_label,
+                       const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                       uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges);
+
 /* Host-resident benchmark helper: number of kernels launched by this context so far, and the wall time
  * (ms) of the last densify / commit / prove calls. */
 unsigned long long lasso_launch_count(const lasso_ctx*);

@@ -12,8 +12,8 @@ importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    Context, DensifiedRepresentation, LassoError, MsmJob, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof,
-    Strategy, bind_bot, bind_top, commit_rows, eq_evals, gather_lookup_polys, gens_points_needed, lib,
-    library_path, materialize_subtables, msm, sample_generators, sumcheck_bind_round_arbitrary, sumcheck_round_arbitrary,
-    sumcheck_round_cubic,
+    Context, CustomStrategy, DensifiedRepresentation, LassoError, MsmJob, SparsePolyCommitmentGens,
+    SparsePolynomialEvaluationProof, Strategy, bind_bot, bind_top, commit_rows, eq_evals, gather_lookup_polys,
+    gens_points_needed, lib, library_path, materialize_subtables, msm, sample_generators, sumcheck_bind_round_arbitrary,
+    sumcheck_round_arbitrary, sumcheck_round_cubic, sumcheck_round_custom, trace_combine_lookups,
 )

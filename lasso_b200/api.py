@@ -86,6 +86,157 @@ class Strategy:
         return (self.C if self.kind == LT else 1) + 1
 
 
+# ------------------------------------------------------------------ caller-defined strategies
+OP_ADD, OP_SUB, OP_MUL, OP_MULK, OP_ADDK = 0, 1, 2, 3, 4
+LASSO_ERR_STRATEGY = 4
+FR_MODULUS = 2**252 + 27742317777372353535851937790883648493
+MAX_MEMORIES, MAX_OPS, MAX_CONSTANTS, MAX_DEGREE = 16, 128, 64, 16
+
+
+class _Value:
+    """A value of the traced combine_lookups: an SSA slot and its degree in the memory values."""
+
+    __slots__ = ("tr", "slot", "degree")
+
+    def __init__(self, tr, slot, degree):
+        self.tr, self.slot, self.degree = tr, slot, degree
+
+    def __add__(self, o):
+        return self.tr.binary(OP_ADD, self, o)
+
+    __radd__ = __add__
+
+    def __sub__(self, o):
+        if isinstance(o, (int, np.integer)):
+            return self.tr.binary(OP_ADD, self, -int(o))
+        return self.tr.binary(OP_SUB, self, o)
+
+    def __rsub__(self, o):  # o - self, o an int
+        return self.tr.binary(OP_ADD, self.tr.binary(OP_MUL, self, -1), o)
+
+    def __mul__(self, o):
+        return self.tr.binary(OP_MUL, self, o)
+
+    __rmul__ = __mul__
+
+    def __neg__(self):
+        return self.tr.binary(OP_MUL, self, -1)
+
+
+class _Tracer:
+    def __init__(self, num_memories):
+        self.alpha = num_memories
+        self.program, self.constants, self._kidx = [], [], {}
+
+    def _const(self, x):
+        x %= FR_MODULUS
+        if x not in self._kidx:
+            self._kidx[x] = len(self.constants)
+            self.constants.append(x)
+        return self._kidx[x]
+
+    def _emit(self, op, a, b, degree):
+        self.program.append((op, a, b))
+        return _Value(self, self.alpha + len(self.program) - 1, degree)
+
+    def binary(self, op, a, b):
+        if isinstance(b, _Value):
+            if b.tr is not self:
+                raise ValueError("combine_lookups mixes values of two traces")
+            deg = a.degree + b.degree if op == OP_MUL else max(a.degree, b.degree)
+            return self._emit(op, a.slot, b.slot, deg)
+        if not isinstance(b, (int, np.integer)):
+            return NotImplemented
+        return self._emit(OP_MULK if op == OP_MUL else OP_ADDK, a.slot, self._const(int(b)), a.degree)
+
+
+def trace_combine_lookups(combine_lookups, num_memories):
+    """Trace combine_lookups(vals), vals a list of num_memories symbolic values, through + - * (Python ints are constants
+    mod l, negatives allowed) into the SSA program of lasso_strategy_create.  -> (program (n, 3) int32, constants
+    (k, 4) uint64 Montgomery limbs, degree of g)."""
+    tr = _Tracer(num_memories)
+    g = combine_lookups([_Value(tr, k, 1) for k in range(num_memories)])
+    if not isinstance(g, _Value) or g.tr is not tr:
+        raise LassoError(LASSO_ERR_STRATEGY, "combine_lookups must return an expression of the memory values")
+    if not tr.program or g.slot != num_memories + len(tr.program) - 1:  # g is an input or an earlier value
+        g = tr._emit(OP_ADDK, g.slot, tr._const(0), g.degree)
+    prog = np.array(tr.program, dtype=np.int32).reshape(-1, 3)
+    consts = np.zeros((len(tr.constants), 4), dtype=np.uint64)
+    for k, x in enumerate(tr.constants):
+        m = x * 2**256 % FR_MODULUS
+        consts[k] = [(m >> (64 * i)) & (2**64 - 1) for i in range(4)]
+    return prog, consts, g.degree
+
+
+class CustomStrategy:
+    """A caller-defined SubtableStrategy<F, C, M> (src/subtables/mod.rs:31-93):
+    - tables: materialize_subtables(), num_subtables arrays of M = 2^log_m integers below 2^32;
+    - combine_lookups: a Python function of a list of num_memories values, written as the trait's method with + - *;
+    - g_poly_degree: declared as in the trait; at least the degree of combine_lookups;
+    - memory_to_subtable / memory_to_dimension: the trait's maps as lists (default i % num_subtables and
+      i // num_subtables over num_memories = C * num_subtables memories).
+    With ctx=None only the host description is built (tracing and checks); otherwise it is uploaded to ctx's device."""
+
+    def __init__(self, ctx, C_, log_m, tables, combine_lookups, g_poly_degree, memory_to_subtable=None,
+                 memory_to_dimension=None):
+        self.C, self.log_m, self.g_poly_degree = int(C_), int(log_m), int(g_poly_degree)
+        self.tables = []
+        for t in tables:
+            t = np.asarray(t)
+            if t.shape != (1 << self.log_m,):
+                raise LassoError(LASSO_ERR_STRATEGY, "every table needs 2^log_m entries")
+            if t.size and (int(t.min()) < 0 or int(t.max()) >= 1 << 32):
+                raise LassoError(LASSO_ERR_STRATEGY, "table entries must be integers in [0, 2^32)")
+            self.tables.append(np.ascontiguousarray(t, dtype=np.uint32))
+        nsub = len(self.tables)
+        if memory_to_subtable is None and memory_to_dimension is None:
+            alpha = self.C * nsub
+            memory_to_subtable = [i % nsub for i in range(alpha)]
+            memory_to_dimension = [i // nsub for i in range(alpha)]
+        if memory_to_subtable is None or memory_to_dimension is None or len(memory_to_subtable) != len(memory_to_dimension):
+            raise LassoError(LASSO_ERR_STRATEGY, "memory_to_subtable and memory_to_dimension need the same length")
+        self.memory_to_subtable = np.ascontiguousarray(memory_to_subtable, dtype=np.int32)
+        self.memory_to_dimension = np.ascontiguousarray(memory_to_dimension, dtype=np.int32)
+        if not 1 <= self.num_memories <= MAX_MEMORIES:
+            raise LassoError(LASSO_ERR_STRATEGY, "num_memories must be in 1..16")
+        self.program, self.constants, self.degree = trace_combine_lookups(combine_lookups, self.num_memories)
+        if self.g_poly_degree < self.degree:
+            raise LassoError(LASSO_ERR_STRATEGY, "declared g_poly_degree %d is below the degree %d of combine_lookups"
+                             % (self.g_poly_degree, self.degree))
+        self.ctx, self._h = ctx, None
+        if ctx is not None:
+            h = C.c_void_p()
+            _chk(lib().lasso_strategy_create(
+                ctx._h, self.C, self.log_m, nsub, _ptr_array(self.tables), self.num_memories, _p(self.memory_to_subtable),
+                _p(self.memory_to_dimension), _p(self.program), int(self.program.shape[0]), _p(self.constants),
+                int(self.constants.shape[0]), self.g_poly_degree, C.byref(h)))
+            self._h = h
+
+    @property
+    def num_subtables(self):
+        return len(self.tables)
+
+    @property
+    def num_memories(self):
+        return int(self.memory_to_subtable.shape[0])
+
+    @property
+    def sumcheck_poly_degree(self):
+        return self.g_poly_degree + 1
+
+    def close(self):
+        if self._h:
+            lib().lasso_strategy_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            if self._h and self.ctx._h:
+                self.close()
+        except Exception:
+            pass
+
+
 class Context:
     """One per GPU: device, stream, memory pool, scratch."""
 
@@ -184,6 +335,14 @@ def sumcheck_round_arbitrary(ctx, S, polys):
     out = np.zeros((S.sumcheck_poly_degree + 1, 4), dtype=np.uint64)
     _chk(lib().lasso_sumcheck_round_arbitrary(ctx._h, S.kind, S.C, S.log_m, S.log_r, _ptr_array(polys),
                                               C.c_size_t(polys[0].shape[0]), _p(out)))
+    return out
+
+
+def sumcheck_round_custom(ctx, S, polys):
+    """sumcheck_round_arbitrary for a CustomStrategy: g_poly_degree + 2 evaluations."""
+    polys = [_fr(p) for p in polys]
+    out = np.zeros((S.sumcheck_poly_degree + 1, 4), dtype=np.uint64)
+    _chk(lib().lasso_sumcheck_round_custom(ctx._h, S._h, _ptr_array(polys), C.c_size_t(polys[0].shape[0]), _p(out)))
     return out
 
 
@@ -383,7 +542,12 @@ class SparsePolynomialEvaluationProof:
         out = ctx._buf("proof", cap, np.uint8)
         chal = ctx._buf("challenges", (1 << 14, 4), np.uint64)
         n, nch = C.c_size_t(0), C.c_size_t(0)
-        _chk(lib().lasso_prove(ctx._h, strategy.kind, strategy.log_r, dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h,
-                               transcript_label, tape_label, _p(seed), _p(out), C.c_size_t(cap), C.byref(n), _p(chal),
-                               C.c_size_t(chal.shape[0]), C.byref(nch)))
+        tail = (dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, transcript_label, tape_label, _p(seed), _p(out),
+                C.c_size_t(cap), C.byref(n), _p(chal), C.c_size_t(chal.shape[0]), C.byref(nch))
+        if isinstance(strategy, CustomStrategy):
+            if strategy._h is None:
+                raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
+            _chk(lib().lasso_prove_custom(ctx._h, strategy._h, *tail))
+        else:
+            _chk(lib().lasso_prove(ctx._h, strategy.kind, strategy.log_r, *tail))
         return cls(bytes(out[: n.value]), chal[: nch.value].copy())

@@ -15,6 +15,19 @@ struct lasso_gens {
 struct lasso_dense {
   Dense* d;
 };
+// a caller-defined SubtableStrategy, resident on the context's device
+struct lasso_strategy {
+  Ctx* c = nullptr;
+  CustomStrategy cs;
+  DBuf<CustomIns> ops;
+  DBuf<fr_t> consts, tables_fr;
+  DBuf<uint32_t> tables_u32;
+  Strategy S() const {
+    Strategy s{STRAT_CUSTOM, cs.C, cs.log_m, 0};
+    s.custom = &cs;
+    return s;
+  }
+};
 
 struct lasso_msm_job {
   Ctx* c = nullptr;
@@ -51,6 +64,94 @@ static int fail(int code, const std::string& msg) {
 static bool is_pow2(size_t x) { return x && !(x & (x - 1)); }
 static constexpr size_t kMsmLargeMin = 1 << 14;  // below this the row kernels (c = 8, buckets in shared memory) win
 static Strategy mkS(int kind, int C, int log_M, int log_R) { return Strategy{kind, C, log_M, log_R}; }
+
+// Checks a custom strategy's descriptor (everything but the tables' contents) and fills cs with its shape, the degree
+// of g and the instructions with SSA slots mapped to physical slots.  "" = valid, else the reason.
+static std::string custom_check(int C, int log_m, int nsub, int alpha, const int* sub, const int* dim, const int32_t* prog,
+                                int n_ops, const uint64_t* consts, int n_consts, int degree, CustomStrategy& cs,
+                                std::vector<CustomIns>& ins) {
+  if (C < 1 || C > 16) return "C must be in 1..16";
+  if (log_m < 2 || log_m > 24) return "log_m must be in 2..24";
+  if (alpha < 1 || alpha > kCustomMaxMemories) return "num_memories must be in 1..16";
+  if (nsub < 1 || nsub > alpha) return "num_subtables must be in 1..num_memories";
+  if (!sub || !dim || !prog) return "null map or program";
+  for (int i = 0; i < alpha; i++) {
+    if (sub[i] < 0 || sub[i] >= nsub) return "memory_to_subtable_index out of range";
+    if (dim[i] < 0 || dim[i] >= C) return "memory_to_dimension_index out of range";
+  }
+  if (n_ops < 1 || n_ops > kCustomMaxOps) return "the program needs 1..128 instructions";
+  if (n_consts < 0 || n_consts > kCustomMaxConsts) return "at most 64 constants";
+  if (n_consts > 0 && !consts) return "null constants";
+  for (int k = 0; k < n_consts; k++) {
+    fr_t x;
+    memcpy(x.v, consts + 4 * k, 32);
+    if (!fr_eq(fr_reduce_once(x.v), x)) return "constant " + std::to_string(k) + " is not a canonical Montgomery residue";
+  }
+  // operands refer to earlier slots; degree by propagation (an input has degree 1)
+  const int nvals = alpha + n_ops;
+  std::vector<int> deg(nvals, 1), last_use(nvals, -1);
+  for (int j = 0; j < n_ops; j++) {
+    const int op = prog[3 * j], a = prog[3 * j + 1], b = prog[3 * j + 2];
+    if (op < CUSTOM_ADD || op > CUSTOM_ADDK) return "instruction " + std::to_string(j) + ": unknown opcode";
+    const bool konst = op == CUSTOM_MULK || op == CUSTOM_ADDK;
+    if (a < 0 || a >= alpha + j) return "instruction " + std::to_string(j) + ": operand a does not name an earlier slot";
+    if (konst ? (b < 0 || b >= n_consts) : (b < 0 || b >= alpha + j))
+      return "instruction " + std::to_string(j) + (konst ? ": constant index out of range" : ": operand b does not name an earlier slot");
+    int d = op == CUSTOM_MUL ? deg[a] + deg[b] : (konst ? deg[a] : std::max(deg[a], deg[b]));
+    deg[alpha + j] = std::min(d, 1 << 20);
+    last_use[a] = j;
+    if (!konst) last_use[b] = j;
+  }
+  const int gdeg = deg[nvals - 1];
+  if (degree < 1 || degree > kCustomMaxDegree) return "g_poly_degree must be in 1..16";
+  if (degree < gdeg)
+    return "declared g_poly_degree " + std::to_string(degree) + " is below the program's degree " + std::to_string(gdeg);
+  // physical slots by liveness: an operand's slot is free again after its last use, before the result is stored
+  std::vector<int> phys(nvals, -1), free_slots;
+  int n_slots = 0;
+  ins.resize(n_ops);
+  for (int j = 0; j < n_ops; j++) {
+    const int op = prog[3 * j], a = prog[3 * j + 1], b = prog[3 * j + 2];
+    const bool konst = op == CUSTOM_MULK || op == CUSTOM_ADDK;
+    ins[j].op = op;
+    ins[j].a = a < alpha ? -1 - a : phys[a];
+    ins[j].b = konst ? b : (b < alpha ? -1 - b : phys[b]);
+    for (int v : {a, konst ? -1 : b})
+      if (v >= alpha && last_use[v] == j && phys[v] >= 0) {
+        free_slots.push_back(phys[v]);
+        phys[v] = -1;
+      }
+    if (j + 1 == n_ops) {
+      ins[j].dst = -1;  // g itself stays in registers
+      break;
+    }
+    int s;
+    if (!free_slots.empty()) {
+      s = free_slots.back();
+      free_slots.pop_back();
+    } else {
+      s = n_slots++;
+    }
+    ins[j].dst = s;
+    if (last_use[alpha + j] < 0) free_slots.push_back(s);  // dead value: stored, never read
+    else phys[alpha + j] = s;
+  }
+  if (n_slots > kCustomMaxSlots) return "the program keeps more than 16 intermediate values live at once";
+  cs = CustomStrategy{};
+  cs.C = C;
+  cs.log_m = log_m;
+  cs.nsub = nsub;
+  cs.alpha = alpha;
+  cs.degree = degree;
+  cs.n_ops = n_ops;
+  cs.n_consts = n_consts;
+  cs.n_slots = n_slots;
+  for (int i = 0; i < alpha; i++) {
+    cs.sub[i] = sub[i];
+    cs.dim[i] = dim[i];
+  }
+  return "";
+}
 
 extern "C" {
 
@@ -517,13 +618,13 @@ int lasso_commit(lasso_ctx* h, const lasso_dense* d, const lasso_gens* g, uint8_
   LB_CATCH
 }
 
-int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
-                const lasso_gens* g, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
-                uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
-                size_t challenges_cap, size_t* n_challenges) {
-  LB_TRY_CTX(h)
-  Strategy S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
-  if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
+}  // extern "C"
+
+// lasso_prove / lasso_prove_custom after the strategy has been checked
+static int prove_checked(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
+                         const lasso_gens* g, const char* transcript_label, const char* tape_label,
+                         const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                         uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
   // assert_eq!(r.len(), log2(dense.s))  surge.rs:131
   if (r_len != log2_exact_or_ceil(d->d->s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");
   std::vector<fr_t> rv(r_len);
@@ -547,6 +648,100 @@ int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uin
   if (b.size() > proof_cap) return fail(LASSO_ERR_LENGTH, "prove: output buffer too small");
   memcpy(proof_out, b.data(), b.size());
   return 0;
+}
+
+extern "C" {
+
+int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
+                const lasso_gens* g, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
+                uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
+                size_t challenges_cap, size_t* n_challenges) {
+  LB_TRY_CTX(h)
+  Strategy S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
+  if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
+  return prove_checked(h, S, d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
+                       challenges_out, challenges_cap, n_challenges);
+  LB_CATCH
+}
+
+// ---- caller-defined strategies
+int lasso_strategy_create(lasso_ctx* h, int C, int log_m, int num_subtables, const uint32_t* const* tables,
+                          int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
+                          const int32_t* program, int n_ops, const uint64_t* constants, int n_constants, int g_degree,
+                          lasso_strategy** out) {
+  if (out) *out = nullptr;
+  CustomStrategy cs;
+  std::vector<CustomIns> ins;
+  const std::string why = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
+                                       n_ops, constants, n_constants, g_degree, cs, ins);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "strategy: " + why);
+  if (!out || !tables) return fail(LASSO_ERR_STRATEGY, "strategy: null tables or output");
+  for (int k = 0; k < num_subtables; k++)
+    if (!tables[k]) return fail(LASSO_ERR_STRATEGY, "strategy: null table");
+  const size_t M = (size_t)1 << log_m;
+  uint32_t mx = 0;
+  for (int k = 0; k < num_subtables; k++)
+    for (size_t i = 0; i < M; i++) mx = std::max(mx, tables[k][i]);
+  cs.tbits = mx ? 32u - (unsigned)__builtin_clz(mx) : 1u;
+  LB_TRY_CTX(h)
+  Ctx* c = h->c;
+  std::unique_ptr<lasso_strategy> s(new lasso_strategy());
+  s->c = c;
+  s->ops.alloc(c, ins.size());
+  s->consts.alloc(c, std::max(n_constants, 1));
+  s->tables_fr.alloc(c, (size_t)num_subtables * M);
+  s->tables_u32.alloc(c, (size_t)num_subtables * M);
+  LB_CUDA_CHECK(cudaMemcpyAsync(s->ops.p, ins.data(), ins.size() * sizeof(CustomIns), cudaMemcpyHostToDevice, c->st));
+  if (n_constants)
+    LB_CUDA_CHECK(cudaMemcpyAsync(s->consts.p, constants, (size_t)n_constants * 32, cudaMemcpyHostToDevice, c->st));
+  for (int k = 0; k < num_subtables; k++)
+    LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_u32.p + k * M, tables[k], M * 4, cudaMemcpyHostToDevice, c->st));
+  launch_from_u32(s->tables_u32.p, s->tables_fr.p, (size_t)num_subtables * M, c->st);
+  LB_LAUNCH_CHECK();
+  g_launches += 1;
+  c->sync();  // the sources are caller memory
+  cs.d_ops = s->ops.p;
+  cs.d_consts = s->consts.p;
+  cs.d_tables_fr = s->tables_fr.p;
+  cs.d_tables_u32 = s->tables_u32.p;
+  s->cs = cs;
+  *out = s.release();
+  return 0;
+  LB_CATCH
+}
+void lasso_strategy_destroy(lasso_strategy* s) {
+  if (!s) return;
+  cudaSetDevice(s->c->device);
+  delete s;
+}
+int lasso_sumcheck_round_custom(lasso_ctx* h, const lasso_strategy* s, const uint64_t* const* polys, size_t len,
+                                uint64_t* evals_out) {
+  LB_TRY_CTX(h)
+  if (!s || s->c != h->c) return fail(LASSO_ERR_STRATEGY, "strategy was created on another context");
+  if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "len must be a power of two >= 2");
+  Ctx* c = h->c;
+  const Strategy S = s->S();
+  const int np = S.num_memories() + 1, npts = S.sumcheck_poly_degree() + 1;
+  DBuf<fr_t> d(c, (size_t)np * len);
+  for (int k = 0; k < np; k++)
+    LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
+  const Finalize f = c->fin_begin();
+  launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
+  g_launches += 1;
+  c->fin_wait(f, (fr_t*)evals_out, npts);
+  return 0;
+  LB_CATCH
+}
+int lasso_prove_custom(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, const uint64_t* r, size_t r_len,
+                       const lasso_gens* g, const char* transcript_label, const char* tape_label,
+                       const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                       uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
+  LB_TRY_CTX(h)
+  if (!s || s->c != h->c) return fail(LASSO_ERR_STRATEGY, "strategy was created on another context");
+  if ((size_t)s->cs.C != d->d->C || (size_t)s->cs.log_m != d->d->log_m)
+    return fail(LASSO_ERR_STRATEGY, "strategy (C, log_m) differ from the densified representation");
+  return prove_checked(h, s->S(), d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
+                       challenges_out, challenges_cap, n_challenges);
   LB_CATCH
 }
 

@@ -6,26 +6,64 @@
 
 namespace lb {
 
-enum StrategyKind { STRAT_AND = 0, STRAT_OR = 1, STRAT_XOR = 2, STRAT_LT = 3, STRAT_RANGE = 4 };
+// STRAT_CUSTOM is internal: a caller-defined strategy (lasso_strategy_create), described by a CustomStrategy
+enum StrategyKind { STRAT_AND = 0, STRAT_OR = 1, STRAT_XOR = 2, STRAT_LT = 3, STRAT_RANGE = 4, STRAT_CUSTOM = 5 };
+
+// ---- caller-defined strategies: tables as data, combine_lookups as a straight-line program over Fr
+// Limits: 2 * alpha circuits must fit one batched grand product (32), the round message (degree + 2 elements) one
+// publication region, the program and its constants the shared memory of a CTA.
+static constexpr int kCustomMaxMemories = 16, kCustomMaxOps = 128, kCustomMaxConsts = 64, kCustomMaxDegree = 16;
+static constexpr int kCustomMaxSlots = 16;  // live intermediate values of a program (after slot allocation)
+enum CustomOp { CUSTOM_ADD = 0, CUSTOM_SUB = 1, CUSTOM_MUL = 2, CUSTOM_MULK = 3, CUSTOM_ADDK = 4 };
+// One instruction after slot allocation: dst is a physical slot; an operand a (and b for ADD, SUB, MUL) is a physical
+// slot when >= 0 and memory value k when it is -1 - k; for MULK and ADDK b indexes the constants.
+struct CustomIns {
+  int op, dst, a, b;
+};
+struct CustomStrategy {
+  int C, log_m, nsub, alpha, degree;       // degree: the declared g_poly_degree
+  int n_ops, n_consts, n_slots;
+  int sub[kCustomMaxMemories], dim[kCustomMaxMemories];
+  unsigned tbits;                          // bit width of the largest table entry (>= 1)
+  const CustomIns* d_ops = nullptr;        // device: n_ops instructions
+  const fr_t* d_consts = nullptr;          // device: n_consts Montgomery constants
+  const fr_t* d_tables_fr = nullptr;       // device: nsub x M Montgomery elements
+  const uint32_t* d_tables_u32 = nullptr;  // device: nsub x M values
+};
 
 // Runtime stand-in for the reference's `impl SubtableStrategy<F, C, M>` const generics
 // (src/subtables/mod.rs:31-93).
 struct Strategy {
   int kind, C, log_m, log_r;
+  const CustomStrategy* custom = nullptr;  // kind == STRAT_CUSTOM
   int M() const { return 1 << log_m; }
-  int num_subtables() const { return kind == STRAT_LT ? 2 : (kind == STRAT_RANGE ? 3 : 1); }
-  int num_memories() const { return kind == STRAT_LT ? 2 * C : C; }
-  int g_poly_degree() const { return kind == STRAT_LT ? C : 1; }
+  int num_subtables() const {
+    if (kind == STRAT_CUSTOM) return custom->nsub;
+    return kind == STRAT_LT ? 2 : (kind == STRAT_RANGE ? 3 : 1);
+  }
+  int num_memories() const {
+    if (kind == STRAT_CUSTOM) return custom->alpha;
+    return kind == STRAT_LT ? 2 * C : C;
+  }
+  int g_poly_degree() const {
+    if (kind == STRAT_CUSTOM) return custom->degree;
+    return kind == STRAT_LT ? C : 1;
+  }
   int sumcheck_poly_degree() const { return g_poly_degree() + 1; }
   // src/subtables/mod.rs:64-74, range_check.rs:62-73
   int memory_to_subtable_index(int i) const {
+    if (kind == STRAT_CUSTOM) return custom->sub[i];
     if (kind == STRAT_RANGE) {
       if (i * log_m > log_r) return 2;
       return ((i + 1) * log_m > log_r) ? 1 : 0;
     }
     return i % num_subtables();
   }
-  int memory_to_dimension_index(int i) const { return kind == STRAT_RANGE ? i : i / num_subtables(); }
+  int memory_to_dimension_index(int i) const {
+    if (kind == STRAT_CUSTOM) return custom->dim[i];
+    return kind == STRAT_RANGE ? i : i / num_subtables();
+  }
+  // built-in strategies only: a custom one is validated when it is created (capi.cu)
   bool valid() const {
     if (!(kind >= 0 && kind <= 4 && C >= 1 && C <= 16 && log_m >= 2 && log_m <= 24 && (log_m % 2 == 0 || kind == STRAT_RANGE)))
       return false;
@@ -63,6 +101,8 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
 bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t stride, size_t q, const fr_t& r,
                                          const Finalize& fin, size_t min_q, cudaStream_t st);
 int sumcheck_max_blocks();
+// per-device function attributes (dynamic shared memory opt-in of the custom-strategy kernels)
+void poly_init_device();
 
 // ---- K3: batched cubic round evaluation (sumcheck.rs:49-93) ----
 // A, B: ncirc device pointers each to 2*half elements; Ceq: 2*half elements.  The batching coefficients of
@@ -80,7 +120,8 @@ void launch_sumcheck_bind_eval_cubic_comb(fr_t* const* d_A, fr_t* const* d_B, co
                                           const fr_t& r, const CubicCoeffs& cf, int scale, const Finalize& fin, cudaStream_t st);
 
 // ---- K5: subtables (subtables/*.rs) ----
-// tables_fr: nsub x M Montgomery elements; tables_u32: nsub x M raw values
+// tables_fr: nsub x M Montgomery elements; tables_u32: nsub x M raw values.  Built-in strategies only: a custom
+// strategy's tables are uploaded once when it is created and used in place.
 void launch_materialize_subtables(const Strategy& S, fr_t* tables_fr, uint32_t* tables_u32, cudaStream_t st);
 // E_k[j] = T_sub(k)[nz_dim(k)[j]] for k < alpha (subtables/mod.rs:78-92). nz: C x s (u32).
 void launch_gather_lookup_polys(const Strategy& S, const fr_t* tables_fr, const uint32_t* tables_u32,

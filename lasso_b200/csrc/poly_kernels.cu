@@ -401,6 +401,163 @@ __global__ void __launch_bounds__(128)
   finalize_last_stage(fin, gridDim.x, NP);
 }
 
+// ------------------------------------------------------------------------------------ K2/K7 for custom strategies
+// combine_lookups is a straight-line program (CustomIns, kernels.cuh) run by one interpreter per thread.  The program
+// and its constants are staged into shared memory once per CTA; the intermediate values of a thread live in
+// shared memory too, in n_slots physical slots (the host allocates them by liveness).  A memory value operand is
+// formed on the fly from the polynomial (after the first evaluation point the loads hit L1).  The instruction stream is
+// the same for every thread, so the dispatch on the opcode never diverges.
+static constexpr int kCustomThreads = 128;
+
+// d * t for a small integer t (t <= kCustomMaxDegree + 1): double-and-add, cheaper than a Montgomery product
+__device__ __forceinline__ fr_t fr_mul_small(const fr_t& d, int t) {
+  fr_t r = fr_zero();
+#pragma unroll 1
+  for (int b = 4; b >= 0; b--) {
+    r = fr_dbl(r);
+    if ((t >> b) & 1) r = fr_add(r, d);
+  }
+  return r;
+}
+// slot s of this thread: 8 words, word-major across the CTA so that a warp's accesses are conflict-free
+__device__ __forceinline__ fr_t custom_ld(const uint32_t* sm, int s) {
+  fr_t r;
+#pragma unroll
+  for (int l = 0; l < 8; l++) r.v[l] = sm[(s * 8 + l) * kCustomThreads + threadIdx.x];
+  return r;
+}
+__device__ __forceinline__ void custom_st(uint32_t* sm, int s, const fr_t& x) {
+#pragma unroll
+  for (int l = 0; l < 8; l++) sm[(s * 8 + l) * kCustomThreads + threadIdx.x] = x.v[l];
+}
+// g(x_0, .., x_{alpha-1}); input(k) yields x_k
+template <class Input>
+__device__ __forceinline__ fr_t custom_run(const CustomIns* ops, int n_ops, const fr_t* consts, uint32_t* slots,
+                                           Input input) {
+  fr_t r = fr_zero();
+#pragma unroll 1
+  for (int j = 0; j < n_ops; j++) {
+    const CustomIns in = ops[j];
+    const fr_t a = in.a >= 0 ? custom_ld(slots, in.a) : input(-1 - in.a);
+    if (in.op == CUSTOM_MULK) {
+      r = fr_mul(a, consts[in.b]);
+    } else if (in.op == CUSTOM_ADDK) {
+      r = fr_add(a, consts[in.b]);
+    } else {
+      const fr_t b = in.b >= 0 ? custom_ld(slots, in.b) : input(-1 - in.b);
+      r = in.op == CUSTOM_ADD ? fr_add(a, b) : (in.op == CUSTOM_SUB ? fr_sub(a, b) : fr_mul(a, b));
+    }
+    if (j + 1 < n_ops) custom_st(slots, in.dst, r);
+  }
+  return r;
+}
+// shared memory: instructions | constants | slots of every thread | (round kernel) accumulators of every thread
+static size_t custom_smem_bytes(const CustomStrategy& cs, int npoints) {
+  return (size_t)cs.n_ops * sizeof(CustomIns) + (size_t)cs.n_consts * sizeof(fr_t) +
+         (size_t)(cs.n_slots + npoints) * sizeof(fr_t) * kCustomThreads;
+}
+__device__ __forceinline__ void custom_stage(const CustomStrategy& cs, CustomIns*& ops, fr_t*& consts, uint32_t*& slots) {
+  extern __shared__ __align__(32) unsigned char custom_sm[];
+  consts = (fr_t*)custom_sm;  // first: 32-byte alignment
+  ops = (CustomIns*)(consts + cs.n_consts);
+  slots = (uint32_t*)(ops + cs.n_ops);
+  for (int j = threadIdx.x; j < cs.n_ops; j += blockDim.x) ops[j] = cs.d_ops[j];
+  for (int j = threadIdx.x; j < cs.n_consts; j += blockDim.x) consts[j] = cs.d_consts[j];
+  __syncthreads();
+}
+
+// One round of prove_arbitrary (sumcheck.rs:179-237) for any program: per index pair i and point t = 0..npts-1,
+// eq(t) * g(x(t)) with x_k(t) = lo_k + t (hi_k - lo_k).  The npts accumulators sit after the slots.
+__global__ void __launch_bounds__(kCustomThreads)
+    sc_eval_custom_kernel(CustomStrategy cs, const fr_t* base, size_t stride, size_t half, int npts, Finalize fin) {
+  __shared__ fr_t scratch[kCustomThreads / 32];
+  __shared__ fr_t res[kCustomMaxDegree + 2];
+  __shared__ int s_last;
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(cs, ops, consts, slots);
+  uint32_t* acc = slots + cs.n_slots * 8 * kCustomThreads;
+  for (int t = 0; t < npts; t++) custom_st(acc, t, fr_zero());
+  const fr_t* eq = base + (size_t)cs.alpha * stride;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
+    const fr_t q0 = ld_fr(eq + i), dq = fr_sub(ld_fr(eq + half + i), q0);
+    fr_t cq = q0;
+#pragma unroll 1
+    for (int t = 0; t < npts; t++) {
+      const fr_t g = custom_run(ops, cs.n_ops, consts, slots, [&](int k) {
+        const fr_t* P = base + (size_t)k * stride;
+        const fr_t lo = ld_fr(P + i);
+        if (t == 0) return lo;
+        const fr_t hi = ld_fr(P + half + i);
+        return t == 1 ? hi : fr_add(lo, fr_mul_small(fr_sub(hi, lo), t));
+      });
+      custom_st(acc, t, fr_add(custom_ld(acc, t), fr_mul(g, cq)));
+      cq = fr_add(cq, dq);
+    }
+  }
+  for (int t = 0; t < npts; t++) {
+    fr_t v[1] = {custom_ld(acc, t)};
+    block_sum_fr<1>(v, scratch);
+    if (threadIdx.x == 0) res[t] = v[0];
+  }
+  __syncthreads();
+  if (gridDim.x == 1) {
+    if ((int)threadIdx.x < npts) finalize_publish(fin, threadIdx.x, res[threadIdx.x]);
+    return;
+  }
+  if ((int)threadIdx.x < npts) fin.partial[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = res[threadIdx.x];
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = (atomicAdd(fin.counter, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!s_last) return;
+  finalize_last_stage(fin, gridDim.x, npts);
+}
+
+// subtables/mod.rs:186-216 for any program: sum_k eq[k] * g(E_1[k], ..., E_alpha[k])
+__global__ void __launch_bounds__(kCustomThreads)
+    claim_custom_kernel(CustomStrategy cs, const fr_t* base, size_t stride, size_t n, fr_t* partial) {
+  __shared__ fr_t scratch[kCustomThreads / 32];
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(cs, ops, consts, slots);
+  fr_t acc[1] = {fr_zero()};
+  const fr_t* eq = base + (size_t)cs.alpha * stride;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const fr_t g = custom_run(ops, cs.n_ops, consts, slots, [&](int k) { return ld_fr(base + (size_t)k * stride + i); });
+    acc[0] = fr_add(acc[0], fr_mul(g, ld_fr(eq + i)));
+  }
+  block_sum_fr<1>(acc, scratch);
+  if (threadIdx.x == 0) partial[blockIdx.x] = acc[0];
+}
+
+// dynamic shared memory above the default 48 KiB needs an opt-in per kernel and device (at context creation): the
+// largest program's
+void poly_init_device() {
+  CustomStrategy cs{};
+  cs.n_ops = kCustomMaxOps;
+  cs.n_consts = kCustomMaxConsts;
+  cs.n_slots = kCustomMaxSlots;
+  const int bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 2);
+  LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  LB_CUDA_CHECK(cudaFuncSetAttribute(claim_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+}
+// grid: one wave of as many CTAs as fit an SM at this shared-memory size
+static int custom_grid(size_t n, size_t smem) {
+  int per_sm = (int)((200u << 10) / (smem + 1024));
+  if (per_sm < 1) per_sm = 1;
+  if (per_sm > kBlocksPerSM * 2) per_sm = kBlocksPerSM * 2;
+  return grid_for(n, kCustomThreads, kNumSMs * per_sm);
+}
+static void launch_eval_custom(const CustomStrategy& cs, const fr_t* base, size_t stride, size_t half, int npts,
+                               const Finalize& fin, cudaStream_t st) {
+  const size_t smem = custom_smem_bytes(cs, npts);
+  sc_eval_custom_kernel<<<custom_grid(half, smem), kCustomThreads, smem, st>>>(cs, base, stride, half, npts, fin);
+  LB_LAUNCH_CHECK();
+}
+
 // combine_lookups weights are F::from(1u64 << (i * inc)): inc = log2 of the chunk size (and.rs:45-53, range_check.rs:78-86)
 static int linear_inc(const Strategy& S) { return S.kind == STRAT_RANGE ? S.log_m : S.log_m / 2; }
 
@@ -413,7 +570,9 @@ static void launch_lt(const fr_t* base, size_t stride, size_t half, const Finali
 void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t stride, size_t half, const Finalize& fin,
                                     cudaStream_t st) {
   int blocks;
-  if (S.kind == STRAT_LT) {
+  if (S.kind == STRAT_CUSTOM) {
+    launch_eval_custom(*S.custom, base, stride, half, S.sumcheck_poly_degree() + 1, fin, st);
+  } else if (S.kind == STRAT_LT) {
     blocks = grid_for(half, 128, kMaxBlocks);
     switch (S.C) {
       case 1: launch_lt<1>(base, stride, half, fin, blocks, st); break;
@@ -449,7 +608,7 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
 bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t stride, size_t q, const fr_t& r,
                                          const Finalize& fin, size_t min_q, cudaStream_t st) {
   static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
-  if (S.kind == STRAT_LT || q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
+  if (S.kind == STRAT_LT || S.kind == STRAT_CUSTOM || q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
   sc_bind_eval_linear_kernel<<<grid_for(q, kThreads, kNumSMs * 2), kThreads, 0, st>>>(base, stride, S.num_memories(), q, r,
                                                                                        linear_inc(S), fin);
   LB_LAUNCH_CHECK();
@@ -489,7 +648,11 @@ __global__ void __launch_bounds__(kThreads)
 void launch_sumcheck_claim(const Strategy& S, const fr_t* base, size_t stride, size_t n, fr_t* partial, fr_t* out,
                            cudaStream_t st) {
   int blocks = grid_for(n);
-  if (S.kind == STRAT_LT)
+  if (S.kind == STRAT_CUSTOM) {
+    const size_t smem = custom_smem_bytes(*S.custom, 0);
+    blocks = custom_grid(n, smem);
+    claim_custom_kernel<<<blocks, kCustomThreads, smem, st>>>(*S.custom, base, stride, n, partial);
+  } else if (S.kind == STRAT_LT)
     claim_lt_kernel<<<blocks, kThreads, 0, st>>>(base, stride, S.C, n, partial);
   else
     claim_linear_kernel<<<blocks, kThreads, 0, st>>>(base, stride, S.num_memories(), n, linear_inc(S), partial);
@@ -751,6 +914,7 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 void launch_materialize_subtables(const Strategy& S, fr_t* tables_fr, uint32_t* tables_u32, cudaStream_t st) {
+  if (S.kind == STRAT_CUSTOM) throw std::runtime_error("a custom strategy's tables are uploaded, not materialised");
   size_t n = (size_t)S.M() * S.num_subtables();
   materialize_kernel<<<grid_for(n), kThreads, 0, st>>>(S.kind, S.num_subtables(), S.log_m, S.log_r, tables_fr,
                                                        tables_u32);

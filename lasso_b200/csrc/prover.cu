@@ -233,6 +233,7 @@ Ctx* ctx_create(int device) {
   msm_init_device();      // per-device function attributes (dynamic shared memory opt-in)
   msm_large_init_device();
   densify_init_device();
+  poly_init_device();
   LB_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_aux, cudaEventDisableTiming));
   LB_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_stage, cudaEventDisableTiming));
   const char* sp = getenv("LASSO_B200_SPANS");
@@ -1395,16 +1396,23 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
 
   // ---- Subtables::new (subtables/mod.rs:116-129): materialise (replicated, 2-6 MiB), gather, merge
   const size_t nv_d = g.nv_d, nd_loc = ((size_t)1 << nv_d) / G;
+  // a custom strategy's tables were uploaded when it was created: used in place
+  const bool custom = S.kind == STRAT_CUSTOM;
   const int nsub = S.num_subtables();
-  DBuf<fr_t> tables_fr(c, (size_t)nsub * M);
-  DBuf<uint32_t> tables_u32(c, (size_t)nsub * M);
+  DBuf<fr_t> tables_fr_buf(c, custom ? 0 : (size_t)nsub * M);
+  DBuf<uint32_t> tables_u32_buf(c, custom ? 0 : (size_t)nsub * M);
+  const fr_t* tables_fr = custom ? S.custom->d_tables_fr : tables_fr_buf.p;
+  const uint32_t* tables_u32 = custom ? S.custom->d_tables_u32 : tables_u32_buf.p;
   DBuf<fr_t> E(c, nd_loc);          // combined_poly = E_0 | .. | E_{alpha-1} | 0-pad (this rank's shard)
   DBuf<uint32_t> E_u32(c, nd_loc);  // same values as integers for the small-scalar commit
   {
     SpanTimer sp(c, "Subtables.new");
-    launch_materialize_subtables(S, tables_fr.p, tables_u32.p, c->st);
-    launch_gather_lookup_polys(S, tables_fr.p, tables_u32.p, dense.nz(), s_loc, E.p, s_loc, E_u32.p, c->st);
-    g_launches += 2;
+    if (!custom) {
+      launch_materialize_subtables(S, tables_fr_buf.p, tables_u32_buf.p, c->st);
+      g_launches += 1;
+    }
+    launch_gather_lookup_polys(S, tables_fr, tables_u32, dense.nz(), s_loc, E.p, s_loc, E_u32.p, c->st);
+    g_launches += 1;
     if (nd_loc > alpha * s_loc) {
       launch_fill_zero(E.p + alpha * s_loc, nd_loc - alpha * s_loc, c->st);
       LB_CUDA_CHECK(cudaMemsetAsync(E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
@@ -1415,7 +1423,8 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
   // ---- comm_derefs (surge.rs:136-140, subtables/mod.rs:177-184, 382-393)
   {
     SpanTimer sp(c, "Subtables.commit");
-    unsigned tbits = S.kind == STRAT_LT ? 1 : (S.kind == STRAT_RANGE ? (unsigned)S.log_m : (unsigned)(S.log_m / 2));
+    unsigned tbits = custom ? S.custom->tbits
+                            : (S.kind == STRAT_LT ? 1 : (S.kind == STRAT_RANGE ? (unsigned)S.log_m : (unsigned)(S.log_m / 2)));
     comm_E = commit_u32(c, g, E_u32.p, nv_d, tbits);
     w.vec_pts(comm_E);
   }
@@ -1480,7 +1489,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
         pc->reset(new Circuit());
         circuit_alloc(c, **pc, s, G > 1 ? rtree_all.p + (slot++) * 2 * (size_t)G : nullptr);
       }
-      launch_gp_fingerprints_mem(tables_fr.p + k * M, dense.fin(j), M_loc, G, gr, gamma, tau, init[i]->tree.p,
+      launch_gp_fingerprints_mem(tables_fr + k * M, dense.fin(j), M_loc, G, gr, gamma, tau, init[i]->tree.p,
                                  fin[i]->tree.p, c->st);
       launch_gp_fingerprints_ops(dense.dim(j), E.p + i * s_loc, dense.read(j), s_loc, gamma, tau, rd[i]->tree.p,
                                  wr[i]->tree.p, c->st);

@@ -4,7 +4,9 @@ One GPU per rank by default (torch.distributed over NCCL carries the job id and 
 LASSO_SHARD_SAME_GPU=1 every rank uses GPU 0 (gloo for the plumbing) — the exchanges of the sharded proof (shared
 host segments + CUDA IPC exchange buffers, csrc/comm.cu) do not need one device per rank, so a single-GPU box can
 run this check too.
-usage: torchrun --nproc-per-node N tools/sharded_check.py [kind C log_m log_r lookups same]"""
+With --custom every strategy is a caller-defined one (lasso_b200.CustomStrategy): the built-in cases re-expressed as
+programs plus tables that are not built in, checked against the oracle for caller-defined strategies (oracle_custom/).
+usage: torchrun --nproc-per-node N tools/sharded_check.py [--custom] [kind C log_m log_r lookups same]"""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -13,6 +15,8 @@ import torch
 import torch.distributed as dist
 import lasso_b200 as lb
 import oracle_lib as ol
+import custom_builtins as cb
+import oracle_custom_lib as oc
 
 rank = int(os.environ.get("RANK", 0)); local = int(os.environ.get("LOCAL_RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
 same_gpu = os.environ.get("LASSO_SHARD_SAME_GPU") == "1"
@@ -25,18 +29,28 @@ else:
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
 cases = [(2, 4, 16, 0, 1 << 12, 1), (3, 4, 4, 0, 128, 0), (0, 1, 16, 0, 1 << 10, 1), (4, 3, 8, 40, 256, 0), (3, 8, 8, 0, 512, 0),
          (1, 2, 8, 0, 700, 0)]
-if len(sys.argv) > 6:
-    cases = [tuple(int(x) for x in sys.argv[1:7])]
+custom = "--custom" in sys.argv
+argv = [a for a in sys.argv if a != "--custom"]
+if len(argv) > 6:
+    cases = [tuple(int(x) for x in argv[1:7])]
+if custom:  # new tables: kind = -1 - their index in cb.NEW_TABLES
+    cases += [(-1 - i, 0, 0, 0, 300 + i, 0) for i in range(len(cb.NEW_TABLES))]
 ctx = lb.Context(local)
 ctx.init_comm()
 ok = True
 for kind, C, log_m, log_r, n, same in cases:
-    rng = np.random.default_rng(kind * 7 + C)
+    if kind < 0:
+        S = cb.NEW_TABLES[sorted(cb.NEW_TABLES)[-1 - kind]](ctx)
+        C, log_m = S.C, S.log_m
+    elif custom:
+        S = cb.as_custom(ctx, kind, C, log_m, log_r)
+    else:
+        S = lb.Strategy(kind, C, log_m, log_r)
+    rng = np.random.default_rng(kind * 7 + C if kind >= 0 else 1000 - kind)
     col = rng.integers(0, 1 << log_m, size=(n, 1), dtype=np.uint64)
     idx = np.ascontiguousarray(np.repeat(col, C, axis=1) if same else rng.integers(0, 1 << log_m, size=(n, C), dtype=np.uint64))
     s = 1 << (n - 1).bit_length()
     r = ol.rand_fr(rng, s.bit_length() - 1); seed = ol.rand_fr(rng, 1)[0]
-    S = lb.Strategy(kind, C, log_m, log_r)
     need = lb.gens_points_needed(C, s, S.num_memories, log_m)
     stream = np.ascontiguousarray(ol.generators(max(need, 300))[:need])
     gens = lb.SparsePolyCommitmentGens.new(ctx, b"g", C, s, S.num_memories, log_m, stream=stream)
@@ -46,12 +60,15 @@ for kind, C, log_m, log_r, n, same in cases:
     proof = lb.SparsePolynomialEvaluationProof.prove(ctx, S, dense, r, gens, tape_seed=seed)
     dt = time.time() - t0
     if rank == 0:
-        ref = ol.prove(kind, C, log_m, log_r, idx, r, stream, seed, flags=1)
+        if custom:
+            ref = oc.prove(S, idx, r, stream, seed, flags=1)
+        else:
+            ref = ol.prove(kind, C, log_m, log_r, idx, r, stream, seed, flags=1)
         good = ref["rc"] == 0 and com == ref["commitment"] and proof.bytes == ref["proof"]
         nch = min(len(proof.challenges), len(ref["challenges"]))
         first_bad = next((i for i in range(nch) if (proof.challenges[i] != ref["challenges"][i]).any()), None)
-        print("case kind=%d C=%d log_m=%d n=%d world=%d: %s (%.1f ms, commit_ok=%s, first diverging challenge=%s)" % (
-            kind, C, log_m, n, world, "OK" if good else "MISMATCH", dt * 1e3, com == ref["commitment"], first_bad), flush=True)
+        print("case %skind=%d C=%d log_m=%d n=%d world=%d: %s (%.1f ms, commit_ok=%s, first diverging challenge=%s)" % (
+            "custom " if custom else "", kind, C, log_m, n, world, "OK" if good else "MISMATCH", dt * 1e3, com == ref["commitment"], first_bad), flush=True)
         ok = ok and good
 # an out-of-range index (densified.rs:46) in the LAST rank's block of rows: every rank must report it (the verdict is
 # agreed through the round-message path; nobody may be left waiting in the exchange that follows)
