@@ -73,7 +73,9 @@ struct MsmLargePlan {
   size_t max_entries = 0, max_units = 0;
 };
 int msm_large_window_bits(size_t n);
-MsmLargePlan msm_large_plan(size_t n, unsigned max_bits);
+// c_force != 0 replaces msm_large_window_bits(n) (tests of the widths the size rule never picks); the small-scalar
+// clamp and the limits below still apply
+MsmLargePlan msm_large_plan(size_t n, unsigned max_bits, int c_force = 0);
 size_t msm_large_scratch_bytes(const MsmLargePlan& p);
 void msm_large_init_device();
 // bases: arkworks affine (x, y) Montgomery limbs; term i uses base i % n_pool when n_pool != 0 (bench inputs), else base i

@@ -477,11 +477,12 @@ int msm_large_window_bits(size_t n) {
   if (c > 17) c = 17;
   return c;
 }
-MsmLargePlan msm_large_plan(size_t n, unsigned max_bits) {
+MsmLargePlan msm_large_plan(size_t n, unsigned max_bits, int c_force) {
   MsmLargePlan p;
   p.n = n;
   p.nbits = max_bits < 1 ? 1 : (int)max_bits;
-  p.c = msm_large_window_bits(n);
+  if (c_force != 0 && (c_force < 2 || c_force > 20)) throw std::runtime_error("msm_large: forced window width outside 2..20");
+  p.c = c_force ? c_force : msm_large_window_bits(n);
   if (p.c > p.nbits + 1) p.c = p.nbits + 1 < 2 ? 2 : p.nbits + 1;  // small scalars: one window holds them
   p.nw = (p.nbits + 2 + p.c - 1) / p.c;                             // c nw >= nbits + 2  =>  s + bias < 2^(c nw)
   if (p.nw > 32) throw std::runtime_error("msm_large: more than 32 windows");

@@ -1,77 +1,22 @@
 // Test harness: one extern "C" wrapper per launcher of kernels.cuh / msm.cuh that the C ABI does not expose on its own.
-// Linked from the library's own kernel objects (lasso_b200/_build/poly_kernels.o, msm_kernels.o), so the tests run
+// Linked from the library's own kernel objects (lasso_b200/_build/poly_kernels.o, msm_kernels.o, msm_large.o,
+// msm_final.o), so the tests run
 // exactly the code the prover runs.  Every wrapper copies its host inputs to the device, calls ONE launcher on a stream
 // of its own, synchronises, copies every output (in-place arrays included) back and frees what it allocated.  Field
 // elements are 4 x u64 Montgomery limbs (the fr_t layout), points arkworks affine (x, y) Montgomery limbs.
-// Return codes: 0 ok, -1 a launcher threw (std::runtime_error), -2 a CUDA error, -3 a publication slot did not carry
-// the message's tag, -4 bad arguments.
-#include <cuda_runtime.h>
-
-#include <cstdint>
-#include <cstdio>
+// Return codes: see harness_common.cuh.
 #include <cstring>
-#include <stdexcept>
-#include <vector>
 
-#include "../../lasso_b200/csrc/kernels.cuh"
-#include "../../lasso_b200/csrc/msm.cuh"
 #include "../../lasso_b200/csrc/pub_codec.hpp"
+#include "harness_common.cuh"
 
 using namespace lb;
+using kh::guarded;
+using kh::HarnessError;
+using kh::Scope;
+using kh::ck;
 
 namespace {
-
-struct HarnessError {
-  int code;
-};
-
-void ck(cudaError_t e) {
-  if (e != cudaSuccess) {
-    fprintf(stderr, "kernel harness: CUDA error %s\n", cudaGetErrorString(e));
-    throw HarnessError{-2};
-  }
-}
-
-// every device allocation of one call; freed when the call returns, whatever happens
-struct Scope {
-  std::vector<void*> dev, host;
-  cudaStream_t st = nullptr;
-  Scope() { ck(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking)); }
-  ~Scope() {
-    if (st) cudaStreamSynchronize(st);
-    for (void* p : dev) cudaFree(p);
-    for (void* p : host) cudaFreeHost(p);
-    if (st) cudaStreamDestroy(st);
-  }
-  template <class T>
-  T* alloc(size_t count) {
-    void* p = nullptr;
-    ck(cudaMalloc(&p, count * sizeof(T) + 16));
-    dev.push_back(p);
-    ck(cudaMemsetAsync(p, 0, count * sizeof(T) + 16, st));
-    return (T*)p;
-  }
-  template <class T>
-  T* up(const void* h, size_t count) {
-    T* d = alloc<T>(count);
-    if (count) ck(cudaMemcpyAsync(d, h, count * sizeof(T), cudaMemcpyHostToDevice, st));
-    return d;
-  }
-  template <class T>
-  void down(void* h, const T* d, size_t count) {
-    if (count) ck(cudaMemcpyAsync(h, d, count * sizeof(T), cudaMemcpyDeviceToHost, st));
-  }
-  // an array of device pointers to n arrays of `len` elements each, filled from host[k * len ..]
-  fr_t* const* ptr_array(const uint64_t* host, int n, size_t len, std::vector<fr_t*>& ptrs) {
-    ptrs.resize(n);
-    for (int k = 0; k < n; k++) ptrs[k] = up<fr_t>(host + (size_t)k * len * 4, len);
-    return up<fr_t*>(ptrs.data(), n);
-  }
-  void sync() {
-    ck(cudaStreamSynchronize(st));
-    ck(cudaGetLastError());
-  }
-};
 
 // one publication region in mapped pinned host memory (as the prover's Ctx), tag 1
 struct Pub {
@@ -122,28 +67,6 @@ fr_t fr_of(const uint64_t* x) {
   fr_t r;
   memcpy(r.v, x, 32);
   return r;
-}
-
-bool g_inited = false;
-void init() {
-  if (g_inited) return;
-  poly_init_device();
-  msm_init_device();
-  g_inited = true;
-}
-
-template <class F>
-int guarded(F f) {
-  try {
-    init();
-    f();
-    return 0;
-  } catch (const HarnessError& e) {
-    return e.code;
-  } catch (const std::runtime_error& e) {
-    fprintf(stderr, "kernel harness: %s\n", e.what());
-    return -1;
-  }
 }
 
 }  // namespace
@@ -474,6 +397,42 @@ int kh_msm_rows_direct_u32(const KhTables* t, const uint32_t* scalars, int nrows
     s.sync();
     s.down(out, dout, (size_t)nrows * 4);
     s.sync();
+  });
+}
+
+// ---------------------------------------------------------------- one large MSM (msm_large.cu, msm_final.cu)
+// bases: n_pool arkworks affine points (x, y Montgomery limbs), term i uses base i % n_pool; scalars: n Montgomery
+// elements.  launch_msm_large_prep, then the plan for the widest scalar (c_force != 0: that window width, subject to
+// the plan's small-scalar clamp and limits), then launch_msm_large twice on the same scratch: out_ext = (x, y, t, z)
+// arkworks limbs, out_raw = un-normalised internal (X, Y, Z, T), 32 u32.
+// info: c, nw, nbits, NB, S, nlev, lev_L[0 .. 8).
+int kh_msm_large(const uint64_t* bases, size_t n_pool, const uint64_t* scalars, size_t n, int c_force, uint64_t* out_ext,
+                 uint32_t* out_raw, int* info) {
+  if (n == 0 || n_pool == 0 || n_pool > n) return -4;
+  return guarded([&] {
+    Scope s;
+    const fq_t* db = s.up<fq_t>(bases, n_pool * 2);
+    const fr_t* dsc = s.up<fr_t>(scalars, n);
+    pt_niels* niels = s.alloc<pt_niels>(n);
+    fr_t* canon = s.alloc<fr_t>(n);
+    unsigned* d_max_bits = s.alloc<unsigned>(1);
+    launch_msm_large_prep(db, dsc, n, n_pool == n ? 0 : n_pool, niels, canon, d_max_bits, s.st);
+    unsigned max_bits = 0;
+    s.down(&max_bits, d_max_bits, 1);
+    s.sync();
+    const MsmLargePlan p = msm_large_plan(n, max_bits, c_force);
+    void* scratch = s.alloc<uint8_t>(msm_large_scratch_bytes(p));
+    fq_t* oe = s.alloc<fq_t>(4);
+    uint32_t* orw = s.alloc<uint32_t>(32);
+    launch_msm_large(p, niels, canon, scratch, oe, nullptr, s.st);
+    launch_msm_large(p, niels, canon, scratch, nullptr, orw, s.st);
+    s.sync();
+    s.down(out_ext, oe, 4);
+    s.down(out_raw, orw, 32);
+    s.sync();
+    const int head[6] = {p.c, p.nw, p.nbits, (int)p.NB, (int)p.S, p.nlev};
+    for (int k = 0; k < 6; k++) info[k] = head[k];
+    for (int k = 0; k < 8; k++) info[6 + k] = (int)p.lev_L[k];
   });
 }
 

@@ -35,6 +35,10 @@ def lib():
         L.kh_msm_direct.argtypes = [V, V, I, V]
         L.kh_bullet_fused.argtypes = [V, V, V, V, S, S, I, V, V, V, V, V, V, V, V]
         L.kh_msm_rows_direct_u32.argtypes = [V, V, I, I, I, I, I, I, V]
+        L.kh_msm_large.argtypes = [V, S, V, S, I, V, V, V]
+        L.kh_arith.argtypes = [I, I, S, V, V, V, V]
+        L.kh_arith_op_name.argtypes = [I]
+        L.kh_arith_op_name.restype = C.c_char_p
         _lib = L
     return _lib
 
@@ -43,6 +47,17 @@ def call(name, *args):
     """call a wrapper; a non-zero return code is a failure of the launch under test"""
     rc = getattr(lib(), name)(*args)
     assert rc == 0, "%s returned %d (-1: the launcher threw, -2: CUDA error, -3: publication tag missing)" % (name, rc)
+
+
+def op_ids(name_fn):
+    """{operation name: id} of an arithmetic op table, from its kh_arith_op_name-style name function"""
+    ids, i = {}, 0
+    while True:
+        s = name_fn(i)
+        if s is None:
+            return ids
+        ids[s.decode()] = i
+        i += 1
 
 
 class Tables:
