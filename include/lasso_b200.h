@@ -173,8 +173,8 @@ int lasso_prove(lasso_ctx*, int strategy, int log_R, lasso_dense*, const uint64_
  *
  * A SubtableStrategy (subtables/mod.rs:31-93) given as data instead of one of the built-in kinds above:
  *  - C, log_m: the const generics, 1 <= C <= 16, 2 <= log_m <= 24 (log_m may be odd);
- *  - tables[k], k < num_subtables: materialize_subtables() as M = 2^log_m u32 values each (entries must be integers
- *    below 2^32: the commitments and openings run over them as integers);
+ *  - tables[k], k < num_subtables: materialize_subtables() as M = 2^log_m u32 values each (integers below 2^32;
+ *    lasso_strategy_create_fr below takes tables of arbitrary field elements);
  *  - mem_to_subtable[i], mem_to_dimension[i], i < num_memories (alpha): memory_to_subtable_index /
  *    memory_to_dimension_index; 1 <= num_subtables <= alpha <= 16 (2 alpha grand-product circuits in one batch);
  *  - program (n_ops instructions of 3 int32 {op, a, b}): combine_lookups in SSA form.  Slots 0..alpha-1 hold the
@@ -193,6 +193,17 @@ int lasso_strategy_create(lasso_ctx*, int C, int log_m, int num_subtables, const
                           int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
                           const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
                           int g_degree, lasso_strategy** out);
+/* The same with tables of arbitrary field elements: tables[k] holds M Fr values, 4 Montgomery limbs each (a Rust
+ * caller passes materialize_subtables()[k].as_ptr() as it is).  Every other parameter and check as above; an entry that
+ * is not a canonical Montgomery residue also fails with LASSO_ERR_STRATEGY before a CUDA call.  When every entry is
+ * below 2^32 the strategy is the one lasso_strategy_create makes of those integers.  Otherwise it is full-width: only
+ * the Montgomery tables are uploaded, and the lookup values are committed with ceil((w + 2) / 8) signed 8-bit windows,
+ * w the bit width of the widest entry.  An entry l - k costs the full width: it is committed as the canonical integer
+ * it is, never as -k, since the generators may carry a torsion component. */
+int lasso_strategy_create_fr(lasso_ctx*, int C, int log_m, int num_subtables, const uint64_t* const* tables,
+                             int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
+                             const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
+                             int g_degree, lasso_strategy** out);
 void lasso_strategy_destroy(lasso_strategy*);
 /* lasso_sumcheck_round_arbitrary for a custom strategy: polys = num_memories + 1 arrays of `len` elements (the last
  * one eq); evals_out receives g_degree + 2 elements. */

@@ -13,7 +13,7 @@ importing works without a GPU, but creating a Context raises.
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
     Context, CustomStrategy, DensifiedRepresentation, LassoError, MsmJob, SparsePolyCommitmentGens,
-    SparsePolynomialEvaluationProof, Strategy, bind_bot, bind_top, commit_rows, eq_evals, gather_lookup_polys,
+    SparsePolynomialEvaluationProof, Strategy, bind_bot, bind_top, commit_rows, eq_evals, fr_from_ints, gather_lookup_polys,
     gens_points_needed, lib, library_path, materialize_subtables, msm, sample_generators, sumcheck_bind_round_arbitrary,
     sumcheck_round_arbitrary, sumcheck_round_cubic, sumcheck_round_custom, trace_combine_lookups,
 )

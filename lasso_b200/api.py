@@ -168,9 +168,33 @@ def trace_combine_lookups(combine_lookups, num_memories):
     return prog, consts, g.degree
 
 
+def fr_from_ints(values):
+    """Python integers (any sign, any size) -> (n, 4) uint64 Montgomery limbs of their residues mod l: the Fr layout of
+    the binding, e.g. a CustomStrategy table of differences fr_from_ints([a - b for ...])."""
+    vals = [int(v) % FR_MODULUS * 2**256 % FR_MODULUS for v in values]
+    out = np.zeros((len(vals), 4), dtype=np.uint64)
+    for i in range(4):
+        out[:, i] = [(v >> (64 * i)) & (2**64 - 1) for v in vals]
+    return out
+
+
+def _is_canonical(limbs):
+    """per row of (n, 4) uint64 limbs: the 256-bit integer they hold is below l"""
+    below = np.zeros(limbs.shape[0], dtype=bool)
+    equal = np.ones(limbs.shape[0], dtype=bool)
+    for i in range(3, -1, -1):
+        li = np.uint64((FR_MODULUS >> (64 * i)) & (2**64 - 1))
+        below |= equal & (limbs[:, i] < li)
+        equal &= limbs[:, i] == li
+    return below
+
+
 class CustomStrategy:
     """A caller-defined SubtableStrategy<F, C, M> (src/subtables/mod.rs:31-93):
-    - tables: materialize_subtables(), num_subtables arrays of M = 2^log_m integers below 2^32;
+    - tables: materialize_subtables(), num_subtables tables of M = 2^log_m entries, each either a 1-D array of integers
+      below 2^32 or an (M, 4) uint64 array of Fr in Montgomery limbs (any field element; see fr_from_ints).  When any
+      table is (M, 4) all of them are kept in that form (fr_tables) and the strategy is made by
+      lasso_strategy_create_fr;
     - combine_lookups: a Python function of a list of num_memories values, written as the trait's method with + - *;
     - g_poly_degree: declared as in the trait; at least the degree of combine_lookups;
     - memory_to_subtable / memory_to_dimension: the trait's maps as lists (default i % num_subtables and
@@ -181,13 +205,22 @@ class CustomStrategy:
                  memory_to_dimension=None):
         self.C, self.log_m, self.g_poly_degree = int(C_), int(log_m), int(g_poly_degree)
         self.tables = []
-        for t in tables:
-            t = np.asarray(t)
+        raw = [np.asarray(t) for t in tables]
+        self.fr_tables = any(t.ndim == 2 for t in raw)
+        for t in raw:
+            if t.ndim == 2:
+                if t.shape != (1 << self.log_m, 4) or t.dtype != np.uint64:
+                    raise LassoError(LASSO_ERR_STRATEGY, "a field-element table is a (2^log_m, 4) uint64 array")
+                if not _is_canonical(t).all():
+                    raise LassoError(LASSO_ERR_STRATEGY, "a table entry is not a canonical Montgomery residue")
+                self.tables.append(np.ascontiguousarray(t))
+                continue
             if t.shape != (1 << self.log_m,):
                 raise LassoError(LASSO_ERR_STRATEGY, "every table needs 2^log_m entries")
             if t.size and (int(t.min()) < 0 or int(t.max()) >= 1 << 32):
                 raise LassoError(LASSO_ERR_STRATEGY, "table entries must be integers in [0, 2^32)")
-            self.tables.append(np.ascontiguousarray(t, dtype=np.uint32))
+            t = np.ascontiguousarray(t, dtype=np.uint32)
+            self.tables.append(fr_from_ints(t.tolist()) if self.fr_tables else t)
         nsub = len(self.tables)
         if memory_to_subtable is None and memory_to_dimension is None:
             alpha = self.C * nsub
@@ -206,7 +239,8 @@ class CustomStrategy:
         self.ctx, self._h = ctx, None
         if ctx is not None:
             h = C.c_void_p()
-            _chk(lib().lasso_strategy_create(
+            create = lib().lasso_strategy_create_fr if self.fr_tables else lib().lasso_strategy_create
+            _chk(create(
                 ctx._h, self.C, self.log_m, nsub, _ptr_array(self.tables), self.num_memories, _p(self.memory_to_subtable),
                 _p(self.memory_to_dimension), _p(self.program), int(self.program.shape[0]), _p(self.constants),
                 int(self.constants.shape[0]), self.g_poly_degree, C.byref(h)))

@@ -665,6 +665,40 @@ int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uin
 }
 
 // ---- caller-defined strategies
+// Uploads a checked strategy: tables_u32 (integers, mirrored into Montgomery form on the device) or tables_fr
+// (Montgomery, full width: no u32 copy), exactly one of them non-null.
+static int strategy_upload(Ctx* c, CustomStrategy cs, const std::vector<CustomIns>& ins, const uint64_t* constants,
+                           int n_constants, const uint32_t* const* tables_u32, const uint64_t* const* tables_fr,
+                           lasso_strategy** out) {
+  const size_t M = (size_t)1 << cs.log_m;
+  std::unique_ptr<lasso_strategy> s(new lasso_strategy());
+  s->c = c;
+  s->ops.alloc(c, ins.size());
+  s->consts.alloc(c, std::max(n_constants, 1));
+  s->tables_fr.alloc(c, (size_t)cs.nsub * M);
+  if (tables_u32) s->tables_u32.alloc(c, (size_t)cs.nsub * M);
+  LB_CUDA_CHECK(cudaMemcpyAsync(s->ops.p, ins.data(), ins.size() * sizeof(CustomIns), cudaMemcpyHostToDevice, c->st));
+  if (n_constants)
+    LB_CUDA_CHECK(cudaMemcpyAsync(s->consts.p, constants, (size_t)n_constants * 32, cudaMemcpyHostToDevice, c->st));
+  if (tables_u32) {
+    for (int k = 0; k < cs.nsub; k++)
+      LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_u32.p + k * M, tables_u32[k], M * 4, cudaMemcpyHostToDevice, c->st));
+    launch_from_u32(s->tables_u32.p, s->tables_fr.p, (size_t)cs.nsub * M, c->st);
+    LB_LAUNCH_CHECK();
+    g_launches += 1;
+  } else {
+    for (int k = 0; k < cs.nsub; k++)
+      LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_fr.p + k * M, tables_fr[k], M * 32, cudaMemcpyHostToDevice, c->st));
+  }
+  c->sync();  // the sources are caller memory
+  cs.d_ops = s->ops.p;
+  cs.d_consts = s->consts.p;
+  cs.d_tables_fr = s->tables_fr.p;
+  cs.d_tables_u32 = s->tables_u32.p;
+  s->cs = cs;
+  *out = s.release();
+  return 0;
+}
 int lasso_strategy_create(lasso_ctx* h, int C, int log_m, int num_subtables, const uint32_t* const* tables,
                           int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
                           const int32_t* program, int n_ops, const uint64_t* constants, int n_constants, int g_degree,
@@ -684,29 +718,46 @@ int lasso_strategy_create(lasso_ctx* h, int C, int log_m, int num_subtables, con
     for (size_t i = 0; i < M; i++) mx = std::max(mx, tables[k][i]);
   cs.tbits = mx ? 32u - (unsigned)__builtin_clz(mx) : 1u;
   LB_TRY_CTX(h)
-  Ctx* c = h->c;
-  std::unique_ptr<lasso_strategy> s(new lasso_strategy());
-  s->c = c;
-  s->ops.alloc(c, ins.size());
-  s->consts.alloc(c, std::max(n_constants, 1));
-  s->tables_fr.alloc(c, (size_t)num_subtables * M);
-  s->tables_u32.alloc(c, (size_t)num_subtables * M);
-  LB_CUDA_CHECK(cudaMemcpyAsync(s->ops.p, ins.data(), ins.size() * sizeof(CustomIns), cudaMemcpyHostToDevice, c->st));
-  if (n_constants)
-    LB_CUDA_CHECK(cudaMemcpyAsync(s->consts.p, constants, (size_t)n_constants * 32, cudaMemcpyHostToDevice, c->st));
+  return strategy_upload(h->c, cs, ins, constants, n_constants, tables, nullptr, out);
+  LB_CATCH
+}
+int lasso_strategy_create_fr(lasso_ctx* h, int C, int log_m, int num_subtables, const uint64_t* const* tables,
+                             int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
+                             const int32_t* program, int n_ops, const uint64_t* constants, int n_constants, int g_degree,
+                             lasso_strategy** out) {
+  if (out) *out = nullptr;
+  CustomStrategy cs;
+  std::vector<CustomIns> ins;
+  const std::string why = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
+                                       n_ops, constants, n_constants, g_degree, cs, ins);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "strategy: " + why);
+  if (!out || !tables) return fail(LASSO_ERR_STRATEGY, "strategy: null tables or output");
   for (int k = 0; k < num_subtables; k++)
-    LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_u32.p + k * M, tables[k], M * 4, cudaMemcpyHostToDevice, c->st));
-  launch_from_u32(s->tables_u32.p, s->tables_fr.p, (size_t)num_subtables * M, c->st);
-  LB_LAUNCH_CHECK();
-  g_launches += 1;
-  c->sync();  // the sources are caller memory
-  cs.d_ops = s->ops.p;
-  cs.d_consts = s->consts.p;
-  cs.d_tables_fr = s->tables_fr.p;
-  cs.d_tables_u32 = s->tables_u32.p;
-  s->cs = cs;
-  *out = s.release();
-  return 0;
+    if (!tables[k]) return fail(LASSO_ERR_STRATEGY, "strategy: null table");
+  const size_t M = (size_t)1 << log_m;
+  // canonical values: every entry a canonical Montgomery residue; the widest one fixes the commitment's windows
+  std::vector<uint32_t> small((size_t)num_subtables * M);
+  unsigned bits = 1;
+  for (int k = 0; k < num_subtables; k++)
+    for (size_t i = 0; i < M; i++) {
+      fr_t x;
+      memcpy(x.v, tables[k] + 4 * i, 32);
+      if (!fr_eq(fr_reduce_once(x.v), x)) return fail(LASSO_ERR_STRATEGY, "strategy: a table entry is not a canonical field element");
+      const fr_t v = fr_to_canonical(x);
+      for (int l = 7; l >= 0; l--)
+        if (v.v[l]) {
+          bits = std::max(bits, 32u * (unsigned)l + 32u - (unsigned)__builtin_clz(v.v[l]));
+          break;
+        }
+      small[k * M + i] = v.v[0];
+    }
+  cs.tbits = bits;
+  std::vector<const uint32_t*> rows(num_subtables);
+  for (int k = 0; k < num_subtables; k++) rows[k] = small.data() + k * M;
+  LB_TRY_CTX(h)
+  // entries below 2^32: exactly the strategy lasso_strategy_create makes of those integers
+  if (!cs.full_width()) return strategy_upload(h->c, cs, ins, constants, n_constants, rows.data(), nullptr, out);
+  return strategy_upload(h->c, cs, ins, constants, n_constants, nullptr, tables, out);
   LB_CATCH
 }
 void lasso_strategy_destroy(lasso_strategy* s) {

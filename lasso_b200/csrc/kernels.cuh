@@ -24,11 +24,13 @@ struct CustomStrategy {
   int C, log_m, nsub, alpha, degree;       // degree: the declared g_poly_degree
   int n_ops, n_consts, n_slots;
   int sub[kCustomMaxMemories], dim[kCustomMaxMemories];
-  unsigned tbits;                          // bit width of the largest table entry (>= 1)
+  unsigned tbits;                          // bit width of the largest table entry (>= 1, <= 253)
   const CustomIns* d_ops = nullptr;        // device: n_ops instructions
   const fr_t* d_consts = nullptr;          // device: n_consts Montgomery constants
   const fr_t* d_tables_fr = nullptr;       // device: nsub x M Montgomery elements
-  const uint32_t* d_tables_u32 = nullptr;  // device: nsub x M values
+  const uint32_t* d_tables_u32 = nullptr;  // device: nsub x M values; null when full_width()
+  // an entry at or above 2^32: the lookup values are committed and opened from their Montgomery form only
+  bool full_width() const { return tbits > 32; }
 };
 
 // Runtime stand-in for the reference's `impl SubtableStrategy<F, C, M>` const generics
@@ -143,6 +145,10 @@ int bound_max_chunks();
 // out[k] = <z_k, eq>, z_k = base + k*stride, k < npolys, n elements each
 void launch_multi_dot_u32(const uint32_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
                           cudaStream_t st);
+// the same two over Montgomery Fr polynomials (lookup values of a table of arbitrary field elements)
+void launch_bound_fr(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out, cudaStream_t st);
+void launch_multi_dot_fr(const fr_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
+                         cudaStream_t st);
 // Reed-Solomon fingerprints (memory_checking.rs:236-310).  init/final over M cells, read/write over s ops.
 // M_local cells of this rank; local cell i = global address i*G + g; `table` is the full M-entry table
 void launch_gp_fingerprints_mem(const fr_t* table, const fr_t* final_fr, size_t M_local, int G, int g,

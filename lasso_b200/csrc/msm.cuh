@@ -58,6 +58,12 @@ void launch_centre_constant(const pt_niels* M16, int ncols, pt_ext* K16, cudaStr
 void launch_msm_rows_direct_u32(const pt_niels* M, size_t npts, const pt_niels* M16, const pt_ext* K16, const uint32_t* scalars,
                                 size_t row_stride, int nrows, int ncols, int nw, int col_mul, int col_add, pt_ext* partials,
                                 fq_t* out_ext, uint32_t* out_comp, uint32_t* out_raw, cudaStream_t st);
+// the same rows over Montgomery Fr scalars (made canonical in the kernel), nw signed 8-bit windows over M only: every
+// scalar v needs v + sum_{w < nw} 128 * 2^(8w) < 2^(8 nw), which msm_windows_for_bits(bits of v) guarantees; column map
+// and outputs as launch_msm_rows_direct_u32
+void launch_msm_rows_direct_fr(const pt_niels* M, size_t npts, const fr_t* scalars, size_t row_stride, int nrows, int ncols,
+                               int nw, int col_mul, int col_add, pt_ext* partials, fq_t* out_ext, uint32_t* out_comp,
+                               uint32_t* out_raw, cudaStream_t st);
 void msm_init_device();
 
 // ---- one large variable-base MSM (msm_large.cu): the reference's Pippenger with a large window, buckets in HBM

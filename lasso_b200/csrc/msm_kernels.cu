@@ -1009,6 +1009,75 @@ void launch_msm_rows_direct_u32(const pt_niels* M, size_t npts, const pt_niels* 
   LB_LAUNCH_CHECK();
 }
 
+// Field-valued polynomials (a caller's table of arbitrary field elements): as msm_rows_direct_u32_kernel, but the
+// scalars are Montgomery Fr elements, made canonical in registers, and cut into nw signed 8-bit digits by the offset
+// trick over 256 bits: b = v + sum_{w < nw} 128 * 2^(8w), digit w = byte w of b - 128.  Exact when b < 2^(8 nw), so
+// for every v below 2^(8 nw - 2) (msm_windows_for_bits); 2^(8 nw - 1) - 1 would carry out of the top window.
+// One running 256-bit shift walks the digits, so the loop body (one mixed addition) exists once, whatever nw.
+__global__ void __launch_bounds__(MSM_T)
+    msm_rows_direct_fr_kernel(const pt_niels* M, size_t npts, const fr_t* scalars, size_t row_stride, int ncols, int nw,
+                              int col_mul, int col_add, pt_ext* partials) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  uint32_t* buf = reinterpret_cast<uint32_t*>(smem_raw);  // SoA point storage, MSM_T points
+  const int tid = threadIdx.x, row = blockIdx.x;
+  const fr_t* srow = scalars + (size_t)row * row_stride;
+  uint32_t off[8];  // the offset: 0x80 in each of the nw low bytes
+#pragma unroll
+  for (int l = 0; l < 8; l++) {
+    const int nb = nw - 4 * l;  // bytes of this word below the top window
+    off[l] = nb >= 4 ? 0x80808080u : (nb <= 0 ? 0u : 0x80808080u >> (8 * (4 - nb)));
+  }
+  pt_ext acc = pt_identity();
+  for (int c = tid; c < ncols; c += MSM_T) {
+    const fr_t x = ld_fr(srow + c);
+    if (fr_is_zero(x)) continue;
+    const fr_t v = fr_to_canonical(x);
+    uint32_t b[8];
+    uint64_t carry = 0;
+#pragma unroll
+    for (int l = 0; l < 8; l++) {
+      const uint64_t t = (uint64_t)v.v[l] + off[l] + carry;
+      b[l] = (uint32_t)t;
+      carry = t >> 32;
+    }
+    const pt_niels* mc = M + ((size_t)c * col_mul + col_add) * 128;
+    for (int w = 0; w < nw; w++) {
+      const int d = (int)(b[0] & 0xffu) - 128;
+      if (d != 0) {
+        pt_niels n = ld_niels(mc + (size_t)w * npts * 128 + ((d < 0 ? -d : d) - 1));
+        acc = pt_madd(acc, d < 0 ? niels_neg(n) : n);
+      }
+#pragma unroll
+      for (int l = 0; l < 7; l++) b[l] = __funnelshift_r(b[l], b[l + 1], 8);
+      b[7] >>= 8;
+    }
+  }
+  sm_store_pt(buf, MSM_T, tid, acc);
+  __syncthreads();
+  for (int d = MSM_T / 2; d >= 1; d >>= 1) {
+    if (tid < d) {
+      acc = pt_add(acc, sm_load_pt(buf, MSM_T, tid + d));
+      sm_store_pt(buf, MSM_T, tid, acc);
+    }
+    __syncthreads();
+  }
+  if (tid == 0) partials[row] = acc;
+}
+void launch_msm_rows_direct_fr(const pt_niels* M, size_t npts, const fr_t* scalars, size_t row_stride, int nrows, int ncols,
+                               int nw, int col_mul, int col_add, pt_ext* partials, fq_t* out_ext, uint32_t* out_comp,
+                               uint32_t* out_raw, cudaStream_t st) {
+  if (nrows <= 0) return;
+  if (nw < 1 || nw > kMsmFullWindows) throw std::runtime_error("msm_rows_direct_fr: nw must be in 1..32");
+  msm_rows_direct_fr_kernel<<<nrows, MSM_T, 32 * MSM_T * sizeof(uint32_t), st>>>(M, npts, scalars, row_stride, ncols, nw,
+                                                                              col_mul, col_add, partials);
+  LB_LAUNCH_CHECK();
+  if (out_raw)
+    msm_finish_kernel<<<nrows, 32, 0, st>>>(partials, nrows, 1, 1, 1, out_ext, out_comp, out_raw);
+  else
+    normalize_rows_kernel<<<(nrows + 31) / 32, 32, 0, st>>>(partials, nrows, out_ext, out_comp);
+  LB_LAUNCH_CHECK();
+}
+
 // Launch geometry.  wpc = windows per CTA (all of them over a shifted table), ngroups = window groups,
 // chunk_cols = columns per CTA: at most MSM_CHUNK list entries (columns x windows) per CTA; with only a few
 // rows (Bulletproofs rounds) the columns are split further so that about one CTA per SM exists.

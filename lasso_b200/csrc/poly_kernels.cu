@@ -1058,6 +1058,56 @@ void launch_multi_dot_u32(const uint32_t* base, size_t stride, int npolys, const
   reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
   LB_LAUNCH_CHECK();
 }
+// The Fr twins, for the lookup values of a caller's table of arbitrary field elements (no u32 mirror): a Montgomery
+// product per term.  Same chunks x R_size partials and the same second passes as the u32 forms.
+__global__ void __launch_bounds__(kThreads)
+    bound_fr_kernel(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, size_t rows_per_chunk, fr_t* partial) {
+  __shared__ fr_t sL[64];
+  const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t j0 = (size_t)blockIdx.y * rows_per_chunk;
+  size_t j1 = j0 + rows_per_chunk;
+  if (j1 > L_size) j1 = L_size;
+  fr_t acc = fr_zero();
+  for (size_t jb = j0; jb < j1; jb += 64) {
+    __syncthreads();
+    if (threadIdx.x < 64 && jb + threadIdx.x < j1) sL[threadIdx.x] = ld_fr(L + jb + threadIdx.x);
+    __syncthreads();
+    const size_t je = jb + 64 < j1 ? jb + 64 : j1;
+    if (i < R_size)
+      for (size_t j = jb; j < je; j++) acc = fr_add(acc, fr_mul(sL[j - jb], ld_fr(Z + j * R_size + i)));
+  }
+  if (i < R_size) st_fr(partial + (size_t)blockIdx.y * R_size + i, acc);
+}
+void launch_bound_fr(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out, cudaStream_t st) {
+  int chunks = (int)(L_size < (size_t)kBoundChunks ? L_size : (size_t)kBoundChunks);
+  size_t rows_per_chunk = (L_size + chunks - 1) / chunks;
+  dim3 grid((unsigned)((R_size + kThreads - 1) / kThreads), chunks);
+  bound_fr_kernel<<<grid, kThreads, 0, st>>>(Z, L, L_size, R_size, rows_per_chunk, partial);
+  LB_LAUNCH_CHECK();
+  bound_reduce_kernel<<<(unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st>>>(partial, chunks, R_size, out);
+  LB_LAUNCH_CHECK();
+}
+__global__ void __launch_bounds__(kThreads)
+    multi_dot_fr_kernel(const fr_t* base, size_t stride, const fr_t* eq, size_t n, fr_t* partial) {
+  __shared__ fr_t scratch[kThreads / 32];
+  const fr_t* P = base + (size_t)blockIdx.y * stride;
+  fr_t acc[1] = {fr_zero()};
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    acc[0] = fr_add(acc[0], fr_mul(ld_fr(eq + i), ld_fr(P + i)));
+  block_sum_fr<1>(acc, scratch);
+  if (threadIdx.x == 0) partial[(size_t)blockIdx.y * gridDim.x + blockIdx.x] = acc[0];
+}
+void launch_multi_dot_fr(const fr_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
+                         cudaStream_t st) {
+  int per = kMaxBlocks / npolys;
+  if (per < 1) per = 1;
+  int bx = grid_for(n, kThreads, per);
+  dim3 grid(bx, npolys);
+  multi_dot_fr_kernel<<<grid, kThreads, 0, st>>>(base, stride, eq, n, partial);
+  LB_LAUNCH_CHECK();
+  reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
+  LB_LAUNCH_CHECK();
+}
 
 // memory_checking.rs:249-252: hash(a, v, t) = t*gamma^2 + v*gamma + a - tau
 __global__ void __launch_bounds__(kThreads)

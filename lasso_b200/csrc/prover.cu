@@ -475,6 +475,61 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
   return msm_rows(c, g, d_vals_loc, 1, R_loc, (int)L, (int)R_loc, nw, false);
 }
 
+// The same commitment of a field-valued polynomial (Montgomery, shard as commit_u32) whose entries have at most
+// max_bits bits.  No sign folding: v is committed as the canonical integer it is, so an entry l - k costs the full
+// width (folding it to -k is exact only in the prime-order subgroup, and the generators are the caller's).
+static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_loc, size_t nv, unsigned max_bits) {
+  size_t L = (size_t)1 << (nv / 2), R = (size_t)1 << (nv - nv / 2);
+  if (R + 2 > g.n_points) throw std::runtime_error("generator stream too short for this polynomial");
+  const int G = c->world;
+  size_t R_loc = loc(c, R);
+  if (!(g.d_multiples.p && R + 2 <= g.n_direct)) {
+    DBuf<fr_t> canon(c, L * R_loc);
+    launch_canonicalize(d_vals_loc, canon.p, L * R_loc, c->d_flag, c->st);
+    g_launches += 1;
+    return msm_rows(c, g, canon.p, 8, R_loc, (int)L, (int)R_loc, kMsmFullWindows, false);
+  }
+  // rows as direct sums over the 8-bit digit-multiples tables: one table entry per non-zero signed digit
+  const int nw = msm_windows_for_bits(max_bits);
+  std::vector<uint8_t> out(L * 32);
+  DBuf<pt_ext> part(c, L);
+  DBuf<uint32_t> comp(c, L * 8);
+  if (G == 1) {
+    launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, comp.p,
+                              nullptr, c->st);
+    g_launches += 2;
+  } else {  // this rank's columns of every row -> partial points -> gather-then-add over the ranks
+    DBuf<uint32_t> raw(c, (size_t)(G + 1) * L * 32);
+    uint32_t* mine = raw.p + (size_t)G * L * 32;
+    launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R_loc, (int)L, (int)R_loc, nw, G, c->rank, part.p,
+                              nullptr, nullptr, mine, c->st);
+    comm_allgather(c, mine, raw.p, L * 128);
+    launch_sum_raw_points(raw.p, G, (int)L, nullptr, comp.p, nullptr, c->st);
+    g_launches += 3;
+  }
+  c->d2h(out.data(), comp.p, out.size());
+  return out;
+}
+
+// The lookup values E as the openings and the derefs commitment read them: the u32 mirror when every table entry
+// is below 2^32, else (u32 == nullptr) the Montgomery form.  The implicit form wraps an integer-valued u32 polynomial.
+struct PolySrc {
+  const uint32_t* u32;
+  const fr_t* fr;
+  PolySrc(const uint32_t* u) : u32(u), fr(nullptr) {}
+  PolySrc(const uint32_t* u, const fr_t* f) : u32(u), fr(f) {}
+};
+static std::vector<uint8_t> commit_src(Ctx* c, const Gens& g, PolySrc Z, size_t nv, unsigned max_bits) {
+  return Z.u32 ? commit_u32(c, g, Z.u32, nv, max_bits) : commit_fr(c, g, Z.fr, nv, max_bits);
+}
+static void multi_dot_src(PolySrc Z, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
+                          cudaStream_t st) {
+  if (Z.u32)
+    launch_multi_dot_u32(Z.u32, stride, npolys, eq, n, partial, out, st);
+  else
+    launch_multi_dot_fr(Z.fr, stride, npolys, eq, n, partial, out, st);
+}
+
 // ---------------------------------------------------------------------------------------------- densify
 Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m, int* err) {
   SpanTimer sp(c, "Densify");
@@ -1132,13 +1187,13 @@ __global__ void set_elems_kernel(fr_t* dst, fr_t a, fr_t b) {
 }
 
 // PolyEvalProof::prove (dense_mlpoly.rs:301-359) -> DotProductProofLog::prove (dot_product.rs:166-249)
-// -> BulletReductionProof::prove (bullet.rs:40-154).  Z_u32: this rank's shard of an integer-valued polynomial of
-// 2^nv elements, i.e. for every one of the L rows the R/G columns congruent to the rank.
+// -> BulletReductionProof::prove (bullet.rs:40-154).  Z: this rank's shard of a polynomial of 2^nv elements, i.e. for
+// every one of the L rows the R/G columns congruent to the rank.
 // One proof sharded over G GPUs: LZ = L . Z is computed on the column shards and all-gathered (R elements); from
 // there on the opening runs REPLICATED on every rank — its vectors are only R = 2^(nv - nv/2) long and every round
 // is latency-bound, so splitting its two-row MSMs would add an exchange per round and save nothing.  Every rank
 // computes the same points and the same transcript.
-static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const uint32_t* Z_u32, size_t nv,
+static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z, size_t nv,
                                                const std::vector<fr_t>& r, const fr_t& Zr, Transcript& transcript,
                                                RandomTape& tape) {
   SpanTimer sp(c, "DensePolyEval.prove");
@@ -1155,8 +1210,11 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const uint
   eq_evals_dev(c, r, 0, lv, Lvec.p);  // rows are not sharded: L is replicated
   eq_evals_dev(c, r, lv, rv, b.p);    // a_vec of the dot product proof = R
   if ((size_t)bound_max_chunks() * n_loc > c->partial_elems) throw std::runtime_error("bound scratch too small");
-  // x_vec = LZ (this rank's columns) over the u32 mirror of the polynomial
-  launch_bound_u32(Z_u32, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
+  // x_vec = LZ (this rank's columns)
+  if (Z.u32)
+    launch_bound_u32(Z.u32, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
+  else
+    launch_bound_fr(Z.fr, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
   g_launches += 2;
   if (G > 1) comm_gather_vector(c, a_loc.p, n_loc, a_gath.p, a.p);
 
@@ -1354,7 +1412,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, const uint
 
 // CombinedTableEvalProof::prove (subtables/mod.rs:284-313 + prove_single 230-281) and the two analogous
 // n-to-1 reductions of HashLayerProof::prove: fold `evals` with bound_poly_var_bot in reverse challenge order.
-static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, const uint32_t* Z_u32, size_t nv, std::vector<fr_t> evals,
+static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, PolySrc Z, size_t nv, std::vector<fr_t> evals,
                                            bool pad_before_append, const char* evals_label, const char* chal_label,
                                            const char* joint_label, const std::vector<fr_t>& r,
                                            Transcript& transcript, RandomTape& tape) {
@@ -1374,7 +1432,7 @@ static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, const uint32_t
   std::vector<fr_t> r_joint = challenges;
   r_joint.insert(r_joint.end(), r.begin(), r.end());
   transcript.append_scalar(joint_label, joint);
-  return prove_poly_eval(c, g, Z_u32, nv, r_joint, joint, transcript, tape);
+  return prove_poly_eval(c, g, Z, nv, r_joint, joint, transcript, tape);
 }
 
 // ---------------------------------------------------------------------------------------------- prove
@@ -1403,8 +1461,10 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
   DBuf<uint32_t> tables_u32_buf(c, custom ? 0 : (size_t)nsub * M);
   const fr_t* tables_fr = custom ? S.custom->d_tables_fr : tables_fr_buf.p;
   const uint32_t* tables_u32 = custom ? S.custom->d_tables_u32 : tables_u32_buf.p;
+  const bool full_width = custom && S.custom->full_width();
   DBuf<fr_t> E(c, nd_loc);          // combined_poly = E_0 | .. | E_{alpha-1} | 0-pad (this rank's shard)
-  DBuf<uint32_t> E_u32(c, nd_loc);  // same values as integers for the small-scalar commit
+  DBuf<uint32_t> E_u32(c, full_width ? 0 : nd_loc);  // same values as integers for the small-scalar commit
+  const PolySrc E_src(E_u32.p, E.p);  // what the derefs commitment and openings read
   {
     SpanTimer sp(c, "Subtables.new");
     if (!custom) {
@@ -1415,7 +1475,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     g_launches += 1;
     if (nd_loc > alpha * s_loc) {
       launch_fill_zero(E.p + alpha * s_loc, nd_loc - alpha * s_loc, c->st);
-      LB_CUDA_CHECK(cudaMemsetAsync(E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
+      if (E_u32.p) LB_CUDA_CHECK(cudaMemsetAsync(E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
     }
   }
   ByteWriter w;
@@ -1425,7 +1485,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     SpanTimer sp(c, "Subtables.commit");
     unsigned tbits = custom ? S.custom->tbits
                             : (S.kind == STRAT_LT ? 1 : (S.kind == STRAT_RANGE ? (unsigned)S.log_m : (unsigned)(S.log_m / 2)));
-    comm_E = commit_u32(c, g, E_u32.p, nv_d, tbits);
+    comm_E = commit_src(c, g, E_src, nv_d, tbits);
     w.vec_pts(comm_E);
   }
   auto absorb_comm_E = [&]() {  // ~700 Keccak permutations (2^11 points): done while the device prepares the sumcheck
@@ -1459,12 +1519,12 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
   {
     SpanTimer sp(c, "CombinedEval.prove");
     eq_evals_shard(c, r_z, 0, log_s, eqtab.p);
-    launch_multi_dot_u32(E_u32.p, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
+    multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
     g_launches += 2;
     reduce_to_host(c, c->d_small, (int)alpha, eval_derefs.data());
     w.arr_fr(eval_derefs);
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
-    ser_dpl(w, prove_joint(c, g, E_u32.p, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
+    ser_dpl(w, prove_joint(c, g, E_src, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
                            "joint_claim_eval", r_z, transcript, tape));
   }
   // ---- memory checking (surge.rs:186-198)
@@ -1547,7 +1607,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     transcript.append_protocol_name("Lasso HashLayerProof");
     std::vector<fr_t> eval_derefs2(alpha), eval_dim(C), eval_read(C), eval_final(C);
     eq_evals_shard(c, rand_ops, 0, rand_ops.size(), eqtab.p);
-    launch_multi_dot_u32(E_u32.p, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
+    multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
     launch_multi_dot_u32(dense.d_l_u32.p, s_loc, (int)(2 * C), eqtab.p, s_loc, c->d_partial + 65536, c->d_small + 64, c->st);
     g_launches += 4;
     {
@@ -1561,7 +1621,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     }
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
     DotProductProofLogBytes proof_derefs =
-        prove_joint(c, g, E_u32.p, nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
+        prove_joint(c, g, E_src, nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
                     "joint_claim_eval", rand_ops, transcript, tape);
     eq_evals_shard(c, rand_mem, 0, rand_mem.size(), eqtab.p);
     launch_multi_dot_u32(dense.d_m_u32.p, M_loc, (int)C, eqtab.p, M_loc, c->d_partial, c->d_small, c->st);

@@ -218,27 +218,20 @@ CustomStrategy make(size_t C, size_t log_m, size_t nsub, const uint32_t* tables,
   S.K = ldvec(K, n_k);
   return S;
 }
-
-}  // namespace
-
-#define ORC_CUSTOM_ARGS                                                                                             \
-  size_t C, size_t log_m, size_t nsub, const uint32_t *tables, size_t alpha, const int32_t *sub, const int32_t *dim, \
-      const int32_t *prog, size_t n_ops, const uint64_t *K, size_t n_k, size_t degree
-#define ORC_CUSTOM make(C, log_m, nsub, tables, alpha, sub, dim, prog, n_ops, K, n_k, degree)
-
-extern "C" {
-
-void orc_custom_combine_lookups(ORC_CUSTOM_ARGS, const uint64_t* vals, uint64_t* out) {
-  stfr(out, ORC_CUSTOM.combine_lookups(ldvec(vals, alpha).data()));
+// the same with tables = nsub x M Fr (4 Montgomery limbs each, row-major): entries of any width
+CustomStrategy make_fr(size_t C, size_t log_m, size_t nsub, const uint64_t* tables, size_t alpha, const int32_t* sub,
+                       const int32_t* dim, const int32_t* prog, size_t n_ops, const uint64_t* K, size_t n_k,
+                       size_t degree) {
+  const uint32_t zero = 0;
+  CustomStrategy S = make(C, log_m, 0, &zero, alpha, sub, dim, prog, n_ops, K, n_k, degree);
+  const size_t M = pow2(log_m);
+  for (size_t k = 0; k < nsub; k++) S.tables.push_back(ldvec(tables + 4 * k * M, M));
+  return S;
 }
-void orc_custom_evaluate_subtable_mle(ORC_CUSTOM_ARGS, size_t idx, const uint64_t* point, size_t npoint,
-                                      uint64_t* out) {
-  stfr(out, ORC_CUSTOM.evaluate_subtable_mle(idx, ldvec(point, npoint)));
-}
+
 // one round of the primary sumcheck's evaluation loop (sumcheck.rs:179-237): polys = (alpha+1) x len, the last eq
-void orc_custom_sumcheck_round(ORC_CUSTOM_ARGS, const uint64_t* polys, size_t len, uint64_t* evals_out) {
-  const CustomStrategy S = ORC_CUSTOM;
-  const size_t np = alpha + 1, deg = degree + 1, half = len / 2;
+void sumcheck_round(const CustomStrategy& S, const uint64_t* polys, size_t len, uint64_t* evals_out) {
+  const size_t alpha = S.num_memories(), np = alpha + 1, deg = S.degree + 1, half = len / 2;
   auto g = [&](const std::vector<Fr>& v) { return S.combine_lookups(v.data()) * v[alpha]; };
   std::vector<Fr> ev(deg + 1, Fr::zero()), cur(np), nxt(np);
   for (size_t i = 0; i < half; i++) {
@@ -255,15 +248,14 @@ void orc_custom_sumcheck_round(ORC_CUSTOM_ARGS, const uint64_t* polys, size_t le
   }
   memcpy(evals_out, ev.data(), (deg + 1) * 32);
 }
-// Densify -> commit -> prove (-> verify), as orc_prove in oracle/capi.cpp.  indices: n x C row-major; gens: affine
-// generator stream of n_gens points.  flags: bit0 = run verify, bit1 = tamper with the claimed evaluation before
-// verifying, bit2 = tamper with a memory-checking evaluation instead.  Returns 0 ok; 1 verify rejected; < 0 error.
-int orc_custom_prove(ORC_CUSTOM_ARGS, const uint64_t* indices, size_t n, const uint64_t* r, const uint64_t* gens,
-                     size_t n_gens, const uint64_t* tape_seed, int flags, uint8_t* proof_out, size_t proof_cap,
-                     size_t* proof_len, uint8_t* commit_out, size_t commit_cap, size_t* commit_len,
-                     uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
+
+// Densify -> commit -> prove (-> verify): see orc_custom_prove
+int prove_all(const CustomStrategy& S, const uint64_t* indices, size_t n, const uint64_t* r, const uint64_t* gens,
+              size_t n_gens, const uint64_t* tape_seed, int flags, uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+              uint8_t* commit_out, size_t commit_cap, size_t* commit_len, uint64_t* challenges_out, size_t challenges_cap,
+              size_t* n_challenges) {
   try {
-    const CustomStrategy S = ORC_CUSTOM;
+    const size_t C = S.C, log_m = S.log_m, alpha = S.num_memories();
     std::vector<std::vector<size_t>> idx(n, std::vector<size_t>(C));
     for (size_t j = 0; j < n; j++)
       for (size_t i = 0; i < C; i++) idx[j][i] = indices[j * C + i];
@@ -298,6 +290,60 @@ int orc_custom_prove(ORC_CUSTOM_ARGS, const uint64_t* indices, size_t n, const u
     fprintf(stderr, "orc_custom_prove: %s\n", e.what());
     return -1;
   }
+}
+
+}  // namespace
+
+#define ORC_CUSTOM_ARGS                                                                                             \
+  size_t C, size_t log_m, size_t nsub, const uint32_t *tables, size_t alpha, const int32_t *sub, const int32_t *dim, \
+      const int32_t *prog, size_t n_ops, const uint64_t *K, size_t n_k, size_t degree
+#define ORC_CUSTOM make(C, log_m, nsub, tables, alpha, sub, dim, prog, n_ops, K, n_k, degree)
+#define ORC_CUSTOM_ARGS_FR                                                                                          \
+  size_t C, size_t log_m, size_t nsub, const uint64_t *tables, size_t alpha, const int32_t *sub, const int32_t *dim, \
+      const int32_t *prog, size_t n_ops, const uint64_t *K, size_t n_k, size_t degree
+#define ORC_CUSTOM_FR make_fr(C, log_m, nsub, tables, alpha, sub, dim, prog, n_ops, K, n_k, degree)
+
+extern "C" {
+
+void orc_custom_combine_lookups(ORC_CUSTOM_ARGS, const uint64_t* vals, uint64_t* out) {
+  stfr(out, ORC_CUSTOM.combine_lookups(ldvec(vals, alpha).data()));
+}
+void orc_custom_evaluate_subtable_mle(ORC_CUSTOM_ARGS, size_t idx, const uint64_t* point, size_t npoint,
+                                      uint64_t* out) {
+  stfr(out, ORC_CUSTOM.evaluate_subtable_mle(idx, ldvec(point, npoint)));
+}
+// one round of the primary sumcheck's evaluation loop (sumcheck.rs:179-237): polys = (alpha+1) x len, the last eq
+void orc_custom_sumcheck_round(ORC_CUSTOM_ARGS, const uint64_t* polys, size_t len, uint64_t* evals_out) {
+  sumcheck_round(ORC_CUSTOM, polys, len, evals_out);
+}
+// Densify -> commit -> prove (-> verify), as orc_prove in oracle/capi.cpp.  indices: n x C row-major; gens: affine
+// generator stream of n_gens points.  flags: bit0 = run verify, bit1 = tamper with the claimed evaluation before
+// verifying, bit2 = tamper with a memory-checking evaluation instead.  Returns 0 ok; 1 verify rejected; < 0 error.
+int orc_custom_prove(ORC_CUSTOM_ARGS, const uint64_t* indices, size_t n, const uint64_t* r, const uint64_t* gens,
+                     size_t n_gens, const uint64_t* tape_seed, int flags, uint8_t* proof_out, size_t proof_cap,
+                     size_t* proof_len, uint8_t* commit_out, size_t commit_cap, size_t* commit_len,
+                     uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
+  return prove_all(ORC_CUSTOM, indices, n, r, gens, n_gens, tape_seed, flags, proof_out, proof_cap, proof_len, commit_out,
+                   commit_cap, commit_len, challenges_out, challenges_cap, n_challenges);
+}
+
+// _fr twins: the tables as nsub x M Fr (Montgomery limbs) instead of u32
+void orc_custom_combine_lookups_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* vals, uint64_t* out) {
+  stfr(out, ORC_CUSTOM_FR.combine_lookups(ldvec(vals, alpha).data()));
+}
+void orc_custom_evaluate_subtable_mle_fr(ORC_CUSTOM_ARGS_FR, size_t idx, const uint64_t* point, size_t npoint,
+                                         uint64_t* out) {
+  stfr(out, ORC_CUSTOM_FR.evaluate_subtable_mle(idx, ldvec(point, npoint)));
+}
+void orc_custom_sumcheck_round_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* polys, size_t len, uint64_t* evals_out) {
+  sumcheck_round(ORC_CUSTOM_FR, polys, len, evals_out);
+}
+int orc_custom_prove_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* indices, size_t n, const uint64_t* r, const uint64_t* gens,
+                        size_t n_gens, const uint64_t* tape_seed, int flags, uint8_t* proof_out, size_t proof_cap,
+                        size_t* proof_len, uint8_t* commit_out, size_t commit_cap, size_t* commit_len,
+                        uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
+  return prove_all(ORC_CUSTOM_FR, indices, n, r, gens, n_gens, tape_seed, flags, proof_out, proof_cap, proof_len,
+                   commit_out, commit_cap, commit_len, challenges_out, challenges_cap, n_challenges);
 }
 
 }  // extern "C"

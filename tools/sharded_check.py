@@ -6,7 +6,9 @@ host segments + CUDA IPC exchange buffers, csrc/comm.cu) do not need one device 
 run this check too.
 With --custom every strategy is a caller-defined one (lasso_b200.CustomStrategy): the built-in cases re-expressed as
 programs plus tables that are not built in, checked against the oracle for caller-defined strategies (oracle_custom/).
-usage: torchrun --nproc-per-node N tools/sharded_check.py [--custom] [kind C log_m log_r lookups same]"""
+With --fr the strategies are caller-defined ones over tables of arbitrary field elements (tests/field_tables.py, the
+full-width commitment and openings), checked the same way.
+usage: torchrun --nproc-per-node N tools/sharded_check.py [--custom | --fr] [kind C log_m log_r lookups same]"""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -17,6 +19,8 @@ import lasso_b200 as lb
 import oracle_lib as ol
 import custom_builtins as cb
 import oracle_custom_lib as oc
+import oracle_custom_fr_lib as ocf
+import field_tables as ft
 
 rank = int(os.environ.get("RANK", 0)); local = int(os.environ.get("LOCAL_RANK", 0)); world = int(os.environ.get("WORLD_SIZE", 1))
 same_gpu = os.environ.get("LASSO_SHARD_SAME_GPU") == "1"
@@ -29,17 +33,22 @@ else:
     dist.init_process_group("nccl", device_id=torch.device("cuda", local))
 cases = [(2, 4, 16, 0, 1 << 12, 1), (3, 4, 4, 0, 128, 0), (0, 1, 16, 0, 1 << 10, 1), (4, 3, 8, 40, 256, 0), (3, 8, 8, 0, 512, 0),
          (1, 2, 8, 0, 700, 0)]
-custom = "--custom" in sys.argv
-argv = [a for a in sys.argv if a != "--custom"]
+fr = "--fr" in sys.argv
+custom = "--custom" in sys.argv or fr
+argv = [a for a in sys.argv if a not in ("--custom", "--fr")]
 if len(argv) > 6:
     cases = [tuple(int(x) for x in argv[1:7])]
-if custom:  # new tables: kind = -1 - their index in cb.NEW_TABLES
+if fr:  # field-element tables: kind = -100 - their index in ft.INTS; C = 2, odd log_m, degree 2
+    cases = [(-100 - i, 2, 7, 0, 600 + i, 0) for i in range(len(ft.INTS))]
+elif custom:  # new tables: kind = -1 - their index in cb.NEW_TABLES
     cases += [(-1 - i, 0, 0, 0, 300 + i, 0) for i in range(len(cb.NEW_TABLES))]
 ctx = lb.Context(local)
 ctx.init_comm()
 ok = True
 for kind, C, log_m, log_r, n, same in cases:
-    if kind < 0:
+    if kind <= -100:
+        S = ft.strategy(ctx, sorted(ft.INTS)[-100 - kind], C, log_m, 2, nsub=2)
+    elif kind < 0:
         S = cb.NEW_TABLES[sorted(cb.NEW_TABLES)[-1 - kind]](ctx)
         C, log_m = S.C, S.log_m
     elif custom:
@@ -61,7 +70,7 @@ for kind, C, log_m, log_r, n, same in cases:
     dt = time.time() - t0
     if rank == 0:
         if custom:
-            ref = oc.prove(S, idx, r, stream, seed, flags=1)
+            ref = (ocf if fr else oc).prove(S, idx, r, stream, seed, flags=1)
         else:
             ref = ol.prove(kind, C, log_m, log_r, idx, r, stream, seed, flags=1)
         good = ref["rc"] == 0 and com == ref["commitment"] and proof.bytes == ref["proof"]
