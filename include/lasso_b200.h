@@ -41,7 +41,8 @@ enum {
   LASSO_ERR_INDEX_RANGE = 3, /* debug_assert!(memory_address < m)           lasso/densified.rs:46 */
   LASSO_ERR_STRATEGY = 4,    /* unknown / unsupported strategy parameters */
   LASSO_ERR_GENS = 5,        /* generator set too small for the polynomial  poly/commitments.rs:85 */
-  LASSO_ERR_MULTISET = 6     /* assert_eq!(hash_init*hash_write, hash_read*hash_final) memory_checking.rs:689 */
+  LASSO_ERR_MULTISET = 6,    /* assert_eq!(hash_init*hash_write, hash_read*hash_final) memory_checking.rs:689 */
+  LASSO_ERR_POINTER = 7      /* a buffer that must be device memory of the context's GPU is not */
 };
 
 const char* lasso_last_error(void);
@@ -148,6 +149,25 @@ void lasso_gens_destroy(lasso_gens*);
 /* DensifiedRepresentation::from_lookup_indices  lasso/densified.rs:21-75.
  * indices: n_lookups x C row-major `usize` (the reference's &Vec<[usize; C]>). */
 int lasso_densify(lasso_ctx*, const uint64_t* indices, size_t n_lookups, size_t C, size_t log_m, lasso_dense** out);
+/* DensifiedRepresentation::from_lookup_indices with the index matrix in DEVICE memory of the context's GPU (e.g. a
+ * torch CUDA tensor, or lookups a kernel of the caller wrote): no host narrowing, no upload, the GPU sort at every size.
+ *  - entry (k, i), k < n_lookups, i < C, is indices[k * row_stride + i * col_stride] (strides in elements, so
+ *    transposed and sliced views need no copy), an UNSIGNED integer of elem_bytes = 4 or 8.  It is compared with m in
+ *    its full width: an entry >= m (a signed -1 included) returns LASSO_ERR_INDEX_RANGE, creates no dense and leaves
+ *    the context usable;
+ *  - the addresses of the first and the last entry must both be device memory of the context's device
+ *    (cudaPointerGetAttributes); otherwise (host, pinned, managed or another GPU's memory) LASSO_ERR_POINTER, before
+ *    any launch;
+ *  - elem_bytes not 4 or 8, and the n_lookups, C, log_m lasso_densify rejects, return LASSO_ERR_STRATEGY;
+ *  - stream (a cudaStream_t of the context's device, NULL = the legacy default stream): the matrix is read only after
+ *    all work enqueued on `stream` before the call, and work enqueued on `stream` after the call returns is ordered
+ *    after those reads (a caching allocator may free or reuse the matrix in stream order).  The call returns once
+ *    the range verdict is known; the sort may still run, stream-ordered like lasso_densify's;
+ *  - on a sharded context the call is collective like lasso_densify: every rank passes the WHOLE matrix, on its own
+ *    GPU, checks all of it (so every rank reaches the same verdict without an exchange), sorts it and keeps its shard;
+ *  - lasso_last_timings reports its wall time as the densify time. */
+int lasso_densify_device(lasso_ctx*, const void* indices, size_t elem_bytes, size_t n_lookups, size_t C,
+                         size_t row_stride, size_t col_stride, size_t log_m, void* stream, lasso_dense** out);
 void lasso_dense_destroy(lasso_dense*);
 size_t lasso_dense_s(const lasso_dense*);
 /* copies of the public fields (densified.rs:8-18) back to the host, for inspection / tests:

@@ -4,6 +4,7 @@ Field elements are numpy uint64 arrays (..., 4): ark-ff Montgomery limbs.  Affin
 extended points (..., 16)."""
 import ctypes as C
 import os
+import sys
 
 import numpy as np
 
@@ -88,7 +89,7 @@ class Strategy:
 
 # ------------------------------------------------------------------ caller-defined strategies
 OP_ADD, OP_SUB, OP_MUL, OP_MULK, OP_ADDK = 0, 1, 2, 3, 4
-LASSO_ERR_STRATEGY = 4
+LASSO_ERR_INDEX_RANGE, LASSO_ERR_STRATEGY, LASSO_ERR_POINTER = 3, 4, 7
 FR_MODULUS = 2**252 + 27742317777372353535851937790883648493
 MAX_MEMORIES, MAX_OPS, MAX_CONSTANTS, MAX_DEGREE = 16, 128, 64, 16
 
@@ -518,12 +519,34 @@ class DensifiedRepresentation:
 
     @classmethod
     def from_lookup_indices(cls, ctx, indices, log_m):
+        """indices: n x C lookup indices.  A numpy array (or anything numpy converts, CPU tensors included) is narrowed
+        on the host and uploaded (lasso_densify).  A torch CUDA tensor of dtype int64 or int32 stays where it is
+        (lasso_densify_device): any strides, read in the order of torch's current stream of its device; its entries are
+        read as unsigned integers, so a negative one is out of range (LassoError code 3)."""
+        torch = sys.modules.get("torch")  # a CUDA tensor exists only if torch is loaded already
+        if torch is not None and isinstance(indices, torch.Tensor) and indices.is_cuda:
+            return cls._from_device_tensor(ctx, indices, log_m, torch)
         idx = np.ascontiguousarray(indices, dtype=np.uint64)
         assert idx.ndim == 2
         h = C.c_void_p()
         _chk(lib().lasso_densify(ctx._h, _p(idx), C.c_size_t(idx.shape[0]), C.c_size_t(idx.shape[1]),
                                  C.c_size_t(log_m), C.byref(h)))
         return cls(ctx, h, idx.shape[1], log_m)
+
+    @classmethod
+    def _from_device_tensor(cls, ctx, t, log_m, torch):
+        if t.dtype not in (torch.int64, torch.int32):
+            raise LassoError(LASSO_ERR_STRATEGY, "CUDA lookup indices must be int64 or int32, not %s" % t.dtype)
+        if t.ndim != 2:
+            raise LassoError(LASSO_ERR_STRATEGY, "CUDA lookup indices must be an n x C matrix, not %d-dimensional" % t.ndim)
+        n, c = t.shape
+        row_stride, col_stride = t.stride()
+        stream = torch.cuda.current_stream(t.device).cuda_stream
+        h = C.c_void_p()
+        _chk(lib().lasso_densify_device(ctx._h, C.c_void_p(t.data_ptr()), C.c_size_t(t.element_size()), C.c_size_t(n),
+                                        C.c_size_t(c), C.c_size_t(row_stride), C.c_size_t(col_stride), C.c_size_t(log_m),
+                                        C.c_void_p(stream), C.byref(h)))
+        return cls(ctx, h, c, log_m)
 
     def _read(self, which, n, width):
         out = np.zeros((n, width) if width > 1 else (n,), dtype=np.uint64)

@@ -564,6 +564,22 @@ int lasso_densify(lasso_ctx* h, const uint64_t* indices, size_t n_lookups, size_
   return 0;
   LB_CATCH
 }
+int lasso_densify_device(lasso_ctx* h, const void* indices, size_t elem_bytes, size_t n_lookups, size_t C,
+                         size_t row_stride, size_t col_stride, size_t log_m, void* stream, lasso_dense** out) {
+  LB_TRY_CTX(h)
+  *out = nullptr;
+  auto t0 = std::chrono::steady_clock::now();
+  int err = 0;
+  Dense* d = densify_device(h->c, indices, elem_bytes, n_lookups, C, row_stride, col_stride, log_m,
+                            static_cast<cudaStream_t>(stream), &err);
+  if (err == 3) return fail(LASSO_ERR_INDEX_RANGE, "densify_device: an index is >= m");
+  if (err == 7) return fail(LASSO_ERR_POINTER, "densify_device: the indices are not device memory of the context's GPU");
+  if (!d) return fail(LASSO_ERR_STRATEGY, "densify_device: invalid input");
+  h->c->t_densify_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  *out = new lasso_dense{d};
+  return 0;
+  LB_CATCH
+}
 void lasso_dense_destroy(lasso_dense* d) {
   if (!d) return;
   delete d->d;

@@ -6,8 +6,8 @@
 // index k) then has read[k] = p - start[a], start = the exclusive scan of the per-address counts (= final).
 // The stable sort is an LSD radix sort with 8-bit digits over packed (address << 32 | k) words, all C dimensions
 // in the same launches (blockIdx.y = dimension):
-//   extract_kernel   column `dim` of the row-major index matrix -> packed words (zero-padded to s, densified.rs:33-37),
-//                    this rank's shard of dim, per-address counts (RED atomics)
+//   extract_kernel   column `dim` of the (strided, u32 or u64) index matrix -> range check, packed words (zero-padded to
+//                    s, densified.rs:33-37), this rank's shard of dim, per-address counts (RED atomics)
 //   per 8-bit digit (ceil(log_m / 8) passes):
 //     radix_hist_kernel     digit histogram of every tile of 2048 elements -> H[dim][bin][tile]
 //     scan_*_kernel         exclusive scan of H in (bin, tile) order = where each tile's run of each digit starts
@@ -28,20 +28,35 @@ static constexpr int kRadixTile = kRadixThreads * kRadixRounds;  // 2048 element
 static constexpr uint32_t kDzScanTile = 4096;
 
 // ---------------------------------------------------------------------------------------------- extract
-// idx: n x C u32 row-major (already narrowed and range-checked on the host while staging it into pinned memory)
+// Entry (k, dim) of the index matrix is idx[k * row_stride + dim * col_stride], an unsigned integer of T's full width
+// (T = uint32_t or unsigned long long).  It is compared with m BEFORE any narrowing, so an int64 2^32 + 5 or a -1 of
+// either width is out of range; such an entry raises *bad and is replaced by address 0 (as the host scan does), so it
+// is never used as an address.  bad == nullptr: the caller has range-checked the entries already.
+template <class T>
 __global__ void __launch_bounds__(256)
-    dz_extract_kernel(const uint32_t* idx, size_t n, size_t s, int C, uint32_t m, int G, int g, unsigned long long* packed,
-                      uint32_t* count, uint32_t* dim_loc_base, size_t dim_stride) {
+    dz_extract_kernel(const T* idx, size_t row_stride, size_t col_stride, size_t n, size_t s, uint32_t m, int G, int g,
+                      unsigned long long* packed, uint32_t* count, uint32_t* dim_loc_base, size_t dim_stride,
+                      unsigned* bad) {
   const int dim = blockIdx.y;
   unsigned long long* out = packed + (size_t)dim * s;
   uint32_t* cnt = count + (size_t)dim * m;
   uint32_t* dim_loc = dim_loc_base + (size_t)dim * dim_stride;
+  const T* col = idx + (size_t)dim * col_stride;
+  bool violation = false;
   for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < s; k += (size_t)gridDim.x * blockDim.x) {
-    const uint32_t a = k < n ? idx[k * C + dim] : 0u;
+    uint32_t a = 0u;
+    if (k < n) {
+      const T v = col[k * row_stride];
+      if (v < (T)m)
+        a = (uint32_t)v;
+      else
+        violation = true;
+    }
     out[k] = ((unsigned long long)a << 32) | (unsigned long long)k;
     atomicAdd(cnt + a, 1u);
     if ((int)(k % G) == g) dim_loc[k / G] = a;
   }
+  if (violation && bad) *bad = 1u;
 }
 
 // ---------------------------------------------------------------------------------------------- radix pass
@@ -219,13 +234,14 @@ size_t densify_scratch_words(size_t s, int C, size_t log_m) {
   const size_t H = (size_t)C * 256 * ntiles;
   const size_t scan_len = std::max((size_t)256 * ntiles, m);
   const size_t tsums = (size_t)C * ((scan_len + kDzScanTile - 1) / kDzScanTile + 1);
+  // + 64 spare words, the last of them the range flag of launch_densify
   return 2 * 2 * (size_t)C * s /* two packed arrays of u64 */ + (size_t)C * m /* counts / start */ + H + tsums + 64;
 }
-// d_idx: n x C u32 on the device.  Outputs are this rank's shards: dim_i at dim_loc + i * dim_stride (likewise
-// read, final).  Returns the number of kernels launched.
-int launch_densify(const uint32_t* d_idx, size_t n, size_t s, int C, size_t log_m, int G, int g, uint32_t* scratch,
-                   uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride, uint32_t* final_loc,
-                   size_t final_stride, cudaStream_t st) {
+// Outputs are this rank's shards: dim_i at dim_loc + i * dim_stride (likewise read, final).  Returns the number of
+// kernels launched.
+int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
+                   uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
+                   uint32_t* final_loc, size_t final_stride, cudaStream_t st) {
   const uint32_t m = 1u << log_m;
   const uint32_t ntiles = (uint32_t)((s + kRadixTile - 1) / kRadixTile);
   unsigned long long* pa = reinterpret_cast<unsigned long long*>(scratch);
@@ -233,14 +249,26 @@ int launch_densify(const uint32_t* d_idx, size_t n, size_t s, int C, size_t log_
   uint32_t* count = reinterpret_cast<uint32_t*>(pb + (size_t)C * s);
   uint32_t* H = count + (size_t)C * m;
   uint32_t* tsums = H + (size_t)C * 256 * ntiles;
+  unsigned* bad = check ? reinterpret_cast<unsigned*>(scratch + densify_scratch_words(s, C, log_m) - 1) : nullptr;
   int launches = 0;
   LB_CUDA_CHECK(cudaMemsetAsync(count, 0, (size_t)C * m * 4, st));
+  if (bad) LB_CUDA_CHECK(cudaMemsetAsync(bad, 0, sizeof(unsigned), st));
   {
     size_t bx = (s + 255) / 256;
     if (bx > (size_t)kNumSMs * 8) bx = kNumSMs * 8;
-    dz_extract_kernel<<<dim3((unsigned)bx, (unsigned)C), 256, 0, st>>>(d_idx, n, s, C, m, G, g, pa, count, dim_loc, dim_stride);
+    const dim3 grid((unsigned)bx, (unsigned)C);
+    if (idx.elem_bytes == 8)
+      dz_extract_kernel<<<grid, 256, 0, st>>>(static_cast<const unsigned long long*>(idx.p), idx.row_stride, idx.col_stride,
+                                              n, s, m, G, g, pa, count, dim_loc, dim_stride, bad);
+    else
+      dz_extract_kernel<<<grid, 256, 0, st>>>(static_cast<const uint32_t*>(idx.p), idx.row_stride, idx.col_stride, n, s, m,
+                                              G, g, pa, count, dim_loc, dim_stride, bad);
     LB_LAUNCH_CHECK();
     launches++;
+  }
+  if (check) {  // the verdict, and the point after which the index matrix is no longer read
+    LB_CUDA_CHECK(cudaMemcpyAsync(check->h_bad, bad, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
+    LB_CUDA_CHECK(cudaEventRecord(check->ev, st));
   }
   unsigned long long *cur = pa, *nxt = pb;
   for (int shift = 0; shift < (int)log_m; shift += 8) {  // LSD: least significant digit first, every pass stable

@@ -183,10 +183,24 @@ void launch_scale(const fr_t* in, fr_t* out, size_t n, const fr_t& k, cudaStream
 void densify_init_device();
 bool densify_gpu_supported(size_t s, size_t log_m);
 size_t densify_scratch_words(size_t s, int C, size_t log_m);
-// d_idx: n x C u32 (device).  All C dimensions at once; outputs are this rank's shards (rank g of G: accesses k = i*G + g,
-// addresses a = i*G + g): dim_i at dim_loc + i*dim_stride, read_i at read_loc + i*read_stride, final_i likewise.
-int launch_densify(const uint32_t* d_idx, size_t n, size_t s, int C, size_t log_m, int G, int g, uint32_t* scratch,
-                   uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride, uint32_t* final_loc,
-                   size_t final_stride, cudaStream_t st);
+// The index matrix as the extract kernel reads it, on the device: entry (k, i) is p[k * row_stride + i * col_stride]
+// (strides in elements), an unsigned integer of elem_bytes = 4 or 8.
+struct DzIndices {
+  const void* p;
+  int elem_bytes;
+  size_t row_stride, col_stride;
+};
+// For entries nobody has range-checked: the extract kernel raises a flag when an entry is >= m (and uses address 0
+// instead); launch_densify copies the flag to h_bad (pinned) and records ev right after the extract, before it enqueues
+// the rest of the sort.  ev also marks the last read of the index matrix.
+struct DzRangeCheck {
+  unsigned* h_bad;
+  cudaEvent_t ev;
+};
+// All C dimensions at once; outputs are this rank's shards (rank g of G: accesses k = i*G + g, addresses a = i*G + g):
+// dim_i at dim_loc + i*dim_stride, read_i at read_loc + i*read_stride, final_i likewise.  check may be null.
+int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
+                   uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
+                   uint32_t* final_loc, size_t final_stride, cudaStream_t st);
 
 }  // namespace lb

@@ -236,6 +236,7 @@ Ctx* ctx_create(int device) {
   poly_init_device();
   LB_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_aux, cudaEventDisableTiming));
   LB_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_stage, cudaEventDisableTiming));
+  LB_CUDA_CHECK(cudaEventCreateWithFlags(&c->ev_caller, cudaEventDisableTiming));
   const char* sp = getenv("LASSO_B200_SPANS");
   c->span_sync = sp && sp[0] == '1';
   return c.release();
@@ -250,6 +251,7 @@ void ctx_destroy(Ctx* c) {
   cudaFree(c->d_flag);
   if (c->ev_aux) cudaEventDestroy(c->ev_aux);
   if (c->ev_stage) cudaEventDestroy(c->ev_stage);
+  if (c->ev_caller) cudaEventDestroy(c->ev_caller);
   if (c->h_stage) cudaFreeHost(c->h_stage);
   if (c->h_mapped) cudaFreeHost(c->h_mapped);
   if (c->h_pub && c->h_pub_owned) cudaFreeHost(c->h_pub);
@@ -531,14 +533,11 @@ static void multi_dot_src(PolySrc Z, size_t stride, int npolys, const fr_t* eq, 
 }
 
 // ---------------------------------------------------------------------------------------------- densify
-Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m, int* err) {
-  SpanTimer sp(c, "Densify");
-  *err = 0;
-  if (n == 0 || C == 0 || C > 16 || log_m < 1 || log_m > 28) {
-    *err = 4;
-    return nullptr;
-  }
-  const size_t G = (size_t)c->world, gr = (size_t)c->rank;
+// A Dense of the shape densify produces for (n, C, log_m) on this context, its arrays not yet allocated; nullptr for
+// the shapes densify rejects (n >= 1, 1 <= C <= 16, 1 <= log_m <= 28, and s, m >= 2G on a sharded context)
+static std::unique_ptr<Dense> dense_shape(Ctx* c, size_t n, size_t C, size_t log_m) {
+  if (n == 0 || C == 0 || C > 16 || log_m < 1 || log_m > 28) return nullptr;
+  const size_t G = (size_t)c->world;
   std::unique_ptr<Dense> d(new Dense());
   d->ctx = c;
   d->C = C;
@@ -547,14 +546,42 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
   d->m = (size_t)1 << log_m;
   d->nv_l = log2_exact_or_ceil(next_pow2(2 * C * d->s));
   d->nv_m = log2_exact_or_ceil(next_pow2(C)) + log_m;
-  const size_t s = d->s, m = d->m;
-  if (G > 1 && (s < 2 * G || m < 2 * G)) {
+  if (G > 1 && (d->s < 2 * G || d->m < 2 * G)) return nullptr;
+  d->s_loc = d->s / G;
+  d->m_loc = d->m / G;
+  return d;
+}
+// The part both entry points share once the index matrix is on the device: d's arrays and their zero padding, the
+// stable radix sort (densify_kernels.cu; when one proof is sharded every rank sorts the whole sequence and stores
+// only its shard) and DensePolynomial::from_usize + merge.  All of it stream-ordered on c->st, nothing waited for.
+static void densify_on_device(Ctx* c, Dense* d, size_t n, const DzIndices& idx, const DzRangeCheck* check) {
+  const size_t G = (size_t)c->world, gr = (size_t)c->rank;
+  const size_t C = d->C, s = d->s, s_loc = d->s_loc, m_loc = d->m_loc;
+  const size_t nl = ((size_t)1 << d->nv_l) / G, nm = ((size_t)1 << d->nv_m) / G;  // local lengths
+  d->d_l_u32.alloc(c, nl);
+  d->d_m_u32.alloc(c, nm);
+  d->d_l_fr.alloc(c, nl);
+  d->d_m_fr.alloc(c, nm);
+  DBuf<uint32_t> scratch(c, densify_scratch_words(s, (int)C, d->log_m));
+  if (nl > 2 * C * s_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_l_u32.p + 2 * C * s_loc, 0, (nl - 2 * C * s_loc) * 4, c->st));
+  if (nm > C * m_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_m_u32.p + C * m_loc, 0, (nm - C * m_loc) * 4, c->st));
+  g_launches += launch_densify(idx, check, n, s, (int)C, d->log_m, (int)G, (int)gr, scratch.p, d->d_l_u32.p, s_loc,
+                               d->d_l_u32.p + C * s_loc, s_loc, d->d_m_u32.p, m_loc, c->st);
+  launch_from_u32(d->d_l_u32.p, d->d_l_fr.p, nl, c->st);  // DensePolynomial::from_usize + merge
+  launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
+  g_launches += 2;
+}
+
+Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m, int* err) {
+  SpanTimer sp(c, "Densify");
+  *err = 0;
+  std::unique_ptr<Dense> d = dense_shape(c, n, C, log_m);
+  if (!d) {
     *err = 4;
     return nullptr;
   }
-  d->s_loc = s / G;
-  d->m_loc = m / G;
-  const size_t s_loc = d->s_loc, m_loc = d->m_loc;
+  const size_t G = (size_t)c->world, gr = (size_t)c->rank;
+  const size_t s = d->s, m = d->m, s_loc = d->s_loc, m_loc = d->m_loc;
   const size_t nl = ((size_t)1 << d->nv_l) / G, nm = ((size_t)1 << d->nv_m) / G;  // local lengths
   {
     const char* hd = getenv("LASSO_B200_HOST_DENSIFY");
@@ -564,12 +591,7 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
     // launches cost more than the scan).
     const bool want_gpu = (gd && gd[0] == '1') || s >= ((size_t)1 << 15) || G > 1;
     if (densify_gpu_supported(s, log_m) && want_gpu && !(hd && hd[0] == '1')) {
-      // upload the raw index matrix, derive dim / read / final on the device.  When one proof is sharded every rank
-      // does this for the whole sequence and stores only its shard.
-      d->d_l_u32.alloc(c, nl);
-      d->d_m_u32.alloc(c, nm);
-      d->d_l_fr.alloc(c, nl);
-      d->d_m_fr.alloc(c, nm);
+      // upload the raw index matrix, derive dim / read / final on the device (densify_on_device).
       // narrow usize -> u32 (and range-check, densified.rs:46) while staging into pinned memory: half the PCIe
       // bytes and a full-rate copy.  Pipelined: the matrix is cut into pieces, a few host threads narrow them
       // round-robin, and the upload of a piece starts as soon as it is staged (the copy of the early pieces overlaps
@@ -587,7 +609,6 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
       const uint64_t* src = indices + row0 * C;
       uint32_t* stage = c->stage(std::max<size_t>(total, 1));
       DBuf<uint32_t> d_idx(c, G * rows_per * C), d_mine(c, G > 1 ? rows_per * C : 0);
-      DBuf<uint32_t> scratch(c, densify_scratch_words(s, (int)C, log_m));
       uint32_t* d_dst = G > 1 ? d_mine.p : d_idx.p;
       {
         const size_t npieces = total >= (1u << 20) ? 64 : 1, nthreads = npieces > 1 ? (total >= (1u << 25) ? 16 : total >= (1u << 22) ? 8 : 4) : 1;
@@ -647,13 +668,8 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
         }
         if (G > 1) comm_allgather(c, d_mine.p, d_idx.p, rows_per * C * sizeof(uint32_t));
       }
-      if (nl > 2 * C * s_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_l_u32.p + 2 * C * s_loc, 0, (nl - 2 * C * s_loc) * 4, c->st));
-      if (nm > C * m_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_m_u32.p + C * m_loc, 0, (nm - C * m_loc) * 4, c->st));
-      g_launches += launch_densify(d_idx.p, n, s, (int)C, log_m, (int)G, (int)gr, scratch.p, d->d_l_u32.p, s_loc,
-                                   d->d_l_u32.p + C * s_loc, s_loc, d->d_m_u32.p, m_loc, c->st);
-      launch_from_u32(d->d_l_u32.p, d->d_l_fr.p, nl, c->st);  // DensePolynomial::from_usize + merge
-      launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
-      g_launches += 2;
+      // the staged entries are range-checked: the u32 matrix, row-major, needs no flag
+      densify_on_device(c, d.get(), n, DzIndices{d_idx.p, 4, C, 1}, nullptr);
       // no stream sync here: everything downstream is stream-ordered, and the staging buffer is guarded by ev_stage
       return d.release();
     }
@@ -723,6 +739,50 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
   launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
   g_launches += 2;
   c->sync();
+  return d.release();
+}
+
+static bool device_memory_of(const Ctx* c, const void* p) {
+  cudaPointerAttributes a;
+  if (cudaPointerGetAttributes(&a, p) != cudaSuccess) {
+    (void)cudaGetLastError();  // not a pointer CUDA knows: not an error of the context
+    return false;
+  }
+  return a.type == cudaMemoryTypeDevice && a.device == c->device;
+}
+// densify from an index matrix in device memory of the context's GPU (lasso_densify_device): no staging, the GPU sort
+// at every size, the range check in the extract kernel.  `caller`: the stream the matrix is ordered on.
+Dense* densify_device(Ctx* c, const void* indices, size_t elem_bytes, size_t n, size_t C, size_t row_stride,
+                      size_t col_stride, size_t log_m, cudaStream_t caller, int* err) {
+  SpanTimer sp(c, "Densify");
+  *err = 0;
+  std::unique_ptr<Dense> d = elem_bytes == 4 || elem_bytes == 8 ? dense_shape(c, n, C, log_m) : nullptr;
+  if (!d || !densify_gpu_supported(d->s, log_m)) {
+    *err = 4;
+    return nullptr;
+  }
+  // the first and the last entry must both lie in device memory of this GPU (host, pinned and other GPUs' memory fail)
+  size_t last = 0, a = 0, b = 0;
+  const bool wraps = __builtin_mul_overflow(n - 1, row_stride, &a) || __builtin_mul_overflow(C - 1, col_stride, &b) ||
+                     __builtin_add_overflow(a, b, &last) || __builtin_mul_overflow(last, elem_bytes, &last) ||
+                     (uintptr_t)indices > UINTPTR_MAX - last;
+  if (!indices || wraps || !device_memory_of(c, indices) || !device_memory_of(c, (const char*)indices + last)) {
+    *err = 7;
+    return nullptr;
+  }
+  // the matrix is read only after the work the caller enqueued on `caller` before this call
+  LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
+  LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
+  unsigned* h_bad = reinterpret_cast<unsigned*>(c->h_pin);
+  const DzRangeCheck check{h_bad, c->ev_aux};
+  densify_on_device(c, d.get(), n, DzIndices{indices, (int)elem_bytes, row_stride, col_stride}, &check);
+  // the caller's later work on `caller` (a caching allocator freeing the matrix, say) comes after the last read of it
+  LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
+  LB_CUDA_CHECK(cudaEventSynchronize(c->ev_aux));  // the verdict; the sort may still run
+  if (*h_bad) {
+    *err = 3;
+    return nullptr;
+  }
   return d.release();
 }
 

@@ -66,6 +66,7 @@ struct Ctx {
   uint32_t pub_seq = 0;
   static constexpr size_t kPubBytes = (size_t)kPubMaxReaders * kPubRegions * kPubElems * kPubSlotWords * 8;  // 1 MiB
   cudaEvent_t ev_aux = nullptr;  // marks a device->host copy that overlaps later launches on the same stream
+  cudaEvent_t ev_caller = nullptr;  // densify_device: the caller's stream up to the call (the index matrix is ready)
   cudaEvent_t ev_stage = nullptr;  // recorded after the last upload out of h_stage (the buffer is reused by the next densify)
   bool stage_busy = false;
   // host-thread placement (bind_host_threads): the CPUs the library's helper threads may use
@@ -275,6 +276,9 @@ Gens* gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t c
                   size_t log_m);
 size_t gens_points_needed(size_t c, size_t s, size_t num_memories, size_t log_m);
 Dense* densify(Ctx*, const uint64_t* indices, size_t n_lookups, size_t C, size_t log_m, int* err);
+// *err: 3 an entry >= m, 4 bad shape or elem_bytes, 7 the matrix is not device memory of the context's GPU
+Dense* densify_device(Ctx*, const void* indices, size_t elem_bytes, size_t n_lookups, size_t C, size_t row_stride,
+                      size_t col_stride, size_t log_m, cudaStream_t caller, int* err);
 std::vector<uint8_t> commit(Ctx*, const Dense&, const Gens&);
 std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr_t>& r, const Gens&,
                            const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,

@@ -8,7 +8,9 @@ With --custom every strategy is a caller-defined one (lasso_b200.CustomStrategy)
 programs plus tables that are not built in, checked against the oracle for caller-defined strategies (oracle_custom/).
 With --fr the strategies are caller-defined ones over tables of arbitrary field elements (tests/field_tables.py, the
 full-width commitment and openings), checked the same way.
-usage: torchrun --nproc-per-node N tools/sharded_check.py [--custom | --fr] [kind C log_m log_r lookups same]"""
+With --device every rank passes the whole index matrix as a torch CUDA tensor on its own GPU (lasso_densify_device;
+int64, and int32 for every other case) instead of a numpy array.
+usage: torchrun --nproc-per-node N tools/sharded_check.py [--custom | --fr] [--device] [kind C log_m log_r lookups same]"""
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -35,7 +37,8 @@ cases = [(2, 4, 16, 0, 1 << 12, 1), (3, 4, 4, 0, 128, 0), (0, 1, 16, 0, 1 << 10,
          (1, 2, 8, 0, 700, 0)]
 fr = "--fr" in sys.argv
 custom = "--custom" in sys.argv or fr
-argv = [a for a in sys.argv if a not in ("--custom", "--fr")]
+device = "--device" in sys.argv
+argv = [a for a in sys.argv if a not in ("--custom", "--fr", "--device")]
 if len(argv) > 6:
     cases = [tuple(int(x) for x in argv[1:7])]
 if fr:  # field-element tables: kind = -100 - their index in ft.INTS; C = 2, odd log_m, degree 2
@@ -44,8 +47,17 @@ elif custom:  # new tables: kind = -1 - their index in cb.NEW_TABLES
     cases += [(-1 - i, 0, 0, 0, 300 + i, 0) for i in range(len(cb.NEW_TABLES))]
 ctx = lb.Context(local)
 ctx.init_comm()
+
+
+def indices(idx, i=0):
+    """the matrix as from_lookup_indices gets it: numpy, or with --device a CUDA tensor (int32 for every other case)"""
+    if not device:
+        return idx
+    return torch.from_numpy(idx.astype(np.int32 if i % 2 else np.int64)).to(torch.device("cuda", local))
+
+
 ok = True
-for kind, C, log_m, log_r, n, same in cases:
+for i, (kind, C, log_m, log_r, n, same) in enumerate(cases):
     if kind <= -100:
         S = ft.strategy(ctx, sorted(ft.INTS)[-100 - kind], C, log_m, 2, nsub=2)
     elif kind < 0:
@@ -64,7 +76,7 @@ for kind, C, log_m, log_r, n, same in cases:
     stream = np.ascontiguousarray(ol.generators(max(need, 300))[:need])
     gens = lb.SparsePolyCommitmentGens.new(ctx, b"g", C, s, S.num_memories, log_m, stream=stream)
     t0 = time.time()
-    dense = lb.DensifiedRepresentation.from_lookup_indices(ctx, idx, log_m)
+    dense = lb.DensifiedRepresentation.from_lookup_indices(ctx, indices(idx, i), log_m)
     com = dense.commit(gens)
     proof = lb.SparsePolynomialEvaluationProof.prove(ctx, S, dense, r, gens, tape_seed=seed)
     dt = time.time() - t0
@@ -76,8 +88,8 @@ for kind, C, log_m, log_r, n, same in cases:
         good = ref["rc"] == 0 and com == ref["commitment"] and proof.bytes == ref["proof"]
         nch = min(len(proof.challenges), len(ref["challenges"]))
         first_bad = next((i for i in range(nch) if (proof.challenges[i] != ref["challenges"][i]).any()), None)
-        print("case %skind=%d C=%d log_m=%d n=%d world=%d: %s (%.1f ms, commit_ok=%s, first diverging challenge=%s)" % (
-            "custom " if custom else "", kind, C, log_m, n, world, "OK" if good else "MISMATCH", dt * 1e3, com == ref["commitment"], first_bad), flush=True)
+        print("case %s%skind=%d C=%d log_m=%d n=%d world=%d: %s (%.1f ms, commit_ok=%s, first diverging challenge=%s)" % (
+            "custom " if custom else "", "device " if device else "", kind, C, log_m, n, world, "OK" if good else "MISMATCH", dt * 1e3, com == ref["commitment"], first_bad), flush=True)
         ok = ok and good
 # an out-of-range index (densified.rs:46) in the LAST rank's block of rows: every rank must report it (the verdict is
 # agreed through the round-message path; nobody may be left waiting in the exchange that follows)
@@ -85,7 +97,7 @@ n_bad = 1 << 12
 bad = np.zeros((n_bad, 2), dtype=np.uint64)
 bad[n_bad - 3, 1] = 1 << 8
 try:
-    lb.DensifiedRepresentation.from_lookup_indices(ctx, bad, 8)
+    lb.DensifiedRepresentation.from_lookup_indices(ctx, indices(bad), 8)
     bad_ok = False
 except lb.LassoError as e:
     bad_ok = e.code == 3
