@@ -183,7 +183,10 @@ int lasso_commit(lasso_ctx*, const lasso_dense*, const lasso_gens*, uint8_t* out
  * r: log2(s) Fr elements.  transcript_label: Transcript::new(label) (b"example" in bench.rs:59);
  * tape_label / tape_seed: RandomTape::new(b"proof") seeded with an explicit scalar (the reference draws it
  * from ark_std::test_rng()).  proof_out receives the ark-serialize (compressed) bytes of the proof struct.
- * challenges_out (optional) receives every Fiat-Shamir challenge in order (4 limbs each). */
+ * challenges_out (optional) receives every Fiat-Shamir challenge in order (4 limbs each).
+ * LASSO_ERR_STRATEGY, before any launch, for the parameters lasso_sumcheck_round_arbitrary rejects and for LT with
+ * C > 8: its 2C memories make 4C grand-product circuits, above the 32 that one batched grand product holds.  The
+ * per-loop entry points above accept LT up to C = 16. */
 int lasso_prove(lasso_ctx*, int strategy, int log_R, lasso_dense*, const uint64_t* r, size_t r_len,
                 const lasso_gens*, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
                 uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,

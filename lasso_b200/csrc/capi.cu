@@ -675,6 +675,9 @@ int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uin
   LB_TRY_CTX(h)
   Strategy S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
   if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
+  if (!S.provable())
+    return fail(LASSO_ERR_STRATEGY, "prove: " + std::to_string(2 * S.num_memories()) +
+                                        " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)");
   return prove_checked(h, S, d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
                        challenges_out, challenges_cap, n_challenges);
   LB_CATCH

@@ -75,6 +75,9 @@ struct Strategy {
     if (kind == STRAT_RANGE && log_r < 0) return false;
     return true;
   }
+  // valid() and a proof the prover can run: every memory makes two grand-product circuits and one batched grand
+  // product holds 32 (CubicCoeffs, TreePtrs), so LT needs C <= 8; the round entry points take C up to 16
+  bool provable() const { return valid() && 2 * num_memories() <= 32; }
 };
 
 struct FrVec {  // small vector passed by value as a kernel parameter (challenge points, weights)
