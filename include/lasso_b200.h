@@ -42,7 +42,8 @@ enum {
   LASSO_ERR_STRATEGY = 4,    /* unknown / unsupported strategy parameters */
   LASSO_ERR_GENS = 5,        /* generator set too small for the polynomial  poly/commitments.rs:85 */
   LASSO_ERR_MULTISET = 6,    /* assert_eq!(hash_init*hash_write, hash_read*hash_final) memory_checking.rs:689 */
-  LASSO_ERR_POINTER = 7      /* a buffer that must be device memory of the context's GPU is not */
+  LASSO_ERR_POINTER = 7,     /* a buffer that must be device memory of the context's GPU is not */
+  LASSO_ERR_VALUE = 8        /* a field element that is not a canonical Montgomery residue (< l) */
 };
 
 const char* lasso_last_error(void);
@@ -238,6 +239,79 @@ int lasso_prove_custom(lasso_ctx*, const lasso_strategy*, lasso_dense*, const ui
                        const lasso_gens*, const char* transcript_label, const char* tape_label,
                        const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
                        uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges);
+
+/* ---------------------------------------------------------------- transcripts and dense polynomials
+ *
+ * For a caller that composes Lasso into a larger protocol: its own multilinear polynomials committed and opened on the
+ * GPU, bound by one Fiat-Shamir transcript the caller holds across calls.
+ *
+ * ProofTranscript (utils/transcript.rs:6-72) over merlin, and RandomTape (utils/random.rs:9-39).  Host objects: they
+ * need no context and no GPU.  Labels are NUL-terminated; scalars are 4 Montgomery limbs and must be canonical
+ * residues (LASSO_ERR_VALUE otherwise); points are 32-byte ark-serialize compressed encodings, absorbed as given.
+ * append_scalars / append_points frame the vector with the begin/end markers of the reference. */
+typedef struct lasso_transcript lasso_transcript;
+typedef struct lasso_random_tape lasso_random_tape;
+int lasso_transcript_create(const char* label, lasso_transcript** out); /* Transcript::new(label) */
+void lasso_transcript_destroy(lasso_transcript*);
+int lasso_transcript_append_message(lasso_transcript*, const char* label, const uint8_t* msg, size_t len);
+int lasso_transcript_append_u64(lasso_transcript*, const char* label, uint64_t x);
+int lasso_transcript_append_protocol_name(lasso_transcript*, const char* name);
+int lasso_transcript_append_scalar(lasso_transcript*, const char* label, const uint64_t s[4]);
+int lasso_transcript_append_scalars(lasso_transcript*, const char* label, const uint64_t* s, size_t n);
+int lasso_transcript_append_point(lasso_transcript*, const char* label, const uint8_t point[32]);
+int lasso_transcript_append_points(lasso_transcript*, const char* label, const uint8_t* points, size_t n);
+/* PolyCommitment::append_to_transcript (poly/dense_mlpoly.rs:281-289) of serialised commitment bytes (lasso_poly_commit's
+ * output: a u64 count, then 32 bytes per point); LASSO_ERR_LENGTH when len != 8 + 32 * count */
+int lasso_transcript_append_poly_commitment(lasso_transcript*, const char* label, const uint8_t* bytes, size_t len);
+int lasso_transcript_challenge_scalar(lasso_transcript*, const char* label, uint64_t out[4]);
+int lasso_transcript_challenge_vector(lasso_transcript*, const char* label, size_t n, uint64_t* out);
+/* RandomTape::new(label) seeded with an explicit scalar, as lasso_prove's tape is */
+int lasso_random_tape_create(const char* label, const uint64_t seed[4], lasso_random_tape** out);
+void lasso_random_tape_destroy(lasso_random_tape*);
+int lasso_random_tape_random_scalar(lasso_random_tape*, const char* label, uint64_t out[4]);
+int lasso_random_tape_random_vector(lasso_random_tape*, const char* label, size_t n, uint64_t* out);
+
+/* PolyCommitmentGens (poly/dense_mlpoly.rs:31-45) from an explicit generator stream: with R = 2^(num_vars - num_vars/2),
+ * G_0..G_{R-1} = stream[0..R), Q = stream[R], h = stream[R+1] (poly/commitments.rs:21-44, dot_product.rs:146-149).
+ * Its own type: it cannot be passed to lasso_commit or lasso_prove.  Builds the same device tables a lasso_gens of the
+ * same R builds (window table, digit-multiples tables; LASSO_B200_NO_MULTIPLES and LASSO_B200_TABLE_GB apply): about
+ * 14 GB of HBM at R = 2^12.  LASSO_ERR_GENS when n_points < R + 2, LASSO_ERR_LENGTH when num_vars > 28. */
+typedef struct lasso_poly_gens lasso_poly_gens;
+typedef struct lasso_poly lasso_poly;
+size_t lasso_poly_gens_points_needed(size_t num_vars); /* R + 2 */
+int lasso_poly_gens_create(lasso_ctx*, const uint64_t* stream_affine, size_t n_points, size_t num_vars,
+                           lasso_poly_gens** out);
+void lasso_poly_gens_destroy(lasso_poly_gens*);
+/* DensePolynomial::new (poly/dense_mlpoly.rs:62-71): a device-resident copy of `len` evaluations, 4 Montgomery limbs
+ * each.  len must be a power of two (LASSO_ERR_NOT_POW2, 0 included) and at most 2^28 (LASSO_ERR_LENGTH).  Every
+ * evaluation must be a canonical residue: otherwise LASSO_ERR_VALUE, found by the ingest pass on the device (the one
+ * error reported after a launch; no polynomial is made and the context stays usable).  A polynomial whose values are
+ * all integers below 2^32 is committed and opened through the 16-bit digit tables, a wider one with ceil((w + 2) / 8)
+ * signed 8-bit windows, w the bit width of its widest value; both give the same bytes.
+ * lasso_poly_create reads host memory (len x 4 u64, contiguous).  lasso_poly_create_device reads DEVICE memory of the
+ * context's GPU: row i at Z + i * row_stride (row_stride in u64, >= 4, else LASSO_ERR_LENGTH), limbs contiguous.  The
+ * first and the last row must be device memory of the context's device, otherwise LASSO_ERR_POINTER before any launch;
+ * the rows are read after the work enqueued on `stream` (NULL = the legacy default stream) before the call, and later
+ * work on `stream` is ordered after those reads.  The library keeps its own copy: the caller may free Z on return.
+ * Not available on a sharded context (LASSO_ERR_STRATEGY). */
+int lasso_poly_create(lasso_ctx*, const uint64_t* Z, size_t len, lasso_poly** out);
+int lasso_poly_create_device(lasso_ctx*, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
+                             lasso_poly** out);
+size_t lasso_poly_num_vars(const lasso_poly*);
+void lasso_poly_destroy(lasso_poly*);
+/* DensePolynomial::commit (poly/dense_mlpoly.rs:152-181) without blinds -> PolyCommitment { C: Vec<G> } serialised
+ * with ark-serialize (compressed): a u64 count L = 2^(num_vars/2), then 32 bytes per row.  *out_len receives the size
+ * (also when cap is too small: LASSO_ERR_LENGTH).  LASSO_ERR_GENS when the generators' R differs from the
+ * polynomial's (poly/commitments.rs:85). */
+int lasso_poly_commit(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, uint8_t* out, size_t cap, size_t* out_len);
+/* DensePolynomial::evaluate (poly/dense_mlpoly.rs:229-235): Z(r), r_len == num_vars (LASSO_ERR_LENGTH otherwise) */
+int lasso_poly_evaluate(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t r_len, uint64_t out[4]);
+/* PolyEvalProof::prove (poly/dense_mlpoly.rs:301-359) without blinds: proof_out receives the ark-serialize (compressed)
+ * PolyEvalProof, C_Zr_out (may be null) the compressed C_Zr_prime returned alongside it.  The transcript and the tape
+ * are advanced in place, so later calls continue them.  Errors as lasso_poly_commit and lasso_poly_evaluate. */
+int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, const uint64_t* r, size_t r_len,
+                          const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* random_tape,
+                          uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]);
 
 /* Host-resident benchmark helper: number of kernels launched by this context so far, and the wall time
  * (ms) of the last densify / commit / prove calls. */

@@ -18,6 +18,22 @@ pub struct lasso_dense {
 pub struct lasso_msm_job {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct lasso_transcript {
+    _p: [u8; 0],
+}
+#[repr(C)]
+pub struct lasso_random_tape {
+    _p: [u8; 0],
+}
+#[repr(C)]
+pub struct lasso_poly_gens {
+    _p: [u8; 0],
+}
+#[repr(C)]
+pub struct lasso_poly {
+    _p: [u8; 0],
+}
 
 extern "C" {
     pub fn lasso_last_error() -> *const c_char;
@@ -70,6 +86,40 @@ extern "C" {
                        g: *const lasso_gens, transcript_label: *const c_char, tape_label: *const c_char, tape_seed: *const u64,
                        proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize, challenges_out: *mut u64,
                        challenges_cap: usize, n_challenges: *mut usize) -> c_int;
+    // a caller's transcript and dense polynomials (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_transcript_create(label: *const c_char, out: *mut *mut lasso_transcript) -> c_int;
+    pub fn lasso_transcript_destroy(t: *mut lasso_transcript);
+    pub fn lasso_transcript_append_message(t: *mut lasso_transcript, label: *const c_char, msg: *const u8, len: usize) -> c_int;
+    pub fn lasso_transcript_append_u64(t: *mut lasso_transcript, label: *const c_char, x: u64) -> c_int;
+    pub fn lasso_transcript_append_protocol_name(t: *mut lasso_transcript, name: *const c_char) -> c_int;
+    pub fn lasso_transcript_append_scalar(t: *mut lasso_transcript, label: *const c_char, s: *const u64) -> c_int;
+    pub fn lasso_transcript_append_scalars(t: *mut lasso_transcript, label: *const c_char, s: *const u64, n: usize) -> c_int;
+    pub fn lasso_transcript_append_point(t: *mut lasso_transcript, label: *const c_char, point: *const u8) -> c_int;
+    pub fn lasso_transcript_append_points(t: *mut lasso_transcript, label: *const c_char, points: *const u8, n: usize) -> c_int;
+    pub fn lasso_transcript_append_poly_commitment(t: *mut lasso_transcript, label: *const c_char, bytes: *const u8,
+                                                   len: usize) -> c_int;
+    pub fn lasso_transcript_challenge_scalar(t: *mut lasso_transcript, label: *const c_char, out: *mut u64) -> c_int;
+    pub fn lasso_transcript_challenge_vector(t: *mut lasso_transcript, label: *const c_char, n: usize, out: *mut u64) -> c_int;
+    pub fn lasso_random_tape_create(label: *const c_char, seed: *const u64, out: *mut *mut lasso_random_tape) -> c_int;
+    pub fn lasso_random_tape_destroy(t: *mut lasso_random_tape);
+    pub fn lasso_random_tape_random_scalar(t: *mut lasso_random_tape, label: *const c_char, out: *mut u64) -> c_int;
+    pub fn lasso_random_tape_random_vector(t: *mut lasso_random_tape, label: *const c_char, n: usize, out: *mut u64) -> c_int;
+    pub fn lasso_poly_gens_points_needed(num_vars: usize) -> usize;
+    pub fn lasso_poly_gens_create(ctx: *mut lasso_ctx, stream: *const u64, n_points: usize, num_vars: usize,
+                                  out: *mut *mut lasso_poly_gens) -> c_int;
+    pub fn lasso_poly_gens_destroy(g: *mut lasso_poly_gens);
+    pub fn lasso_poly_create(ctx: *mut lasso_ctx, z: *const u64, len: usize, out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_create_device(ctx: *mut lasso_ctx, z: *const u64, len: usize, row_stride: usize, stream: *mut c_void,
+                                    out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_num_vars(p: *const lasso_poly) -> usize;
+    pub fn lasso_poly_destroy(p: *mut lasso_poly);
+    pub fn lasso_poly_commit(ctx: *mut lasso_ctx, p: *const lasso_poly, g: *const lasso_poly_gens, out: *mut u8, cap: usize,
+                             out_len: *mut usize) -> c_int;
+    pub fn lasso_poly_evaluate(ctx: *mut lasso_ctx, p: *const lasso_poly, r: *const u64, r_len: usize, out: *mut u64) -> c_int;
+    pub fn lasso_poly_eval_prove(ctx: *mut lasso_ctx, p: *const lasso_poly, g: *const lasso_poly_gens, r: *const u64,
+                                 r_len: usize, zr: *const u64, transcript: *mut lasso_transcript,
+                                 random_tape: *mut lasso_random_tape, proof_out: *mut u8, proof_cap: usize,
+                                 proof_len: *mut usize, c_zr_out: *mut u8) -> c_int;
     pub fn lasso_launch_count(ctx: *const lasso_ctx) -> u64;
     pub fn lasso_last_timings(ctx: *const lasso_ctx, out_ms: *mut f64);
 }

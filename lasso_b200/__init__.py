@@ -7,13 +7,21 @@ Host-side mirror of the reference's surface for that path (names follow the Rust
     SparsePolyCommitmentGens.new(ctx, label, c, s, num_memories, log_m)  src/lasso/surge.rs:32
     SparsePolynomialEvaluationProof.prove(ctx, strategy, dense, r, gens, ...)   src/lasso/surge.rs:119
 
+and, for a caller that composes Lasso into a larger protocol, its own dense polynomials on its own transcript:
+
+    Transcript(label), RandomTape(label, seed)                           src/utils/{transcript,random}.rs
+    PolyCommitmentGens.new(ctx, label, num_vars)                         src/poly/dense_mlpoly.rs:38
+    DensePolynomial(ctx, Z).commit(gens) / .evaluate(r)                  src/poly/dense_mlpoly.rs:152, 229
+    PolyEvalProof.prove(ctx, poly, r, Zr, gens, transcript, random_tape)    src/poly/dense_mlpoly.rs:301
+
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    Context, CustomStrategy, DensifiedRepresentation, LassoError, MsmJob, SparsePolyCommitmentGens,
-    SparsePolynomialEvaluationProof, Strategy, bind_bot, bind_top, commit_rows, eq_evals, fr_from_ints, gather_lookup_polys,
-    gens_points_needed, lib, library_path, materialize_subtables, msm, sample_generators, sumcheck_bind_round_arbitrary,
+    Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
+    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Transcript, bind_bot, bind_top,
+    commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,
+    msm, poly_gens_points_needed, sample_generators, sumcheck_bind_round_arbitrary,
     sumcheck_round_arbitrary, sumcheck_round_cubic, sumcheck_round_custom, trace_combine_lookups,
 )

@@ -41,6 +41,10 @@ def lib():
         L.lasso_dense_read.restype = C.c_size_t
         L.lasso_launch_count.restype = C.c_ulonglong
         L.lasso_spans.restype = C.c_size_t
+        L.lasso_poly_gens_points_needed.restype = C.c_size_t
+        L.lasso_poly_gens_points_needed.argtypes = [C.c_size_t]
+        L.lasso_poly_num_vars.restype = C.c_size_t
+        L.lasso_transcript_append_u64.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
         _lib = L
     return _lib
 
@@ -89,6 +93,7 @@ class Strategy:
 
 # ------------------------------------------------------------------ caller-defined strategies
 OP_ADD, OP_SUB, OP_MUL, OP_MULK, OP_ADDK = 0, 1, 2, 3, 4
+LASSO_ERR_LENGTH, LASSO_ERR_NOT_POW2, LASSO_ERR_GENS, LASSO_ERR_VALUE = 1, 2, 5, 8
 LASSO_ERR_INDEX_RANGE, LASSO_ERR_STRATEGY, LASSO_ERR_POINTER = 3, 4, 7
 FR_MODULUS = 2**252 + 27742317777372353535851937790883648493
 MAX_MEMORIES, MAX_OPS, MAX_CONSTANTS, MAX_DEGREE = 16, 128, 64, 16
@@ -608,3 +613,228 @@ class SparsePolynomialEvaluationProof:
         else:
             _chk(lib().lasso_prove(ctx._h, strategy.kind, strategy.log_r, *tail))
         return cls(bytes(out[: n.value]), chal[: nch.value].copy())
+
+
+# ------------------------------------------------------------------ dense polynomials on a caller's transcript
+def _label(label):
+    """a transcript label: bytes (or str) without a NUL byte"""
+    if isinstance(label, str):
+        label = label.encode()
+    if not isinstance(label, (bytes, bytearray)) or b"\0" in label:
+        raise LassoError(LASSO_ERR_LENGTH, "a label is bytes without a NUL byte, not %r" % (label,))
+    return bytes(label)
+
+
+def _limbs(a, n=None, what="scalars"):
+    """Fr elements as (k, 4) uint64 Montgomery limbs (k = n when given)"""
+    a = np.asarray(a)
+    if a.dtype != np.uint64 or a.ndim == 0 or a.shape[-1] != 4:
+        raise LassoError(LASSO_ERR_LENGTH, "%s are uint64 Montgomery limbs of shape (..., 4)" % what)
+    a = np.ascontiguousarray(a).reshape(-1, 4)
+    if n is not None and a.shape[0] != n:
+        raise LassoError(LASSO_ERR_LENGTH, "%s: %d elements, expected %d" % (what, a.shape[0], n))
+    return a
+
+
+def _compressed(points):
+    """32-byte compressed points: one bytes object of 32 k bytes, or a sequence of 32-byte objects"""
+    b = bytes(points) if isinstance(points, (bytes, bytearray, memoryview)) else b"".join(bytes(p) for p in points)
+    if len(b) % 32:
+        raise LassoError(LASSO_ERR_LENGTH, "compressed points are 32 bytes each, got %d bytes" % len(b))
+    return b
+
+
+class Transcript:
+    """merlin Transcript with the reference's ProofTranscript methods (src/utils/transcript.rs:6-72).  A host object: no
+    context or GPU needed.  Scalars are (4,) uint64 Montgomery limbs, points 32-byte compressed encodings."""
+
+    def __init__(self, label):
+        h = C.c_void_p()
+        _chk(lib().lasso_transcript_create(_label(label), C.byref(h)))
+        self._h = h
+
+    def append_message(self, label, msg):
+        msg = bytes(msg)
+        _chk(lib().lasso_transcript_append_message(self._h, _label(label), msg, C.c_size_t(len(msg))))
+
+    def append_u64(self, label, x):
+        _chk(lib().lasso_transcript_append_u64(self._h, _label(label), int(x)))
+
+    def append_protocol_name(self, name):
+        _chk(lib().lasso_transcript_append_protocol_name(self._h, _label(name)))
+
+    def append_scalar(self, label, s):
+        _chk(lib().lasso_transcript_append_scalar(self._h, _label(label), _p(_limbs(s, 1, "a scalar"))))
+
+    def append_scalars(self, label, scalars):
+        s = _limbs(scalars)
+        _chk(lib().lasso_transcript_append_scalars(self._h, _label(label), _p(s), C.c_size_t(s.shape[0])))
+
+    def append_point(self, label, point):
+        b = _compressed(point)
+        if len(b) != 32:
+            raise LassoError(LASSO_ERR_LENGTH, "a point is 32 bytes")
+        _chk(lib().lasso_transcript_append_point(self._h, _label(label), b))
+
+    def append_points(self, label, points):
+        b = _compressed(points)
+        _chk(lib().lasso_transcript_append_points(self._h, _label(label), b, C.c_size_t(len(b) // 32)))
+
+    def append_poly_commitment(self, label, commitment):
+        """PolyCommitment::append_to_transcript (src/poly/dense_mlpoly.rs:281-289) of DensePolynomial.commit's bytes"""
+        b = bytes(commitment)
+        _chk(lib().lasso_transcript_append_poly_commitment(self._h, _label(label), b, C.c_size_t(len(b))))
+
+    def challenge_scalar(self, label):
+        out = np.zeros(4, dtype=np.uint64)
+        _chk(lib().lasso_transcript_challenge_scalar(self._h, _label(label), _p(out)))
+        return out
+
+    def challenge_vector(self, label, n):
+        out = np.zeros((int(n), 4), dtype=np.uint64)
+        _chk(lib().lasso_transcript_challenge_vector(self._h, _label(label), C.c_size_t(int(n)), _p(out)))
+        return out
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lasso_transcript_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class RandomTape:
+    """RandomTape::new(label) (src/utils/random.rs:15-30) seeded with an explicit scalar instead of test_rng()."""
+
+    def __init__(self, label, seed):
+        h = C.c_void_p()
+        _chk(lib().lasso_random_tape_create(_label(label), _p(_limbs(seed, 1, "the seed")), C.byref(h)))
+        self._h = h
+
+    def random_scalar(self, label):
+        out = np.zeros(4, dtype=np.uint64)
+        _chk(lib().lasso_random_tape_random_scalar(self._h, _label(label), _p(out)))
+        return out
+
+    def random_vector(self, label, n):
+        out = np.zeros((int(n), 4), dtype=np.uint64)
+        _chk(lib().lasso_random_tape_random_vector(self._h, _label(label), C.c_size_t(int(n)), _p(out)))
+        return out
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lasso_random_tape_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+def poly_gens_points_needed(num_vars):
+    """R + 2 generators, R = 2^(num_vars - num_vars // 2)"""
+    return int(lib().lasso_poly_gens_points_needed(C.c_size_t(int(num_vars))))
+
+
+class PolyCommitmentGens:
+    """src/poly/dense_mlpoly.rs:31-45: G_0..G_{R-1}, Q, h from one generator stream"""
+
+    def __init__(self, ctx, handle, stream, num_vars):
+        self.ctx, self._h, self.stream, self.num_vars = ctx, handle, stream, num_vars
+
+    @classmethod
+    def new(cls, ctx, label, num_vars, stream=None):
+        if stream is None:
+            stream = sample_generators(_label(label), poly_gens_points_needed(num_vars))
+        stream = _fr(stream, 8)
+        h = C.c_void_p()
+        _chk(lib().lasso_poly_gens_create(ctx._h, _p(stream), C.c_size_t(stream.shape[0]), C.c_size_t(int(num_vars)),
+                                          C.byref(h)))
+        return cls(ctx, h, stream, int(num_vars))
+
+    def __del__(self):
+        try:
+            if self._h and self.ctx._h:
+                lib().lasso_poly_gens_destroy(self._h)
+        except Exception:
+            pass
+
+
+def _poly_source(Z):
+    """-> ("host", contiguous (n, 4) uint64 array) or ("device", tensor, row stride); raises on anything else"""
+    torch = sys.modules.get("torch")  # a CUDA tensor exists only if torch is loaded already
+    if torch is not None and isinstance(Z, torch.Tensor) and Z.is_cuda:
+        if Z.dtype not in (torch.int64, getattr(torch, "uint64", torch.int64)):
+            raise LassoError(LASSO_ERR_LENGTH, "a CUDA polynomial is int64 or uint64 limbs, not %s" % Z.dtype)
+        if Z.ndim != 2 or Z.shape[1] != 4:
+            raise LassoError(LASSO_ERR_LENGTH, "a CUDA polynomial is an (n, 4) tensor of limbs, not %s" % (tuple(Z.shape),))
+        if Z.stride(1) != 1:
+            raise LassoError(LASSO_ERR_LENGTH, "the 4 limbs of an evaluation must be contiguous (stride 1)")
+        return "device", Z, (Z.stride(0) if Z.shape[0] > 1 else 4)
+    a = np.asarray(Z)
+    if a.dtype == np.int64:
+        a = a.view(np.uint64)
+    if a.dtype != np.uint64 or a.ndim != 2 or a.shape[1] != 4:
+        raise LassoError(LASSO_ERR_LENGTH, "a polynomial is an (n, 4) uint64 array of Montgomery limbs")
+    return "host", np.ascontiguousarray(a), 4
+
+
+class DensePolynomial:
+    """DensePolynomial<Fr> (src/poly/dense_mlpoly.rs:13-235), resident on ctx's GPU.  Z: the 2^num_vars evaluations as
+    an (n, 4) uint64 numpy array of Montgomery limbs, or a torch CUDA tensor (int64 or uint64, limbs contiguous, any row
+    stride) read in the order of torch's current stream.  The library keeps its own copy."""
+
+    def __init__(self, ctx, Z):
+        kind, src, row_stride = _poly_source(Z)
+        h = C.c_void_p()
+        if kind == "device":
+            torch = sys.modules["torch"]
+            stream = torch.cuda.current_stream(src.device).cuda_stream
+            _chk(lib().lasso_poly_create_device(ctx._h, C.c_void_p(src.data_ptr()), C.c_size_t(src.shape[0]),
+                                                C.c_size_t(row_stride), C.c_void_p(stream), C.byref(h)))
+        else:
+            _chk(lib().lasso_poly_create(ctx._h, _p(src), C.c_size_t(src.shape[0]), C.byref(h)))
+        self.ctx, self._h = ctx, h
+        self.num_vars = int(lib().lasso_poly_num_vars(h))
+
+    def commit(self, gens):
+        """DensePolynomial::commit without blinds -> the ark-serialize bytes of PolyCommitment"""
+        cap = 8 + 32 * (1 << (self.num_vars // 2))
+        out = np.zeros(cap, dtype=np.uint8)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_poly_commit(self.ctx._h, self._h, gens._h, _p(out), C.c_size_t(cap), C.byref(n)))
+        return bytes(out[: n.value])
+
+    def evaluate(self, r):
+        r = _limbs(r, what="r")
+        out = np.zeros(4, dtype=np.uint64)
+        _chk(lib().lasso_poly_evaluate(self.ctx._h, self._h, _p(r), C.c_size_t(r.shape[0]), _p(out)))
+        return out
+
+    def __del__(self):
+        try:
+            if self._h and self.ctx._h:
+                lib().lasso_poly_destroy(self._h)
+        except Exception:
+            pass
+
+
+class PolyEvalProof:
+    """src/poly/dense_mlpoly.rs:291-359.  `.bytes` is the ark-serialize (compressed) PolyEvalProof, `.C_Zr` the 32-byte
+    compressed C_Zr_prime that PolyEvalProof::prove returns alongside it."""
+
+    def __init__(self, data, C_Zr):
+        self.bytes, self.C_Zr = data, C_Zr
+
+    @classmethod
+    def prove(cls, ctx, poly, r, Zr, gens, transcript, random_tape):
+        """advances transcript and random_tape in place"""
+        r = _limbs(r, what="r")
+        Zr = _limbs(Zr, 1, "Zr")
+        cap = 2 * (8 + 32 * 32) + 4 * 32
+        out = np.zeros(cap, dtype=np.uint8)
+        czr = np.zeros(32, dtype=np.uint8)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_poly_eval_prove(ctx._h, poly._h, gens._h, _p(r), C.c_size_t(r.shape[0]), _p(Zr), transcript._h,
+                                         random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
+        return cls(bytes(out[: n.value]), czr.tobytes())

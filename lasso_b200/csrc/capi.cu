@@ -29,6 +29,22 @@ struct lasso_strategy {
   }
 };
 
+// host objects: a caller's Fiat-Shamir transcript and random tape, continued across calls
+struct lasso_transcript {
+  Transcript t;
+};
+struct lasso_random_tape {
+  RandomTape t;
+};
+// PolyCommitmentGens: a generator set of one R = 2^(num_vars - num_vars/2)
+struct lasso_poly_gens {
+  Gens* g;
+  size_t num_vars;
+};
+struct lasso_poly {
+  Poly* p;
+};
+
 struct lasso_msm_job {
   Ctx* c = nullptr;
   size_t n = 0, n_pool = 0;
@@ -812,6 +828,255 @@ int lasso_prove_custom(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, co
     return fail(LASSO_ERR_STRATEGY, "strategy (C, log_m) differ from the densified representation");
   return prove_checked(h, s->S(), d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
                        challenges_out, challenges_cap, n_challenges);
+  LB_CATCH
+}
+
+// ---- transcripts and random tapes (host only: no context, no device)
+#define LB_TRY_T(t) \
+  try {             \
+    if (!(t)) return fail(LASSO_ERR_LENGTH, "null transcript");
+int lasso_transcript_create(const char* label, lasso_transcript** out) {
+  LB_TRY
+  if (!out || !label) return fail(LASSO_ERR_LENGTH, "transcript: null label or output");
+  *out = new lasso_transcript{Transcript(label)};
+  return 0;
+  LB_CATCH
+}
+void lasso_transcript_destroy(lasso_transcript* t) { delete t; }
+int lasso_transcript_append_message(lasso_transcript* t, const char* label, const uint8_t* msg, size_t len) {
+  LB_TRY_T(t)
+  if (len && !msg) return fail(LASSO_ERR_LENGTH, "transcript: null message");
+  t->t.append_message(label, msg, len);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_u64(lasso_transcript* t, const char* label, uint64_t x) {
+  LB_TRY_T(t)
+  t->t.append_u64(label, x);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_protocol_name(lasso_transcript* t, const char* name) {
+  LB_TRY_T(t)
+  t->t.append_protocol_name(name);
+  return 0;
+  LB_CATCH
+}
+// the scalars of the caller are Montgomery limbs; a non-canonical one would serialise to another residue's bytes
+static bool load_scalars(const uint64_t* s, size_t n, std::vector<fr_t>& out) {
+  out.resize(n);
+  for (size_t i = 0; i < n; i++) {
+    memcpy(out[i].v, s + 4 * i, 32);
+    if (!fr_eq(fr_reduce_once(out[i].v), out[i])) return false;
+  }
+  return true;
+}
+int lasso_transcript_append_scalar(lasso_transcript* t, const char* label, const uint64_t s[4]) {
+  LB_TRY_T(t)
+  std::vector<fr_t> v;
+  if (!load_scalars(s, 1, v)) return fail(LASSO_ERR_VALUE, "transcript: the scalar is not a canonical residue");
+  t->t.append_scalar(label, v[0]);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_scalars(lasso_transcript* t, const char* label, const uint64_t* s, size_t n) {
+  LB_TRY_T(t)
+  std::vector<fr_t> v;
+  if (n && !s) return fail(LASSO_ERR_LENGTH, "transcript: null scalars");
+  if (!load_scalars(s, n, v)) return fail(LASSO_ERR_VALUE, "transcript: a scalar is not a canonical residue");
+  t->t.append_scalars(label, v.data(), n);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_point(lasso_transcript* t, const char* label, const uint8_t point[32]) {
+  LB_TRY_T(t)
+  t->t.append_point_compressed(label, point);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_points(lasso_transcript* t, const char* label, const uint8_t* points, size_t n) {
+  LB_TRY_T(t)
+  if (n && !points) return fail(LASSO_ERR_LENGTH, "transcript: null points");
+  t->t.append_message(label, std::string("begin_append_vector"));
+  for (size_t i = 0; i < n; i++) t->t.append_point_compressed(label, points + 32 * i);
+  t->t.append_message(label, std::string("end_append_vector"));
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_poly_commitment(lasso_transcript* t, const char* label, const uint8_t* bytes, size_t len) {
+  LB_TRY_T(t)
+  uint64_t n = 0;
+  if (!bytes || len < 8) return fail(LASSO_ERR_LENGTH, "poly commitment: shorter than its count");
+  memcpy(&n, bytes, 8);
+  if (n > (len - 8) / 32 || len != 8 + 32 * n) return fail(LASSO_ERR_LENGTH, "poly commitment: length != 8 + 32 * count");
+  t->t.append_message(label, std::string("poly_commitment_begin"));
+  for (uint64_t i = 0; i < n; i++) t->t.append_point_compressed("poly_commitment_share", bytes + 8 + 32 * i);
+  t->t.append_message(label, std::string("poly_commitment_end"));
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_challenge_scalar(lasso_transcript* t, const char* label, uint64_t out[4]) {
+  LB_TRY_T(t)
+  const fr_t c = t->t.challenge_scalar(label);
+  memcpy(out, c.v, 32);
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_challenge_vector(lasso_transcript* t, const char* label, size_t n, uint64_t* out) {
+  LB_TRY_T(t)
+  if (n && !out) return fail(LASSO_ERR_LENGTH, "transcript: null output");
+  for (size_t i = 0; i < n; i++) {
+    const fr_t c = t->t.challenge_scalar(label);
+    memcpy(out + 4 * i, c.v, 32);
+  }
+  return 0;
+  LB_CATCH
+}
+int lasso_random_tape_create(const char* label, const uint64_t seed[4], lasso_random_tape** out) {
+  LB_TRY
+  if (!out || !label || !seed) return fail(LASSO_ERR_LENGTH, "random tape: null label, seed or output");
+  std::vector<fr_t> s;
+  if (!load_scalars(seed, 1, s)) return fail(LASSO_ERR_VALUE, "random tape: the seed is not a canonical residue");
+  *out = new lasso_random_tape{RandomTape(label, s[0])};
+  return 0;
+  LB_CATCH
+}
+void lasso_random_tape_destroy(lasso_random_tape* t) { delete t; }
+int lasso_random_tape_random_scalar(lasso_random_tape* t, const char* label, uint64_t out[4]) {
+  return lasso_random_tape_random_vector(t, label, 1, out);
+}
+int lasso_random_tape_random_vector(lasso_random_tape* t, const char* label, size_t n, uint64_t* out) {
+  LB_TRY_T(t)
+  if (n && !out) return fail(LASSO_ERR_LENGTH, "random tape: null output");
+  const std::vector<fr_t> v = t->t.random_vector(label, n);
+  for (size_t i = 0; i < n; i++) memcpy(out + 4 * i, v[i].v, 32);
+  return 0;
+  LB_CATCH
+}
+
+// ---- dense polynomials of the caller
+static int poly_ctx_check(lasso_ctx* h) {
+  if (h->c->world > 1) return fail(LASSO_ERR_STRATEGY, "dense polynomials are not available on a sharded context");
+  return 0;
+}
+size_t lasso_poly_gens_points_needed(size_t num_vars) { return poly_R(num_vars) + 2; }
+int lasso_poly_gens_create(lasso_ctx* h, const uint64_t* stream_affine, size_t n_points, size_t num_vars,
+                           lasso_poly_gens** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!out || !stream_affine) return fail(LASSO_ERR_GENS, "poly gens: null stream or output");
+  if (num_vars > 28) return fail(LASSO_ERR_LENGTH, "poly gens: num_vars <= 28");
+  if (n_points < poly_R(num_vars) + 2) return fail(LASSO_ERR_GENS, "poly gens: stream shorter than lasso_poly_gens_points_needed()");
+  Gens* g = poly_gens_create(h->c, stream_affine, n_points, num_vars);
+  *out = new lasso_poly_gens{g, num_vars};
+  return 0;
+  LB_CATCH
+}
+void lasso_poly_gens_destroy(lasso_poly_gens* g) {
+  if (!g) return;
+  cudaSetDevice(g->g->ctx->device);
+  delete g->g;
+  delete g;
+}
+static int poly_new(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, bool device, void* stream,
+                    lasso_poly** out) {
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!out) return fail(LASSO_ERR_LENGTH, "poly: null output");
+  if (!is_pow2(len)) return fail(LASSO_ERR_NOT_POW2, "poly: the length must be a power of two (dense_mlpoly.rs:63-66)");
+  if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly: at most 2^28 evaluations");
+  if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly: row_stride must be at least 4 u64");
+  if (!device && !Z) return fail(LASSO_ERR_POINTER, "poly: null evaluations");
+  int err = 0;
+  Poly* p = poly_create(h->c, Z, len, row_stride, device, static_cast<cudaStream_t>(stream), &err);
+  if (err == 7) return fail(LASSO_ERR_POINTER, "poly: the evaluations are not device memory of the context's GPU");
+  if (err == 8) return fail(LASSO_ERR_VALUE, "poly: an evaluation is not a canonical Montgomery residue");
+  *out = new lasso_poly{p};
+  return 0;
+}
+int lasso_poly_create(lasso_ctx* h, const uint64_t* Z, size_t len, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_new(h, Z, len, 4, false, nullptr, out);
+  LB_CATCH
+}
+int lasso_poly_create_device(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
+                             lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_new(h, Z, len, row_stride, true, stream, out);
+  LB_CATCH
+}
+size_t lasso_poly_num_vars(const lasso_poly* p) { return p ? p->p->nv : 0; }
+void lasso_poly_destroy(lasso_poly* p) {
+  if (!p) return;
+  cudaSetDevice(p->p->ctx->device);
+  delete p->p;
+  delete p;
+}
+// the checks every use of a polynomial shares: same context, and the generators' R equals the polynomial's
+static int poly_use_check(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g) {
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!p || p->p->ctx != h->c) return fail(LASSO_ERR_STRATEGY, "poly: created on another context");
+  if (g) {
+    if (g->g->ctx != h->c) return fail(LASSO_ERR_GENS, "poly gens: created on another context");
+    // commitments.rs:85 asserts gens.n == the row length
+    if (poly_R(g->num_vars) != poly_R(p->p->nv)) return fail(LASSO_ERR_GENS, "poly gens: R differs from the polynomial's");
+  }
+  return 0;
+}
+int lasso_poly_commit(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, uint8_t* out, size_t cap,
+                      size_t* out_len) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, g)) return rc;
+  if (!g) return fail(LASSO_ERR_GENS, "poly commit: null generators");
+  const size_t need = 8 + 32 * ((size_t)1 << (p->p->nv / 2));
+  if (out_len) *out_len = need;
+  if (!out || cap < need) return fail(LASSO_ERR_LENGTH, "poly commit: output buffer too small");
+  auto t0 = std::chrono::steady_clock::now();
+  const std::vector<uint8_t> b = poly_commit(h->c, *p->p, *g->g);
+  h->c->t_commit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  memcpy(out, b.data(), b.size());
+  return 0;
+  LB_CATCH
+}
+static int load_point(const Poly& p, const uint64_t* r, size_t r_len, std::vector<fr_t>& rv) {
+  if (r_len != p.nv) return fail(LASSO_ERR_LENGTH, "poly: r.len() != num_vars");
+  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "poly: null point");
+  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "poly: a coordinate of r is not a canonical residue");
+  return 0;
+}
+int lasso_poly_evaluate(lasso_ctx* h, const lasso_poly* p, const uint64_t* r, size_t r_len, uint64_t out[4]) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  std::vector<fr_t> rv;
+  if (const int rc = load_point(*p->p, r, r_len, rv)) return rc;
+  const fr_t v = poly_evaluate(h->c, *p->p, rv);
+  memcpy(out, v.v, 32);
+  return 0;
+  LB_CATCH
+}
+int lasso_poly_eval_prove(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, const uint64_t* r, size_t r_len,
+                          const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* tape,
+                          uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, g)) return rc;
+  if (!g) return fail(LASSO_ERR_GENS, "poly eval proof: null generators");
+  if (!transcript || !tape) return fail(LASSO_ERR_LENGTH, "poly eval proof: null transcript or random tape");
+  std::vector<fr_t> rv, zr;
+  if (const int rc = load_point(*p->p, r, r_len, rv)) return rc;
+  if (!load_scalars(Zr, 1, zr)) return fail(LASSO_ERR_VALUE, "poly eval proof: Zr is not a canonical residue");
+  // the proof's size is fixed by num_vars: L_vec and R_vec of log2(R) points, delta, beta, z1, z2
+  const size_t lg = p->p->nv - p->p->nv / 2, need = 2 * (8 + 32 * lg) + 4 * 32;
+  if (proof_len) *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "poly eval proof: output buffer too small");
+  auto t0 = std::chrono::steady_clock::now();
+  uint8_t czr[32];
+  const std::vector<uint8_t> b = poly_eval_prove(h->c, *p->p, *g->g, rv, zr[0], transcript->t, tape->t, czr);
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (b.size() != need) return fail(-1, "poly eval proof: unexpected proof size");
+  memcpy(proof_out, b.data(), b.size());
+  if (C_Zr_out) memcpy(C_Zr_out, czr, 32);
+  return 0;
   LB_CATCH
 }
 

@@ -155,6 +155,11 @@ class Transcript {
     strobe_.meta_ad(&len, 4, true);
     strobe_.prf(out, n);
   }
+  void append_u64(const char* label, uint64_t x) {  // merlin: the 8 little-endian bytes
+    uint8_t b[8];
+    for (int i = 0; i < 8; i++) b[i] = (uint8_t)(x >> (8 * i));
+    append_message(label, b, 8);
+  }
   void append_protocol_name(const char* name) { append_message("protocol-name", std::string(name)); }
   void append_scalar(const char* label, const fr_t& s) {
     uint8_t b[32];

@@ -182,6 +182,13 @@ void launch_bullet_scalars(const fr_t* a, const fr_t* w, size_t n_loc, size_t m,
                            fr_t* sR, cudaStream_t st);
 void launch_scale(const fr_t* in, fr_t* out, size_t n, const fr_t& k, cudaStream_t st);
 
+// ---- ingest of a caller's dense polynomial (dense_poly_kernels.cu) ----
+// dst[i] <- row i of src (4 u64 Montgomery limbs, rows row_stride u64 apart; src == dst with row_stride 4 is allowed);
+// flags[0] |= 1 when a row is not a canonical residue (< l), flags[1] = max bit width of the canonical values
+void launch_poly_ingest(const uint64_t* src, size_t row_stride, size_t n, fr_t* dst, unsigned* flags, cudaStream_t st);
+// out[i] <- the integer value of in[i] (every value below 2^32)
+void launch_poly_mirror_u32(const fr_t* in, size_t n, uint32_t* out, cudaStream_t st);
+
 // ---- densify on the GPU (densify_kernels.cu; densified.rs:33-56): stable LSD radix sort by address ----
 void densify_init_device();
 bool densify_gpu_supported(size_t s, size_t log_m);

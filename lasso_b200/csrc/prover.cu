@@ -280,28 +280,17 @@ size_t gens_points_needed(size_t c, size_t s, size_t num_memories, size_t log_m)
   size_t mx = std::max(nv_l, std::max(nv_m, nv_d));
   return ((size_t)1 << (mx - mx / 2)) + 2;
 }
-Gens* gens_create(Ctx* c, const uint64_t* stream_affine, size_t n_points, size_t cc, size_t s, size_t num_memories,
-                  size_t log_m) {
-  if (n_points < gens_points_needed(cc, s, num_memories, log_m)) return nullptr;
-  std::unique_ptr<Gens> g(new Gens());
-  g->ctx = c;
-  g->n_points = n_points;
-  g->c = cc;
-  g->s = s;
-  g->num_memories = num_memories;
-  g->log_m = log_m;
-  g->nv_l = log2_exact_or_ceil(next_pow2(2 * cc * s));
-  g->nv_m = log2_exact_or_ceil(next_pow2(cc)) + log_m;
-  g->nv_d = log2_exact_or_ceil(next_pow2(num_memories * s));
+// The device side of a generator stream, shared by SparsePolyCommitmentGens and PolyCommitmentGens: the stream, its
+// fixed-base window table and the digit-multiples tables of the generators the widest opening uses, R_size = widest_R
+// generators + Q + h (dense_mlpoly.rs:301-316)
+static void gens_build_tables(Ctx* c, Gens* g, const uint64_t* stream_affine, size_t n_points, size_t widest_R) {
   g->d_bases_ark.alloc(c, n_points * 2);
   LB_CUDA_CHECK(cudaMemcpyAsync(g->d_bases_ark.p, stream_affine, n_points * 64, cudaMemcpyHostToDevice, c->st));
   g->d_table.alloc(c, (size_t)kMsmFullWindows * n_points);
   launch_build_table(g->d_bases_ark.p, n_points, g->d_table.p, n_points, kMsmFullWindows, c->st);
   g_launches += kMsmFullWindows;
   {
-    // widest opening: R_size = 2^(nv - nv/2) generators + Q + h (dense_mlpoly.rs:301-316)
-    size_t nv = std::max(g->nv_l, std::max(g->nv_m, g->nv_d));
-    size_t nd = ((size_t)1 << (nv - nv / 2)) + 2;
+    size_t nd = widest_R + 2;
     const char* off = getenv("LASSO_B200_NO_MULTIPLES");
     // The tables are an optimisation: if the device cannot hold them (cap, or an allocation failure on a smaller
     // or busier GPU) the prover silently keeps the bucket / 8-bit paths — outputs do not depend on it.
@@ -335,6 +324,31 @@ Gens* gens_create(Ctx* c, const uint64_t* stream_affine, size_t n_points, size_t
     }
   }
   c->sync();
+}
+Gens* gens_create(Ctx* c, const uint64_t* stream_affine, size_t n_points, size_t cc, size_t s, size_t num_memories,
+                  size_t log_m) {
+  if (n_points < gens_points_needed(cc, s, num_memories, log_m)) return nullptr;
+  std::unique_ptr<Gens> g(new Gens());
+  g->ctx = c;
+  g->n_points = n_points;
+  g->c = cc;
+  g->s = s;
+  g->num_memories = num_memories;
+  g->log_m = log_m;
+  g->nv_l = log2_exact_or_ceil(next_pow2(2 * cc * s));
+  g->nv_m = log2_exact_or_ceil(next_pow2(cc)) + log_m;
+  g->nv_d = log2_exact_or_ceil(next_pow2(num_memories * s));
+  const size_t nv = std::max(g->nv_l, std::max(g->nv_m, g->nv_d));
+  gens_build_tables(c, g.get(), stream_affine, n_points, poly_R(nv));
+  return g.release();
+}
+Gens* poly_gens_create(Ctx* c, const uint64_t* stream_affine, size_t n_points, size_t num_vars) {
+  if (n_points < poly_R(num_vars) + 2) return nullptr;
+  std::unique_ptr<Gens> g(new Gens());
+  g->ctx = c;
+  g->n_points = n_points;
+  g->nv_l = g->nv_m = g->nv_d = num_vars;
+  gens_build_tables(c, g.get(), stream_affine, n_points, poly_R(num_vars));
   return g.release();
 }
 
@@ -1222,6 +1236,7 @@ struct DotProductProofLogBytes {  // dot_product.rs:152-159 field order
   std::vector<uint8_t> L_vec, R_vec;  // 32 B per point
   uint8_t delta[32], beta[32];
   fr_t z1, z2;
+  uint8_t Cy[32];  // not serialised: the commitment to y that PolyEvalProof::prove returns as C_Zr_prime
 };
 static void ser_dpl(ByteWriter& w, const DotProductProofLogBytes& p) {
   w.vec_pts(p.L_vec);
@@ -1349,6 +1364,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     if (m != 1) launch_round(0);  // round 0 needs no challenge: it runs while the host absorbs Cx, Cy, a
     transcript.append_point_compressed("Cx", CxCy);
     transcript.append_point_compressed("Cy", CxCy + 32);
+    memcpy(out.Cy, CxCy + 32, 32);
     LB_CUDA_CHECK(cudaEventSynchronize(c->ev_aux));
     transcript.append_scalars_bytes("a", c->h_pin, n);
     sp1.reset(new SpanTimer(c, "PE.3 bullet rounds"));
@@ -1387,6 +1403,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
       g_launches += 1;
       std::vector<uint8_t> Cy = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
       transcript.append_point_compressed("Cy", Cy.data());
+      memcpy(out.Cy, Cy.data(), 32);
       // append_scalars(b"a", a_vec): canonical bytes straight from the device
       DBuf<fr_t> canon(c, n);
       launch_canonicalize(b.p, canon.p, n, c->d_flag, c->st);
@@ -1706,6 +1723,88 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     ser_dpl(w, proof_derefs);
   }
   c->sync();
+  return w.b;
+}
+
+// ---------------------------------------------------------------------------------------------- dense polynomials
+// DensePolynomial::new (dense_mlpoly.rs:62-71) from the caller's evaluations.  Both sources go through the same ingest
+// kernel: host rows are first uploaded into the polynomial's own buffer and checked there in place.  The caller checks
+// len (a power of two, at most 2^28) and row_stride (>= 4).
+Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err) {
+  SpanTimer sp(c, "DensePolynomial.new");
+  *err = 0;
+  if (device) {  // the first and the last row must both lie in device memory of this GPU
+    size_t last = 0;
+    const bool wraps = __builtin_mul_overflow(len - 1, row_stride, &last) || __builtin_add_overflow(last, (size_t)3, &last) ||
+                       __builtin_mul_overflow(last, sizeof(uint64_t), &last) || (uintptr_t)Z > UINTPTR_MAX - last;
+    if (!Z || wraps || !device_memory_of(c, Z) || !device_memory_of(c, (const char*)Z + last)) {
+      *err = 7;
+      return nullptr;
+    }
+  }
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->len = len;
+  p->nv = log2_exact_or_ceil(len);
+  p->d_fr.alloc(c, len);
+  DBuf<unsigned> flags(c, 2);
+  LB_CUDA_CHECK(cudaMemsetAsync(flags.p, 0, 2 * sizeof(unsigned), c->st));
+  if (device) {
+    // the rows are read only after the work the caller enqueued on `caller` before this call, and the caller's later
+    // work on `caller` (a caching allocator freeing the tensor, say) comes after the last read of them
+    LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
+    LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
+    launch_poly_ingest(Z, row_stride, len, p->d_fr.p, flags.p, c->st);
+    LB_CUDA_CHECK(cudaEventRecord(c->ev_aux, c->st));
+    LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
+  } else {
+    LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, Z, len * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+    launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, len, p->d_fr.p, flags.p, c->st);
+  }
+  g_launches += 1;
+  unsigned f[2];
+  c->d2h(f, flags.p, sizeof f);
+  if (f[0]) {
+    *err = 8;
+    return nullptr;
+  }
+  p->bits = f[1];
+  // integer values: the u32 mirror feeds commit_u32 / bound_u32 / multi_dot_u32, which give the same bytes as the
+  // Montgomery forms (lasso_strategy_create_fr sets the same precedent)
+  if (p->bits <= 32) {
+    p->d_u32.alloc(c, len);
+    launch_poly_mirror_u32(p->d_fr.p, len, p->d_u32.p, c->st);
+    g_launches += 1;
+  }
+  return p.release();
+}
+static PolySrc poly_src(const Poly& p) { return PolySrc(p.d_u32.p, p.d_fr.p); }
+// DensePolynomial::commit (dense_mlpoly.rs:152-181, no blinds) -> PolyCommitment { C: Vec<G> }
+std::vector<uint8_t> poly_commit(Ctx* c, const Poly& p, const Gens& g) {
+  SpanTimer sp(c, "DensePolynomial.commit");
+  ByteWriter w;
+  w.vec_pts(commit_src(c, g, poly_src(p), p.nv, std::max(p.bits, 1u)));
+  return w.b;
+}
+// DensePolynomial::evaluate (dense_mlpoly.rs:229-235): <Z, eq(r)>
+fr_t poly_evaluate(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
+  SpanTimer sp(c, "DensePolynomial.evaluate");
+  DBuf<fr_t> eq(c, p.len);
+  eq_evals_dev(c, r, 0, p.nv, eq.p);
+  multi_dot_src(poly_src(p), p.len, 1, eq.p, p.len, c->d_partial, c->d_small, c->st);
+  g_launches += 2;
+  fr_t out;
+  c->d2h(&out, c->d_small, sizeof out);
+  return out;
+}
+// PolyEvalProof::prove (dense_mlpoly.rs:301-359, no blinds) on the caller's transcript and tape
+std::vector<uint8_t> poly_eval_prove(Ctx* c, const Poly& p, const Gens& g, const std::vector<fr_t>& r, const fr_t& Zr,
+                                     Transcript& transcript, RandomTape& tape, uint8_t C_Zr[32]) {
+  const DotProductProofLogBytes proof = prove_poly_eval(c, g, poly_src(p), p.nv, r, Zr, transcript, tape);
+  c->sync();
+  memcpy(C_Zr, proof.Cy, 32);
+  ByteWriter w;
+  ser_dpl(w, proof);
   return w.b;
 }
 

@@ -233,6 +233,16 @@ struct Dense {
   const fr_t* fin(size_t i) const { return d_m_fr.p + i * m_loc; }
 };
 
+// DensePolynomial<Fr> (poly/dense_mlpoly.rs:13-18) of a caller, device resident: the library's own copy of its
+// evaluations, checked canonical on the way in (dense_poly_kernels.cu)
+struct Poly {
+  Ctx* ctx = nullptr;
+  size_t len = 0, nv = 0;
+  unsigned bits = 0;     // bit width of the widest value as an integer (0: the zero polynomial)
+  DBuf<fr_t> d_fr;       // Montgomery form
+  DBuf<uint32_t> d_u32;  // the same values as integers when bits <= 32 (commit_u32 / bound_u32), else empty
+};
+
 // ark-serialize (compressed) writer
 struct ByteWriter {
   std::vector<uint8_t> b;
@@ -284,6 +294,22 @@ std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr
                            const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,
                            std::vector<fr_t>* challenges);
 void sample_generators(const std::string& label, size_t count, uint64_t* out_affine);
+
+// dense polynomials of a caller (prover.cu): PolyCommitmentGens, DensePolynomial::{new, commit, evaluate},
+// PolyEvalProof::prove.  Single-GPU contexts only.
+static constexpr size_t kPolyMaxLen = (size_t)1 << 28;
+inline size_t poly_R(size_t num_vars) { return (size_t)1 << (num_vars - num_vars / 2); }
+// PolyCommitmentGens::new (dense_mlpoly.rs:38-45) from an explicit stream: G_0..G_{R-1}, Q = stream[R], h = stream[R+1];
+// nullptr when n_points < R + 2
+Gens* poly_gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t num_vars);
+// Z: len rows of 4 u64 Montgomery limbs, row_stride u64 apart; host memory, or device memory of the context's GPU
+// (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory
+Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err);
+std::vector<uint8_t> poly_commit(Ctx*, const Poly&, const Gens&);  // serialised PolyCommitment
+fr_t poly_evaluate(Ctx*, const Poly&, const std::vector<fr_t>& r);
+// serialised PolyEvalProof; C_Zr receives the compressed commitment to Zr the reference returns alongside it
+std::vector<uint8_t> poly_eval_prove(Ctx*, const Poly&, const Gens&, const std::vector<fr_t>& r, const fr_t& Zr,
+                                     Transcript&, RandomTape&, uint8_t C_Zr[32]);
 
 // comm.cu
 void comm_unique_id(uint8_t out[128]);

@@ -1,0 +1,236 @@
+// ORACLE FOR DENSE POLYNOMIALS ON A CALLER'S TRANSCRIPT — TEST INFRASTRUCTURE ONLY.
+//
+// lasso_b200's lasso_transcript_* / lasso_random_tape_* / lasso_poly_* expose the reference's dense-polynomial items to
+// a caller that holds its own Fiat-Shamir transcript.  The oracle in oracle/ restates those items (PolyCommitmentGens,
+// DensePolynomial::commit / evaluate, PolyEvalProof::prove / verify_plain, ProofTranscript, RandomTape) but drives them
+// only inside its own round trips; this file puts C entry points on the same code that take and return what the
+// library takes and returns: serialised bytes, an explicit generator stream, and transcript / tape objects that live
+// across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof.
+#include "../oracle/lasso.hpp"
+
+using namespace oracle;
+
+namespace {
+
+Fr ldfr(const uint64_t* p) { return Fr::from_raw(p); }
+void stfr(uint64_t* p, const Fr& f) { memcpy(p, f.l, 32); }
+std::vector<Fr> ldvec(const uint64_t* p, size_t n) {
+  std::vector<Fr> v(n);
+  for (size_t i = 0; i < n; i++) v[i] = ldfr(p + 4 * i);
+  return v;
+}
+std::vector<Affine> ldstream(const uint64_t* p, size_t n) {
+  std::vector<Affine> s(n);
+  for (size_t i = 0; i < n; i++) s[i] = Affine{Fq::from_raw(p + 8 * i), Fq::from_raw(p + 8 * i + 4)};
+  return s;
+}
+bool ldpoint(const uint8_t* in, Point& out) {
+  Affine a;
+  if (!decompress(in, a)) return false;
+  out = Point::from_affine(a);
+  return true;
+}
+void put_u64(std::vector<uint8_t>& b, uint64_t v) {
+  for (int i = 0; i < 8; i++) b.push_back((uint8_t)(v >> (8 * i)));
+}
+void put_point(std::vector<uint8_t>& b, const Point& p) {
+  uint8_t c[32];
+  p.compress(c);
+  b.insert(b.end(), c, c + 32);
+}
+void put_fr(std::vector<uint8_t>& b, const Fr& f) {
+  uint8_t c[32];
+  f.to_bytes(c);
+  b.insert(b.end(), c, c + 32);
+}
+// ark-serialize (compressed) of PolyCommitment { C: Vec<G> }
+std::vector<uint8_t> ser_commitment(const PolyCommitment& c) {
+  std::vector<uint8_t> b;
+  put_u64(b, c.C.size());
+  for (const Point& p : c.C) put_point(b, p);
+  return b;
+}
+// PolyEvalProof { proof: DotProductProofLog { bullet_reduction_proof { L_vec, R_vec }, delta, beta, z1, z2 } }
+std::vector<uint8_t> ser_proof(const PolyEvalProof& p) {
+  std::vector<uint8_t> b;
+  const DotProductProofLog& d = p.proof;
+  put_u64(b, d.bullet_reduction_proof.L_vec.size());
+  for (const Point& q : d.bullet_reduction_proof.L_vec) put_point(b, q);
+  put_u64(b, d.bullet_reduction_proof.R_vec.size());
+  for (const Point& q : d.bullet_reduction_proof.R_vec) put_point(b, q);
+  put_point(b, d.delta);
+  put_point(b, d.beta);
+  put_fr(b, d.z1);
+  put_fr(b, d.z2);
+  return b;
+}
+struct Reader {
+  const uint8_t* p;
+  size_t n, at = 0;
+  bool ok = true;
+  const uint8_t* take(size_t k) {
+    if (!ok || n - at < k) {
+      ok = false;
+      return nullptr;
+    }
+    at += k;
+    return p + at - k;
+  }
+  uint64_t u64() {
+    const uint8_t* b = take(8);
+    uint64_t v = 0;
+    if (b) memcpy(&v, b, 8);
+    return v;
+  }
+  Point point() {
+    const uint8_t* b = take(32);
+    Point q = Point::zero();
+    if (b && !ldpoint(b, q)) ok = false;
+    return q;
+  }
+  std::vector<Point> points() {
+    const uint64_t k = u64();
+    std::vector<Point> v;
+    if (k > (n - at) / 32) ok = false;
+    for (uint64_t i = 0; ok && i < k; i++) v.push_back(point());
+    return v;
+  }
+  Fr fr() {  // ark rejects a non-canonical encoding
+    const uint8_t* b = take(32);
+    if (!b) return Fr::zero();
+    Fr f = Fr::from_bytes32_mod_order(b);
+    uint8_t back[32];
+    f.to_bytes(back);
+    if (memcmp(back, b, 32)) ok = false;
+    return f;
+  }
+};
+
+}  // namespace
+
+extern "C" {
+
+// ---- ProofTranscript (utils/transcript.rs) and RandomTape (utils/random.rs), one call per method
+void* orcd_transcript_new(const char* label) { return new Transcript(label); }
+void orcd_transcript_free(void* t) { delete (Transcript*)t; }
+void orcd_transcript_append_message(void* t, const char* label, const uint8_t* msg, size_t n) {
+  ((Transcript*)t)->append_message(label, msg, n);
+}
+void orcd_transcript_append_u64(void* t, const char* label, uint64_t x) { ((Transcript*)t)->append_u64(label, x); }
+void orcd_transcript_append_protocol_name(void* t, const char* name) { ((Transcript*)t)->append_protocol_name(name); }
+void orcd_transcript_append_scalar(void* t, const char* label, const uint64_t* s) {
+  ((Transcript*)t)->append_scalar(label, ldfr(s));
+}
+void orcd_transcript_append_scalars(void* t, const char* label, const uint64_t* s, size_t n) {
+  ((Transcript*)t)->append_scalars(label, ldvec(s, n));
+}
+// points as 32-byte compressed encodings: decompressed, then appended through the oracle's own compression
+int orcd_transcript_append_point(void* t, const char* label, const uint8_t* p32) {
+  Point q;
+  if (!ldpoint(p32, q)) return 1;
+  ((Transcript*)t)->append_point(label, q);
+  return 0;
+}
+int orcd_transcript_append_points(void* t, const char* label, const uint8_t* pts, size_t n) {  // transcript.rs:50-56
+  std::vector<Point> v(n);
+  for (size_t i = 0; i < n; i++)
+    if (!ldpoint(pts + 32 * i, v[i])) return 1;
+  Transcript& tr = *(Transcript*)t;
+  tr.append_message(label, "begin_append_vector");
+  for (const Point& q : v) tr.append_point(label, q);
+  tr.append_message(label, "end_append_vector");
+  return 0;
+}
+// PolyCommitment::append_to_transcript (dense_mlpoly.rs:281-289) of serialised commitment bytes
+int orcd_transcript_append_poly_commitment(void* t, const char* label, const uint8_t* bytes, size_t len) {
+  Reader rd{bytes, len};
+  PolyCommitment c;
+  c.C = rd.points();
+  if (!rd.ok || rd.at != len) return 1;
+  c.append_to_transcript(label, *(Transcript*)t);
+  return 0;
+}
+void orcd_transcript_challenge_scalar(void* t, const char* label, uint64_t* out) {
+  stfr(out, ((Transcript*)t)->challenge_scalar(label));
+}
+void orcd_transcript_challenge_vector(void* t, const char* label, size_t n, uint64_t* out) {
+  std::vector<Fr> v = ((Transcript*)t)->challenge_vector(label, n);
+  for (size_t i = 0; i < n; i++) stfr(out + 4 * i, v[i]);
+}
+void* orcd_tape_new(const char* label, const uint64_t* seed) { return new RandomTape(label, ldfr(seed)); }
+void orcd_tape_free(void* t) { delete (RandomTape*)t; }
+void orcd_tape_random_vector(void* t, const char* label, size_t n, uint64_t* out) {
+  std::vector<Fr> v = ((RandomTape*)t)->random_vector(label, n);
+  for (size_t i = 0; i < n; i++) stfr(out + 4 * i, v[i]);
+}
+
+// ---- DensePolynomial / PolyCommitmentGens / PolyEvalProof (dense_mlpoly.rs)
+// Z: n = 2^nv Montgomery elements; stream: n_points affine generators (G.., Q, h for R = 2^(nv - nv/2))
+// commit: out receives the serialised PolyCommitment; returns its length, 0 when the stream is too short or cap too small
+size_t orcd_poly_commit(const uint64_t* Z, size_t n, const uint64_t* stream, size_t n_points, uint8_t* out, size_t cap) {
+  try {
+    DensePolynomial poly(ldvec(Z, n));
+    size_t l, r;
+    EqPolynomial::compute_factored_lens(poly.num_vars, l, r);
+    if (n_points < pow2(r) + 2) return 0;
+    PolyCommitmentGens gens = PolyCommitmentGens::make(poly.num_vars, ldstream(stream, n_points));
+    std::vector<uint8_t> b = ser_commitment(poly.commit(gens));
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_poly_commit: %s\n", e.what());
+    return 0;
+  }
+}
+void orcd_evaluate(const uint64_t* Z, size_t n, const uint64_t* r, uint64_t* out) {
+  DensePolynomial poly(ldvec(Z, n));
+  stfr(out, poly.evaluate(ldvec(r, poly.num_vars)));
+}
+// PolyEvalProof::prove on a caller's transcript and tape: returns the proof's length (0 on error); C_Zr_out = the
+// compressed C_Zr_prime (Zr * Q + 0 * h)
+size_t orcd_poly_prove(const uint64_t* Z, size_t n, const uint64_t* r, const uint64_t* Zr, const uint64_t* stream,
+                       size_t n_points, void* transcript, void* tape, uint8_t* out, size_t cap, uint8_t* C_Zr_out) {
+  try {
+    DensePolynomial poly(ldvec(Z, n));
+    size_t l, rr;
+    EqPolynomial::compute_factored_lens(poly.num_vars, l, rr);
+    if (n_points < pow2(rr) + 2) return 0;
+    PolyCommitmentGens gens = PolyCommitmentGens::make(poly.num_vars, ldstream(stream, n_points));
+    PolyEvalProof proof = PolyEvalProof::prove(poly, ldvec(r, poly.num_vars), ldfr(Zr), gens, *(Transcript*)transcript,
+                                               *(RandomTape*)tape);
+    commit_scalar(ldfr(Zr), Fr::zero(), gens.gens.gens_1).compress(C_Zr_out);
+    std::vector<uint8_t> b = ser_proof(proof);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_poly_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// PolyEvalProof::verify_plain (dense_mlpoly.rs:388-400) of serialised bytes: 0 accepted, 1 rejected, 2 the commitment
+// or the proof does not parse
+int orcd_poly_verify(const uint64_t* stream, size_t n_points, size_t nv, const uint8_t* comm, size_t comm_len,
+                     const uint8_t* proof, size_t proof_len, const uint64_t* r, const uint64_t* Zr, void* transcript) {
+  size_t l, rr;
+  EqPolynomial::compute_factored_lens(nv, l, rr);
+  if (n_points < pow2(rr) + 2) return 2;
+  PolyCommitmentGens gens = PolyCommitmentGens::make(nv, ldstream(stream, n_points));
+  Reader rc{comm, comm_len};
+  PolyCommitment c;
+  c.C = rc.points();
+  if (!rc.ok || rc.at != comm_len || c.C.size() != pow2(l)) return 2;
+  Reader rp{proof, proof_len};
+  PolyEvalProof p;
+  p.proof.bullet_reduction_proof.L_vec = rp.points();
+  p.proof.bullet_reduction_proof.R_vec = rp.points();
+  p.proof.delta = rp.point();
+  p.proof.beta = rp.point();
+  p.proof.z1 = rp.fr();
+  p.proof.z2 = rp.fr();
+  if (!rp.ok || rp.at != proof_len) return 2;
+  return p.verify_plain(gens, *(Transcript*)transcript, ldvec(r, nv), ldfr(Zr), c) ? 0 : 1;
+}
+
+}  // extern "C"
