@@ -312,6 +312,38 @@ int lasso_poly_evaluate(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t
 int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, const uint64_t* r, size_t r_len,
                           const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* random_tape,
                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]);
+/* EqPolynomial::new(r).evals() (poly/eq_poly.rs:21-38) as a polynomial of the context, r[0] the most significant
+ * variable: 2^r_len evaluations, r_len <= 28 (LASSO_ERR_LENGTH), each coordinate a canonical residue (LASSO_ERR_VALUE). */
+int lasso_poly_create_eq(lasso_ctx*, const uint64_t* r, size_t r_len, lasso_poly** out);
+
+/* ---------------------------------------------------------------- sumchecks over a caller's polynomials
+ *
+ * A combining function g(x_0..x_{n_inputs-1}) in the program format of lasso_strategy_create (slots 0..n_inputs-1 are
+ * the inputs, instruction j writes slot n_inputs + j, the last instruction's slot is g), its constants, and the declared
+ * combined_degree.  The rules of lasso_strategy_create apply: 1 <= n_inputs <= 16, 1 <= n_ops <= 128, at most 64
+ * constants, each a canonical residue, operands name earlier slots, at most 16 intermediate values live at once,
+ * 1 <= degree <= 16 and at least the program's degree; LASSO_ERR_STRATEGY otherwise.  A host object: it needs no context
+ * and no GPU. */
+typedef struct lasso_comb lasso_comb;
+int lasso_comb_create(int n_inputs, const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
+                      int degree, lasso_comb** out);
+void lasso_comb_destroy(lasso_comb*);
+/* SumcheckInstanceProof::prove_arbitrary (subprotocols/sumcheck.rs:149-260): num_rounds rounds of the sumcheck of
+ * sum_x g(polys[0](x), .., polys[n_polys-1](x)) on the caller's transcript, which is advanced in place.  The caller's
+ * polynomials are NOT modified (the reference binds them in place): they can be opened at r afterwards.  The same
+ * polynomial may appear several times.
+ *  - proof_out: the ark-serialize bytes of SumcheckInstanceProof, 8 + num_rounds * (8 + 32 * degree) bytes (*proof_len
+ *    receives the size, also when proof_cap is too small);
+ *  - r_out: the num_rounds challenges; final_evals_out: n_polys values, element 0 of each polynomial after the binds
+ *    (its evaluation at r when num_rounds == num_vars);
+ *  - claim_out (may be NULL): e_0 + e_1 of the first round, i.e. the sum over the hypercube.
+ * Errors, each returned before any launch and before the transcript is touched: LASSO_ERR_STRATEGY for n_polys !=
+ * n_inputs, a polynomial of another context or a sharded context; LASSO_ERR_LENGTH for polynomials of different
+ * num_vars, num_rounds outside 1..num_vars, proof_cap too small, or a null transcript or output.  The working memory
+ * (n_polys x 2^(num_vars-1) elements when num_rounds >= 2) is allocated before the first transcript write. */
+int lasso_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
+                         size_t num_rounds, lasso_transcript*, uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                         uint64_t* r_out, uint64_t* final_evals_out, uint64_t claim_out[4]);
 
 /* Host-resident benchmark helper: number of kernels launched by this context so far, and the wall time
  * (ms) of the last densify / commit / prove calls. */

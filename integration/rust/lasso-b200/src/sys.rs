@@ -34,6 +34,10 @@ pub struct lasso_poly_gens {
 pub struct lasso_poly {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct lasso_comb {
+    _p: [u8; 0],
+}
 
 extern "C" {
     pub fn lasso_last_error() -> *const c_char;
@@ -120,6 +124,15 @@ extern "C" {
                                  r_len: usize, zr: *const u64, transcript: *mut lasso_transcript,
                                  random_tape: *mut lasso_random_tape, proof_out: *mut u8, proof_cap: usize,
                                  proof_len: *mut usize, c_zr_out: *mut u8) -> c_int;
+    pub fn lasso_poly_create_eq(ctx: *mut lasso_ctx, r: *const u64, r_len: usize, out: *mut *mut lasso_poly) -> c_int;
+    // sumchecks over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_comb_create(n_inputs: c_int, program: *const i32, n_ops: c_int, constants: *const u64, n_constants: c_int,
+                             degree: c_int, out: *mut *mut lasso_comb) -> c_int;
+    pub fn lasso_comb_destroy(g: *mut lasso_comb);
+    pub fn lasso_sumcheck_prove(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly, n_polys: usize,
+                                num_rounds: usize, transcript: *mut lasso_transcript, proof_out: *mut u8, proof_cap: usize,
+                                proof_len: *mut usize, r_out: *mut u64, final_evals_out: *mut u64, claim_out: *mut u64)
+                                -> c_int;
     pub fn lasso_launch_count(ctx: *const lasso_ctx) -> u64;
     pub fn lasso_last_timings(ctx: *const lasso_ctx, out_ms: *mut f64);
 }

@@ -13,14 +13,17 @@ and, for a caller that composes Lasso into a larger protocol, its own dense poly
     PolyCommitmentGens.new(ctx, label, num_vars)                         src/poly/dense_mlpoly.rs:38
     DensePolynomial(ctx, Z).commit(gens) / .evaluate(r)                  src/poly/dense_mlpoly.rs:152, 229
     PolyEvalProof.prove(ctx, poly, r, Zr, gens, transcript, random_tape)    src/poly/dense_mlpoly.rs:301
+    DensePolynomial.eq(ctx, r)                                           src/poly/eq_poly.rs:21
+    SumcheckInstanceProof.prove_arbitrary(ctx, polys, Comb(fn, k), transcript)   src/subprotocols/sumcheck.rs:149
 
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
-    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Transcript, bind_bot, bind_top,
+    Comb, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
+    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, SumcheckInstanceProof, Transcript,
+    bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,
     msm, poly_gens_points_needed, sample_generators, sumcheck_bind_round_arbitrary,
     sumcheck_round_arbitrary, sumcheck_round_cubic, sumcheck_round_custom, trace_combine_lookups,

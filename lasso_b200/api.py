@@ -797,6 +797,17 @@ class DensePolynomial:
         self.ctx, self._h = ctx, h
         self.num_vars = int(lib().lasso_poly_num_vars(h))
 
+    @classmethod
+    def eq(cls, ctx, r):
+        """EqPolynomial::new(r).evals() (src/poly/eq_poly.rs:21-38) on ctx's GPU, r[0] the most significant variable"""
+        r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+        h = C.c_void_p()
+        _chk(lib().lasso_poly_create_eq(ctx._h, _p(r), C.c_size_t(r.shape[0]), C.byref(h)))
+        self = cls.__new__(cls)
+        self.ctx, self._h = ctx, h
+        self.num_vars = int(lib().lasso_poly_num_vars(h))
+        return self
+
     def commit(self, gens):
         """DensePolynomial::commit without blinds -> the ark-serialize bytes of PolyCommitment"""
         cap = 8 + 32 * (1 << (self.num_vars // 2))
@@ -838,3 +849,71 @@ class PolyEvalProof:
         _chk(lib().lasso_poly_eval_prove(ctx._h, poly._h, gens._h, _p(r), C.c_size_t(r.shape[0]), _p(Zr), transcript._h,
                                          random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
         return cls(bytes(out[: n.value]), czr.tobytes())
+
+
+# ------------------------------------------------------------------ sumchecks over a caller's polynomials
+class Comb:
+    """A combining function g(x_0, .., x_{n_inputs-1}) of SumcheckInstanceProof.prove_arbitrary
+    (src/subprotocols/sumcheck.rs:149-260): fn(vals), vals a list of n_inputs values, written with + - * and Python
+    integers (constants mod l), traced into the program of lasso_comb_create.  degree = combined_degree, the number of
+    evaluation points minus one; None means the traced degree.  A host object: no context or GPU needed."""
+
+    def __init__(self, fn, n_inputs, degree=None):
+        program, constants, traced = trace_combine_lookups(fn, int(n_inputs))
+        self._create(program, constants, int(n_inputs), traced if degree is None else int(degree))
+        self.traced_degree = traced
+
+    @classmethod
+    def from_program(cls, program, constants, n_inputs, degree):
+        """the program format of lasso_comb_create as it is: (n, 3) int32 {op, a, b}, (k, 4) uint64 Montgomery constants"""
+        self = cls.__new__(cls)
+        program = np.ascontiguousarray(program, dtype=np.int32).reshape(-1, 3)
+        constants = np.ascontiguousarray(constants, dtype=np.uint64).reshape(-1, 4)
+        self._create(program, constants, int(n_inputs), int(degree))
+        self.traced_degree = None
+        return self
+
+    def _create(self, program, constants, n_inputs, degree):
+        self._h = None
+        self.program, self.constants, self.n_inputs, self.degree = program, constants, n_inputs, degree
+        h = C.c_void_p()
+        _chk(lib().lasso_comb_create(n_inputs, _p(program), int(program.shape[0]), _p(constants) if constants.size else None,
+                                     int(constants.shape[0]), degree, C.byref(h)))
+        self._h = h
+
+    def __del__(self):
+        try:
+            if self._h:
+                lib().lasso_comb_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class SumcheckInstanceProof:
+    """src/subprotocols/sumcheck.rs:12-328.  `.bytes` is the ark-serialize (compressed) proof, `.r` the challenges,
+    `.final_evals` the value of every polynomial at r after the binds, `.claim` the sum over the hypercube."""
+
+    def __init__(self, data, r, final_evals, claim):
+        self.bytes, self.r, self.final_evals, self.claim = data, r, final_evals, claim
+
+    @classmethod
+    def prove_arbitrary(cls, ctx, polys, comb, transcript, num_rounds=None):
+        """prove_arbitrary over DensePolynomials of ctx (all of one num_vars; the same one may appear several times) on
+        the caller's transcript, advanced in place.  The polynomials are not modified.  num_rounds=None: num_vars."""
+        polys = list(polys)
+        if num_rounds is None:
+            num_rounds = polys[0].num_vars if polys else 0
+        num_rounds = int(num_rounds)
+        arr = (C.c_void_p * max(len(polys), 1))()
+        for i, p in enumerate(polys):
+            arr[i] = p._h.value
+        cap = 8 + max(num_rounds, 0) * (8 + 32 * comb.degree)
+        out = np.zeros(cap, dtype=np.uint8)
+        r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
+        fin = np.zeros((max(len(polys), 1), 4), dtype=np.uint64)
+        claim = np.zeros(4, dtype=np.uint64)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_sumcheck_prove(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.c_size_t(num_rounds),
+                                        transcript._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin), _p(claim)))
+        return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim)

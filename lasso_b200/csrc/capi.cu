@@ -44,6 +44,10 @@ struct lasso_poly_gens {
 struct lasso_poly {
   Poly* p;
 };
+// a combining function of lasso_sumcheck_prove: a host object
+struct lasso_comb {
+  Comb g;
+};
 
 struct lasso_msm_job {
   Ctx* c = nullptr;
@@ -81,20 +85,11 @@ static bool is_pow2(size_t x) { return x && !(x & (x - 1)); }
 static constexpr size_t kMsmLargeMin = 1 << 14;  // below this the row kernels (c = 8, buckets in shared memory) win
 static Strategy mkS(int kind, int C, int log_M, int log_R) { return Strategy{kind, C, log_M, log_R}; }
 
-// Checks a custom strategy's descriptor (everything but the tables' contents) and fills cs with its shape, the degree
-// of g and the instructions with SSA slots mapped to physical slots.  "" = valid, else the reason.
-static std::string custom_check(int C, int log_m, int nsub, int alpha, const int* sub, const int* dim, const int32_t* prog,
-                                int n_ops, const uint64_t* consts, int n_consts, int degree, CustomStrategy& cs,
-                                std::vector<CustomIns>& ins) {
-  if (C < 1 || C > 16) return "C must be in 1..16";
-  if (log_m < 2 || log_m > 24) return "log_m must be in 2..24";
-  if (alpha < 1 || alpha > kCustomMaxMemories) return "num_memories must be in 1..16";
-  if (nsub < 1 || nsub > alpha) return "num_subtables must be in 1..num_memories";
-  if (!sub || !dim || !prog) return "null map or program";
-  for (int i = 0; i < alpha; i++) {
-    if (sub[i] < 0 || sub[i] >= nsub) return "memory_to_subtable_index out of range";
-    if (dim[i] < 0 || dim[i] >= C) return "memory_to_dimension_index out of range";
-  }
+// Checks a straight-line program over alpha inputs (slots 0..alpha-1) with its constants and declared degree (named
+// `what` in the reasons) and maps its SSA slots to physical slots: ins receives the instructions, *n_slots_out the
+// number of physical slots.  Shared by custom strategies and combining functions.  "" = valid, else the reason.
+static std::string program_check(int alpha, const int32_t* prog, int n_ops, const uint64_t* consts, int n_consts, int degree,
+                                 const std::string& what, std::vector<CustomIns>& ins, int* n_slots_out) {
   if (n_ops < 1 || n_ops > kCustomMaxOps) return "the program needs 1..128 instructions";
   if (n_consts < 0 || n_consts > kCustomMaxConsts) return "at most 64 constants";
   if (n_consts > 0 && !consts) return "null constants";
@@ -119,9 +114,9 @@ static std::string custom_check(int C, int log_m, int nsub, int alpha, const int
     if (!konst) last_use[b] = j;
   }
   const int gdeg = deg[nvals - 1];
-  if (degree < 1 || degree > kCustomMaxDegree) return "g_poly_degree must be in 1..16";
+  if (degree < 1 || degree > kCustomMaxDegree) return what + " must be in 1..16";
   if (degree < gdeg)
-    return "declared g_poly_degree " + std::to_string(degree) + " is below the program's degree " + std::to_string(gdeg);
+    return "declared " + what + " " + std::to_string(degree) + " is below the program's degree " + std::to_string(gdeg);
   // physical slots by liveness: an operand's slot is free again after its last use, before the result is stored
   std::vector<int> phys(nvals, -1), free_slots;
   int n_slots = 0;
@@ -153,6 +148,26 @@ static std::string custom_check(int C, int log_m, int nsub, int alpha, const int
     else phys[alpha + j] = s;
   }
   if (n_slots > kCustomMaxSlots) return "the program keeps more than 16 intermediate values live at once";
+  *n_slots_out = n_slots;
+  return "";
+}
+// Checks a custom strategy's descriptor (everything but the tables' contents) and fills cs with its shape, the degree
+// of g and the instructions with SSA slots mapped to physical slots.  "" = valid, else the reason.
+static std::string custom_check(int C, int log_m, int nsub, int alpha, const int* sub, const int* dim, const int32_t* prog,
+                                int n_ops, const uint64_t* consts, int n_consts, int degree, CustomStrategy& cs,
+                                std::vector<CustomIns>& ins) {
+  if (C < 1 || C > 16) return "C must be in 1..16";
+  if (log_m < 2 || log_m > 24) return "log_m must be in 2..24";
+  if (alpha < 1 || alpha > kCustomMaxMemories) return "num_memories must be in 1..16";
+  if (nsub < 1 || nsub > alpha) return "num_subtables must be in 1..num_memories";
+  if (!sub || !dim || !prog) return "null map or program";
+  for (int i = 0; i < alpha; i++) {
+    if (sub[i] < 0 || sub[i] >= nsub) return "memory_to_subtable_index out of range";
+    if (dim[i] < 0 || dim[i] >= C) return "memory_to_dimension_index out of range";
+  }
+  int n_slots = 0;
+  const std::string why = program_check(alpha, prog, n_ops, consts, n_consts, degree, "g_poly_degree", ins, &n_slots);
+  if (!why.empty()) return why;
   cs = CustomStrategy{};
   cs.C = C;
   cs.log_m = log_m;
@@ -1076,6 +1091,73 @@ int lasso_poly_eval_prove(lasso_ctx* h, const lasso_poly* p, const lasso_poly_ge
   if (b.size() != need) return fail(-1, "poly eval proof: unexpected proof size");
   memcpy(proof_out, b.data(), b.size());
   if (C_Zr_out) memcpy(C_Zr_out, czr, 32);
+  return 0;
+  LB_CATCH
+}
+int lasso_poly_create_eq(lasso_ctx* h, const uint64_t* r, size_t r_len, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!out) return fail(LASSO_ERR_LENGTH, "eq poly: null output");
+  if (r_len > 28) return fail(LASSO_ERR_LENGTH, "eq poly: at most 28 variables (2^28 evaluations)");
+  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "eq poly: null point");
+  std::vector<fr_t> rv;
+  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "eq poly: a coordinate of r is not a canonical residue");
+  *out = new lasso_poly{poly_create_eq(h->c, rv)};
+  return 0;
+  LB_CATCH
+}
+
+// ---- sumchecks over a caller's polynomials
+int lasso_comb_create(int n_inputs, const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
+                      int degree, lasso_comb** out) {
+  LB_TRY
+  if (out) *out = nullptr;
+  if (!out) return fail(LASSO_ERR_STRATEGY, "comb: null output");
+  if (n_inputs < 1 || n_inputs > kCombMaxInputs) return fail(LASSO_ERR_STRATEGY, "comb: n_inputs must be in 1..16");
+  if (!program) return fail(LASSO_ERR_STRATEGY, "comb: null program");
+  Comb g;
+  const std::string why = program_check(n_inputs, program, n_ops, constants, n_constants, degree, "degree", g.ins, &g.n_slots);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "comb: " + why);
+  g.n_inputs = n_inputs;
+  g.degree = degree;
+  g.consts.resize(n_constants);
+  if (n_constants) memcpy(g.consts.data(), constants, (size_t)n_constants * 32);
+  *out = new lasso_comb{std::move(g)};
+  return 0;
+  LB_CATCH
+}
+void lasso_comb_destroy(lasso_comb* g) { delete g; }
+int lasso_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly* const* polys, size_t n_polys,
+                         size_t num_rounds, lasso_transcript* transcript, uint8_t* proof_out, size_t proof_cap,
+                         size_t* proof_len, uint64_t* r_out, uint64_t* final_evals_out, uint64_t claim_out[4]) {
+  LB_TRY_CTX(h)
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!g) return fail(LASSO_ERR_STRATEGY, "sumcheck: null combining function");
+  if (!polys || n_polys != (size_t)g->g.n_inputs)
+    return fail(LASSO_ERR_STRATEGY, "sumcheck: " + std::to_string(n_polys) + " polynomials for a combining function of " +
+                                        std::to_string(g->g.n_inputs) + " inputs");
+  for (size_t j = 0; j < n_polys; j++)
+    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  const size_t nv = polys[0]->p->nv;
+  for (size_t j = 1; j < n_polys; j++)
+    if (polys[j]->p->nv != nv) return fail(LASSO_ERR_LENGTH, "sumcheck: the polynomials have different num_vars");
+  if (num_rounds < 1 || num_rounds > nv) return fail(LASSO_ERR_LENGTH, "sumcheck: num_rounds must be in 1..num_vars");
+  // SumcheckInstanceProof: a u64 count, then per round a u64 length and the degree coefficients except the linear one
+  const size_t need = 8 + num_rounds * (8 + 32 * (size_t)g->g.degree);
+  if (proof_len) *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "sumcheck: output buffer too small");
+  if (!transcript || !r_out || !final_evals_out) return fail(LASSO_ERR_LENGTH, "sumcheck: null transcript or output");
+  std::vector<const Poly*> ps(n_polys);
+  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
+  auto t0 = std::chrono::steady_clock::now();
+  const SumcheckOut o = sumcheck_prove(h->c, g->g, ps.data(), (int)n_polys, num_rounds, transcript->t);
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (o.proof.size() != need) return fail(-1, "sumcheck: unexpected proof size");
+  memcpy(proof_out, o.proof.data(), need);
+  for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
+  for (size_t j = 0; j < n_polys; j++) memcpy(final_evals_out + 4 * j, o.final_evals[j].v, 32);
+  if (claim_out) memcpy(claim_out, o.claim.v, 32);
   return 0;
   LB_CATCH
 }

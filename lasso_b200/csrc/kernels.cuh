@@ -106,8 +106,33 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
 bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t stride, size_t q, const fr_t& r,
                                          const Finalize& fin, size_t min_q, cudaStream_t st);
 int sumcheck_max_blocks();
-// per-device function attributes (dynamic shared memory opt-in of the custom-strategy kernels)
+// per-device function attributes (dynamic shared memory opt-in of the custom-strategy and combining-function kernels)
 void poly_init_device();
+
+// ---- K2 over a caller's polynomials (lasso_sumcheck_prove): g(P_0, .., P_{k-1}) with no eq factor ----
+// A combining function g of n_inputs values in the program format of the custom strategies (CustomIns after slot
+// allocation); d_ops and d_consts are device copies.
+static constexpr int kCombMaxInputs = 16;
+struct CombProgram {
+  int n_inputs, degree, n_ops, n_consts, n_slots;
+  const CustomIns* d_ops;
+  const fr_t* d_consts;
+};
+// the k input polynomials as independent device pointers, passed by value
+struct CombPtrs {
+  fr_t* p[kCombMaxInputs];
+};
+// One round (sumcheck.rs:179-237): the degree + 1 sums over i < half of g(x(t)), x_k(t) = lo_k + t (hi_k - lo_k),
+// lo_k = in.p[k][i], hi_k = in.p[k][half + i]; one launch, published through fin.
+void launch_sumcheck_eval_comb(const CombProgram& g, const CombPtrs& in, size_t half, const Finalize& fin, cudaStream_t st);
+// dst.p[k][i] <- src.p[k][i] + r (src.p[k][half + i] - src.p[k][i]) for k < n, i < half; dst == src binds in place
+void launch_bind_comb(const CombPtrs& src, const CombPtrs& dst, int n, size_t half, const fr_t& r, cudaStream_t st);
+// The bind above from length 4q to 2q fused with the evaluation of the next round over the bound values, one launch.
+// Returns false (nothing launched) when q < min_q (0: the default threshold below which two launches are quicker).
+bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, const CombPtrs& dst, size_t q, const fr_t& r,
+                                    const Finalize& fin, size_t min_q, cudaStream_t st);
+// value k < n: src.p[k][0] + r (src.p[k][half] - src.p[k][0]), element 0 of the last bind, published through fin
+void launch_final_comb(const CombPtrs& src, int n, size_t half, const fr_t& r, const Finalize& fin, cudaStream_t st);
 
 // ---- K3: batched cubic round evaluation (sumcheck.rs:49-93) ----
 // A, B: ncirc device pointers each to 2*half elements; Ceq: 2*half elements.  The batching coefficients of

@@ -452,11 +452,14 @@ __device__ __forceinline__ fr_t custom_run(const CustomIns* ops, int n_ops, cons
   return r;
 }
 // shared memory: instructions | constants | slots of every thread | (round kernel) accumulators of every thread
-static size_t custom_smem_bytes(const CustomStrategy& cs, int npoints) {
+// (Prog: a CustomStrategy or a CombProgram)
+template <class Prog>
+static size_t custom_smem_bytes(const Prog& cs, int npoints) {
   return (size_t)cs.n_ops * sizeof(CustomIns) + (size_t)cs.n_consts * sizeof(fr_t) +
          (size_t)(cs.n_slots + npoints) * sizeof(fr_t) * kCustomThreads;
 }
-__device__ __forceinline__ void custom_stage(const CustomStrategy& cs, CustomIns*& ops, fr_t*& consts, uint32_t*& slots) {
+template <class Prog>
+__device__ __forceinline__ void custom_stage(const Prog& cs, CustomIns*& ops, fr_t*& consts, uint32_t*& slots) {
   extern __shared__ __align__(32) unsigned char custom_sm[];
   consts = (fr_t*)custom_sm;  // first: 32-byte alignment
   ops = (CustomIns*)(consts + cs.n_consts);
@@ -533,6 +536,110 @@ __global__ void __launch_bounds__(kCustomThreads)
   if (threadIdx.x == 0) partial[blockIdx.x] = acc[0];
 }
 
+// ------------------------------------------------------------------------------------ K2 over a caller's polynomials
+// prove_arbitrary (sumcheck.rs:149-260) for a combining function g of k independent polynomials, no eq factor (a caller
+// that wants one passes eq as an input).  The same interpreter as the custom strategies; the inputs are k pointers.
+// acc[t] += g(x(t)) for the pair i, x_k(t) = lo_k + t (hi_k - lo_k), lo_k = in.p[k][i], hi_k = in.p[k][half + i]
+__device__ __forceinline__ void comb_accumulate(const CombProgram& pg, const CustomIns* ops, const fr_t* consts,
+                                                uint32_t* slots, uint32_t* acc, const CombPtrs& in, size_t half, size_t i,
+                                                int npts) {
+#pragma unroll 1
+  for (int t = 0; t < npts; t++) {
+    const fr_t g = custom_run(ops, pg.n_ops, consts, slots, [&](int k) {
+      const fr_t* P = in.p[k];
+      const fr_t lo = ld_fr(P + i);
+      if (t == 0) return lo;
+      const fr_t hi = ld_fr(P + half + i);
+      return t == 1 ? hi : fr_add(lo, fr_mul_small(fr_sub(hi, lo), t));
+    });
+    custom_st(acc, t, fr_add(custom_ld(acc, t), g));
+  }
+}
+// the npts sums of the CTA -> block partials -> the last CTA adds them and publishes (as sc_eval_custom_kernel)
+__device__ __forceinline__ void comb_finish(uint32_t* acc, int npts, const Finalize& fin) {
+  __shared__ fr_t scratch[kCustomThreads / 32];
+  __shared__ fr_t res[kCustomMaxDegree + 1];
+  __shared__ int s_last;
+  for (int t = 0; t < npts; t++) {
+    fr_t v[1] = {custom_ld(acc, t)};
+    block_sum_fr<1>(v, scratch);
+    if (threadIdx.x == 0) res[t] = v[0];
+  }
+  __syncthreads();
+  if (gridDim.x == 1) {
+    if ((int)threadIdx.x < npts) finalize_publish(fin, threadIdx.x, res[threadIdx.x]);
+    return;
+  }
+  if ((int)threadIdx.x < npts) fin.partial[(size_t)threadIdx.x * gridDim.x + blockIdx.x] = res[threadIdx.x];
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) s_last = (atomicAdd(fin.counter, 1u) == gridDim.x - 1);
+  __syncthreads();
+  if (!s_last) return;
+  finalize_last_stage(fin, gridDim.x, npts);
+}
+// One round: degree + 1 evaluation points, the accumulators after the slots in shared memory
+__global__ void __launch_bounds__(kCustomThreads)
+    sc_eval_comb_kernel(CombProgram pg, const __grid_constant__ CombPtrs in, size_t half, Finalize fin) {
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(pg, ops, consts, slots);
+  const int npts = pg.degree + 1;
+  uint32_t* acc = slots + pg.n_slots * 8 * kCustomThreads;
+  for (int t = 0; t < npts; t++) custom_st(acc, t, fr_zero());
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x)
+    comb_accumulate(pg, ops, consts, slots, acc, in, half, i, npts);
+  comb_finish(acc, npts, fin);
+}
+// The bind of round j-1 and the evaluation of round j in one pass: thread i folds src elements i, i+q, i+2q, i+3q of
+// every input to dst elements i, i+q, then evaluates the pair i of the bound inputs.  The bound values are read back
+// from dst after the stores (this thread's own stores: L1 or L2 hits) rather than kept in shared memory, which at
+// 64 B per input per thread would not fit next to the slots and accumulators for k = 16.  Every element of src is read
+// once, so the round costs 4 reads + 2 writes of 32 B per input and pair instead of 4 + 2 (bind) + 2 (evaluation).
+// In place (src == dst) is safe: elements i and i+q are read and written by thread i only.
+__global__ void __launch_bounds__(kCustomThreads)
+    sc_bind_eval_comb_kernel(CombProgram pg, const __grid_constant__ CombPtrs src, const __grid_constant__ CombPtrs dst, size_t q,
+                             fr_t r, Finalize fin) {
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(pg, ops, consts, slots);
+  const int npts = pg.degree + 1;
+  uint32_t* acc = slots + pg.n_slots * 8 * kCustomThreads;
+  for (int t = 0; t < npts; t++) custom_st(acc, t, fr_zero());
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < q; i += (size_t)gridDim.x * blockDim.x) {
+#pragma unroll 1
+    for (int k = 0; k < pg.n_inputs; k++) {
+      const fr_t* S = src.p[k];
+      fr_t* D = dst.p[k];
+      const fr_t a0 = ld_fr_stream(S + i), a1 = ld_fr_stream(S + q + i);
+      const fr_t a2 = ld_fr_stream(S + 2 * q + i), a3 = ld_fr_stream(S + 3 * q + i);
+      st_fr(D + i, fr_add(a0, fr_mul(r, fr_sub(a2, a0))));
+      st_fr(D + q + i, fr_add(a1, fr_mul(r, fr_sub(a3, a1))));
+    }
+    comb_accumulate(pg, ops, consts, slots, acc, dst, q, i, npts);
+  }
+  comb_finish(acc, npts, fin);
+}
+// dense_mlpoly.rs:209-216 over the pointer descriptor, one input per blockIdx.y
+__global__ void __launch_bounds__(kThreads) bind_comb_kernel(const __grid_constant__ CombPtrs src, const __grid_constant__ CombPtrs dst,
+                                                             size_t half, fr_t r) {
+  const fr_t* Z = src.p[blockIdx.y];
+  fr_t* out = dst.p[blockIdx.y];
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
+    const fr_t lo = ld_fr_stream(Z + i), hi = ld_fr_stream(Z + half + i);
+    st_fr(out + i, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
+  }
+}
+// the final evaluations: only element 0 of the last bind is read (sumcheck.rs:258), so only it is computed
+__global__ void final_comb_kernel(const __grid_constant__ CombPtrs src, int n, size_t half, fr_t r, Finalize fin) {
+  const int k = threadIdx.x;
+  if (k >= n) return;
+  const fr_t lo = ld_fr(src.p[k]), hi = ld_fr(src.p[k] + half);
+  finalize_publish(fin, k, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
+}
+
 // dynamic shared memory above the default 48 KiB needs an opt-in per kernel and device (at context creation): the
 // largest program's
 void poly_init_device() {
@@ -543,6 +650,9 @@ void poly_init_device() {
   const int bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 2);
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   LB_CUDA_CHECK(cudaFuncSetAttribute(claim_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  const int comb_bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 1);
+  LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
+  LB_CUDA_CHECK(cudaFuncSetAttribute(sc_bind_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
 }
 // grid: one wave of as many CTAs as fit an SM at this shared-memory size
 static int custom_grid(size_t n, size_t smem) {
@@ -613,6 +723,34 @@ bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t s
                                                                                        linear_inc(S), fin);
   LB_LAUNCH_CHECK();
   return true;
+}
+
+// ---- sumcheck over a caller's polynomials
+void launch_sumcheck_eval_comb(const CombProgram& g, const CombPtrs& in, size_t half, const Finalize& fin, cudaStream_t st) {
+  const size_t smem = custom_smem_bytes(g, g.degree + 1);
+  sc_eval_comb_kernel<<<custom_grid(half, smem), kCustomThreads, smem, st>>>(g, in, half, fin);
+  LB_LAUNCH_CHECK();
+}
+void launch_bind_comb(const CombPtrs& src, const CombPtrs& dst, int n, size_t half, const fr_t& r, cudaStream_t st) {
+  if (half == 0 || n == 0) return;
+  int per = kNumSMs * kBindBlocksPerSM / n;
+  if (per < kNumSMs / 4) per = kNumSMs / 4;
+  bind_comb_kernel<<<dim3(grid_for(half, kThreads, per), n), kThreads, 0, st>>>(src, dst, half, r);
+  LB_LAUNCH_CHECK();
+}
+// The same threshold as the primary sumcheck's fused rounds: below q = 2^15 a round is a latency chain
+bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, const CombPtrs& dst, size_t q, const fr_t& r,
+                                    const Finalize& fin, size_t min_q, cudaStream_t st) {
+  static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
+  if (q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
+  const size_t smem = custom_smem_bytes(g, g.degree + 1);
+  sc_bind_eval_comb_kernel<<<custom_grid(q, smem), kCustomThreads, smem, st>>>(g, src, dst, q, r, fin);
+  LB_LAUNCH_CHECK();
+  return true;
+}
+void launch_final_comb(const CombPtrs& src, int n, size_t half, const fr_t& r, const Finalize& fin, cudaStream_t st) {
+  final_comb_kernel<<<1, 32, 0, st>>>(src, n, half, r, fin);
+  LB_LAUNCH_CHECK();
 }
 
 // subtables/mod.rs:186-216: sum_k eq[k] * g(E_1[k], ..., E_alpha[k]) over the whole hypercube

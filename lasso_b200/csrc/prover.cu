@@ -1807,5 +1807,81 @@ std::vector<uint8_t> poly_eval_prove(Ctx* c, const Poly& p, const Gens& g, const
   ser_dpl(w, proof);
   return w.b;
 }
+Poly* poly_create_eq(Ctx* c, const std::vector<fr_t>& r) {
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->nv = r.size();
+  p->len = (size_t)1 << p->nv;
+  p->bits = 253;  // the width of l: eq values are committed through the Fr windows
+  p->d_fr.alloc(c, p->len);
+  eq_evals_dev(c, r, 0, p->nv, p->d_fr.p);
+  return p.release();
+}
+
+// ---------------------------------------------------------------------------------------------- caller sumchecks
+// prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first evaluates the
+// caller's buffers; each later one binds the previous challenge and evaluates, fused from q = 2^15 pairs up, else a
+// bind and an evaluation) and one kernel that binds the last challenge into element 0 of every input and publishes the
+// k final evaluations.  LASSO_B200_UNFUSED_SUMCHECK (read per call, for A/B runs in one process) never fuses.
+SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int k, size_t num_rounds,
+                           Transcript& transcript) {
+  SpanTimer sp(c, "Sumcheck.prove_arbitrary");
+  const size_t nv = polys[0]->nv, npts = (size_t)g.degree + 1;
+  // every allocation before the first transcript write: a failure leaves the caller's transcript as it was
+  DBuf<fr_t> ws;
+  if (num_rounds >= 2) ws.alloc(c, (size_t)k << (nv - 1));
+  // the program, one upload: constants (32-byte aligned) then instructions
+  const size_t cbytes = g.consts.size() * sizeof(fr_t), ibytes = g.ins.size() * sizeof(CustomIns);
+  std::vector<uint8_t> staged(cbytes + ibytes);
+  if (cbytes) memcpy(staged.data(), g.consts.data(), cbytes);
+  memcpy(staged.data() + cbytes, g.ins.data(), ibytes);
+  DBuf<uint8_t> prog(c, staged.size());
+  LB_CUDA_CHECK(cudaMemcpyAsync(prog.p, staged.data(), staged.size(), cudaMemcpyHostToDevice, c->st));
+  const CombProgram pg{g.n_inputs, g.degree, (int)g.ins.size(), (int)g.consts.size(), g.n_slots,
+                       reinterpret_cast<const CustomIns*>(prog.p + cbytes), reinterpret_cast<const fr_t*>(prog.p)};
+  CombPtrs src{}, dst{};
+  for (int j = 0; j < k; j++) {
+    src.p[j] = polys[j]->d_fr.p;
+    if (ws.p) dst.p[j] = ws.p + ((size_t)j << (nv - 1));
+  }
+  const bool unfused = getenv("LASSO_B200_UNFUSED_SUMCHECK") != nullptr;
+  SumcheckOut out;
+  ByteWriter w;
+  w.u64(num_rounds);
+  std::vector<fr_t> evals(npts);
+  size_t len = polys[0]->len;  // the length of the arrays src points to
+  fr_t r_prev = fr_zero();
+  for (size_t j = 0; j < num_rounds; j++) {
+    const Finalize f = c->fin_begin();
+    if (j == 0) {
+      launch_sumcheck_eval_comb(pg, src, len / 2, f, c->st);
+      g_launches += 1;
+    } else {  // bind the previous challenge (caller buffers -> workspace, then in place) and evaluate
+      if (!unfused && launch_sumcheck_bind_eval_comb(pg, src, dst, len / 4, r_prev, f, 0, c->st)) {
+        g_launches += 1;
+      } else {
+        launch_bind_comb(src, dst, k, len / 2, r_prev, c->st);
+        launch_sumcheck_eval_comb(pg, dst, len / 4, f, c->st);
+        g_launches += 2;
+      }
+      src = dst;
+      len /= 2;
+    }
+    c->fin_wait(f, evals.data(), (int)npts);
+    if (j == 0) out.claim = fr_add(evals[0], evals[1]);
+    const std::vector<fr_t> coeffs = unipoly_from_evals(evals);
+    unipoly_append(coeffs, transcript);
+    r_prev = transcript.challenge_scalar("challenge_nextround");
+    out.r.push_back(r_prev);
+    w.vec_fr(unipoly_compress(coeffs));
+  }
+  out.final_evals.resize(k);
+  const Finalize f = c->fin_begin();
+  launch_final_comb(src, k, len / 2, r_prev, f, c->st);
+  g_launches += 1;
+  c->fin_wait(f, out.final_evals.data(), k);
+  out.proof = std::move(w.b);
+  return out;
+}
 
 }  // namespace lb

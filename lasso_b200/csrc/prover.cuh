@@ -310,6 +310,25 @@ fr_t poly_evaluate(Ctx*, const Poly&, const std::vector<fr_t>& r);
 // serialised PolyEvalProof; C_Zr receives the compressed commitment to Zr the reference returns alongside it
 std::vector<uint8_t> poly_eval_prove(Ctx*, const Poly&, const Gens&, const std::vector<fr_t>& r, const fr_t& Zr,
                                      Transcript&, RandomTape&, uint8_t C_Zr[32]);
+// EqPolynomial::new(r).evals() (eq_poly.rs:21-38) as a full-width polynomial (no u32 mirror); r.size() <= 28
+Poly* poly_create_eq(Ctx*, const std::vector<fr_t>& r);
+
+// A combining function g(x_0..x_{n_inputs-1}) of SumcheckInstanceProof::prove_arbitrary: a checked program (capi.cu)
+// with its slots allocated, and the declared combined_degree.  Host only.
+struct Comb {
+  int n_inputs = 0, degree = 0, n_slots = 0;
+  std::vector<CustomIns> ins;
+  std::vector<fr_t> consts;
+};
+struct SumcheckOut {
+  std::vector<uint8_t> proof;  // ark-serialize (compressed) SumcheckInstanceProof
+  std::vector<fr_t> r, final_evals;
+  fr_t claim;  // e_0 + e_1 of the first round: the sum over the hypercube
+};
+// SumcheckInstanceProof::prove_arbitrary (sumcheck.rs:149-260) over polys[0..k), k == g.n_inputs, all of one num_vars,
+// 1 <= num_rounds <= num_vars (the caller checks).  The polynomials are not modified: the first bind writes into a
+// workspace of k x 2^(num_vars-1) elements, allocated before the transcript is touched.
+SumcheckOut sumcheck_prove(Ctx*, const Comb& g, const Poly* const* polys, int k, size_t num_rounds, Transcript&);
 
 // comm.cu
 void comm_unique_id(uint8_t out[128]);

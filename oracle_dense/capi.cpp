@@ -106,6 +106,41 @@ struct Reader {
   }
 };
 
+// A combining function as lasso_comb_create takes it: 3 ints {op, a, b} per instruction, slots 0..n-1 the inputs,
+// instruction j writes slot n + j, the last slot is g; op: 0 a + b, 1 a - b, 2 a * b, 3 a * K[b], 4 a + K[b].
+// Interpreted directly, SSA slot by SSA slot (no slot allocation).  Taken as given: the GPU library checks it.
+struct Program {
+  size_t n;
+  std::vector<int32_t> prog;
+  std::vector<Fr> K;
+  Fr operator()(const Fr* vals) const {
+    Fr s[16 + 128];
+    const size_t m = prog.size() / 3;
+    for (size_t j = 0; j < n; j++) s[j] = vals[j];
+    for (size_t j = 0; j < m; j++) {
+      const int32_t op = prog[3 * j], a = prog[3 * j + 1], b = prog[3 * j + 2];
+      switch (op) {
+        case 0: s[n + j] = s[a] + s[b]; break;
+        case 1: s[n + j] = s[a] - s[b]; break;
+        case 2: s[n + j] = s[a] * s[b]; break;
+        case 3: s[n + j] = s[a] * K[b]; break;
+        default: s[n + j] = s[a] + K[b]; break;
+      }
+    }
+    return s[n + m - 1];
+  }
+};
+// ark-serialize (compressed) of SumcheckInstanceProof { compressed_polys: Vec<CompressedUniPoly> }
+std::vector<uint8_t> ser_sumcheck(const SumcheckInstanceProof& p) {
+  std::vector<uint8_t> b;
+  put_u64(b, p.compressed_polys.size());
+  for (const CompressedUniPoly& c : p.compressed_polys) {
+    put_u64(b, c.coeffs_except_linear_term.size());
+    for (const Fr& f : c.coeffs_except_linear_term) put_fr(b, f);
+  }
+  return b;
+}
+
 }  // namespace
 
 extern "C" {
@@ -231,6 +266,61 @@ int orcd_poly_verify(const uint64_t* stream, size_t n_points, size_t nv, const u
   p.proof.z2 = rp.fr();
   if (!rp.ok || rp.at != proof_len) return 2;
   return p.verify_plain(gens, *(Transcript*)transcript, ldvec(r, nv), ldfr(Zr), c) ? 0 : 1;
+}
+
+// ---- SumcheckInstanceProof (subprotocols/sumcheck.rs)
+// prove_arbitrary on copies of polys (k x len Montgomery elements, row-major) with the program interpreted on the host,
+// on a caller's transcript.  out: the serialised proof (returns its length, 0 on error); r_out: num_rounds challenges;
+// final_out: k values; claim_out: e_0 + e_1 of the first round; round_evals_out (may be null): num_rounds x (degree + 1)
+// evaluations of the round polynomials at 0..degree.
+size_t orcd_sumcheck_prove(const uint64_t* polys, size_t k, size_t len, size_t num_rounds, const int32_t* prog, size_t n_ops,
+                           const uint64_t* K, size_t n_k, size_t degree, void* transcript, uint8_t* out, size_t cap,
+                           uint64_t* r_out, uint64_t* final_out, uint64_t* claim_out, uint64_t* round_evals_out) {
+  try {
+    std::vector<DensePolynomial> ps;
+    for (size_t j = 0; j < k; j++) ps.emplace_back(ldvec(polys + 4 * len * j, len));
+    const Program g{k, std::vector<int32_t>(prog, prog + 3 * n_ops), ldvec(K, n_k)};
+    std::vector<Fr> r, final_evals;
+    std::vector<std::vector<Fr>> rounds;
+    SumcheckInstanceProof proof = SumcheckInstanceProof::prove_arbitrary(
+        num_rounds, ps, [&](const Fr* v) { return g(v); }, degree, *(Transcript*)transcript, r, final_evals, nullptr, &rounds);
+    std::vector<uint8_t> b = ser_sumcheck(proof);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+    for (size_t j = 0; j < k; j++) stfr(final_out + 4 * j, final_evals[j]);
+    stfr(claim_out, rounds[0][0] + rounds[0][1]);
+    if (round_evals_out)
+      for (size_t j = 0; j < num_rounds; j++)
+        for (size_t t = 0; t <= degree; t++) stfr(round_evals_out + 4 * (j * (degree + 1) + t), rounds[j][t]);
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_sumcheck_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// SumcheckInstanceProof::verify (sumcheck.rs:286-328) of serialised bytes: 0 accepted (e_out = the final claim,
+// r_out = num_rounds challenges), 1 rejected, 2 the bytes do not parse
+int orcd_sumcheck_verify(const uint8_t* bytes, size_t n, const uint64_t* claim, size_t num_rounds, size_t degree,
+                         void* transcript, uint64_t* e_out, uint64_t* r_out) {
+  Reader rd{bytes, n};
+  SumcheckInstanceProof p;
+  const uint64_t rounds = rd.u64();
+  for (uint64_t j = 0; rd.ok && j < rounds; j++) {
+    const uint64_t m = rd.u64();
+    if (m > (n - rd.at) / 32) rd.ok = false;
+    CompressedUniPoly c;
+    for (uint64_t i = 0; rd.ok && i < m; i++) c.coeffs_except_linear_term.push_back(rd.fr());
+    if (c.coeffs_except_linear_term.empty()) rd.ok = false;
+    p.compressed_polys.push_back(c);
+  }
+  if (!rd.ok || rd.at != n) return 2;
+  Fr e;
+  std::vector<Fr> r;
+  if (!p.verify(ldfr(claim), num_rounds, degree, *(Transcript*)transcript, e, r)) return 1;
+  stfr(e_out, e);
+  for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+  return 0;
 }
 
 }  // extern "C"
