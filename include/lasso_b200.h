@@ -344,6 +344,43 @@ void lasso_comb_destroy(lasso_comb*);
 int lasso_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
                          size_t num_rounds, lasso_transcript*, uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
                          uint64_t* r_out, uint64_t* final_evals_out, uint64_t claim_out[4]);
+/* Q(x) = g(polys[0](x), .., polys[n_polys-1](x)) at every point of the hypercube, e.g. the fingerprints
+ * h(a, v, t) = t gamma^2 + v gamma + a - tau of offline memory checking (lasso/memory_checking.rs:251-252).  g's
+ * declared degree is not used.  The result is a full-width polynomial like lasso_poly_create_eq (committed through the
+ * Fr windows): it can be committed, evaluated, opened, summed over or made a grand-product circuit.  Errors, before any
+ * launch: LASSO_ERR_STRATEGY for n_polys != n_inputs, a polynomial of another context or a sharded context;
+ * LASSO_ERR_LENGTH for polynomials of different num_vars or a null output. */
+int lasso_poly_create_comb(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
+                           lasso_poly** out);
+
+/* ---------------------------------------------------------------- grand products over a caller's polynomials
+ *
+ * GrandProductCircuit::new (subprotocols/grand_product.rs:38-58) over a polynomial of the context with
+ * 1 <= num_vars <= 28 (LASSO_ERR_LENGTH otherwise; a single evaluation has no layers).  Layer 0 is the polynomial
+ * itself: it is neither copied nor modified, and it MUST outlive the circuit.  The layers above it (2^num_vars - 2
+ * elements) are built on the GPU when the circuit is created; the product of all evaluations (`evaluate`,
+ * grand_product.rs:60-65) is then a host value.  LASSO_ERR_STRATEGY for a polynomial of another context or a sharded
+ * context. */
+typedef struct lasso_gp_circuit lasso_gp_circuit;
+int lasso_gp_circuit_create(lasso_ctx*, const lasso_poly*, lasso_gp_circuit** out);
+int lasso_gp_circuit_evaluate(const lasso_gp_circuit*, uint64_t out[4]);
+size_t lasso_gp_circuit_num_vars(const lasso_gp_circuit*);
+void lasso_gp_circuit_destroy(lasso_gp_circuit*);
+/* BatchedGrandProductArgument::prove (subprotocols/grand_product.rs:100-201) over n circuits of one num_vars v on the
+ * caller's transcript, which is advanced in place.  The caller appends the products (lasso_gp_circuit_evaluate) to the
+ * transcript first if its protocol does (lasso/memory_checking.rs:683-713).
+ *  - proof_out: the ark-serialize bytes of BatchedGrandProductArgument, 8 + v (24 + 64 n) + 52 v (v - 1) bytes
+ *    (*proof_len receives the size, also when proof_cap is too small);
+ *  - r_out: the v coordinates of rand; claims_out: n values, the final claims_to_verify, which equal P_k(rand) for the
+ *    circuits' polynomials P_k.
+ * The proof binds the circuits' own layers in place, as the reference does, so a circuit can be proven once; its
+ * polynomial (layer 0) is not modified and can be opened at rand afterwards.
+ * Errors, each returned before any launch and before the transcript is touched: LASSO_ERR_STRATEGY for n == 0 or
+ * n > 32, a circuit of another context, a sharded context, a circuit already proven or the same circuit twice;
+ * LASSO_ERR_LENGTH for circuits of different num_vars, proof_cap too small, or a null transcript or output.  The working
+ * memory is allocated before the first transcript write. */
+int lasso_gp_prove(lasso_ctx*, const lasso_gp_circuit* const* circuits, size_t n, lasso_transcript*, uint8_t* proof_out,
+                   size_t proof_cap, size_t* proof_len, uint64_t* r_out, uint64_t* claims_out);
 
 /* Host-resident benchmark helper: number of kernels launched by this context so far, and the wall time
  * (ms) of the last densify / commit / prove calls. */

@@ -38,6 +38,10 @@ pub struct lasso_poly {
 pub struct lasso_comb {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct lasso_gp_circuit {
+    _p: [u8; 0],
+}
 
 extern "C" {
     pub fn lasso_last_error() -> *const c_char;
@@ -133,6 +137,16 @@ extern "C" {
                                 num_rounds: usize, transcript: *mut lasso_transcript, proof_out: *mut u8, proof_cap: usize,
                                 proof_len: *mut usize, r_out: *mut u64, final_evals_out: *mut u64, claim_out: *mut u64)
                                 -> c_int;
+    pub fn lasso_poly_create_comb(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly,
+                                  n_polys: usize, out: *mut *mut lasso_poly) -> c_int;
+    // grand products over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_gp_circuit_create(ctx: *mut lasso_ctx, poly: *const lasso_poly, out: *mut *mut lasso_gp_circuit) -> c_int;
+    pub fn lasso_gp_circuit_evaluate(c: *const lasso_gp_circuit, out: *mut u64) -> c_int;
+    pub fn lasso_gp_circuit_num_vars(c: *const lasso_gp_circuit) -> usize;
+    pub fn lasso_gp_circuit_destroy(c: *mut lasso_gp_circuit);
+    pub fn lasso_gp_prove(ctx: *mut lasso_ctx, circuits: *const *const lasso_gp_circuit, n: usize,
+                          transcript: *mut lasso_transcript, proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize,
+                          r_out: *mut u64, claims_out: *mut u64) -> c_int;
     pub fn lasso_launch_count(ctx: *const lasso_ctx) -> u64;
     pub fn lasso_last_timings(ctx: *const lasso_ctx, out_ms: *mut f64);
 }

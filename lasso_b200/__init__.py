@@ -15,13 +15,16 @@ and, for a caller that composes Lasso into a larger protocol, its own dense poly
     PolyEvalProof.prove(ctx, poly, r, Zr, gens, transcript, random_tape)    src/poly/dense_mlpoly.rs:301
     DensePolynomial.eq(ctx, r)                                           src/poly/eq_poly.rs:21
     SumcheckInstanceProof.prove_arbitrary(ctx, polys, Comb(fn, k), transcript)   src/subprotocols/sumcheck.rs:149
+    DensePolynomial.from_comb(ctx, comb, polys)                          (pointwise g(P_0, .., P_{k-1}))
+    GrandProductCircuit(ctx, poly).evaluate()                            src/subprotocols/grand_product.rs:38, 60
+    BatchedGrandProductArgument.prove(ctx, circuits, transcript)         src/subprotocols/grand_product.rs:100
 
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    Comb, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
+    BatchedGrandProductArgument, Comb, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
     RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, SumcheckInstanceProof, Transcript,
     bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,

@@ -44,6 +44,7 @@ def lib():
         L.lasso_poly_gens_points_needed.restype = C.c_size_t
         L.lasso_poly_gens_points_needed.argtypes = [C.c_size_t]
         L.lasso_poly_num_vars.restype = C.c_size_t
+        L.lasso_gp_circuit_num_vars.restype = C.c_size_t
         L.lasso_transcript_append_u64.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
         _lib = L
     return _lib
@@ -798,15 +799,31 @@ class DensePolynomial:
         self.num_vars = int(lib().lasso_poly_num_vars(h))
 
     @classmethod
+    def _wrap(cls, ctx, h):
+        self = cls.__new__(cls)
+        self.ctx, self._h = ctx, h
+        self.num_vars = int(lib().lasso_poly_num_vars(h))
+        return self
+
+    @classmethod
     def eq(cls, ctx, r):
         """EqPolynomial::new(r).evals() (src/poly/eq_poly.rs:21-38) on ctx's GPU, r[0] the most significant variable"""
         r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
         h = C.c_void_p()
         _chk(lib().lasso_poly_create_eq(ctx._h, _p(r), C.c_size_t(r.shape[0]), C.byref(h)))
-        self = cls.__new__(cls)
-        self.ctx, self._h = ctx, h
-        self.num_vars = int(lib().lasso_poly_num_vars(h))
-        return self
+        return cls._wrap(ctx, h)
+
+    @classmethod
+    def from_comb(cls, ctx, comb, polys):
+        """Q(x) = comb(P_0(x), .., P_{k-1}(x)) at every point of the hypercube, on ctx's GPU (comb.degree is not used),
+        e.g. the fingerprints t gamma^2 + v gamma + a - tau of offline memory checking"""
+        polys = list(polys)
+        arr = (C.c_void_p * max(len(polys), 1))()
+        for i, p in enumerate(polys):
+            arr[i] = p._h.value
+        h = C.c_void_p()
+        _chk(lib().lasso_poly_create_comb(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.byref(h)))
+        return cls._wrap(ctx, h)
 
     def commit(self, gens):
         """DensePolynomial::commit without blinds -> the ark-serialize bytes of PolyCommitment"""
@@ -917,3 +934,59 @@ class SumcheckInstanceProof:
         _chk(lib().lasso_sumcheck_prove(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.c_size_t(num_rounds),
                                         transcript._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin), _p(claim)))
         return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim)
+
+
+# ------------------------------------------------------------------ grand products over a caller's polynomials
+class GrandProductCircuit:
+    """src/subprotocols/grand_product.rs:14-66 over a DensePolynomial of ctx with 1 <= num_vars <= 28: the layers above
+    the polynomial are built on ctx's GPU; the polynomial itself is layer 0, neither copied nor modified, and the circuit
+    keeps a reference to it.  A circuit can be proven once (the proof binds its layers)."""
+
+    def __init__(self, ctx, poly):
+        h = C.c_void_p()
+        _chk(lib().lasso_gp_circuit_create(ctx._h, poly._h, C.byref(h)))
+        self.ctx, self.poly, self._h = ctx, poly, h
+        self.num_vars = int(lib().lasso_gp_circuit_num_vars(h))
+
+    def evaluate(self):
+        """the product of all evaluations, (4,) uint64 Montgomery limbs"""
+        out = np.zeros(4, dtype=np.uint64)
+        _chk(lib().lasso_gp_circuit_evaluate(self._h, _p(out)))
+        return out
+
+    def __del__(self):
+        try:
+            if self._h and self.ctx._h:
+                lib().lasso_gp_circuit_destroy(self._h)
+        except Exception:
+            pass
+
+
+class BatchedGrandProductArgument:
+    """src/subprotocols/grand_product.rs:68-262.  `.bytes` is the ark-serialize (compressed) proof, `.r` the point rand
+    (num_vars x 4), `.claims` the final claims (n x 4), the circuits' polynomials evaluated at rand."""
+
+    def __init__(self, data, r, claims):
+        self.bytes, self.r, self.claims = data, r, claims
+
+    @staticmethod
+    def proof_len(n, num_vars):
+        return 8 + num_vars * (24 + 64 * n) + 52 * num_vars * (num_vars - 1)
+
+    @classmethod
+    def prove(cls, ctx, circuits, transcript):
+        """BatchedGrandProductArgument::prove over 1..32 GrandProductCircuits of one num_vars on the caller's transcript,
+        advanced in place"""
+        circuits = list(circuits)
+        arr = (C.c_void_p * max(len(circuits), 1))()
+        for i, c in enumerate(circuits):
+            arr[i] = c._h.value
+        v = circuits[0].num_vars if circuits else 0
+        cap = cls.proof_len(len(circuits), v)
+        out = np.zeros(cap, dtype=np.uint8)
+        r = np.zeros((max(v, 1), 4), dtype=np.uint64)
+        claims = np.zeros((max(len(circuits), 1), 4), dtype=np.uint64)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_gp_prove(ctx._h, arr, C.c_size_t(len(circuits)), transcript._h, _p(out), C.c_size_t(cap),
+                                  C.byref(n), _p(r), _p(claims)))
+        return cls(bytes(out[: n.value]), r[:v], claims[: len(circuits)])

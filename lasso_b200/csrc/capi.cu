@@ -48,6 +48,13 @@ struct lasso_poly {
 struct lasso_comb {
   Comb g;
 };
+// GrandProductCircuit over a caller's polynomial (layer 0, not owned); proving binds its layers, so it is proven once
+struct lasso_gp_circuit {
+  Ctx* c;
+  std::unique_ptr<Circuit> ci;
+  fr_t product;
+  mutable bool proven;
+};
 
 struct lasso_msm_job {
   Ctx* c = nullptr;
@@ -1158,6 +1165,89 @@ int lasso_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly* co
   for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
   for (size_t j = 0; j < n_polys; j++) memcpy(final_evals_out + 4 * j, o.final_evals[j].v, 32);
   if (claim_out) memcpy(claim_out, o.claim.v, 32);
+  return 0;
+  LB_CATCH
+}
+int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* const* polys, size_t n_polys,
+                           lasso_poly** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!g) return fail(LASSO_ERR_STRATEGY, "comb poly: null combining function");
+  if (!polys || n_polys != (size_t)g->g.n_inputs)
+    return fail(LASSO_ERR_STRATEGY, "comb poly: " + std::to_string(n_polys) + " polynomials for a combining function of " +
+                                        std::to_string(g->g.n_inputs) + " inputs");
+  for (size_t j = 0; j < n_polys; j++)
+    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  for (size_t j = 1; j < n_polys; j++)
+    if (polys[j]->p->nv != polys[0]->p->nv) return fail(LASSO_ERR_LENGTH, "comb poly: the polynomials have different num_vars");
+  if (!out) return fail(LASSO_ERR_LENGTH, "comb poly: null output");
+  std::vector<const Poly*> ps(n_polys);
+  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
+  *out = new lasso_poly{poly_create_comb(h->c, g->g, ps.data(), (int)n_polys)};
+  return 0;
+  LB_CATCH
+}
+
+// ---- grand products over a caller's polynomials
+int lasso_gp_circuit_create(lasso_ctx* h, const lasso_poly* p, lasso_gp_circuit** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  if (!out) return fail(LASSO_ERR_LENGTH, "grand product circuit: null output");
+  if (p->p->nv < 1 || p->p->nv > 28)
+    return fail(LASSO_ERR_LENGTH, "grand product circuit: num_vars must be in 1..28 (a single evaluation has no layers)");
+  fr_t product;
+  Circuit* ci = gp_circuit_create(h->c, *p->p, &product);
+  *out = new lasso_gp_circuit{h->c, std::unique_ptr<Circuit>(ci), product, false};
+  return 0;
+  LB_CATCH
+}
+int lasso_gp_circuit_evaluate(const lasso_gp_circuit* gc, uint64_t out[4]) {
+  if (!gc || !out) return fail(LASSO_ERR_LENGTH, "grand product circuit: null circuit or output");
+  memcpy(out, gc->product.v, 32);
+  return 0;
+}
+size_t lasso_gp_circuit_num_vars(const lasso_gp_circuit* gc) { return gc ? gc->ci->num_layers : 0; }
+void lasso_gp_circuit_destroy(lasso_gp_circuit* gc) {
+  if (!gc) return;
+  cudaSetDevice(gc->c->device);
+  delete gc;
+}
+int lasso_gp_prove(lasso_ctx* h, const lasso_gp_circuit* const* circuits, size_t n, lasso_transcript* transcript,
+                   uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* r_out, uint64_t* claims_out) {
+  LB_TRY_CTX(h)
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!circuits || n == 0 || n > 32)
+    return fail(LASSO_ERR_STRATEGY, "grand product: 1..32 circuits per batch (CubicCoeffs, TreePtrs)");
+  for (size_t k = 0; k < n; k++) {
+    if (!circuits[k] || circuits[k]->c != h->c) return fail(LASSO_ERR_STRATEGY, "grand product: a circuit of another context");
+    if (circuits[k]->proven) return fail(LASSO_ERR_STRATEGY, "grand product: a circuit can be proven once (its layers are bound)");
+    for (size_t j = 0; j < k; j++)
+      if (circuits[j] == circuits[k]) return fail(LASSO_ERR_STRATEGY, "grand product: the same circuit twice in one batch");
+  }
+  const size_t v = circuits[0]->ci->num_layers;
+  for (size_t k = 1; k < n; k++)
+    if (circuits[k]->ci->num_layers != v) return fail(LASSO_ERR_LENGTH, "grand product: the circuits have different num_vars");
+  // per layer i < v: a sumcheck of i cubic rounds (8 + 8 + 104 i) and two vectors of n claims (2 (8 + 32 n))
+  const size_t need = 8 + v * (24 + 64 * n) + 52 * v * (v - 1);
+  if (proof_len) *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "grand product: output buffer too small");
+  if (!transcript || !r_out || !claims_out) return fail(LASSO_ERR_LENGTH, "grand product: null transcript or output");
+  std::vector<Circuit*> cs(n);
+  std::vector<fr_t> products(n);
+  for (size_t k = 0; k < n; k++) {
+    cs[k] = circuits[k]->ci.get();
+    products[k] = circuits[k]->product;
+    circuits[k]->proven = true;
+  }
+  auto t0 = std::chrono::steady_clock::now();
+  const GrandProductOut o = gp_prove(h->c, cs, products, transcript->t);
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (o.proof.size() != need) return fail(-1, "grand product: unexpected proof size");
+  memcpy(proof_out, o.proof.data(), need);
+  for (size_t j = 0; j < v; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
+  for (size_t k = 0; k < n; k++) memcpy(claims_out + 4 * k, o.claims[k].v, 32);
   return 0;
   LB_CATCH
 }

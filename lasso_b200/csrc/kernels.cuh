@@ -89,6 +89,8 @@ struct FrVec {  // small vector passed by value as a kernel parameter (challenge
 void launch_bind_top(fr_t* base, size_t stride, int npolys, size_t half, const fr_t& r, cudaStream_t st);
 // same over an array of independent device pointers (grand-product circuits)
 void launch_bind_top_ptrs(fr_t* const* d_ptrs, int npolys, size_t half, const fr_t& r, cudaStream_t st);
+// out of place: d_dst[k][i] <- Z[i] + r (Z[half + i] - Z[i]), Z = d_src[k], k < npolys (device pointer tables)
+void launch_bind_ptrs(fr_t* const* d_src, fr_t* const* d_dst, int npolys, size_t half, const fr_t& r, cudaStream_t st);
 // out[i] <- Z[2i] + r (Z[2i+1] - Z[2i]), out-of-place
 void launch_bind_bot(const fr_t* Z, fr_t* out, size_t half, const fr_t& r, cudaStream_t st);
 
@@ -133,6 +135,8 @@ bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, c
                                     const Finalize& fin, size_t min_q, cudaStream_t st);
 // value k < n: src.p[k][0] + r (src.p[k][half] - src.p[k][0]), element 0 of the last bind, published through fin
 void launch_final_comb(const CombPtrs& src, int n, size_t half, const fr_t& r, const Finalize& fin, cudaStream_t st);
+// out[i] <- g(in.p[0][i], .., in.p[n_inputs-1][i]) for i < n (g.degree is not used)
+void launch_comb_map(const CombProgram& g, const CombPtrs& in, size_t n, fr_t* out, cudaStream_t st);
 
 // ---- K3: batched cubic round evaluation (sumcheck.rs:49-93) ----
 // A, B: ncirc device pointers each to 2*half elements; Ceq: 2*half elements.  The batching coefficients of
@@ -192,6 +196,8 @@ struct TreePtrs {
 void launch_product_trees(const TreePtrs& trees, int ntrees, size_t N, int slot0, int stop_len, const Finalize& fin,
                           cudaStream_t st);
 int product_trees_launches(size_t N);
+// layer 1 of a grand-product circuit over a caller's polynomial P of 2*half elements: out[i] = P[i] * P[i + half]
+void launch_product_layer1(const fr_t* P, fr_t* out, size_t half, cudaStream_t st);
 // x_k[0] <- x_k[0] + r (x_k[1] - x_k[0]) for the n arrays x_k = d_AB[k]; results also published (Finalize)
 void launch_bind_heads(fr_t* const* d_AB, int n, const fr_t& r, const Finalize& fin, cudaStream_t st);
 // elementwise helpers for the Bulletproofs scalar folds (bullet.rs:125-130)

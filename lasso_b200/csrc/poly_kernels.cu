@@ -42,6 +42,15 @@ __global__ void __launch_bounds__(kThreads) bind_top_ptrs_kernel(fr_t* const* pt
     st_fr(Z + i, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
   }
 }
+// out of place: dst[y][i] <- bind of src[y] (grand products over a caller's polynomials, whose buffers stay untouched)
+__global__ void __launch_bounds__(kThreads) bind_ptrs_kernel(fr_t* const* src, fr_t* const* dst, size_t half, fr_t r) {
+  const fr_t* Z = src[blockIdx.y];
+  fr_t* out = dst[blockIdx.y];
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
+    fr_t lo = ld_fr_stream(Z + i), hi = ld_fr_stream(Z + half + i);
+    st_fr(out + i, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
+  }
+}
 // dense_mlpoly.rs:218-225
 __global__ void __launch_bounds__(kThreads) bind_bot_kernel(const fr_t* Z, fr_t* out, size_t half, fr_t r) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x) {
@@ -69,6 +78,14 @@ void launch_bind_top_ptrs(fr_t* const* d_ptrs, int npolys, size_t half, const fr
   if (per < kNumSMs / 4) per = kNumSMs / 4;
   dim3 grid(grid_for(half, kThreads, per), npolys);
   bind_top_ptrs_kernel<<<grid, kThreads, 0, st>>>(d_ptrs, half, r);
+  LB_LAUNCH_CHECK();
+}
+void launch_bind_ptrs(fr_t* const* d_src, fr_t* const* d_dst, int npolys, size_t half, const fr_t& r, cudaStream_t st) {
+  if (half == 0 || npolys == 0) return;
+  int per = kMaxBlocks / npolys;
+  if (per < kNumSMs / 4) per = kNumSMs / 4;
+  dim3 grid(grid_for(half, kThreads, per), npolys);
+  bind_ptrs_kernel<<<grid, kThreads, 0, st>>>(d_src, d_dst, half, r);
   LB_LAUNCH_CHECK();
 }
 void launch_bind_bot(const fr_t* Z, fr_t* out, size_t half, const fr_t& r, cudaStream_t st) {
@@ -639,6 +656,16 @@ __global__ void final_comb_kernel(const __grid_constant__ CombPtrs src, int n, s
   const fr_t lo = ld_fr(src.p[k]), hi = ld_fr(src.p[k] + half);
   finalize_publish(fin, k, fr_add(lo, fr_mul(r, fr_sub(hi, lo))));
 }
+// out[i] = g(in.p[0][i], .., in.p[k-1][i]): a polynomial formed pointwise from others, one element per thread
+__global__ void __launch_bounds__(kCustomThreads)
+    comb_map_kernel(CombProgram pg, const __grid_constant__ CombPtrs in, size_t n, fr_t* out) {
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(pg, ops, consts, slots);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
+    st_fr(out + i, custom_run(ops, pg.n_ops, consts, slots, [&](int k) { return ld_fr(in.p[k] + i); }));
+}
 
 // dynamic shared memory above the default 48 KiB needs an opt-in per kernel and device (at context creation): the
 // largest program's
@@ -653,6 +680,8 @@ void poly_init_device() {
   const int comb_bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 1);
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_bind_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
+  LB_CUDA_CHECK(cudaFuncSetAttribute(comb_map_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)custom_smem_bytes(cs, 0)));
 }
 // grid: one wave of as many CTAs as fit an SM at this shared-memory size
 static int custom_grid(size_t n, size_t smem) {
@@ -750,6 +779,11 @@ bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, c
 }
 void launch_final_comb(const CombPtrs& src, int n, size_t half, const fr_t& r, const Finalize& fin, cudaStream_t st) {
   final_comb_kernel<<<1, 32, 0, st>>>(src, n, half, r, fin);
+  LB_LAUNCH_CHECK();
+}
+void launch_comb_map(const CombProgram& g, const CombPtrs& in, size_t n, fr_t* out, cudaStream_t st) {
+  const size_t smem = custom_smem_bytes(g, 0);
+  comb_map_kernel<<<custom_grid(n, smem), kCustomThreads, smem, st>>>(g, in, n, out);
   LB_LAUNCH_CHECK();
 }
 
@@ -1328,6 +1362,15 @@ int product_trees_launches(size_t N) {
   int n = 1;
   for (size_t len = N; len > 4096; len /= 2) n++;
   return n;
+}
+// layer 1 of a caller's circuit from its polynomial P (layer 0, only read): out[i] = P[i] * P[i + half]
+__global__ void __launch_bounds__(kThreads) product_layer1_kernel(const fr_t* P, fr_t* out, size_t half) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (size_t)gridDim.x * blockDim.x)
+    st_fr(out + i, fr_mul(ld_fr(P + i), ld_fr(P + half + i)));
+}
+void launch_product_layer1(const fr_t* P, fr_t* out, size_t half, cudaStream_t st) {
+  product_layer1_kernel<<<grid_for(half), kThreads, 0, st>>>(P, out, half);
+  LB_LAUNCH_CHECK();
 }
 // last round of a batched cubic sumcheck (one element pair left per array): bind the 2*ncirc heads with r in
 // place and publish them — they are the layer's claims (grand_product.rs:139-150)

@@ -949,35 +949,6 @@ static SumcheckProof prove_arbitrary(Ctx* c, const Strategy& S, fr_t* base, size
 }
 
 // ---------------------------------------------------------------------------------------------- grand products
-// GrandProductCircuit (grand_product.rs:14-66): layer k is one contiguous array of N/2^k elements,
-// left_vec[k] = first half, right_vec[k] = second half; layer k+1[i] = layer k[i] * layer k[i + N/2^(k+1)].
-// Sharded: layers with N/2^k >= G are held as low-bit shards (local length N/(2^k G)); the layer of global
-// length G is all-gathered and the few layers above it are kept replicated on every rank.
-struct Circuit {
-  DBuf<fr_t> tree;   // local shards: layer 0 at 0 (N/G elements), layer 1 after it, ...
-  fr_t* rtree = nullptr;  // replicated top: layer k_rep (G elements), k_rep + 1, ... (2G slots in a shared allocation; G > 1)
-  size_t N = 0, num_layers = 0;
-  int G = 1;
-  size_t k_rep = 0;  // first replicated layer: N >> k_rep == G
-  bool layer_is_sharded(size_t k) const { return G == 1 || (N >> k) >= 2 * (size_t)G; }
-  size_t layer_len_global(size_t k) const { return N >> k; }
-  fr_t* layer_local(size_t k) const {  // valid for (N >> k) >= G
-    size_t off = 0, len = N / G;
-    for (size_t i = 0; i < k; i++) {
-      off += len;
-      len /= 2;
-    }
-    return tree.p + off;
-  }
-  fr_t* layer_rep(size_t k) const {  // valid for k >= k_rep (G > 1)
-    size_t off = 0, len = (size_t)G;
-    for (size_t i = k_rep; i < k; i++) {
-      off += len;
-      len /= 2;
-    }
-    return rtree + off;
-  }
-};
 static void circuit_alloc(Ctx* c, Circuit& ci, size_t N, fr_t* rtree_slot) {
   ci.N = N;
   ci.G = c->world;
@@ -1056,7 +1027,12 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
   // pointer tables: slot L (< num_layers) = the arrays of layer L, slot num_layers = the replicated tail arrays;
   // all of them are uploaded once, up front (no per-layer copy + sync)
   const size_t nslots = num_layers + 1;
-  DBuf<fr_t*> d_ptrs(c, nslots * 4 * ncirc);
+  // circuits over a caller's polynomials (all or none of a batch): layer 0 is the caller's and is only read; its first
+  // bind goes out of place into layer 1's storage, whose sumcheck is over by then.  Two more tables for that bind:
+  // src [A_0.. | B_0.. | eq] of layer 0, dst [A_0.. | B_0.. | eq'] of layer 1.
+  const bool ext = circuits[0]->ext0 != nullptr && num_layers >= 2;
+  const size_t nbind = 2 * (size_t)ncirc + 1;
+  DBuf<fr_t*> d_ptrs(c, nslots * 4 * ncirc + (ext ? 2 * nbind : 0));
   const size_t eq_cap = std::max<size_t>(circuits[0]->N / 2 / G, (size_t)G);
   DBuf<fr_t> eqbuf(c, eq_cap), eqbuf2(c, std::max<size_t>(eq_cap / 2, 1));
   DBuf<fr_t> tail(c, (size_t)(2 * ncirc + 1) * G);  // replicated remainders of A_k, B_k, C (G elements each)
@@ -1064,10 +1040,23 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
   if (ncirc > 32) throw std::runtime_error("more than 32 circuits in one batched grand product");
   std::vector<fr_t> ev(3), fin((size_t)2 * ncirc);
   // per slot: [A_0..A_{n-1} | B_0..B_{n-1} | A_0,B_0,A_1,B_1,...]
-  std::vector<fr_t*> table(nslots * 4 * ncirc);
+  std::vector<fr_t*> table(d_ptrs.n);
   auto slot_A = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc; };
   auto slot_B = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc + ncirc; };
   auto slot_AB = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc + 2 * ncirc; };
+  fr_t* const* bind_src = d_ptrs.p + nslots * 4 * ncirc;
+  fr_t* const* bind_dst = bind_src + nbind;
+  if (ext) {
+    fr_t** ts = table.data() + nslots * 4 * ncirc;
+    for (int k = 0; k < ncirc; k++) {
+      ts[k] = circuits[k]->layer_local(0);
+      ts[ncirc + k] = ts[k] + circuits[k]->N / 2;
+      ts[nbind + k] = circuits[k]->layer_local(1);
+      ts[nbind + ncirc + k] = ts[nbind + k] + circuits[k]->N / 4;
+    }
+    ts[2 * ncirc] = eqbuf.p;  // the first bind of a layer reads eq from eqbuf and writes eqbuf2
+    ts[nbind + 2 * ncirc] = eqbuf2.p;
+  }
   auto layer_cur = [&](size_t layer_id, bool& replicated_layer) {
     const size_t len_g = circuits[0]->layer_len_global(layer_id);
     replicated_layer = G > 1 && !circuits[0]->layer_is_sharded(layer_id);
@@ -1119,6 +1108,7 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
     fr_t* Ccur = eqbuf.p;
     fr_t* Cnext = eqbuf2.p;
     bool have_evals = false, heads_published = false;
+    bool on_caller = ext && layer_id == 0;  // dA, dB still point at the caller's buffers: nothing may write them
     Finalize fz = c->fin_begin();
     for (;;) {
       if (sharded && cur == 1) {  // all-gather the G-element remainders; the tail rounds run replicated
@@ -1164,7 +1154,24 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
       fr_t r_j = transcript.challenge_scalar("challenge_nextround");
       rand_prod.push_back(r_j);
       auto tp2 = std::chrono::steady_clock::now();
-      if (half > 1) {
+      if (on_caller) {
+        // bind A_k, B_k (and eq, unless this is the last round) out of place into layer 1's storage, unscaled; then
+        // evaluate the next round there, or read the heads with pack_heads below
+        launch_bind_ptrs(bind_src, bind_dst, half > 1 ? (int)nbind : 2 * ncirc, half, r_j, c->st);
+        dA = slot_A(1);
+        dB = slot_B(1);
+        dAB = slot_AB(1);
+        on_caller = false;
+        have_evals = false;
+        g_launches += 1;
+        if (half > 1) {
+          std::swap(Ccur, Cnext);
+          fz = c->fin_begin();
+          launch_sumcheck_eval_cubic_comb(dA, dB, Ccur, ncirc, half / 2, cf, 1, fz, c->st);
+          g_launches += 1;
+          have_evals = true;
+        }
+      } else if (half > 1) {
         // bind with r_j and evaluate the next round in one pass (sumcheck.rs:116-120 + 63-89)
         fz = c->fin_begin(sharded);
         launch_sumcheck_bind_eval_cubic_comb(dA, dB, Ccur, Cnext, ncirc, half, r_j, cf, stored_scaled ? 0 : 1, fz, c->st);
@@ -1229,6 +1236,43 @@ static void ser_gpa(ByteWriter& w, const GPAProof& p) {
     w.vec_fr(l.claims_prod_left);
     w.vec_fr(l.claims_prod_right);
   }
+}
+
+// A caller's circuit: layer 1 from the caller's buffer, then the library's tree from N/2 down.  N = 2: the top layer is
+// the caller's two elements.  Launches: 1 + product_trees_launches(N/2), or the one read-back for N = 2.
+Circuit* gp_circuit_create(Ctx* c, const Poly& p, fr_t* product) {
+  std::unique_ptr<Circuit> ci(new Circuit());
+  ci->N = p.len;
+  ci->num_layers = p.nv;
+  ci->ext0 = p.d_fr.p;
+  fr_t top[2];
+  if (p.len == 2) {
+    c->d2h(top, p.d_fr.p, sizeof top);
+  } else {
+    ci->tree.alloc(c, p.len - 2);
+    launch_product_layer1(p.d_fr.p, ci->tree.p, p.len / 2, c->st);
+    TreePtrs tp{};
+    tp.p[0] = ci->tree.p;
+    const Finalize f = c->fin_begin();
+    launch_product_trees(tp, 1, p.len / 2, 0, 2, f, c->st);
+    g_launches += 1 + product_trees_launches(p.len / 2);
+    c->fin_wait(f, top, 2);
+  }
+  *product = fr_mul(top[0], top[1]);
+  return ci.release();
+}
+GrandProductOut gp_prove(Ctx* c, std::vector<Circuit*>& circuits, const std::vector<fr_t>& products, Transcript& transcript) {
+  GrandProductOut out;
+  const GPAProof p = prove_gpa(c, circuits, products, transcript, out.r);
+  ByteWriter w;
+  ser_gpa(w, p);
+  out.proof = std::move(w.b);
+  // claims_to_verify after the last layer (grand_product.rs:189-195): rand[0] is that layer's r_layer
+  const LayerProof& last = p.back();
+  for (size_t k = 0; k < circuits.size(); k++)
+    out.claims.push_back(fr_add(last.claims_prod_left[k],
+                                fr_mul(out.r[0], fr_sub(last.claims_prod_right[k], last.claims_prod_left[k]))));
+  return out;
 }
 
 // ---------------------------------------------------------------------------------------------- openings
@@ -1819,6 +1863,36 @@ Poly* poly_create_eq(Ctx* c, const std::vector<fr_t>& r) {
 }
 
 // ---------------------------------------------------------------------------------------------- caller sumchecks
+// A combining function on the device: its constants (32-byte aligned) then its instructions, one upload
+struct CombDev {
+  DBuf<uint8_t> prog;
+  CombProgram pg;
+};
+static void comb_upload(Ctx* c, const Comb& g, CombDev& d) {
+  const size_t cbytes = g.consts.size() * sizeof(fr_t), ibytes = g.ins.size() * sizeof(CustomIns);
+  std::vector<uint8_t> staged(cbytes + ibytes);
+  if (cbytes) memcpy(staged.data(), g.consts.data(), cbytes);
+  memcpy(staged.data() + cbytes, g.ins.data(), ibytes);
+  d.prog.alloc(c, staged.size());
+  LB_CUDA_CHECK(cudaMemcpyAsync(d.prog.p, staged.data(), staged.size(), cudaMemcpyHostToDevice, c->st));
+  d.pg = CombProgram{g.n_inputs, g.degree, (int)g.ins.size(), (int)g.consts.size(), g.n_slots,
+                     reinterpret_cast<const CustomIns*>(d.prog.p + cbytes), reinterpret_cast<const fr_t*>(d.prog.p)};
+}
+Poly* poly_create_comb(Ctx* c, const Comb& g, const Poly* const* polys, int k) {
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->nv = polys[0]->nv;
+  p->len = polys[0]->len;
+  p->bits = 253;  // committed through the Fr windows, as an eq polynomial
+  p->d_fr.alloc(c, p->len);
+  CombDev dev;
+  comb_upload(c, g, dev);
+  CombPtrs in{};
+  for (int j = 0; j < k; j++) in.p[j] = polys[j]->d_fr.p;
+  launch_comb_map(dev.pg, in, p->len, p->d_fr.p, c->st);
+  g_launches += 1;
+  return p.release();
+}
 // prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first evaluates the
 // caller's buffers; each later one binds the previous challenge and evaluates, fused from q = 2^15 pairs up, else a
 // bind and an evaluation) and one kernel that binds the last challenge into element 0 of every input and publishes the
@@ -1830,15 +1904,9 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
   // every allocation before the first transcript write: a failure leaves the caller's transcript as it was
   DBuf<fr_t> ws;
   if (num_rounds >= 2) ws.alloc(c, (size_t)k << (nv - 1));
-  // the program, one upload: constants (32-byte aligned) then instructions
-  const size_t cbytes = g.consts.size() * sizeof(fr_t), ibytes = g.ins.size() * sizeof(CustomIns);
-  std::vector<uint8_t> staged(cbytes + ibytes);
-  if (cbytes) memcpy(staged.data(), g.consts.data(), cbytes);
-  memcpy(staged.data() + cbytes, g.ins.data(), ibytes);
-  DBuf<uint8_t> prog(c, staged.size());
-  LB_CUDA_CHECK(cudaMemcpyAsync(prog.p, staged.data(), staged.size(), cudaMemcpyHostToDevice, c->st));
-  const CombProgram pg{g.n_inputs, g.degree, (int)g.ins.size(), (int)g.consts.size(), g.n_slots,
-                       reinterpret_cast<const CustomIns*>(prog.p + cbytes), reinterpret_cast<const fr_t*>(prog.p)};
+  CombDev dev;
+  comb_upload(c, g, dev);
+  const CombProgram& pg = dev.pg;
   CombPtrs src{}, dst{};
   for (int j = 0; j < k; j++) {
     src.p[j] = polys[j]->d_fr.p;

@@ -243,6 +243,40 @@ struct Poly {
   DBuf<uint32_t> d_u32;  // the same values as integers when bits <= 32 (commit_u32 / bound_u32), else empty
 };
 
+// GrandProductCircuit (grand_product.rs:14-66): layer k is one contiguous array of N/2^k elements,
+// left_vec[k] = first half, right_vec[k] = second half; layer k+1[i] = layer k[i] * layer k[i + N/2^(k+1)].
+// Sharded: layers with N/2^k >= G are held as low-bit shards (local length N/(2^k G)); the layer of global
+// length G is all-gathered and the few layers above it are kept replicated on every rank.
+// A caller's circuit (single GPU) has an external layer 0, the caller's polynomial, which is only read: `tree` holds
+// layers 1.. (N - 2 elements), and the prover binds layer 0 out of place into layer 1's storage.
+struct Circuit {
+  DBuf<fr_t> tree;   // local shards: layer 0 at 0 (N/G elements), layer 1 after it, ...  (ext0: layer 1 at 0)
+  fr_t* ext0 = nullptr;   // layer 0 when it is a caller's buffer, else null
+  fr_t* rtree = nullptr;  // replicated top: layer k_rep (G elements), k_rep + 1, ... (2G slots in a shared allocation; G > 1)
+  size_t N = 0, num_layers = 0;
+  int G = 1;
+  size_t k_rep = 0;  // first replicated layer: N >> k_rep == G
+  bool layer_is_sharded(size_t k) const { return G == 1 || (N >> k) >= 2 * (size_t)G; }
+  size_t layer_len_global(size_t k) const { return N >> k; }
+  fr_t* layer_local(size_t k) const {  // valid for (N >> k) >= G
+    if (ext0 && k == 0) return ext0;
+    size_t off = 0, len = N / G;
+    for (size_t i = 0; i < k; i++) {
+      off += len;
+      len /= 2;
+    }
+    return tree.p + (ext0 ? off - N : off);  // ext0: layer 0 is not stored
+  }
+  fr_t* layer_rep(size_t k) const {  // valid for k >= k_rep (G > 1)
+    size_t off = 0, len = (size_t)G;
+    for (size_t i = k_rep; i < k; i++) {
+      off += len;
+      len /= 2;
+    }
+    return rtree + off;
+  }
+};
+
 // ark-serialize (compressed) writer
 struct ByteWriter {
   std::vector<uint8_t> b;
@@ -329,6 +363,21 @@ struct SumcheckOut {
 // 1 <= num_rounds <= num_vars (the caller checks).  The polynomials are not modified: the first bind writes into a
 // workspace of k x 2^(num_vars-1) elements, allocated before the transcript is touched.
 SumcheckOut sumcheck_prove(Ctx*, const Comb& g, const Poly* const* polys, int k, size_t num_rounds, Transcript&);
+// Q(x) = g(polys[0](x), .., polys[k-1](x)) at every point, k == g.n_inputs, all of one num_vars (the caller checks): a
+// full-width polynomial like poly_create_eq
+Poly* poly_create_comb(Ctx*, const Comb& g, const Poly* const* polys, int k);
+
+// grand products over a caller's polynomials (single GPU)
+// GrandProductCircuit::new (grand_product.rs:38-58) with p as layer 0 (p.nv >= 1; p is only read and must outlive the
+// circuit); *product receives evaluate() (grand_product.rs:60-65)
+Circuit* gp_circuit_create(Ctx*, const Poly& p, fr_t* product);
+struct GrandProductOut {
+  std::vector<uint8_t> proof;   // ark-serialize (compressed) BatchedGrandProductArgument
+  std::vector<fr_t> r, claims;  // rand and the final claims_to_verify (P_k(rand))
+};
+// BatchedGrandProductArgument::prove (grand_product.rs:100-201) on the caller's transcript; products[k] = evaluate() of
+// circuits[k], all of one num_vars, at most 32.  The stored layers are bound in place, so a circuit is proven once.
+GrandProductOut gp_prove(Ctx*, std::vector<Circuit*>& circuits, const std::vector<fr_t>& products, Transcript&);
 
 // comm.cu
 void comm_unique_id(uint8_t out[128]);

@@ -322,5 +322,84 @@ int orcd_sumcheck_verify(const uint8_t* bytes, size_t n, const uint64_t* claim, 
   for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
   return 0;
 }
+// out[i] = g(polys[0][i], .., polys[k-1][i]) (k x len Montgomery elements, row-major), the program interpreted on the host
+void orcd_comb_map(const uint64_t* polys, size_t k, size_t len, const int32_t* prog, size_t n_ops, const uint64_t* K, size_t n_k,
+                   uint64_t* out) {
+  const Program g{k, std::vector<int32_t>(prog, prog + 3 * n_ops), ldvec(K, n_k)};
+  std::vector<Fr> vals(k);
+  for (size_t i = 0; i < len; i++) {
+    for (size_t j = 0; j < k; j++) vals[j] = ldfr(polys + 4 * (j * len + i));
+    stfr(out + 4 * i, g(vals.data()));
+  }
+}
+
+// ---- GrandProductCircuit / BatchedGrandProductArgument (subprotocols/grand_product.rs)
+// GrandProductCircuit::new over each of n polynomials (n x len Montgomery elements, row-major, len >= 2), then
+// BatchedGrandProductArgument::prove on a caller's transcript (the products are not appended to it: the caller's
+// protocol does that).  out: the serialised proof (returns its length, 0 on error); products_out: n evaluate() values;
+// rand_out: log2(len) values; claims_out: n final claims_to_verify.
+size_t orcd_gp_prove(const uint64_t* polys, size_t n, size_t len, void* transcript, uint8_t* out, size_t cap,
+                     uint64_t* products_out, uint64_t* rand_out, uint64_t* claims_out) {
+  try {
+    std::vector<GrandProductCircuit> cs;
+    for (size_t k = 0; k < n; k++) cs.emplace_back(DensePolynomial(ldvec(polys + 4 * len * k, len)));
+    std::vector<GrandProductCircuit*> ptrs;
+    for (size_t k = 0; k < n; k++) {
+      stfr(products_out + 4 * k, cs[k].evaluate());
+      ptrs.push_back(&cs[k]);
+    }
+    std::vector<Fr> rand;
+    const BatchedGrandProductArgument p = BatchedGrandProductArgument::prove(ptrs, *(Transcript*)transcript, rand);
+    ByteWriter w;
+    ser(w, p);
+    if (w.b.size() > cap) return 0;
+    memcpy(out, w.b.data(), w.b.size());
+    for (size_t j = 0; j < rand.size(); j++) stfr(rand_out + 4 * j, rand[j]);
+    const LayerProofBatched& last = p.proof.back();  // grand_product.rs:189-195, rand[0] = the last r_layer
+    for (size_t k = 0; k < n; k++)
+      stfr(claims_out + 4 * k, last.claims_prod_left[k] + rand[0] * (last.claims_prod_right[k] - last.claims_prod_left[k]));
+    return w.b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_gp_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// BatchedGrandProductArgument::verify (grand_product.rs:203-261) of serialised bytes against n products of circuits of
+// num_vars variables: 0 accepted (claims_out = the n final claims, rand_out = num_vars values), 1 rejected, 2 the bytes
+// do not parse
+int orcd_gp_verify(const uint8_t* bytes, size_t nbytes, const uint64_t* products, size_t n, size_t num_vars, void* transcript,
+                   uint64_t* claims_out, uint64_t* rand_out) {
+  Reader rd{bytes, nbytes};
+  BatchedGrandProductArgument p;
+  auto frs = [&]() {
+    const uint64_t m = rd.u64();
+    std::vector<Fr> v;
+    if (m > (nbytes - rd.at) / 32) rd.ok = false;
+    for (uint64_t i = 0; rd.ok && i < m; i++) v.push_back(rd.fr());
+    return v;
+  };
+  const uint64_t layers = rd.u64();
+  if (layers > nbytes) rd.ok = false;
+  for (uint64_t l = 0; rd.ok && l < layers; l++) {
+    LayerProofBatched lp;
+    const uint64_t rounds = rd.u64();
+    if (rounds > nbytes) rd.ok = false;
+    for (uint64_t j = 0; rd.ok && j < rounds; j++) {
+      CompressedUniPoly c;
+      c.coeffs_except_linear_term = frs();
+      if (c.coeffs_except_linear_term.empty()) rd.ok = false;
+      lp.proof.compressed_polys.push_back(c);
+    }
+    lp.claims_prod_left = frs();
+    lp.claims_prod_right = frs();
+    p.proof.push_back(std::move(lp));
+  }
+  if (!rd.ok || rd.at != nbytes) return 2;
+  std::vector<Fr> claims, rand;
+  if (!p.verify(ldvec(products, n), pow2(num_vars), *(Transcript*)transcript, claims, rand)) return 1;
+  for (size_t k = 0; k < n; k++) stfr(claims_out + 4 * k, claims[k]);
+  for (size_t j = 0; j < rand.size(); j++) stfr(rand_out + 4 * j, rand[j]);
+  return 0;
+}
 
 }  // extern "C"
