@@ -94,7 +94,11 @@ void launch_bind_ptrs(fr_t* const* d_src, fr_t* const* d_dst, int npolys, size_t
 // out[i] <- Z[2i] + r (Z[2i+1] - Z[2i]), out-of-place
 void launch_bind_bot(const fr_t* Z, fr_t* out, size_t half, const fr_t& r, cudaStream_t st);
 
-// ---- K4: eq evals (eq_poly.rs:21-38); scratch needs 2 * 4096 elements when ell > 12 ----
+// ---- K4: eq evals (eq_poly.rs:21-38) ----
+// ell <= 11: no scratch.  12..22: the two factor tables, 2 * 4096 elements.  23..28: the low table (4096 elements) and
+// the staged high table (2^(ell - 11) elements) after it, 4096 + 2^17 at ell = 28; kEqScratchElems covers every ell <= 28
+// with 4096 elements to spare.
+static constexpr size_t kEqScratchElems = 4096 + ((size_t)1 << 17) + 4096;
 void launch_eq_evals(const FrVec& r, int ell, fr_t* out, fr_t* scratch, cudaStream_t st);
 
 // ---- K2: primary sumcheck round evaluation (sumcheck.rs:179-237) ----

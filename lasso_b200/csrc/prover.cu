@@ -220,7 +220,7 @@ Ctx* ctx_create(int device) {
   LB_CUDA_CHECK(cudaMalloc((void**)&c->d_partial, c->partial_elems * sizeof(fr_t)));
   c->small_elems = 65536;
   LB_CUDA_CHECK(cudaMalloc((void**)&c->d_small, c->small_elems * sizeof(fr_t)));
-  LB_CUDA_CHECK(cudaMalloc((void**)&c->d_eq_scratch, (size_t)(4096 + (1 << 17) + 4096) * sizeof(fr_t)));
+  LB_CUDA_CHECK(cudaMalloc((void**)&c->d_eq_scratch, kEqScratchElems * sizeof(fr_t)));
   LB_CUDA_CHECK(cudaMalloc((void**)&c->d_flag, 64));
   LB_CUDA_CHECK(cudaMemset(c->d_flag, 0, 64));
   LB_CUDA_CHECK(cudaHostAlloc((void**)&c->h_mapped, Ctx::kMappedBytes, cudaHostAllocMapped));

@@ -1,75 +1,21 @@
-// Test harness: one extern "C" wrapper per launcher of kernels.cuh / msm.cuh that the C ABI does not expose on its own.
-// Linked from the library's own kernel objects (lasso_b200/_build/poly_kernels.o, msm_kernels.o, msm_large.o,
-// msm_final.o), so the tests run
-// exactly the code the prover runs.  Every wrapper copies its host inputs to the device, calls ONE launcher on a stream
+// Test harness: one extern "C" wrapper per launcher of kernels.cuh / msm.cuh that the C ABI does not expose on its own
+// (the combining-function, layer-0, ingest and eq launchers are in harness_comb.cu).
+// Linked from the library's own kernel objects (lasso_b200/_build/poly_kernels.o, dense_poly_kernels.o, msm_kernels.o,
+// msm_large.o, msm_final.o), so the tests run exactly the code the prover runs.  Every wrapper copies its host inputs to the device, calls ONE launcher on a stream
 // of its own, synchronises, copies every output (in-place arrays included) back and frees what it allocated.  Field
 // elements are 4 x u64 Montgomery limbs (the fr_t layout), points arkworks affine (x, y) Montgomery limbs.
 // Return codes: see harness_common.cuh.
 #include <cstring>
 
-#include "../../lasso_b200/csrc/pub_codec.hpp"
 #include "harness_common.cuh"
 
 using namespace lb;
-using kh::guarded;
-using kh::HarnessError;
-using kh::Scope;
 using kh::ck;
-
-namespace {
-
-// one publication region in mapped pinned host memory (as the prover's Ctx), tag 1
-struct Pub {
-  unsigned long long* h = nullptr;
-  PubDst dst = {};
-  static constexpr uint32_t kTag = 1;
-  explicit Pub(Scope& s) {
-    const size_t bytes = (size_t)kPubElems * kPubSlotWords * 8;
-    ck(cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped));
-    s.host.push_back(h);
-    memset(h, 0, bytes);
-    unsigned long long* d = nullptr;
-    ck(cudaHostGetDevicePointer((void**)&d, h, 0));
-    dst.dst[0] = d;
-    dst.ndst = 1;
-    dst.tag = kTag;
-  }
-  // elements [v0, v0 + count) -> out (4 x u64 each); every word must carry the tag
-  void decode(int v0, int count, uint64_t* out) const {
-    for (int v = v0; v < v0 + count; v++) {
-      unsigned long long w[5];
-      for (int k = 0; k < 5; k++) {
-        const unsigned long long word = h[(size_t)v * kPubSlotWords + k];
-        if (pub_tag_of(word) != kTag) throw HarnessError{-3};
-        w[k] = word & kPubValueMask;
-      }
-      uint32_t x[8];
-      pub_decode(w, x);
-      memcpy(out + 4 * (size_t)(v - v0), x, 32);
-    }
-  }
-  // elements [v0, v0 + count) must not have been written
-  void expect_empty(int v0, int count) const {
-    for (size_t i = (size_t)v0 * kPubSlotWords; i < (size_t)(v0 + count) * kPubSlotWords; i++)
-      if (h[i] != 0) throw HarnessError{-3};
-  }
-};
-
-Finalize make_fin(Scope& s, const Pub& p, size_t partial_elems) {
-  Finalize f;
-  f.partial = s.alloc<fr_t>(partial_elems);
-  f.counter = s.alloc<unsigned>(1);
-  f.pub = p.dst;
-  return f;
-}
-
-fr_t fr_of(const uint64_t* x) {
-  fr_t r;
-  memcpy(r.v, x, 32);
-  return r;
-}
-
-}  // namespace
+using kh::fr_of;
+using kh::guarded;
+using kh::make_fin;
+using kh::Pub;
+using kh::Scope;
 
 // ---------------------------------------------------------------- window + digit-multiples tables of a generator set
 // Built once per test module with the library's launchers (launch_build_table, launch_build_multiples, optionally

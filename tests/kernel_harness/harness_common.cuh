@@ -1,12 +1,14 @@
-// Test harness plumbing shared by its translation units (harness.cu, arith.cu): error codes, the per-call device
-// allocation scope, and the wrapper that turns exceptions into return codes.
+// Test harness plumbing shared by its translation units (harness.cu, harness_comb.cu, arith.cu, harness_fr.cu): error
+// codes, the per-call device allocation scope, the publication region of the launchers that publish, and the wrapper
+// that turns exceptions into return codes.
 // Return codes: 0 ok, -1 a launcher threw (std::runtime_error), -2 a CUDA error, -3 a publication slot did not carry
-// the message's tag, -4 bad arguments.
+// the message's tag, -4 bad arguments, -5 a repeated launch published different values (harness_comb.cu).
 #pragma once
 #include <cuda_runtime.h>
 
 #include <cstdint>
 #include <cstdio>
+#include <cstring>
 #include <stdexcept>
 #include <vector>
 
@@ -66,6 +68,58 @@ struct Scope {
     ck(cudaGetLastError());
   }
 };
+
+// one publication region in mapped pinned host memory (as the prover's Ctx); messages carry tag 1 unless set_tag
+struct Pub {
+  unsigned long long* h = nullptr;
+  lb::PubDst dst = {};
+  explicit Pub(Scope& s) {
+    const size_t bytes = (size_t)lb::kPubElems * lb::kPubSlotWords * 8;
+    ck(cudaHostAlloc((void**)&h, bytes, cudaHostAllocMapped));
+    s.host.push_back(h);
+    memset(h, 0, bytes);
+    unsigned long long* d = nullptr;
+    ck(cudaHostGetDevicePointer((void**)&d, h, 0));
+    dst.dst[0] = d;
+    dst.ndst = 1;
+    dst.tag = 1;
+  }
+  // the next launch publishes with this tag (a Finalize copied before the call keeps the old one)
+  void set_tag(uint32_t tag) { dst.tag = tag; }
+  // elements [v0, v0 + count) -> out (4 x u64 each); every word must carry the current tag
+  void decode(int v0, int count, uint64_t* out) const {
+    for (int v = v0; v < v0 + count; v++) {
+      unsigned long long w[5];
+      for (int k = 0; k < 5; k++) {
+        const unsigned long long word = h[(size_t)v * lb::kPubSlotWords + k];
+        if (lb::pub_tag_of(word) != dst.tag) throw HarnessError{-3};
+        w[k] = word & lb::kPubValueMask;
+      }
+      uint32_t x[8];
+      lb::pub_decode(w, x);
+      memcpy(out + 4 * (size_t)(v - v0), x, 32);
+    }
+  }
+  // elements [v0, v0 + count) must not have been written
+  void expect_empty(int v0, int count) const {
+    for (size_t i = (size_t)v0 * lb::kPubSlotWords; i < (size_t)(v0 + count) * lb::kPubSlotWords; i++)
+      if (h[i] != 0) throw HarnessError{-3};
+  }
+};
+
+inline lb::Finalize make_fin(Scope& s, const Pub& p, size_t partial_elems) {
+  lb::Finalize f;
+  f.partial = s.alloc<lb::fr_t>(partial_elems);
+  f.counter = s.alloc<unsigned>(1);
+  f.pub = p.dst;
+  return f;
+}
+
+inline lb::fr_t fr_of(const uint64_t* x) {
+  lb::fr_t r;
+  memcpy(r.v, x, 32);
+  return r;
+}
 
 inline bool g_inited = false;
 inline void init() {

@@ -36,6 +36,17 @@ def lib():
         L.kh_bullet_fused.argtypes = [V, V, V, V, S, S, I, V, V, V, V, V, V, V, V]
         L.kh_msm_rows_direct_u32.argtypes = [V, V, I, I, I, I, I, I, V]
         L.kh_msm_large.argtypes = [V, S, V, S, I, V, V, V]
+        L.kh_comb_program.argtypes = [I, V, I, V, I, I, V, V]
+        L.kh_comb_eval.argtypes = [I, V, I, V, I, I, V, V, S, I, V]
+        L.kh_comb_bind_eval.argtypes = [I, V, I, V, I, I, V, V, S, V, S, I, I, V, V, V]
+        L.kh_bind_comb.argtypes = [I, V, V, S, V, I, V]
+        L.kh_final_comb.argtypes = [I, V, S, V, I, V]
+        L.kh_comb_map.argtypes = [I, V, I, V, I, I, V, V, S, V, S]
+        L.kh_product_layer1.argtypes = [V, S, V, S]
+        L.kh_bind_ptrs.argtypes = [I, V, V, S, V, V]
+        L.kh_poly_ingest.argtypes = [V, S, S, V, V]
+        L.kh_poly_mirror_u32.argtypes = [V, S, V]
+        L.kh_eq_evals.argtypes = [I, V, V, S, V, V]
         L.kh_arith.argtypes = [I, I, S, V, V, V, V]
         L.kh_arith_op_name.argtypes = [I]
         L.kh_arith_op_name.restype = C.c_char_p
@@ -46,7 +57,8 @@ def lib():
 def call(name, *args):
     """call a wrapper; a non-zero return code is a failure of the launch under test"""
     rc = getattr(lib(), name)(*args)
-    assert rc == 0, "%s returned %d (-1: the launcher threw, -2: CUDA error, -3: publication tag missing)" % (name, rc)
+    assert rc == 0, ("%s returned %d (-1: the launcher threw, -2: CUDA error, -3: publication tag missing, -4: bad "
+                     "arguments, -5: a repeated launch published different values)" % (name, rc))
 
 
 def op_ids(name_fn):
