@@ -316,6 +316,44 @@ int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*,
  * variable: 2^r_len evaluations, r_len <= 28 (LASSO_ERR_LENGTH), each coordinate a canonical residue (LASSO_ERR_VALUE). */
 int lasso_poly_create_eq(lasso_ctx*, const uint64_t* r, size_t r_len, lasso_poly** out);
 
+/* ---------------------------------------------------------------- many polynomials per call
+ *
+ * DensePolynomial::merge (poly/dense_mlpoly.rs:251-261): a new polynomial holding the evaluations of polys[0..n_polys) one
+ * after another, zero-padded to the next power of two.  Inputs may have different num_vars and may repeat; they are not
+ * modified, and the result owns its own copy, so they may be destroyed afterwards.  It has a u32 mirror (is committed and
+ * opened through the 16-bit tables) iff every input has one, i.e. iff every value is an integer below 2^32.  Copies only:
+ * no kernel is launched.  Errors, before any copy: LASSO_ERR_LENGTH for n_polys == 0, a null array or output, or more
+ * than 2^28 evaluations after padding; LASSO_ERR_STRATEGY for a polynomial of another context or a sharded context. */
+int lasso_poly_create_merge(lasso_ctx*, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out);
+/* DensePolynomial::evaluate (poly/dense_mlpoly.rs:229-235) of n_polys polynomials of one num_vars at one point r: out
+ * receives n_polys x 4 limbs, P_j(r) at out + 4 j.  One eq table serves every polynomial, and the dot kernel reads each of
+ * its elements once per group of 8 inputs.  1 <= n_polys <= 64: the inputs travel as one kernel parameter of 64 pointers,
+ * and the per-input block partials of one launch fill at most 8 x 528 elements of the context's scratch.  Integer and
+ * full-width polynomials may be mixed.  Errors, before any launch: LASSO_ERR_LENGTH for different num_vars,
+ * r_len != num_vars, n_polys outside 1..64, or a null array or output; LASSO_ERR_VALUE for a non-canonical coordinate;
+ * LASSO_ERR_STRATEGY for a polynomial of another context or a sharded context. */
+int lasso_poly_evaluate_batch(lasso_ctx*, const lasso_poly* const* polys, size_t n_polys, const uint64_t* r, size_t r_len,
+                              uint64_t* out);
+/* CombinedTableEvalProof::prove (subtables/mod.rs:229-313) without blinds: opens the merged polynomial `combined` at r for
+ * the n_evals claims `evals` with ONE PolyEvalProof.  The protocol name "Lasso CombinedTableEvalProof" is appended, evals
+ * are zero-padded to a power of two and appended as "evals_ops_val", log2 of that many challenges are drawn
+ * ("challenge_combine_n_to_one"), the padded evals are folded with them (bound_poly_var_bot, last challenge first) into
+ * "joint_claim_eval", and the polynomial is opened at (challenges || r).  proof_out receives the ark-serialize
+ * (compressed) CombinedTableEvalProof, which is its PolyEvalProof alone: the size lasso_poly_eval_prove gives at
+ * combined's num_vars (*proof_len receives it, also when proof_cap is too small).  The transcript and the tape advance in
+ * place.
+ * As in the reference, evals are the caller's claims and are not checked: a wrong one gives a proof the verifier rejects.
+ * For combined = lasso_poly_create_merge(P_0..P_{k-1}) the claim evals[i] = P_i(r) is about block i of combined only when
+ * every P_i has num_vars == r_len (equal sizes); with unequal sizes block i is not component i.
+ * Errors, each returned before any launch and before the transcript or the tape is touched: LASSO_ERR_LENGTH for
+ * num_vars != r_len + log2(next_pow2(n_evals)), n_evals == 0, a too small proof_cap, or a null transcript, tape, evals or
+ * output; LASSO_ERR_GENS for generators whose R differs from the polynomial's; LASSO_ERR_VALUE for a non-canonical eval or
+ * coordinate; LASSO_ERR_STRATEGY for another context or a sharded context.  The opening's working memory is reserved in
+ * the context's memory pool before the first transcript write. */
+int lasso_combined_eval_prove(lasso_ctx*, const lasso_poly* combined, const lasso_poly_gens*, const uint64_t* evals,
+                              size_t n_evals, const uint64_t* r, size_t r_len, lasso_transcript*, lasso_random_tape*,
+                              uint8_t* proof_out, size_t proof_cap, size_t* proof_len);
+
 /* ---------------------------------------------------------------- sumchecks over a caller's polynomials
  *
  * A combining function g(x_0..x_{n_inputs-1}) in the program format of lasso_strategy_create (slots 0..n_inputs-1 are

@@ -129,6 +129,15 @@ extern "C" {
                                  random_tape: *mut lasso_random_tape, proof_out: *mut u8, proof_cap: usize,
                                  proof_len: *mut usize, c_zr_out: *mut u8) -> c_int;
     pub fn lasso_poly_create_eq(ctx: *mut lasso_ctx, r: *const u64, r_len: usize, out: *mut *mut lasso_poly) -> c_int;
+    // many polynomials per call (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_poly_create_merge(ctx: *mut lasso_ctx, polys: *const *const lasso_poly, n_polys: usize,
+                                   out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_evaluate_batch(ctx: *mut lasso_ctx, polys: *const *const lasso_poly, n_polys: usize, r: *const u64,
+                                     r_len: usize, out: *mut u64) -> c_int;
+    pub fn lasso_combined_eval_prove(ctx: *mut lasso_ctx, combined: *const lasso_poly, gens: *const lasso_poly_gens,
+                                     evals: *const u64, n_evals: usize, r: *const u64, r_len: usize,
+                                     transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
+                                     proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize) -> c_int;
     // sumchecks over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
     pub fn lasso_comb_create(n_inputs: c_int, program: *const i32, n_ops: c_int, constants: *const u64, n_constants: c_int,
                              degree: c_int, out: *mut *mut lasso_comb) -> c_int;

@@ -14,6 +14,9 @@ and, for a caller that composes Lasso into a larger protocol, its own dense poly
     DensePolynomial(ctx, Z).commit(gens) / .evaluate(r)                  src/poly/dense_mlpoly.rs:152, 229
     PolyEvalProof.prove(ctx, poly, r, Zr, gens, transcript, random_tape)    src/poly/dense_mlpoly.rs:301
     DensePolynomial.eq(ctx, r)                                           src/poly/eq_poly.rs:21
+    DensePolynomial.merge(ctx, polys)                                    src/poly/dense_mlpoly.rs:251
+    DensePolynomial.evaluate_batch(ctx, polys, r)                        (DensePolynomial::evaluate of many, one eq table)
+    CombinedTableEvalProof.prove(ctx, combined, evals, r, gens, transcript, random_tape)   src/subtables/mod.rs:284
     SumcheckInstanceProof.prove_arbitrary(ctx, polys, Comb(fn, k), transcript)   src/subprotocols/sumcheck.rs:149
     DensePolynomial.from_comb(ctx, comb, polys)                          (pointwise g(P_0, .., P_{k-1}))
     GrandProductCircuit(ctx, poly).evaluate()                            src/subprotocols/grand_product.rs:38, 60
@@ -24,7 +27,7 @@ importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    BatchedGrandProductArgument, Comb, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
+    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
     RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, SumcheckInstanceProof, Transcript,
     bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,

@@ -780,6 +780,15 @@ def _poly_source(Z):
     return "host", np.ascontiguousarray(a), 4
 
 
+def _poly_handles(polys):
+    """a C array of the lasso_poly handles of DensePolynomials (at least one slot)"""
+    polys = list(polys)
+    arr = (C.c_void_p * max(len(polys), 1))()
+    for i, p in enumerate(polys):
+        arr[i] = p._h.value
+    return arr
+
+
 class DensePolynomial:
     """DensePolynomial<Fr> (src/poly/dense_mlpoly.rs:13-235), resident on ctx's GPU.  Z: the 2^num_vars evaluations as
     an (n, 4) uint64 numpy array of Montgomery limbs, or a torch CUDA tensor (int64 or uint64, limbs contiguous, any row
@@ -825,6 +834,26 @@ class DensePolynomial:
         _chk(lib().lasso_poly_create_comb(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.byref(h)))
         return cls._wrap(ctx, h)
 
+    @classmethod
+    def merge(cls, ctx, polys):
+        """DensePolynomial::merge (src/poly/dense_mlpoly.rs:251-261): the evaluations of polys one after another,
+        zero-padded to a power of two, as a new polynomial with its own copy (the inputs are unchanged and may be
+        dropped).  Integer-valued iff every input is."""
+        polys = list(polys)
+        h = C.c_void_p()
+        _chk(lib().lasso_poly_create_merge(ctx._h, _poly_handles(polys), C.c_size_t(len(polys)), C.byref(h)))
+        return cls._wrap(ctx, h)
+
+    @staticmethod
+    def evaluate_batch(ctx, polys, r):
+        """P_j(r) for 1..64 DensePolynomials of one num_vars, over one eq table -> (n, 4) uint64 Montgomery limbs"""
+        polys = list(polys)
+        arr = _poly_handles(polys)
+        r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+        out = np.zeros((max(len(polys), 1), 4), dtype=np.uint64)
+        _chk(lib().lasso_poly_evaluate_batch(ctx._h, arr, C.c_size_t(len(polys)), _p(r), C.c_size_t(r.shape[0]), _p(out)))
+        return out[: len(polys)]
+
     def commit(self, gens):
         """DensePolynomial::commit without blinds -> the ark-serialize bytes of PolyCommitment"""
         cap = 8 + 32 * (1 << (self.num_vars // 2))
@@ -866,6 +895,35 @@ class PolyEvalProof:
         _chk(lib().lasso_poly_eval_prove(ctx._h, poly._h, gens._h, _p(r), C.c_size_t(r.shape[0]), _p(Zr), transcript._h,
                                          random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
         return cls(bytes(out[: n.value]), czr.tobytes())
+
+
+class CombinedTableEvalProof:
+    """src/subtables/mod.rs:225-375 without blinds: n claims P_i(r) about the blocks of one merged polynomial
+    (DensePolynomial.merge) opened with one PolyEvalProof.  `.data` is the ark-serialize (compressed) proof."""
+
+    def __init__(self, data):
+        self.data = data
+
+    @staticmethod
+    def proof_len(num_vars):
+        """the serialised size for a merged polynomial of num_vars variables (that of its PolyEvalProof)"""
+        lg = num_vars - num_vars // 2
+        return 2 * (8 + 32 * lg) + 4 * 32
+
+    @classmethod
+    def prove(cls, ctx, combined, evals, r, gens, transcript, random_tape):
+        """CombinedTableEvalProof::prove over `combined` for the claims `evals` at r (combined.num_vars == len(r) +
+        log2(next_pow2(len(evals)))), on the caller's transcript and tape, advanced in place.  The claims are not checked:
+        a wrong one gives a proof the verifier rejects."""
+        evals = _limbs(evals, what="evals")
+        r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+        cap = cls.proof_len(combined.num_vars)
+        out = np.zeros(cap, dtype=np.uint8)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_combined_eval_prove(ctx._h, combined._h, gens._h, _p(evals), C.c_size_t(evals.shape[0]), _p(r),
+                                             C.c_size_t(r.shape[0]), transcript._h, random_tape._h, _p(out),
+                                             C.c_size_t(cap), C.byref(n)))
+        return cls(bytes(out[: n.value]))
 
 
 # ------------------------------------------------------------------ sumchecks over a caller's polynomials

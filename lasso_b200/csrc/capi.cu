@@ -1050,6 +1050,73 @@ int lasso_poly_create_eq(lasso_ctx* h, const uint64_t* r, size_t r_len, lasso_po
   LB_CATCH
 }
 
+// ---- many polynomials per call: merge, batched evaluation, one combined opening
+int lasso_poly_create_merge(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!polys || n_polys == 0 || !out) return fail(LASSO_ERR_LENGTH, "merge: no polynomials, or a null output");
+  for (size_t j = 0; j < n_polys; j++)
+    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  size_t total = 0;
+  for (size_t j = 0; j < n_polys; j++) {
+    total += polys[j]->p->len;  // each len <= 2^28: the running sum cannot wrap before it passes the limit
+    if (total > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "merge: at most 2^28 evaluations after padding");
+  }
+  std::vector<const Poly*> ps(n_polys);
+  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
+  *out = new lasso_poly{poly_merge(h->c, ps.data(), (int)n_polys)};
+  return 0;
+  LB_CATCH
+}
+int lasso_poly_evaluate_batch(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, const uint64_t* r,
+                              size_t r_len, uint64_t* out) {
+  LB_TRY_CTX(h)
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!polys || n_polys == 0 || n_polys > (size_t)kDotMaxPolys || !out)
+    return fail(LASSO_ERR_LENGTH, "evaluate batch: 1..64 polynomials and an output");
+  for (size_t j = 0; j < n_polys; j++)
+    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  for (size_t j = 1; j < n_polys; j++)
+    if (polys[j]->p->nv != polys[0]->p->nv) return fail(LASSO_ERR_LENGTH, "evaluate batch: the polynomials have different num_vars");
+  std::vector<fr_t> rv;
+  if (const int rc = load_point(*polys[0]->p, r, r_len, rv)) return rc;
+  std::vector<const Poly*> ps(n_polys);
+  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
+  const std::vector<fr_t> v = poly_evaluate_batch(h->c, ps.data(), (int)n_polys, rv);
+  for (size_t j = 0; j < n_polys; j++) memcpy(out + 4 * j, v[j].v, 32);
+  return 0;
+  LB_CATCH
+}
+int lasso_combined_eval_prove(lasso_ctx* h, const lasso_poly* combined, const lasso_poly_gens* g, const uint64_t* evals,
+                              size_t n_evals, const uint64_t* r, size_t r_len, lasso_transcript* transcript,
+                              lasso_random_tape* tape, uint8_t* proof_out, size_t proof_cap, size_t* proof_len) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, combined, g)) return rc;
+  if (!g) return fail(LASSO_ERR_GENS, "combined eval proof: null generators");
+  if (n_evals == 0 || n_evals > kPolyMaxLen || !evals) return fail(LASSO_ERR_LENGTH, "combined eval proof: 1..2^28 evals");
+  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "combined eval proof: null point");
+  // subtables/mod.rs:238-241: the joint polynomial has log2(#evals padded) variables more than r
+  const size_t nv = combined->p->nv;
+  if (nv != r_len + log2_exact_or_ceil(next_pow2(n_evals)))
+    return fail(LASSO_ERR_LENGTH, "combined eval proof: num_vars != r.len() + log2(next_pow2(n_evals))");
+  // the PolyEvalProof of lasso_poly_eval_prove at num_vars
+  const size_t lg = nv - nv / 2, need = 2 * (8 + 32 * lg) + 4 * 32;
+  if (proof_len) *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "combined eval proof: output buffer too small");
+  if (!transcript || !tape) return fail(LASSO_ERR_LENGTH, "combined eval proof: null transcript or random tape");
+  std::vector<fr_t> ev, rv;
+  if (!load_scalars(evals, n_evals, ev)) return fail(LASSO_ERR_VALUE, "combined eval proof: an eval is not a canonical residue");
+  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "combined eval proof: a coordinate of r is not a canonical residue");
+  auto t0 = std::chrono::steady_clock::now();
+  const std::vector<uint8_t> b = combined_eval_prove(h->c, *combined->p, *g->g, ev, rv, transcript->t, tape->t);
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (b.size() != need) return fail(-1, "combined eval proof: unexpected proof size");
+  memcpy(proof_out, b.data(), b.size());
+  return 0;
+  LB_CATCH
+}
+
 // ---- sumchecks over a caller's polynomials
 int lasso_comb_create(int n_inputs, const int32_t* program, int n_ops, const uint64_t* constants, int n_constants,
                       int degree, lasso_comb** out) {

@@ -185,6 +185,16 @@ void launch_multi_dot_u32(const uint32_t* base, size_t stride, int npolys, const
 void launch_bound_fr(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size, fr_t* partial, fr_t* out, cudaStream_t st);
 void launch_multi_dot_fr(const fr_t* base, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
                          cudaStream_t st);
+// out[j] = <P_j, eq> for k independent polynomials of n elements each, P_j = in.p[j] (uint32_t* when u32, the integer
+// mirrors, else fr_t*), 1 <= k <= kDotMaxPolys.  A thread reads each eq element once per group of kDotGroup inputs.
+// Two launches: the dot kernel (ceil(k / kDotGroup) CTA rows, at most kMaxBlocks CTAs) and reduce_partials over k values;
+// partial needs k x kMaxBlocks elements.
+static constexpr int kDotGroup = 8, kDotMaxPolys = 64;
+struct DotPtrs {
+  const void* p[kDotMaxPolys];
+};
+void launch_multi_dot_ptrs(const DotPtrs& in, int k, bool u32, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
+                           cudaStream_t st);
 // Reed-Solomon fingerprints (memory_checking.rs:236-310).  init/final over M cells, read/write over s ops.
 // M_local cells of this rank; local cell i = global address i*G + g; `table` is the full M-entry table
 void launch_gp_fingerprints_mem(const fr_t* table, const fr_t* final_fr, size_t M_local, int G, int g,

@@ -1280,6 +1280,66 @@ void launch_multi_dot_fr(const fr_t* base, size_t stride, int npolys, const fr_t
   reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
   LB_LAUNCH_CHECK();
 }
+// The pointer-table forms, for k independent polynomials of one length (lasso_poly_evaluate_batch): CTA row blockIdx.y
+// takes the group of kDotGroup inputs from kDotGroup * blockIdx.y, and a thread reads each eq element once for all the
+// inputs of its group, which keeps them in kDotGroup accumulators.  Block partials of input j go to
+// partial[j * gridDim.x + blockIdx.x], the layout reduce_partials_kernel sums.
+__global__ void __launch_bounds__(kThreads)
+    multi_dot_ptrs_u32_kernel(const __grid_constant__ DotPtrs in, int k, const fr_t* eq, size_t n, fr_t* partial) {
+  __shared__ fr_t scratch[kDotGroup * kThreads / 32];
+  const int j0 = kDotGroup * blockIdx.y, m = k - j0 < kDotGroup ? k - j0 : kDotGroup;
+  wide_t w[kDotGroup];
+#pragma unroll
+  for (int j = 0; j < kDotGroup; j++) wide_zero(w[j]);
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const fr_t e = ld_fr(eq + i);
+#pragma unroll
+    for (int j = 0; j < kDotGroup; j++)
+      if (j < m) wide_mad(w[j], e, static_cast<const uint32_t*>(in.p[j0 + j])[i]);
+  }
+  fr_t acc[kDotGroup];
+#pragma unroll
+  for (int j = 0; j < kDotGroup; j++) acc[j] = wide_reduce(w[j]);
+  block_sum_fr<kDotGroup>(acc, scratch);
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int j = 0; j < kDotGroup; j++)
+      if (j < m) partial[(size_t)(j0 + j) * gridDim.x + blockIdx.x] = acc[j];
+}
+__global__ void __launch_bounds__(kThreads)
+    multi_dot_ptrs_fr_kernel(const __grid_constant__ DotPtrs in, int k, const fr_t* eq, size_t n, fr_t* partial) {
+  __shared__ fr_t scratch[kDotGroup * kThreads / 32];
+  const int j0 = kDotGroup * blockIdx.y, m = k - j0 < kDotGroup ? k - j0 : kDotGroup;
+  fr_t acc[kDotGroup];
+#pragma unroll
+  for (int j = 0; j < kDotGroup; j++) acc[j] = fr_zero();
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const fr_t e = ld_fr(eq + i);
+#pragma unroll
+    for (int j = 0; j < kDotGroup; j++)
+      if (j < m) acc[j] = fr_add(acc[j], fr_mul(e, ld_fr(static_cast<const fr_t*>(in.p[j0 + j]) + i)));
+  }
+  block_sum_fr<kDotGroup>(acc, scratch);
+  if (threadIdx.x == 0)
+#pragma unroll
+    for (int j = 0; j < kDotGroup; j++)
+      if (j < m) partial[(size_t)(j0 + j) * gridDim.x + blockIdx.x] = acc[j];
+}
+void launch_multi_dot_ptrs(const DotPtrs& in, int k, bool u32, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
+                           cudaStream_t st) {
+  const int groups = (k + kDotGroup - 1) / kDotGroup;
+  int per = kMaxBlocks / groups;
+  if (per < 1) per = 1;
+  const int bx = grid_for(n, kThreads, per);
+  const dim3 grid(bx, groups);
+  if (u32)
+    multi_dot_ptrs_u32_kernel<<<grid, kThreads, 0, st>>>(in, k, eq, n, partial);
+  else
+    multi_dot_ptrs_fr_kernel<<<grid, kThreads, 0, st>>>(in, k, eq, n, partial);
+  LB_LAUNCH_CHECK();
+  reduce_partials_kernel<<<k, kThreads, 0, st>>>(partial, bx, out);
+  LB_LAUNCH_CHECK();
+}
 
 // memory_checking.rs:249-252: hash(a, v, t) = t*gamma^2 + v*gamma + a - tau
 __global__ void __launch_bounds__(kThreads)

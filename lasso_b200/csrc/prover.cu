@@ -1861,6 +1861,84 @@ Poly* poly_create_eq(Ctx* c, const std::vector<fr_t>& r) {
   eq_evals_dev(c, r, 0, p->nv, p->d_fr.p);
   return p.release();
 }
+// DensePolynomial::merge (dense_mlpoly.rs:251-261): the inputs' evaluations one after another, zero-padded to a power of
+// two.  Copies only, no kernel: one device-to-device copy per input and form, a memset per form for the padding.
+Poly* poly_merge(Ctx* c, const Poly* const* polys, int k) {
+  size_t total = 0;
+  unsigned bits = 0;
+  bool mirror = true;
+  for (int j = 0; j < k; j++) {
+    total += polys[j]->len;
+    bits = std::max(bits, polys[j]->bits);
+    mirror = mirror && polys[j]->d_u32.p;
+  }
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->len = next_pow2(total);
+  p->nv = log2_exact_or_ceil(p->len);
+  p->bits = bits;  // the padding is zero: the widest value is an input's
+  p->d_fr.alloc(c, p->len);
+  if (mirror) p->d_u32.alloc(c, p->len);
+  size_t at = 0;
+  for (int j = 0; j < k; j++) {
+    const size_t n = polys[j]->len;
+    LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p + at, polys[j]->d_fr.p, n * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+    if (mirror)
+      LB_CUDA_CHECK(cudaMemcpyAsync(p->d_u32.p + at, polys[j]->d_u32.p, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c->st));
+    at += n;
+  }
+  if (p->len > total) {  // zero is all-zero limbs in Montgomery form too
+    LB_CUDA_CHECK(cudaMemsetAsync(p->d_fr.p + total, 0, (p->len - total) * sizeof(fr_t), c->st));
+    if (mirror) LB_CUDA_CHECK(cudaMemsetAsync(p->d_u32.p + total, 0, (p->len - total) * sizeof(uint32_t), c->st));
+  }
+  return p.release();
+}
+// P_j(r) for k polynomials of one num_vars over ONE eq table: the integer inputs through their u32 mirrors and the others
+// through their Montgomery forms, one pointer-table dot launch (+ its reduction) per form present
+std::vector<fr_t> poly_evaluate_batch(Ctx* c, const Poly* const* polys, int k, const std::vector<fr_t>& r) {
+  SpanTimer sp(c, "DensePolynomial.evaluate_batch");
+  const size_t n = polys[0]->len;
+  DBuf<fr_t> eq(c, n);
+  eq_evals_dev(c, r, 0, polys[0]->nv, eq.p);
+  std::vector<int> order;  // the inputs in the order their values land in d_small: integer ones first
+  for (int form = 0; form < 2; form++) {
+    DotPtrs in{};
+    int m = 0;
+    for (int j = 0; j < k; j++) {
+      const bool u32 = polys[j]->d_u32.p != nullptr;
+      if (u32 != (form == 0)) continue;
+      in.p[m++] = u32 ? static_cast<const void*>(polys[j]->d_u32.p) : static_cast<const void*>(polys[j]->d_fr.p);
+      order.push_back(j);
+    }
+    if (!m) continue;
+    launch_multi_dot_ptrs(in, m, form == 0, eq.p, n, c->d_partial, c->d_small + (order.size() - m), c->st);
+    g_launches += 2;
+  }
+  std::vector<fr_t> got(k), out(k);
+  c->d2h(got.data(), c->d_small, k * sizeof(fr_t));
+  for (int i = 0; i < k; i++) out[order[i]] = got[i];
+  return out;
+}
+// CombinedTableEvalProof::prove (subtables/mod.rs:284-313): the n-to-1 reduction and opening the Lasso proof runs for its
+// derefs (prove_joint), on the caller's polynomial, transcript and tape
+std::vector<uint8_t> combined_eval_prove(Ctx* c, const Poly& p, const Gens& g, const std::vector<fr_t>& evals,
+                                         const std::vector<fr_t>& r, Transcript& transcript, RandomTape& tape) {
+  SpanTimer sp(c, "CombinedEval.prove");
+  {
+    // The opening's device vectors (L, a, b, two weight vectors, their fold targets, the MSM rows and partial points)
+    // take about L + 9 R elements plus a few thousand: reserve 16 R + L + 4096 in the context's pool, which keeps freed
+    // memory, before the first transcript write, so that a short device fails here and leaves the transcript as it was.
+    const size_t R = poly_R(p.nv), L = p.len / R;
+    DBuf<fr_t> reserve(c, 16 * R + L + 4096);
+  }
+  transcript.append_protocol_name("Lasso CombinedTableEvalProof");
+  const DotProductProofLogBytes proof = prove_joint(c, g, poly_src(p), p.nv, evals, true, "evals_ops_val",
+                                                    "challenge_combine_n_to_one", "joint_claim_eval", r, transcript, tape);
+  c->sync();
+  ByteWriter w;
+  ser_dpl(w, proof);
+  return w.b;
+}
 
 // ---------------------------------------------------------------------------------------------- caller sumchecks
 // A combining function on the device: its constants (32-byte aligned) then its instructions, one upload

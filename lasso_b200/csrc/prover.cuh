@@ -346,6 +346,15 @@ std::vector<uint8_t> poly_eval_prove(Ctx*, const Poly&, const Gens&, const std::
                                      Transcript&, RandomTape&, uint8_t C_Zr[32]);
 // EqPolynomial::new(r).evals() (eq_poly.rs:21-38) as a full-width polynomial (no u32 mirror); r.size() <= 28
 Poly* poly_create_eq(Ctx*, const std::vector<fr_t>& r);
+// DensePolynomial::merge (dense_mlpoly.rs:251-261) of k >= 1 polynomials (the caller checks the merged length): a new
+// polynomial of its own, with a u32 mirror iff every input has one
+Poly* poly_merge(Ctx*, const Poly* const* polys, int k);
+// P_j(r) for 1 <= k <= kDotMaxPolys polynomials of one num_vars == r.size() (the caller checks), one eq table
+std::vector<fr_t> poly_evaluate_batch(Ctx*, const Poly* const* polys, int k, const std::vector<fr_t>& r);
+// CombinedTableEvalProof::prove (subtables/mod.rs:284-313) without blinds: the serialised PolyEvalProof at
+// (challenges || r); p.nv == r.size() + log2(next_pow2(evals.size())) (the caller checks)
+std::vector<uint8_t> combined_eval_prove(Ctx*, const Poly& p, const Gens& g, const std::vector<fr_t>& evals,
+                                         const std::vector<fr_t>& r, Transcript&, RandomTape&);
 
 // A combining function g(x_0..x_{n_inputs-1}) of SumcheckInstanceProof::prove_arbitrary: a checked program (capi.cu)
 // with its slots allocated, and the declared combined_degree.  Host only.

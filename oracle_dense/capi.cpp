@@ -402,4 +402,68 @@ int orcd_gp_verify(const uint8_t* bytes, size_t nbytes, const uint64_t* products
   return 0;
 }
 
+// ---- DensePolynomial::merge and CombinedTableEvalProof (dense_mlpoly.rs:251-261, subtables/mod.rs:225-375)
+// merge of k polynomials (polys: their evaluations one after another, lens[j] of polynomial j): out receives the merged
+// evaluations (cap elements); returns their count, 0 when cap is too small
+size_t orcd_merge(const uint64_t* polys, const size_t* lens, size_t k, uint64_t* out, size_t cap) {
+  std::vector<DensePolynomial> ps;
+  size_t at = 0;
+  for (size_t j = 0; j < k; j++) {
+    ps.emplace_back(ldvec(polys + 4 * at, lens[j]));
+    at += lens[j];
+  }
+  const DensePolynomial m = DensePolynomial::merge(ps);
+  if (m.len > cap) return 0;
+  for (size_t i = 0; i < m.len; i++) stfr(out + 4 * i, m.Z[i]);
+  return m.len;
+}
+// CombinedTableEvalProof::prove over the polynomial Z (n = 2^nv elements) for n_evals claims at r (nv - log2 of the
+// padded count coordinates), on a caller's transcript and tape: returns the proof's length (0 on error)
+size_t orcd_combined_eval_prove(const uint64_t* Z, size_t n, const uint64_t* evals, size_t n_evals, const uint64_t* r,
+                                size_t r_len, const uint64_t* stream, size_t n_points, void* transcript, void* tape,
+                                uint8_t* out, size_t cap) {
+  try {
+    DensePolynomial poly(ldvec(Z, n));
+    if (n_evals == 0 || poly.num_vars != r_len + log_2(next_power_of_two(n_evals))) return 0;
+    size_t l, rr;
+    EqPolynomial::compute_factored_lens(poly.num_vars, l, rr);
+    if (n_points < pow2(rr) + 2) return 0;
+    PolyCommitmentGens gens = PolyCommitmentGens::make(poly.num_vars, ldstream(stream, n_points));
+    const CombinedTableEvalProof p = CombinedTableEvalProof::prove(poly, ldvec(evals, n_evals), ldvec(r, r_len), gens,
+                                                                   *(Transcript*)transcript, *(RandomTape*)tape);
+    std::vector<uint8_t> b = ser_proof(p.proof_table_eval);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_combined_eval_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// CombinedTableEvalProof::verify (subtables/mod.rs:315-375) of serialised bytes against the serialised commitment of a
+// polynomial of nv variables: 0 accepted, 1 rejected, 2 the commitment or the proof does not parse or nv does not fit
+int orcd_combined_eval_verify(const uint64_t* stream, size_t n_points, size_t nv, const uint8_t* comm, size_t comm_len,
+                              const uint8_t* proof, size_t proof_len, const uint64_t* evals, size_t n_evals,
+                              const uint64_t* r, size_t r_len, void* transcript) {
+  if (n_evals == 0 || nv != r_len + log_2(next_power_of_two(n_evals))) return 2;
+  size_t l, rr;
+  EqPolynomial::compute_factored_lens(nv, l, rr);
+  if (n_points < pow2(rr) + 2) return 2;
+  PolyCommitmentGens gens = PolyCommitmentGens::make(nv, ldstream(stream, n_points));
+  Reader rc{comm, comm_len};
+  PolyCommitment c;
+  c.C = rc.points();
+  if (!rc.ok || rc.at != comm_len || c.C.size() != pow2(l)) return 2;
+  Reader rp{proof, proof_len};
+  CombinedTableEvalProof p;
+  p.proof_table_eval.proof.bullet_reduction_proof.L_vec = rp.points();
+  p.proof_table_eval.proof.bullet_reduction_proof.R_vec = rp.points();
+  p.proof_table_eval.proof.delta = rp.point();
+  p.proof_table_eval.proof.beta = rp.point();
+  p.proof_table_eval.proof.z1 = rp.fr();
+  p.proof_table_eval.proof.z2 = rp.fr();
+  if (!rp.ok || rp.at != proof_len) return 2;
+  return p.verify(ldvec(r, r_len), ldvec(evals, n_evals), gens, c, *(Transcript*)transcript) ? 0 : 1;
+}
+
 }  // extern "C"
