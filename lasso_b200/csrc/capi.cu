@@ -174,7 +174,6 @@ int lasso_bind_top(lasso_ctx* h, uint64_t* Z, size_t len, const uint64_t r[4]) {
   fr_t rr;
   memcpy(rr.v, r, 32);
   launch_bind_top(d.p, 0, 1, len / 2, rr, c->st);
-  g_launches++;
   LB_CUDA_CHECK(cudaMemcpyAsync(Z, d.p, (len / 2) * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
   return 0;
@@ -189,7 +188,6 @@ int lasso_bind_bot(lasso_ctx* h, uint64_t* Z, size_t len, const uint64_t r[4]) {
   fr_t rr;
   memcpy(rr.v, r, 32);
   launch_bind_bot(d.p, o.p, len / 2, rr, c->st);
-  g_launches++;
   LB_CUDA_CHECK(cudaMemcpyAsync(Z, o.p, (len / 2) * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
   return 0;
@@ -204,7 +202,6 @@ int lasso_eq_evals(lasso_ctx* h, const uint64_t* r, int ell, uint64_t* out) {
   size_t n = (size_t)1 << ell;
   DBuf<fr_t> d(c, n);
   launch_eq_evals(rv, ell, d.p, c->d_eq_scratch, c->st);
-  g_launches += ell <= 11 ? 1 : (ell <= 22 ? 3 : 5);
   LB_CUDA_CHECK(cudaMemcpyAsync(out, d.p, n * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
   return 0;
@@ -223,7 +220,6 @@ int lasso_sumcheck_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M,
     LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
   const Finalize f = c->fin_begin();
   launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
-  g_launches += 1;
   c->fin_wait(f, (fr_t*)evals_out, npts);
   return 0;
   LB_CATCH
@@ -245,9 +241,7 @@ int lasso_sumcheck_bind_round_arbitrary(lasso_ctx* h, int strategy, int C, int l
   if (!launch_sumcheck_bind_eval_arbitrary(S, d.p, len, len / 4, rr, f, 1, c->st)) {
     launch_bind_top(d.p, len, np, len / 2, rr, c->st);
     launch_sumcheck_eval_arbitrary(S, d.p, len, len / 4, f, c->st);
-    g_launches += 1;
   }
-  g_launches += 1;
   c->fin_wait(f, (fr_t*)evals_out, npts);
   for (int k = 0; k < np; k++) c->d2h(polys[k], d.p + (size_t)k * len, (len / 2) * 32);
   return 0;
@@ -278,7 +272,6 @@ int lasso_sumcheck_round_cubic(lasso_ctx* h, int n_circuits, const uint64_t* con
   for (int k = 0; k < n_circuits; k++) {
     const Finalize f = c->fin_begin();
     launch_sumcheck_eval_cubic_comb(pA.p + k, pB.p + k, dC.p, 1, len / 2, cf, 0, f, c->st);
-    g_launches += 1;
     c->fin_wait(f, (fr_t*)out + 3 * (size_t)k, 3);
   }
   return 0;
@@ -292,7 +285,6 @@ int lasso_materialize_subtables(lasso_ctx* h, int strategy, int C, int log_M, in
   size_t M = (size_t)S.M();
   DBuf<fr_t> t(c, M * S.num_subtables());
   launch_materialize_subtables(S, t.p, nullptr, c->st);
-  g_launches++;
   for (int k = 0; k < S.num_subtables(); k++)
     LB_CUDA_CHECK(cudaMemcpyAsync(tables_out[k], t.p + (size_t)k * M, M * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
@@ -317,7 +309,6 @@ int lasso_gather_lookup_polys(lasso_ctx* h, int strategy, int C, int log_M, int 
   LB_CUDA_CHECK(cudaMemcpyAsync(dn.p, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, c->st));
   launch_materialize_subtables(S, t.p, nullptr, c->st);
   launch_gather_lookup_polys(S, t.p, nullptr, dn.p, s, E.p, s, nullptr, c->st);
-  g_launches += 2;
   for (int k = 0; k < S.num_memories(); k++)
     LB_CUDA_CHECK(cudaMemcpyAsync(E_out[k], E.p + (size_t)k * s, s * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
@@ -346,7 +337,6 @@ static void msm_variable_base(Ctx* c, const uint64_t* bases_affine, size_t nbase
   DBuf<fq_t> oe(c, nrows * 4);
   if (c->world == 1) {
     launch_msm_rows(tab.p, nbases, 0, canon.p, 8, ncols, (int)nrows, (int)ncols, nw, 1, 0, part.p, oe.p, nullptr, nullptr, c->st);
-    g_launches += 4;
   } else {
     // collective: every rank passed ITS shard of the terms; partial points are all-gathered and added
     // ("final bucket-sum reduce over NVLink" = gather-then-add, group addition is not an NCCL reduction)
@@ -355,7 +345,6 @@ static void msm_variable_base(Ctx* c, const uint64_t* bases_affine, size_t nbase
     launch_msm_rows(tab.p, nbases, 0, canon.p, 8, ncols, (int)nrows, (int)ncols, nw, 1, 0, part.p, nullptr, nullptr, mine, c->st);
     comm_allgather(c, mine, raw.p, nrows * 128);
     launch_sum_raw_points(raw.p, c->world, (int)nrows, nullptr, nullptr, oe.p, c->st);
-    g_launches += 5;
   }
   LB_CUDA_CHECK(cudaMemcpyAsync(out_ext, oe.p, nrows * 128, cudaMemcpyDeviceToHost, c->st));
   c->sync();
@@ -390,14 +379,13 @@ static void msm_job_once(lasso_msm_job* j) {
   // window count simply follows the widest scalar
   j->plan = msm_large_plan(j->n, max_bits);
   if (c->world == 1) {
-    g_launches += 2 + launch_msm_large(j->plan, j->niels.p, j->canon.p, j->scratch.p, j->out_ext.p, nullptr, c->st);
+    launch_msm_large(j->plan, j->niels.p, j->canon.p, j->scratch.p, j->out_ext.p, nullptr, c->st);
     return;
   }
   uint32_t* mine = j->raw.p + (size_t)c->world * 32;
-  g_launches += 2 + launch_msm_large(j->plan, j->niels.p, j->canon.p, j->scratch.p, nullptr, mine, c->st);
+  launch_msm_large(j->plan, j->niels.p, j->canon.p, j->scratch.p, nullptr, mine, c->st);
   comm_allgather(c, mine, j->raw.p, 128);
   launch_sum_raw_points(j->raw.p, c->world, 1, nullptr, nullptr, j->out_ext.p, c->st);
-  g_launches += 1;
 }
 int lasso_msm_plan_info(size_t n, unsigned max_bits, int out[16]) {
   LB_TRY
@@ -463,7 +451,6 @@ int lasso_msm_job_naive(lasso_ctx* h, lasso_msm_job* j, uint64_t out_xytz[16]) {
   if (c->world > 1) return fail(LASSO_ERR_LENGTH, "msm job: the naive cross-check is single-GPU");
   if (!j->naive_part.p) j->naive_part.alloc(c, (size_t)kNumSMs * 8);
   launch_msm_naive(j->bases.p, j->scalars.p, j->n, j->n_pool == j->n ? 0 : j->n_pool, j->naive_part.p, j->out_ext.p, c->st);
-  g_launches += 2;
   LB_CUDA_CHECK(cudaMemcpyAsync(out_xytz, j->out_ext.p, 128, cudaMemcpyDeviceToHost, c->st));
   c->sync();
   return 0;
@@ -676,8 +663,6 @@ static int strategy_upload(Ctx* c, CustomStrategy cs, const std::vector<CustomIn
     for (int k = 0; k < cs.nsub; k++)
       LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_u32.p + k * M, tables_u32[k], M * 4, cudaMemcpyHostToDevice, c->st));
     launch_from_u32(s->tables_u32.p, s->tables_fr.p, (size_t)cs.nsub * M, c->st);
-    LB_LAUNCH_CHECK();
-    g_launches += 1;
   } else {
     for (int k = 0; k < cs.nsub; k++)
       LB_CUDA_CHECK(cudaMemcpyAsync(s->tables_fr.p + k * M, tables_fr[k], M * 32, cudaMemcpyHostToDevice, c->st));
@@ -770,7 +755,6 @@ int lasso_sumcheck_round_custom(lasso_ctx* h, const lasso_strategy* s, const uin
     LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
   const Finalize f = c->fin_begin();
   launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
-  g_launches += 1;
   c->fin_wait(f, (fr_t*)evals_out, npts);
   return 0;
   LB_CATCH
@@ -1293,7 +1277,6 @@ int lasso_bench_bind(lasso_ctx* h, size_t len, int npolys, int iters, double* av
   for (int i = 0; i < iters; i++) launch_bind_top(d.p, len, npolys, len / 2, r, c->st);
   LB_CUDA_CHECK(cudaEventRecord(e1, c->st));
   LB_CUDA_CHECK(cudaEventSynchronize(e1));
-  g_launches += iters + 3;
   float ms = 0;
   LB_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
   *avg_ms = ms / iters;

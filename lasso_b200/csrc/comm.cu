@@ -273,6 +273,7 @@ static void comm_init_impl(Ctx* c, Xchg* x, const uint8_t id_bytes[128], int ran
   c->h_pub = (unsigned long long*)((uint8_t*)x->seg[rank] + kSegHeaderBytes);
   for (int r = 0; r < world; r++) c->d_pub_reader[r] = readers[r];
   c->pub_seq = 0;
+  c->pub_ring[0] = c->pub_ring[1] = 0;
 }
 
 void comm_destroy(Ctx* c) {
@@ -360,10 +361,8 @@ void comm_allgather(Ctx* c, const void* d_send, void* d_recv, size_t bytes_per_r
     const size_t n16 = chunk / 16;
     unsigned blocks = (unsigned)std::min<size_t>((n16 + 255) / 256, (size_t)kNumSMs);
     if (blocks < 1) blocks = 1;
-    xchg_push_kernel<<<blocks, 256, 0, c->st>>>((const uint4*)((const uint8_t*)d_send + off), n16, peers, c->world,
-                                                c->d_flag + 8, marker, seq);
-    LB_LAUNCH_CHECK();
-    g_launches += 1;
+    launch(xchg_push_kernel, blocks, 256, 0, c->st, (const uint4*)((const uint8_t*)d_send + off), n16, peers, c->world,
+           c->d_flag + 8, marker, seq);
     uint32_t got[8];
     for (int w = 0; w < c->world; w++) c->pub_wait_raw(marker, w, 1, got);  // every rank's block has landed here
     LB_CUDA_CHECK(cudaMemcpy2DAsync((uint8_t*)d_recv + off, bytes_per_rank, x->xbuf[c->rank] + par * kPubMaxReaders * kXchgSlotBytes,
@@ -387,20 +386,15 @@ __global__ void transpose_gathered_kernel(const fr_t* gathered /*[G][npolys]*/, 
 }
 // out[k] = ptrs[k][0] (or base[k*stride]): used to bring the 2*ncirc final claims of a layer to the host in one go
 void pack_heads(Ctx* c, fr_t* const* d_ptrs, const fr_t* base, size_t stride, int npolys, fr_t* d_out) {
-  pack_heads_kernel<<<(npolys + 127) / 128, 128, 0, c->st>>>(d_ptrs, base, stride, npolys, nullptr, d_out);
-  LB_LAUNCH_CHECK();
-  g_launches += 1;
+  launch(pack_heads_kernel, (npolys + 127) / 128, 128, 0, c->st, d_ptrs, base, stride, npolys, nullptr, d_out);
 }
 void comm_gather_heads(Ctx* c, fr_t* const* d_ptrs, const fr_t* base, size_t stride, int npolys, const fr_t* extra, fr_t* d_out) {
   const int total = npolys + (extra ? 1 : 0);
   if ((size_t)total * (c->world + 1) > c->gather_elems) throw std::runtime_error("gather_heads: too many polynomials");
   fr_t* packed = c->d_gather + (size_t)total * c->world;
-  pack_heads_kernel<<<(total + 127) / 128, 128, 0, c->st>>>(d_ptrs, base, stride, npolys, extra, packed);
-  LB_LAUNCH_CHECK();
+  launch(pack_heads_kernel, (total + 127) / 128, 128, 0, c->st, d_ptrs, base, stride, npolys, extra, packed);
   comm_allgather(c, packed, c->d_gather, (size_t)total * sizeof(fr_t));
-  transpose_gathered_kernel<<<(total * c->world + 127) / 128, 128, 0, c->st>>>(c->d_gather, c->world, total, d_out);
-  LB_LAUNCH_CHECK();
-  g_launches += 2;
+  launch(transpose_gathered_kernel, (total * c->world + 127) / 128, 128, 0, c->st, c->d_gather, c->world, total, d_out);
 }
 // in[g * n_loc + j] (rank g's block of n_loc elements) -> out[j * G + g]: the low-bit shards of a vector, interleaved
 __global__ void __launch_bounds__(256) interleave_kernel(const fr_t* in, int world, size_t n_loc, fr_t* out) {
@@ -418,9 +412,8 @@ void comm_gather_vector(Ctx* c, const fr_t* d_shard, size_t n_loc, fr_t* d_scrat
   }
   comm_allgather(c, d_shard, d_scratch, n_loc * sizeof(fr_t));
   const size_t n = n_loc * c->world;
-  interleave_kernel<<<(unsigned)std::min<size_t>((n + 255) / 256, 4 * (size_t)kNumSMs), 256, 0, c->st>>>(d_scratch, c->world, n_loc, d_out);
-  LB_LAUNCH_CHECK();
-  g_launches += 1;
+  launch(interleave_kernel, (unsigned)std::min<size_t>((n + 255) / 256, 4 * (size_t)kNumSMs), 256, 0, c->st, d_scratch,
+         c->world, n_loc, d_out);
 }
 
 }  // namespace lb

@@ -1,11 +1,13 @@
 // lasso_b200 — shared device helpers: 32-byte global loads/stores of field elements,
-// warp-shuffle + shared-memory reductions of Fr partial sums, error checking.
+// warp-shuffle + shared-memory reductions of Fr partial sums, error checking, the kernel launch helper.
 #pragma once
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <cstdio>
 #include <stdexcept>
 #include <string>
+#include <utility>
 
 #include "ed25519.cuh"
 #include "pub_codec.hpp"
@@ -20,13 +22,22 @@ namespace lb {
                                std::to_string(__LINE__));                                             \
   } while (0)
 
-// after every kernel launch: a bad configuration (shared memory opt-in missing on this device, grid too large)
-// fails synchronously and must not go unnoticed
-#define LB_LAUNCH_CHECK() LB_CUDA_CHECK(cudaGetLastError())
-
 static constexpr int kNumSMs = 132;  // H100 SXM
 
+// kernels launched by this library in this process (lasso_launch_count, bench.py's gpu_launches); only launch() adds
+// to it, so copies, memsets and NCCL's own kernels are not counted
+inline std::atomic<unsigned long long> g_launches{0};
+
 #if defined(__CUDACC__)
+// Every kernel launch of the library goes through here.  A bad configuration (shared memory opt-in missing on this
+// device, grid too large) fails synchronously and must not go unnoticed; a launch that was enqueued is counted.
+template <typename... Params, typename... Args>
+void launch(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  kernel<<<grid, block, smem, st>>>(std::forward<Args>(args)...);
+  LB_CUDA_CHECK(cudaGetLastError());
+  g_launches.fetch_add(1, std::memory_order_relaxed);
+}
+
 // One 32-byte element per thread as two 128-bit accesses (the widest global access sm_90 has). The first
 // instruction of a warp touches every 32-byte sector the warp needs; the second is expected to hit those sectors in
 // L1, so DRAM should still see each element once (not profiled; the bind kernel's measured bandwidth, DESIGN.md §7,
@@ -118,7 +129,7 @@ __device__ __forceinline__ void block_sum_fr(fr_t (&v)[NV], fr_t* scratch) {
 // into all G of them — the G replicated host transcripts add the G residues, no collective, no extra launch.
 static constexpr int kPubSlotWords = 8;       // 64 B per element slot (5 words used): never straddles a line
 static constexpr int kPubMaxReaders = 8;      // one node
-static constexpr int kPubRegions = 4;         // ring of regions per writer: consecutive messages never share one
+static constexpr int kPubRegions = 4;         // rings of regions per writer (prover.cuh pub_begin)
 static constexpr int kPubElems = 512;         // elements per region (largest message: 8 * alpha tree tops)
 static constexpr uint32_t kPubTagMod = 8191;  // tags 1..8191 (13 bits, 0 = empty)
 struct PubDst {

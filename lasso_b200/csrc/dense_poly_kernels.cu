@@ -54,8 +54,7 @@ void launch_poly_ingest(const uint64_t* src, size_t row_stride, size_t n, fr_t* 
   size_t b = (n + kIngestThreads - 1) / kIngestThreads;
   if (b > (size_t)kNumSMs * 8) b = (size_t)kNumSMs * 8;
   if (b == 0) return;
-  poly_ingest_kernel<<<(unsigned)b, kIngestThreads, 0, st>>>(src, row_stride, n, dst, flags);
-  LB_LAUNCH_CHECK();
+  launch(poly_ingest_kernel, (unsigned)b, kIngestThreads, 0, st, src, row_stride, n, dst, flags);
 }
 
 __global__ void __launch_bounds__(kIngestThreads) poly_mirror_u32_kernel(const fr_t* in, size_t n, uint32_t* out) {
@@ -66,8 +65,7 @@ void launch_poly_mirror_u32(const fr_t* in, size_t n, uint32_t* out, cudaStream_
   size_t b = (n + kIngestThreads - 1) / kIngestThreads;
   if (b > (size_t)kNumSMs * 8) b = (size_t)kNumSMs * 8;
   if (b == 0) return;
-  poly_mirror_u32_kernel<<<(unsigned)b, kIngestThreads, 0, st>>>(in, n, out);
-  LB_LAUNCH_CHECK();
+  launch(poly_mirror_u32_kernel, (unsigned)b, kIngestThreads, 0, st, in, n, out);
 }
 
 }  // namespace lb

@@ -187,17 +187,13 @@ __global__ void __launch_bounds__(1024)
   for (int k = 0; k < 4; k++)
     if (base + k < len) v[base + k] += o;
 }
-static int scan_exclusive(uint32_t* data, size_t len, int C, uint32_t* tile_sums, cudaStream_t st) {
+static void scan_exclusive(uint32_t* data, size_t len, int C, uint32_t* tile_sums, cudaStream_t st) {
   const uint32_t ntiles = (uint32_t)((len + kDzScanTile - 1) / kDzScanTile);
   dim3 grid(ntiles, (unsigned)C);
-  dz_scan_tiles_kernel<<<grid, 1024, 0, st>>>(data, len, ntiles, tile_sums);
-  LB_LAUNCH_CHECK();
-  if (ntiles == 1) return 1;  // a single tile per dimension: its scan is the result
-  dz_scan_sums_kernel<<<dim3(1, (unsigned)C), 1024, 0, st>>>(tile_sums, ntiles);
-  LB_LAUNCH_CHECK();
-  dz_scan_apply_kernel<<<grid, 1024, 0, st>>>(data, len, ntiles, tile_sums);
-  LB_LAUNCH_CHECK();
-  return 3;
+  launch(dz_scan_tiles_kernel, grid, 1024, 0, st, data, len, ntiles, tile_sums);
+  if (ntiles == 1) return;  // a single tile per dimension: its scan is the result
+  launch(dz_scan_sums_kernel, dim3(1, (unsigned)C), 1024, 0, st, tile_sums, ntiles);
+  launch(dz_scan_apply_kernel, grid, 1024, 0, st, data, len, ntiles, tile_sums);
 }
 
 // ---------------------------------------------------------------------------------------------- results
@@ -237,11 +233,10 @@ size_t densify_scratch_words(size_t s, int C, size_t log_m) {
   // + 64 spare words, the last of them the range flag of launch_densify
   return 2 * 2 * (size_t)C * s /* two packed arrays of u64 */ + (size_t)C * m /* counts / start */ + H + tsums + 64;
 }
-// Outputs are this rank's shards: dim_i at dim_loc + i * dim_stride (likewise read, final).  Returns the number of
-// kernels launched.
-int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
-                   uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
-                   uint32_t* final_loc, size_t final_stride, cudaStream_t st) {
+// Outputs are this rank's shards: dim_i at dim_loc + i * dim_stride (likewise read, final).
+void launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
+                    uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
+                    uint32_t* final_loc, size_t final_stride, cudaStream_t st) {
   const uint32_t m = 1u << log_m;
   const uint32_t ntiles = (uint32_t)((s + kRadixTile - 1) / kRadixTile);
   unsigned long long* pa = reinterpret_cast<unsigned long long*>(scratch);
@@ -250,7 +245,6 @@ int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, si
   uint32_t* H = count + (size_t)C * m;
   uint32_t* tsums = H + (size_t)C * 256 * ntiles;
   unsigned* bad = check ? reinterpret_cast<unsigned*>(scratch + densify_scratch_words(s, C, log_m) - 1) : nullptr;
-  int launches = 0;
   LB_CUDA_CHECK(cudaMemsetAsync(count, 0, (size_t)C * m * 4, st));
   if (bad) LB_CUDA_CHECK(cudaMemsetAsync(bad, 0, sizeof(unsigned), st));
   {
@@ -258,13 +252,11 @@ int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, si
     if (bx > (size_t)kNumSMs * 8) bx = kNumSMs * 8;
     const dim3 grid((unsigned)bx, (unsigned)C);
     if (idx.elem_bytes == 8)
-      dz_extract_kernel<<<grid, 256, 0, st>>>(static_cast<const unsigned long long*>(idx.p), idx.row_stride, idx.col_stride,
-                                              n, s, m, G, g, pa, count, dim_loc, dim_stride, bad);
+      launch(dz_extract_kernel<unsigned long long>, grid, 256, 0, st, static_cast<const unsigned long long*>(idx.p),
+             idx.row_stride, idx.col_stride, n, s, m, G, g, pa, count, dim_loc, dim_stride, bad);
     else
-      dz_extract_kernel<<<grid, 256, 0, st>>>(static_cast<const uint32_t*>(idx.p), idx.row_stride, idx.col_stride, n, s, m,
-                                              G, g, pa, count, dim_loc, dim_stride, bad);
-    LB_LAUNCH_CHECK();
-    launches++;
+      launch(dz_extract_kernel<uint32_t>, grid, 256, 0, st, static_cast<const uint32_t*>(idx.p), idx.row_stride,
+             idx.col_stride, n, s, m, G, g, pa, count, dim_loc, dim_stride, bad);
   }
   if (check) {  // the verdict, and the point after which the index matrix is no longer read
     LB_CUDA_CHECK(cudaMemcpyAsync(check->h_bad, bad, sizeof(unsigned), cudaMemcpyDeviceToHost, st));
@@ -272,25 +264,19 @@ int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, si
   }
   unsigned long long *cur = pa, *nxt = pb;
   for (int shift = 0; shift < (int)log_m; shift += 8) {  // LSD: least significant digit first, every pass stable
-    dz_radix_hist_kernel<<<dim3(ntiles, (unsigned)C), kRadixThreads, 0, st>>>(cur, s, 32 + shift, ntiles, H);
-    LB_LAUNCH_CHECK();
-    launches += 1 + scan_exclusive(H, (size_t)256 * ntiles, C, tsums, st);
-    dz_radix_scatter_kernel<<<dim3(ntiles, (unsigned)C), kRadixThreads, 0, st>>>(cur, nxt, s, 32 + shift, ntiles, H);
-    LB_LAUNCH_CHECK();
-    launches++;
+    launch(dz_radix_hist_kernel, dim3(ntiles, (unsigned)C), kRadixThreads, 0, st, cur, s, 32 + shift, ntiles, H);
+    scan_exclusive(H, (size_t)256 * ntiles, C, tsums, st);
+    launch(dz_radix_scatter_kernel, dim3(ntiles, (unsigned)C), kRadixThreads, 0, st, cur, nxt, s, 32 + shift,
+           ntiles, H);
     std::swap(cur, nxt);
   }
-  dz_final_kernel<<<dim3((m + 255) / 256, (unsigned)C), 256, 0, st>>>(count, m, G, g, final_loc, final_stride);
-  LB_LAUNCH_CHECK();
-  launches += 1 + scan_exclusive(count, m, C, tsums, st);
+  launch(dz_final_kernel, dim3((m + 255) / 256, (unsigned)C), 256, 0, st, count, m, G, g, final_loc, final_stride);
+  scan_exclusive(count, m, C, tsums, st);
   {
     size_t bx = (s + 255) / 256;
     if (bx > (size_t)kNumSMs * 8) bx = kNumSMs * 8;
-    dz_read_kernel<<<dim3((unsigned)bx, (unsigned)C), 256, 0, st>>>(cur, s, m, count, G, g, read_loc, read_stride);
-    LB_LAUNCH_CHECK();
-    launches++;
+    launch(dz_read_kernel, dim3((unsigned)bx, (unsigned)C), 256, 0, st, cur, s, m, count, G, g, read_loc, read_stride);
   }
-  return launches;
 }
 
 }  // namespace lb

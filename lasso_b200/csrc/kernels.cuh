@@ -209,7 +209,6 @@ struct TreePtrs {
 };
 void launch_product_trees(const TreePtrs& trees, int ntrees, size_t N, int slot0, int stop_len, const Finalize& fin,
                           cudaStream_t st);
-int product_trees_launches(size_t N);
 // layer 1 of a grand-product circuit over a caller's polynomial P of 2*half elements: out[i] = P[i] * P[i + half]
 void launch_product_layer1(const fr_t* P, fr_t* out, size_t half, cudaStream_t st);
 // x_k[0] <- x_k[0] + r (x_k[1] - x_k[0]) for the n arrays x_k = d_AB[k]; results also published (Finalize)
@@ -254,8 +253,8 @@ struct DzRangeCheck {
 };
 // All C dimensions at once; outputs are this rank's shards (rank g of G: accesses k = i*G + g, addresses a = i*G + g):
 // dim_i at dim_loc + i*dim_stride, read_i at read_loc + i*read_stride, final_i likewise.  check may be null.
-int launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
-                   uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
-                   uint32_t* final_loc, size_t final_stride, cudaStream_t st);
+void launch_densify(const DzIndices& idx, const DzRangeCheck* check, size_t n, size_t s, int C, size_t log_m, int G, int g,
+                    uint32_t* scratch, uint32_t* dim_loc, size_t dim_stride, uint32_t* read_loc, size_t read_stride,
+                    uint32_t* final_loc, size_t final_stride, cudaStream_t st);
 
 }  // namespace lb

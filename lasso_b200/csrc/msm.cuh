@@ -87,8 +87,8 @@ void msm_large_init_device();
 // bases: arkworks affine (x, y) Montgomery limbs; term i uses base i % n_pool when n_pool != 0 (bench inputs), else base i
 void launch_msm_large_prep(const fq_t* bases_ark, const fr_t* scalars_mont, size_t n, size_t n_pool, pt_niels* niels,
                            fr_t* canon, unsigned* d_max_bits, cudaStream_t st);
-int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* canon, void* scratch, fq_t* out_ext,
-                     uint32_t* out_raw, cudaStream_t st);
+void launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* canon, void* scratch, fq_t* out_ext,
+                      uint32_t* out_raw, cudaStream_t st);
 // msm_final.cu: A = nw x nlev level sums; lgL[k] = log2 of level k's group size
 void launch_msm_final(const pt_ext* A, int nlev, const int* lgL, int nw, int c, fq_t* out_ext, uint32_t* out_raw, cudaStream_t st);
 // independent evaluation for the parity tests: per-term double-and-add + tree sum (partial: kNumSMs * 8 points of scratch)

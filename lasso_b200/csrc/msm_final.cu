@@ -73,8 +73,7 @@ __global__ void __launch_bounds__(32)
 void launch_msm_final(const pt_ext* A, int nlev, const int* lgL, int nw, int c, fq_t* out_ext, uint32_t* out_raw, cudaStream_t st) {
   MsmLgL lg;
   for (int k = 0; k < 8; k++) lg.v[k] = lgL[k];
-  msm_final_kernel<<<1, 32, 0, st>>>(A, nlev, lg, nw, c, out_ext, out_raw);
-  LB_LAUNCH_CHECK();
+  launch(msm_final_kernel, 1, 32, 0, st, A, nlev, lg, nw, c, out_ext, out_raw);
 }
 
 }  // namespace lb

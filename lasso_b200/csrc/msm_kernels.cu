@@ -87,9 +87,8 @@ __global__ void __launch_bounds__(128) table_next_kernel(pt_niels* T, size_t n, 
 }
 void launch_build_table(const fq_t* bases_ark, size_t n, pt_niels* T, size_t stride, int nwindows, cudaStream_t st) {
   unsigned blocks = (unsigned)((n + 127) / 128);
-  table_first_kernel<<<blocks, 128, 0, st>>>(bases_ark, n, T);
-  for (int w = 1; w < nwindows; w++) table_next_kernel<<<blocks, 128, 0, st>>>(T, n, stride, w);
-  LB_LAUNCH_CHECK();
+  launch(table_first_kernel, blocks, 128, 0, st, bases_ark, n, T);
+  for (int w = 1; w < nwindows; w++) launch(table_next_kernel, blocks, 128, 0, st, T, n, stride, w);
 }
 
 // ---------------------------------------------------------------- scalars
@@ -112,8 +111,7 @@ void launch_canonicalize(const fr_t* in, fr_t* out, size_t n, unsigned* d_max_bi
   size_t b = (n + 255) / 256;
   if (b > (size_t)kNumSMs * 8) b = kNumSMs * 8;
   if (b == 0) return;
-  canonicalize_kernel<<<(unsigned)b, 256, 0, st>>>(in, out, n, d_max_bits);
-  LB_LAUNCH_CHECK();
+  launch(canonicalize_kernel, (unsigned)b, 256, 0, st, in, out, n, d_max_bits);
 }
 
 // signed digits (c = 8): byte w of (s + 0x80..80) minus 128.  MsmDigits biases the scalar once; digit(w) with a
@@ -529,8 +527,7 @@ __global__ void __launch_bounds__(128)
 }
 void launch_build_multiples(const pt_niels* T, size_t table_stride, size_t npts, int nwindows, pt_niels* M, cudaStream_t st) {
   const size_t n = (size_t)nwindows * npts;
-  multiples_table_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(T, table_stride, npts, nwindows, M);
-  LB_LAUNCH_CHECK();
+  launch(multiples_table_kernel, (unsigned)((n + 127) / 128), 128, 0, st, T, table_stride, npts, nwindows, M);
 }
 
 // 16-bit multiples of the COMMITMENT generators (the columns of the Hyrax matrices): M16[j][d-1] = d * G_j,
@@ -570,8 +567,7 @@ __global__ void __launch_bounds__(128)
 void launch_build_multiples16(const pt_niels* T, const pt_niels* M, size_t npts8, size_t ncols, size_t col_mul, size_t col_add,
                               pt_niels* M16, cudaStream_t st) {
   const size_t n = ncols * 128;
-  multiples16_table_kernel<<<(unsigned)((n + 127) / 128), 128, 0, st>>>(T, M, npts8, ncols, col_mul, col_add, M16);
-  LB_LAUNCH_CHECK();
+  launch(multiples16_table_kernel, (unsigned)((n + 127) / 128), 128, 0, st, T, M, npts8, ncols, col_mul, col_add, M16);
 }
 
 static constexpr int MSMD_T = 512;  // 128 quads
@@ -858,9 +854,8 @@ void launch_bullet_fused(const pt_niels* M, size_t npts, const fr_t* a_in, const
                          const PubDst& pub, cudaStream_t st) {
   if (m < 2 || n < m) throw std::runtime_error("bullet_fused: m >= 2");
   dim3 grid(bullet_fused_chunks((int)n), 2);
-  bullet_fused_kernel<<<grid, MSMD_T, 0, st>>>(M, npts, a_in, b_in, w_in, a_out, b_out, w_out, (int)n, (int)m, fold, u, uinv,
-                                               blind_L, blind_R, partials, ip_partial, counter, pub);
-  LB_LAUNCH_CHECK();
+  launch(bullet_fused_kernel, grid, MSMD_T, 0, st, M, npts, a_in, b_in, w_in, a_out, b_out, w_out, (int)n, (int)m, fold,
+         u, uinv, blind_L, blind_R, partials, ip_partial, counter, pub);
 }
 
 // two short MSMs over the multiples table; the points go to mapped host memory (msm_finish_quad_kernel)
@@ -876,10 +871,8 @@ void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, 
                        cudaStream_t st) {
   const int nrows = 2, nchunks = msm_direct_chunks(len, 1);
   dim3 grid(nchunks, nrows);
-  msm_direct_kernel<<<grid, MSMD_T, 0, st>>>(M, npts, scalars, len, partials);
-  LB_LAUNCH_CHECK();
-  msm_finish_quad_kernel<<<1, 128 * nrows, 0, st>>>(partials, nrows, nchunks, pub);
-  LB_LAUNCH_CHECK();
+  launch(msm_direct_kernel, grid, MSMD_T, 0, st, M, npts, scalars, len, partials);
+  launch(msm_finish_quad_kernel, 1, 128 * nrows, 0, st, partials, nrows, nchunks, pub);
 }
 
 // ---------------------------------------------------------------- Hyrax row commitments over the multiples table
@@ -990,8 +983,7 @@ __global__ void __launch_bounds__(MSM_T) centre_constant_kernel(const pt_niels* 
   if (tid == 0) *K16 = acc;
 }
 void launch_centre_constant(const pt_niels* M16, int ncols, pt_ext* K16, cudaStream_t st) {
-  centre_constant_kernel<<<1, MSM_T, 32 * MSM_T * sizeof(uint32_t), st>>>(M16, ncols, K16);
-  LB_LAUNCH_CHECK();
+  launch(centre_constant_kernel, 1, MSM_T, 32 * MSM_T * sizeof(uint32_t), st, M16, ncols, K16);
 }
 void launch_msm_rows_direct_u32(const pt_niels* M, size_t npts, const pt_niels* M16, const pt_ext* K16, const uint32_t* scalars,
                                 size_t row_stride, int nrows, int ncols, int nw, int col_mul, int col_add, pt_ext* partials,
@@ -999,14 +991,12 @@ void launch_msm_rows_direct_u32(const pt_niels* M, size_t npts, const pt_niels* 
   if (nrows <= 0) return;
   if (nw < 1) nw = 1;
   if (nw > 5) throw std::runtime_error("msm_rows_direct_u32: more than 5 windows");
-  msm_rows_direct_u32_kernel<<<nrows, MSM_T, 32 * MSM_T * sizeof(uint32_t), st>>>(M, npts, M16, K16, scalars, row_stride,
-                                                                              ncols, nw, col_mul, col_add, partials);
-  LB_LAUNCH_CHECK();
+  launch(msm_rows_direct_u32_kernel, nrows, MSM_T, 32 * MSM_T * sizeof(uint32_t), st, M, npts, M16, K16, scalars,
+         row_stride, ncols, nw, col_mul, col_add, partials);
   if (out_raw)
-    msm_finish_kernel<<<nrows, 32, 0, st>>>(partials, nrows, 1, 1, 1, out_ext, out_comp, out_raw);
+    launch(msm_finish_kernel, nrows, 32, 0, st, partials, nrows, 1, 1, 1, out_ext, out_comp, out_raw);
   else
-    normalize_rows_kernel<<<(nrows + 31) / 32, 32, 0, st>>>(partials, nrows, out_ext, out_comp);
-  LB_LAUNCH_CHECK();
+    launch(normalize_rows_kernel, (nrows + 31) / 32, 32, 0, st, partials, nrows, out_ext, out_comp);
 }
 
 // Field-valued polynomials (a caller's table of arbitrary field elements): as msm_rows_direct_u32_kernel, but the
@@ -1068,14 +1058,12 @@ void launch_msm_rows_direct_fr(const pt_niels* M, size_t npts, const fr_t* scala
                                uint32_t* out_raw, cudaStream_t st) {
   if (nrows <= 0) return;
   if (nw < 1 || nw > kMsmFullWindows) throw std::runtime_error("msm_rows_direct_fr: nw must be in 1..32");
-  msm_rows_direct_fr_kernel<<<nrows, MSM_T, 32 * MSM_T * sizeof(uint32_t), st>>>(M, npts, scalars, row_stride, ncols, nw,
-                                                                              col_mul, col_add, partials);
-  LB_LAUNCH_CHECK();
+  launch(msm_rows_direct_fr_kernel, nrows, MSM_T, 32 * MSM_T * sizeof(uint32_t), st, M, npts, scalars, row_stride, ncols,
+         nw, col_mul, col_add, partials);
   if (out_raw)
-    msm_finish_kernel<<<nrows, 32, 0, st>>>(partials, nrows, 1, 1, 1, out_ext, out_comp, out_raw);
+    launch(msm_finish_kernel, nrows, 32, 0, st, partials, nrows, 1, 1, 1, out_ext, out_comp, out_raw);
   else
-    normalize_rows_kernel<<<(nrows + 31) / 32, 32, 0, st>>>(partials, nrows, out_ext, out_comp);
-  LB_LAUNCH_CHECK();
+    launch(normalize_rows_kernel, (nrows + 31) / 32, 32, 0, st, partials, nrows, out_ext, out_comp);
 }
 
 // Launch geometry.  wpc = windows per CTA (all of them over a shifted table), ngroups = window groups,
@@ -1130,17 +1118,15 @@ void launch_msm_rows(const pt_niels* table, size_t table_stride, int shifted, co
     dim3 grid(g.ngroups, nr, nchunks);
     pt_ext* part = partials + (size_t)r0 * g.ngroups * nchunks;
     if (scalar_limbs == 1)
-      msm_bucket_kernel<1><<<grid, MSM_T, sizeof(MsmSmem), st>>>(
-          table, table_stride, shifted, (const uint32_t*)scalars + (size_t)r0 * row_stride, row_stride, ncols,
-          chunk_cols, nw, g.wpc, col_mul, col_add, part);
+      launch(msm_bucket_kernel<1>, grid, MSM_T, sizeof(MsmSmem), st,
+             table, table_stride, shifted, (const uint32_t*)scalars + (size_t)r0 * row_stride, row_stride, ncols,
+             chunk_cols, nw, g.wpc, col_mul, col_add, part);
     else
-      msm_bucket_kernel<8><<<grid, MSM_T, sizeof(MsmSmem), st>>>(
-          table, table_stride, shifted, (const uint32_t*)scalars + (size_t)r0 * row_stride * 8, row_stride, ncols,
-          chunk_cols, nw, g.wpc, col_mul, col_add, part);
+      launch(msm_bucket_kernel<8>, grid, MSM_T, sizeof(MsmSmem), st,
+             table, table_stride, shifted, (const uint32_t*)scalars + (size_t)r0 * row_stride * 8, row_stride, ncols,
+             chunk_cols, nw, g.wpc, col_mul, col_add, part);
   }
-  LB_LAUNCH_CHECK();
-  msm_finish_kernel<<<nrows, 32, 0, st>>>(partials, nrows, g.ngroups, nchunks, shifted, out_ext, out_comp, out_raw);
-  LB_LAUNCH_CHECK();
+  launch(msm_finish_kernel, nrows, 32, 0, st, partials, nrows, g.ngroups, nchunks, shifted, out_ext, out_comp, out_raw);
 }
 
 // Cross-GPU "bucket-sum reduce": raw[(k * nrows + row) * 32 ..] = partial (X,Y,Z,T) of source k for `row`
@@ -1192,8 +1178,7 @@ __global__ void __launch_bounds__(64)
 }
 void launch_sum_raw_points(const uint32_t* raw, int nsrc, int nrows, uint32_t* out_raw, uint32_t* out_comp, fq_t* out_ext,
                            cudaStream_t st) {
-  sum_raw_points_kernel<<<(nrows + 63) / 64, 64, 0, st>>>(raw, nsrc, nrows, out_raw, out_comp, out_ext);
-  LB_LAUNCH_CHECK();
+  launch(sum_raw_points_kernel, (nrows + 63) / 64, 64, 0, st, raw, nsrc, nrows, out_raw, out_comp, out_ext);
 }
 
 }  // namespace lb

@@ -460,10 +460,8 @@ __global__ void __launch_bounds__(128) msm_naive_sum_kernel(const pt_ext* partia
 void launch_msm_naive(const fq_t* bases_ark, const fr_t* scalars_mont, size_t n, size_t n_pool, pt_ext* partial /* kNumSMs * 8 */,
                       fq_t* out_ext, cudaStream_t st) {
   const int blocks = kNumSMs * 8;
-  msm_naive_terms_kernel<<<blocks, 128, 0, st>>>(bases_ark, scalars_mont, n, n_pool, partial);
-  LB_LAUNCH_CHECK();
-  msm_naive_sum_kernel<<<1, 128, 0, st>>>(partial, blocks, out_ext);
-  LB_LAUNCH_CHECK();
+  launch(msm_naive_terms_kernel, blocks, 128, 0, st, bases_ark, scalars_mont, n, n_pool, partial);
+  launch(msm_naive_sum_kernel, 1, 128, 0, st, partial, blocks, out_ext);
 }
 
 // ---------------------------------------------------------------------------------------------- host side
@@ -525,14 +523,12 @@ void launch_msm_large_prep(const fq_t* bases_ark, const fr_t* scalars_mont, size
                            fr_t* canon, unsigned* d_max_bits, cudaStream_t st) {
   size_t b = (n + 255) / 256;
   if (b > (size_t)kNumSMs * 8) b = kNumSMs * 8;
-  msm_prep_kernel<<<(unsigned)b, 256, 0, st>>>(bases_ark, scalars_mont, n, n_pool, niels, canon, d_max_bits);
-  LB_LAUNCH_CHECK();
+  launch(msm_prep_kernel, (unsigned)b, 256, 0, st, bases_ark, scalars_mont, n, n_pool, niels, canon, d_max_bits);
 }
 // scratch: msm_large_scratch_bytes(plan) bytes.  Outputs (either may be null): out_ext = (x, y, t, z = 1) arkworks
-// limbs; out_raw = un-normalised (X, Y, Z, T) internal limbs (for the cross-GPU gather-then-add).  Returns the number
-// of kernels launched.
-int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* canon, void* scratch, fq_t* out_ext,
-                     uint32_t* out_raw, cudaStream_t st) {
+// limbs; out_raw = un-normalised (X, Y, Z, T) internal limbs (for the cross-GPU gather-then-add).
+void launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* canon, void* scratch, fq_t* out_ext,
+                      uint32_t* out_raw, cudaStream_t st) {
   uint8_t* s = (uint8_t*)scratch;
   auto take = [&](size_t bytes) {
     uint8_t* r = s;
@@ -559,36 +555,25 @@ int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* c
     const int bit = w * p.c + p.c - 1;
     bo.v[bit >> 5] |= 1u << (bit & 31);
   }
-  int launches = 0;
   LB_CUDA_CHECK(cudaMemsetAsync(cnt, 0, ((size_t)p.total + 1) * 4, st));
   LB_CUDA_CHECK(cudaMemsetAsync(fill, 0, ((size_t)p.total + 1) * 4, st));
   LB_CUDA_CHECK(cudaMemsetAsync(totals, 0, 16, st));
   size_t b = (p.n + 255) / 256;
   if (b > (size_t)kNumSMs * 8) b = kNumSMs * 8;
-  msm_hist_kernel<<<(unsigned)b, 256, 0, st>>>(canon, p.n, p.c, p.nw, p.NB1, bo, cnt);
-  LB_LAUNCH_CHECK();
-  msm_scan_tiles_kernel<<<ntiles, 1024, 0, st>>>(cnt, p.total, p.S, off, uoff, tile_sums);
-  LB_LAUNCH_CHECK();
-  msm_scan_sums_kernel<<<1, 1024, 0, st>>>(tile_sums, ntiles, p.total, off, uoff, totals);
-  LB_LAUNCH_CHECK();
-  msm_scan_apply_kernel<<<ntiles, 1024, 0, st>>>(tile_sums, p.total, off, uoff);
-  LB_LAUNCH_CHECK();
-  msm_unit_map_kernel<<<(p.total + 255) / 256, 256, 0, st>>>(uoff, p.total, unit_bucket, multi, totals);
-  LB_LAUNCH_CHECK();
-  launches += 5;
+  launch(msm_hist_kernel, (unsigned)b, 256, 0, st, canon, p.n, p.c, p.nw, p.NB1, bo, cnt);
+  launch(msm_scan_tiles_kernel, ntiles, 1024, 0, st, cnt, p.total, p.S, off, uoff, tile_sums);
+  launch(msm_scan_sums_kernel, 1, 1024, 0, st, tile_sums, ntiles, p.total, off, uoff, totals);
+  launch(msm_scan_apply_kernel, ntiles, 1024, 0, st, tile_sums, p.total, off, uoff);
+  launch(msm_unit_map_kernel, (p.total + 255) / 256, 256, 0, st, uoff, p.total, unit_bucket, multi, totals);
   {
     size_t bx = (p.n + 255) / 256;
     if (bx > (size_t)kNumSMs * 4) bx = kNumSMs * 4;
     dim3 grid((unsigned)bx, (unsigned)p.nw);
-    msm_scatter_kernel<<<grid, 256, 0, st>>>(canon, p.n, p.c, p.NB1, bo, off, fill, entries);
-    LB_LAUNCH_CHECK();
+    launch(msm_scatter_kernel, grid, 256, 0, st, canon, p.n, p.c, p.NB1, bo, off, fill, entries);
   }
-  msm_accum_kernel<<<(unsigned)((p.max_units + 127) / 128), 128, 0, st>>>(niels, entries, cnt, off, uoff, unit_bucket, totals, p.S,
-                                                                        unit_sum);
-  LB_LAUNCH_CHECK();
-  msm_unit_combine_kernel<<<kNumSMs * 4, 256, 0, st>>>(unit_sum, uoff, multi, totals);
-  LB_LAUNCH_CHECK();
-  launches += 3;
+  launch(msm_accum_kernel, (unsigned)((p.max_units + 127) / 128), 128, 0, st, niels, entries, cnt, off, uoff,
+         unit_bucket, totals, p.S, unit_sum);
+  launch(msm_unit_combine_kernel, kNumSMs * 4, 256, 0, st, unit_sum, uoff, multi, totals);
   // bucket reduction, level by level
   MsmLevels lv;
   struct {
@@ -601,10 +586,8 @@ int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* c
     const uint32_t L = p.lev_L[k], n_out = p.lev_n[k];
     pt_ext* run_k = lev_run + (size_t)p.nw * pts_off;
     pt_ext* acc_k = lev_acc + (size_t)p.nw * pts_off;
-    msm_wsum_kernel<<<(unsigned)(((size_t)p.nw * n_out + 127) / 128), 128, 0, st>>>(unit_sum, uoff, p.NB1, prev_run, k, p.nw, items, L,
-                                                                                   run_k, acc_k);
-    LB_LAUNCH_CHECK();
-    launches++;
+    launch(msm_wsum_kernel, (unsigned)(((size_t)p.nw * n_out + 127) / 128), 128, 0, st, unit_sum, uoff, p.NB1,
+           prev_run, k, p.nw, items, L, run_k, acc_k);
     lv.acc[k] = acc_k;
     lv.n[k] = n_out;
     lg.v[k] = 0;
@@ -620,11 +603,9 @@ int launch_msm_large(const MsmLargePlan& p, const pt_niels* niels, const fr_t* c
   }
   {
     dim3 grid((unsigned)p.nw, (unsigned)p.nlev);
-    msm_psum_kernel<<<grid, 256, 0, st>>>(lv, p.nlev, A);
-    LB_LAUNCH_CHECK();
+    launch(msm_psum_kernel, grid, 256, 0, st, lv, p.nlev, A);
   }
   launch_msm_final(A, p.nlev, lg.v, p.nw, p.c, out_ext, out_raw, st);
-  return launches + 2;
 }
 
 }  // namespace lb

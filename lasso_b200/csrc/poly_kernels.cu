@@ -69,29 +69,25 @@ void launch_bind_top(fr_t* base, size_t stride, int npolys, size_t half, const f
   int per = kNumSMs * bps / npolys;
   if (per < kNumSMs / 4) per = kNumSMs / 4;
   dim3 grid(grid_for(half, kThreads, per), npolys);
-  bind_top_kernel<<<grid, kThreads, 0, st>>>(base, stride, half, r);
-  LB_LAUNCH_CHECK();
+  launch(bind_top_kernel, grid, kThreads, 0, st, base, stride, half, r);
 }
 void launch_bind_top_ptrs(fr_t* const* d_ptrs, int npolys, size_t half, const fr_t& r, cudaStream_t st) {
   if (half == 0 || npolys == 0) return;
   int per = kMaxBlocks / npolys;
   if (per < kNumSMs / 4) per = kNumSMs / 4;
   dim3 grid(grid_for(half, kThreads, per), npolys);
-  bind_top_ptrs_kernel<<<grid, kThreads, 0, st>>>(d_ptrs, half, r);
-  LB_LAUNCH_CHECK();
+  launch(bind_top_ptrs_kernel, grid, kThreads, 0, st, d_ptrs, half, r);
 }
 void launch_bind_ptrs(fr_t* const* d_src, fr_t* const* d_dst, int npolys, size_t half, const fr_t& r, cudaStream_t st) {
   if (half == 0 || npolys == 0) return;
   int per = kMaxBlocks / npolys;
   if (per < kNumSMs / 4) per = kNumSMs / 4;
   dim3 grid(grid_for(half, kThreads, per), npolys);
-  bind_ptrs_kernel<<<grid, kThreads, 0, st>>>(d_src, d_dst, half, r);
-  LB_LAUNCH_CHECK();
+  launch(bind_ptrs_kernel, grid, kThreads, 0, st, d_src, d_dst, half, r);
 }
 void launch_bind_bot(const fr_t* Z, fr_t* out, size_t half, const fr_t& r, cudaStream_t st) {
   if (half == 0) return;
-  bind_bot_kernel<<<grid_for(half), kThreads, 0, st>>>(Z, out, half, r);
-  LB_LAUNCH_CHECK();
+  launch(bind_bot_kernel, grid_for(half), kThreads, 0, st, Z, out, half, r);
 }
 
 // ------------------------------------------------------------------------------------ K4
@@ -130,8 +126,7 @@ __global__ void __launch_bounds__(kThreads) eq_outer_kernel(const fr_t* t_hi, co
 }
 void launch_eq_evals(const FrVec& r, int ell, fr_t* out, fr_t* scratch, cudaStream_t st) {
   if (ell <= 11) {
-    eq_small_kernel<<<1, 1024, 0, st>>>(r, 0, ell, out);
-    LB_LAUNCH_CHECK();
+    launch(eq_small_kernel, 1, 1024, 0, st, r, 0, ell, out);
     return;
   }
   int ell_lo = ell / 2 > 11 ? 11 : ell / 2;
@@ -141,21 +136,16 @@ void launch_eq_evals(const FrVec& r, int ell, fr_t* out, fr_t* scratch, cudaStre
     // tail of `out`, stage it in scratch (+4096) because the final pass overwrites that tail, then expand.
     fr_t* hi_tab = out + (((size_t)1 << ell) - ((size_t)1 << ell_hi));
     launch_eq_evals(r, ell_hi, hi_tab, scratch, st);
-    eq_small_kernel<<<1, 1024, 0, st>>>(r, ell_hi, ell_lo, scratch);
-    LB_LAUNCH_CHECK();
+    launch(eq_small_kernel, 1, 1024, 0, st, r, ell_hi, ell_lo, scratch);
     cudaMemcpyAsync(scratch + 4096, hi_tab, sizeof(fr_t) << ell_hi, cudaMemcpyDeviceToDevice, st);
     size_t n = (size_t)1 << ell;
-    eq_outer_kernel<<<grid_for(n), kThreads, 0, st>>>(scratch + 4096, scratch, ell_lo, n, out);
-    LB_LAUNCH_CHECK();
+    launch(eq_outer_kernel, grid_for(n), kThreads, 0, st, scratch + 4096, scratch, ell_lo, n, out);
     return;
   }
-  eq_small_kernel<<<1, 1024, 0, st>>>(r, 0, ell_hi, scratch);
-  LB_LAUNCH_CHECK();
-  eq_small_kernel<<<1, 1024, 0, st>>>(r, ell_hi, ell_lo, scratch + 4096);
-  LB_LAUNCH_CHECK();
+  launch(eq_small_kernel, 1, 1024, 0, st, r, 0, ell_hi, scratch);
+  launch(eq_small_kernel, 1, 1024, 0, st, r, ell_hi, ell_lo, scratch + 4096);
   size_t n = (size_t)1 << ell;
-  eq_outer_kernel<<<grid_for(n), kThreads, 0, st>>>(scratch, scratch + 4096, ell_lo, n, out);
-  LB_LAUNCH_CHECK();
+  launch(eq_outer_kernel, grid_for(n), kThreads, 0, st, scratch, scratch + 4096, ell_lo, n, out);
 }
 
 // ------------------------------------------------------------------------------------ partial-sum reduce
@@ -693,8 +683,7 @@ static int custom_grid(size_t n, size_t smem) {
 static void launch_eval_custom(const CustomStrategy& cs, const fr_t* base, size_t stride, size_t half, int npts,
                                const Finalize& fin, cudaStream_t st) {
   const size_t smem = custom_smem_bytes(cs, npts);
-  sc_eval_custom_kernel<<<custom_grid(half, smem), kCustomThreads, smem, st>>>(cs, base, stride, half, npts, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_eval_custom_kernel, custom_grid(half, smem), kCustomThreads, smem, st, cs, base, stride, half, npts, fin);
 }
 
 // combine_lookups weights are F::from(1u64 << (i * inc)): inc = log2 of the chunk size (and.rs:45-53, range_check.rs:78-86)
@@ -702,8 +691,7 @@ static int linear_inc(const Strategy& S) { return S.kind == STRAT_RANGE ? S.log_
 
 template <int C>
 static void launch_lt(const fr_t* base, size_t stride, size_t half, const Finalize& fin, int blocks, cudaStream_t st) {
-  sc_eval_lt_kernel<C><<<blocks, 128, 0, st>>>(base, stride, half, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_eval_lt_kernel<C>, blocks, 128, 0, st, base, stride, half, fin);
 }
 
 void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t stride, size_t half, const Finalize& fin,
@@ -720,8 +708,7 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
       case 4: launch_lt<4>(base, stride, half, fin, blocks, st); break;
       case 8:
         if (half >= 4096) {  // throughput-bound rounds: two lanes per pair (3 CTAs per SM instead of 2, no spills)
-          sc_eval_lt2_kernel<8><<<grid_for(2 * half, 128, kNumSMs * 6), 128, 0, st>>>(base, stride, half, fin);
-          LB_LAUNCH_CHECK();
+          launch(sc_eval_lt2_kernel<8>, grid_for(2 * half, 128, kNumSMs * 6), 128, 0, st, base, stride, half, fin);
         } else {
           launch_lt<8>(base, stride, half, fin, blocks, st);
         }
@@ -729,14 +716,12 @@ void launch_sumcheck_eval_arbitrary(const Strategy& S, const fr_t* base, size_t 
       default: {
         FrVec tv;
         for (int t = 0; t < 32; t++) tv.v[t] = fr_from_u64((uint64_t)t);
-        sc_eval_lt_generic_kernel<6><<<blocks, 128, 0, st>>>(base, stride, half, S.C, tv, fin);
-        LB_LAUNCH_CHECK();
+        launch(sc_eval_lt_generic_kernel<6>, blocks, 128, 0, st, base, stride, half, S.C, tv, fin);
       }
     }
   } else {
     blocks = grid_for(half);
-    sc_eval_linear_kernel<<<blocks, kThreads, 0, st>>>(base, stride, S.num_memories(), half, linear_inc(S), fin);
-    LB_LAUNCH_CHECK();
+    launch(sc_eval_linear_kernel, blocks, kThreads, 0, st, base, stride, S.num_memories(), half, linear_inc(S), fin);
   }
 }
 // bind with r (length 4q -> 2q) then evaluate the round over the bound polynomials, one launch; only the strategies
@@ -748,24 +733,21 @@ bool launch_sumcheck_bind_eval_arbitrary(const Strategy& S, fr_t* base, size_t s
                                          const Finalize& fin, size_t min_q, cudaStream_t st) {
   static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
   if (S.kind == STRAT_LT || S.kind == STRAT_CUSTOM || q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
-  sc_bind_eval_linear_kernel<<<grid_for(q, kThreads, kNumSMs * 2), kThreads, 0, st>>>(base, stride, S.num_memories(), q, r,
-                                                                                       linear_inc(S), fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_bind_eval_linear_kernel, grid_for(q, kThreads, kNumSMs * 2), kThreads, 0, st, base, stride, S.num_memories(),
+         q, r, linear_inc(S), fin);
   return true;
 }
 
 // ---- sumcheck over a caller's polynomials
 void launch_sumcheck_eval_comb(const CombProgram& g, const CombPtrs& in, size_t half, const Finalize& fin, cudaStream_t st) {
   const size_t smem = custom_smem_bytes(g, g.degree + 1);
-  sc_eval_comb_kernel<<<custom_grid(half, smem), kCustomThreads, smem, st>>>(g, in, half, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_eval_comb_kernel, custom_grid(half, smem), kCustomThreads, smem, st, g, in, half, fin);
 }
 void launch_bind_comb(const CombPtrs& src, const CombPtrs& dst, int n, size_t half, const fr_t& r, cudaStream_t st) {
   if (half == 0 || n == 0) return;
   int per = kNumSMs * kBindBlocksPerSM / n;
   if (per < kNumSMs / 4) per = kNumSMs / 4;
-  bind_comb_kernel<<<dim3(grid_for(half, kThreads, per), n), kThreads, 0, st>>>(src, dst, half, r);
-  LB_LAUNCH_CHECK();
+  launch(bind_comb_kernel, dim3(grid_for(half, kThreads, per), n), kThreads, 0, st, src, dst, half, r);
 }
 // The same threshold as the primary sumcheck's fused rounds: below q = 2^15 a round is a latency chain
 bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, const CombPtrs& dst, size_t q, const fr_t& r,
@@ -773,18 +755,15 @@ bool launch_sumcheck_bind_eval_comb(const CombProgram& g, const CombPtrs& src, c
   static const size_t dflt_min_q = (size_t)bind_env("LASSO_B200_FUSED_MIN_Q", 1 << 15);
   if (q == 0 || q < (min_q ? min_q : dflt_min_q)) return false;
   const size_t smem = custom_smem_bytes(g, g.degree + 1);
-  sc_bind_eval_comb_kernel<<<custom_grid(q, smem), kCustomThreads, smem, st>>>(g, src, dst, q, r, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_bind_eval_comb_kernel, custom_grid(q, smem), kCustomThreads, smem, st, g, src, dst, q, r, fin);
   return true;
 }
 void launch_final_comb(const CombPtrs& src, int n, size_t half, const fr_t& r, const Finalize& fin, cudaStream_t st) {
-  final_comb_kernel<<<1, 32, 0, st>>>(src, n, half, r, fin);
-  LB_LAUNCH_CHECK();
+  launch(final_comb_kernel, 1, 32, 0, st, src, n, half, r, fin);
 }
 void launch_comb_map(const CombProgram& g, const CombPtrs& in, size_t n, fr_t* out, cudaStream_t st) {
   const size_t smem = custom_smem_bytes(g, 0);
-  comb_map_kernel<<<custom_grid(n, smem), kCustomThreads, smem, st>>>(g, in, n, out);
-  LB_LAUNCH_CHECK();
+  launch(comb_map_kernel, custom_grid(n, smem), kCustomThreads, smem, st, g, in, n, out);
 }
 
 // subtables/mod.rs:186-216: sum_k eq[k] * g(E_1[k], ..., E_alpha[k]) over the whole hypercube
@@ -823,14 +802,12 @@ void launch_sumcheck_claim(const Strategy& S, const fr_t* base, size_t stride, s
   if (S.kind == STRAT_CUSTOM) {
     const size_t smem = custom_smem_bytes(*S.custom, 0);
     blocks = custom_grid(n, smem);
-    claim_custom_kernel<<<blocks, kCustomThreads, smem, st>>>(*S.custom, base, stride, n, partial);
+    launch(claim_custom_kernel, blocks, kCustomThreads, smem, st, *S.custom, base, stride, n, partial);
   } else if (S.kind == STRAT_LT)
-    claim_lt_kernel<<<blocks, kThreads, 0, st>>>(base, stride, S.C, n, partial);
+    launch(claim_lt_kernel, blocks, kThreads, 0, st, base, stride, S.C, n, partial);
   else
-    claim_linear_kernel<<<blocks, kThreads, 0, st>>>(base, stride, S.num_memories(), n, linear_inc(S), partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<1, kThreads, 0, st>>>(partial, blocks, out);
-  LB_LAUNCH_CHECK();
+    launch(claim_linear_kernel, blocks, kThreads, 0, st, base, stride, S.num_memories(), n, linear_inc(S), partial);
+  launch(reduce_partials_kernel, 1, kThreads, 0, st, partial, blocks, out);
 }
 
 // ------------------------------------------------------------------------------------ K3
@@ -1029,12 +1006,10 @@ static void launch_cubic_quad(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Ci
   const size_t threads = 4 * (size_t)ncirc * q;
   if (threads <= 1024) {
     unsigned t = (unsigned)((threads + 31) / 32 * 32);
-    sc_cubic_quad_kernel<<<1, t, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
-    LB_LAUNCH_CHECK();
+    launch(sc_cubic_quad_kernel, 1, t, 0, st, d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
   } else {
     unsigned blocks = (unsigned)(((size_t)ncirc * q + 63) / 64);
-    sc_cubic_quad_kernel<<<blocks, 256, 0, st>>>(d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
-    LB_LAUNCH_CHECK();
+    launch(sc_cubic_quad_kernel, blocks, 256, 0, st, d_A, d_B, Cin, Cout, q, lg_q, do_bind, r, ncirc, cf, scale, fin);
   }
 }
 // circuits are strided over blockIdx.y: enough CTAs for ~2 per SM even when a round has few pairs
@@ -1049,15 +1024,14 @@ void launch_sumcheck_bind_eval_cubic_comb(fr_t* const* d_A, fr_t* const* d_B, co
                                           const fr_t& r, const CubicCoeffs& cf, int scale, const Finalize& fin, cudaStream_t st) {
   size_t q = h / 2;
   if (q <= kQuadMaxQ && (q & (q - 1)) == 0) return launch_cubic_quad(d_A, d_B, Cin, Cout, ncirc, q, 1, r, cf, scale, fin, st);
-  sc_bind_eval_cubic_comb_kernel<<<comb_grid(q, ncirc), kThreads, 0, st>>>(d_A, d_B, Cin, Cout, h, r, ncirc, cf, scale, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_bind_eval_cubic_comb_kernel, comb_grid(q, ncirc), kThreads, 0, st, d_A, d_B, Cin, Cout, h, r, ncirc, cf,
+         scale, fin);
 }
 void launch_sumcheck_eval_cubic_comb(fr_t* const* d_A, fr_t* const* d_B, const fr_t* Ceq, int ncirc, size_t half,
                                      const CubicCoeffs& cf, int scale, const Finalize& fin, cudaStream_t st) {
   if (half <= kQuadMaxQ && (half & (half - 1)) == 0)
     return launch_cubic_quad(d_A, d_B, Ceq, nullptr, ncirc, half, 0, fr_zero(), cf, scale, fin, st);
-  sc_eval_cubic_comb_kernel<<<comb_grid(half, ncirc), kThreads, 0, st>>>(d_A, d_B, Ceq, half, ncirc, cf, scale, fin);
-  LB_LAUNCH_CHECK();
+  launch(sc_eval_cubic_comb_kernel, comb_grid(half, ncirc), kThreads, 0, st, d_A, d_B, Ceq, half, ncirc, cf, scale, fin);
 }
 
 // ------------------------------------------------------------------------------------ K5
@@ -1088,9 +1062,8 @@ __global__ void __launch_bounds__(kThreads)
 void launch_materialize_subtables(const Strategy& S, fr_t* tables_fr, uint32_t* tables_u32, cudaStream_t st) {
   if (S.kind == STRAT_CUSTOM) throw std::runtime_error("a custom strategy's tables are uploaded, not materialised");
   size_t n = (size_t)S.M() * S.num_subtables();
-  materialize_kernel<<<grid_for(n), kThreads, 0, st>>>(S.kind, S.num_subtables(), S.log_m, S.log_r, tables_fr,
-                                                       tables_u32);
-  LB_LAUNCH_CHECK();
+  launch(materialize_kernel, grid_for(n), kThreads, 0, st, S.kind, S.num_subtables(), S.log_m, S.log_r, tables_fr,
+         tables_u32);
 }
 struct GatherMap {
   int sub[32], dim[32];
@@ -1117,15 +1090,14 @@ void launch_gather_lookup_polys(const Strategy& S, const fr_t* tables_fr, const 
     map.dim[k] = S.memory_to_dimension_index(k);
   }
   dim3 grid(grid_for(s, kThreads, kMaxBlocks / S.num_memories() + 1), S.num_memories());
-  gather_kernel<<<grid, kThreads, 0, st>>>(map, S.log_m, tables_fr, tables_u32, nz, s, E_fr, E_stride, E_u32);
-  LB_LAUNCH_CHECK();
+  launch(gather_kernel, grid, kThreads, 0, st, map, S.log_m, tables_fr, tables_u32, nz, s, E_fr, E_stride, E_u32);
 }
 __global__ void __launch_bounds__(kThreads) from_u32_kernel(const uint32_t* in, fr_t* out, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     st_fr(out + i, fr_from_u64(in[i]));
 }
 void launch_from_u32(const uint32_t* in, fr_t* out, size_t n, cudaStream_t st) {
-  if (n) from_u32_kernel<<<grid_for(n), kThreads, 0, st>>>(in, out, n);
+  if (n) launch(from_u32_kernel, grid_for(n), kThreads, 0, st, in, out, n);
 }
 void launch_fill_zero(fr_t* out, size_t n, cudaStream_t st) {
   if (n) cudaMemsetAsync(out, 0, n * sizeof(fr_t), st);
@@ -1201,10 +1173,9 @@ void launch_bound_u32(const uint32_t* Z, const fr_t* L, size_t L_size, size_t R_
   size_t rows_per_chunk = (L_size + chunks - 1) / chunks;
   if (rows_per_chunk > ((size_t)1 << 20)) throw std::runtime_error("bound_u32: too many rows per chunk");
   dim3 grid((unsigned)((R_size + kThreads - 1) / kThreads), chunks);
-  bound_u32_kernel<<<grid, kThreads, 0, st>>>(Z, L, L_size, R_size, rows_per_chunk, partial);
-  LB_LAUNCH_CHECK();
-  bound_reduce_kernel<<<(unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st>>>(partial, chunks, R_size, out);
-  LB_LAUNCH_CHECK();
+  launch(bound_u32_kernel, grid, kThreads, 0, st, Z, L, L_size, R_size, rows_per_chunk, partial);
+  launch(bound_reduce_kernel, (unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st, partial, chunks, R_size,
+         out);
 }
 // out[k] = <z_k, eq>, z_k = base + k*stride (u32), k < npolys
 __global__ void __launch_bounds__(kThreads)
@@ -1225,10 +1196,8 @@ void launch_multi_dot_u32(const uint32_t* base, size_t stride, int npolys, const
   if (per < 1) per = 1;
   int bx = grid_for(n, kThreads, per);
   dim3 grid(bx, npolys);
-  multi_dot_u32_kernel<<<grid, kThreads, 0, st>>>(base, stride, eq, n, partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
-  LB_LAUNCH_CHECK();
+  launch(multi_dot_u32_kernel, grid, kThreads, 0, st, base, stride, eq, n, partial);
+  launch(reduce_partials_kernel, npolys, kThreads, 0, st, partial, bx, out);
 }
 // The Fr twins, for the lookup values of a caller's table of arbitrary field elements (no u32 mirror): a Montgomery
 // product per term.  Same chunks x R_size partials and the same second passes as the u32 forms.
@@ -1254,10 +1223,9 @@ void launch_bound_fr(const fr_t* Z, const fr_t* L, size_t L_size, size_t R_size,
   int chunks = (int)(L_size < (size_t)kBoundChunks ? L_size : (size_t)kBoundChunks);
   size_t rows_per_chunk = (L_size + chunks - 1) / chunks;
   dim3 grid((unsigned)((R_size + kThreads - 1) / kThreads), chunks);
-  bound_fr_kernel<<<grid, kThreads, 0, st>>>(Z, L, L_size, R_size, rows_per_chunk, partial);
-  LB_LAUNCH_CHECK();
-  bound_reduce_kernel<<<(unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st>>>(partial, chunks, R_size, out);
-  LB_LAUNCH_CHECK();
+  launch(bound_fr_kernel, grid, kThreads, 0, st, Z, L, L_size, R_size, rows_per_chunk, partial);
+  launch(bound_reduce_kernel, (unsigned)((R_size + kThreads - 1) / kThreads), kThreads, 0, st, partial, chunks, R_size,
+         out);
 }
 __global__ void __launch_bounds__(kThreads)
     multi_dot_fr_kernel(const fr_t* base, size_t stride, const fr_t* eq, size_t n, fr_t* partial) {
@@ -1275,10 +1243,8 @@ void launch_multi_dot_fr(const fr_t* base, size_t stride, int npolys, const fr_t
   if (per < 1) per = 1;
   int bx = grid_for(n, kThreads, per);
   dim3 grid(bx, npolys);
-  multi_dot_fr_kernel<<<grid, kThreads, 0, st>>>(base, stride, eq, n, partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<npolys, kThreads, 0, st>>>(partial, bx, out);
-  LB_LAUNCH_CHECK();
+  launch(multi_dot_fr_kernel, grid, kThreads, 0, st, base, stride, eq, n, partial);
+  launch(reduce_partials_kernel, npolys, kThreads, 0, st, partial, bx, out);
 }
 // The pointer-table forms, for k independent polynomials of one length (lasso_poly_evaluate_batch): CTA row blockIdx.y
 // takes the group of kDotGroup inputs from kDotGroup * blockIdx.y, and a thread reads each eq element once for all the
@@ -1333,12 +1299,10 @@ void launch_multi_dot_ptrs(const DotPtrs& in, int k, bool u32, const fr_t* eq, s
   const int bx = grid_for(n, kThreads, per);
   const dim3 grid(bx, groups);
   if (u32)
-    multi_dot_ptrs_u32_kernel<<<grid, kThreads, 0, st>>>(in, k, eq, n, partial);
+    launch(multi_dot_ptrs_u32_kernel, grid, kThreads, 0, st, in, k, eq, n, partial);
   else
-    multi_dot_ptrs_fr_kernel<<<grid, kThreads, 0, st>>>(in, k, eq, n, partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<k, kThreads, 0, st>>>(partial, bx, out);
-  LB_LAUNCH_CHECK();
+    launch(multi_dot_ptrs_fr_kernel, grid, kThreads, 0, st, in, k, eq, n, partial);
+  launch(reduce_partials_kernel, k, kThreads, 0, st, partial, bx, out);
 }
 
 // memory_checking.rs:249-252: hash(a, v, t) = t*gamma^2 + v*gamma + a - tau
@@ -1365,16 +1329,14 @@ __global__ void __launch_bounds__(kThreads)
 }
 void launch_gp_fingerprints_mem(const fr_t* table, const fr_t* final_fr, size_t M_local, int G, int g,
                                 const fr_t& gamma, const fr_t& tau, fr_t* out_init, fr_t* out_final, cudaStream_t st) {
-  fp_mem_kernel<<<grid_for(M_local), kThreads, 0, st>>>(table, final_fr, M_local, G, g, gamma, fr_sqr(gamma), tau,
-                                                        out_init, out_final);
-  LB_LAUNCH_CHECK();
+  launch(fp_mem_kernel, grid_for(M_local), kThreads, 0, st, table, final_fr, M_local, G, g, gamma, fr_sqr(gamma), tau,
+         out_init, out_final);
 }
 void launch_gp_fingerprints_ops(const fr_t* dim_fr, const fr_t* E_fr, const fr_t* read_fr, size_t s,
                                 const fr_t& gamma, const fr_t& tau, fr_t* out_read, fr_t* out_write,
                                 cudaStream_t st) {
-  fp_ops_kernel<<<grid_for(s), kThreads, 0, st>>>(dim_fr, E_fr, read_fr, s, gamma, fr_sqr(gamma), tau, out_read,
-                                                  out_write);
-  LB_LAUNCH_CHECK();
+  launch(fp_ops_kernel, grid_for(s), kThreads, 0, st, dim_fr, E_fr, read_fr, s, gamma, fr_sqr(gamma), tau, out_read,
+         out_write);
 }
 
 // grand_product.rs:20-58, all product trees of one size at once (single GPU).  A tree is one contiguous array: layer 0 (N elements),
@@ -1410,18 +1372,11 @@ void launch_product_trees(const TreePtrs& trees, int ntrees, size_t N, int slot0
   while (len > 4096) {
     const size_t n_out = len / 2;
     dim3 grid(grid_for(n_out, kThreads, kMaxBlocks / ntrees + 1), ntrees);
-    product_layers_kernel<<<grid, kThreads, 0, st>>>(trees, off, n_out);
-    LB_LAUNCH_CHECK();
+    launch(product_layers_kernel, grid, kThreads, 0, st, trees, off, n_out);
     off += len;
     len = n_out;
   }
-  product_tail_kernel<<<ntrees, 1024, 0, st>>>(trees, off, len, slot0, stop_len, fin);
-  LB_LAUNCH_CHECK();
-}
-int product_trees_launches(size_t N) {
-  int n = 1;
-  for (size_t len = N; len > 4096; len /= 2) n++;
-  return n;
+  launch(product_tail_kernel, ntrees, 1024, 0, st, trees, off, len, slot0, stop_len, fin);
 }
 // layer 1 of a caller's circuit from its polynomial P (layer 0, only read): out[i] = P[i] * P[i + half]
 __global__ void __launch_bounds__(kThreads) product_layer1_kernel(const fr_t* P, fr_t* out, size_t half) {
@@ -1429,8 +1384,7 @@ __global__ void __launch_bounds__(kThreads) product_layer1_kernel(const fr_t* P,
     st_fr(out + i, fr_mul(ld_fr(P + i), ld_fr(P + half + i)));
 }
 void launch_product_layer1(const fr_t* P, fr_t* out, size_t half, cudaStream_t st) {
-  product_layer1_kernel<<<grid_for(half), kThreads, 0, st>>>(P, out, half);
-  LB_LAUNCH_CHECK();
+  launch(product_layer1_kernel, grid_for(half), kThreads, 0, st, P, out, half);
 }
 // last round of a batched cubic sumcheck (one element pair left per array): bind the 2*ncirc heads with r in
 // place and publish them — they are the layer's claims (grand_product.rs:139-150)
@@ -1444,8 +1398,7 @@ __global__ void bind_heads_kernel(fr_t* const* AB, int n, fr_t r, Finalize fin) 
   finalize_publish(fin, k, v);
 }
 void launch_bind_heads(fr_t* const* d_AB, int n, const fr_t& r, const Finalize& fin, cudaStream_t st) {
-  bind_heads_kernel<<<1, (n + 31) / 32 * 32, 0, st>>>(d_AB, n, r, fin);
-  LB_LAUNCH_CHECK();
+  launch(bind_heads_kernel, 1, (n + 31) / 32 * 32, 0, st, d_AB, n, r, fin);
 }
 
 // ---- Bulletproofs scalar-side helpers (bullet.rs:73-134) ----
@@ -1457,8 +1410,7 @@ __global__ void __launch_bounds__(kThreads) fold_ab_kernel(fr_t* a, fr_t* b, siz
   }
 }
 void launch_fold_ab(fr_t* a, fr_t* b, size_t h, const fr_t& u, const fr_t& uinv, cudaStream_t st) {
-  fold_ab_kernel<<<grid_for(h), kThreads, 0, st>>>(a, b, h, u, uinv);
-  LB_LAUNCH_CHECK();
+  launch(fold_ab_kernel, grid_for(h), kThreads, 0, st, a, b, h, u, uinv);
 }
 __global__ void __launch_bounds__(kThreads) cross_ip_kernel(const fr_t* a, const fr_t* b, size_t h, fr_t* partial) {
   __shared__ fr_t scratch[2 * kThreads / 32];
@@ -1475,10 +1427,8 @@ __global__ void __launch_bounds__(kThreads) cross_ip_kernel(const fr_t* a, const
 }
 void launch_cross_inner_products(const fr_t* a, const fr_t* b, size_t h, fr_t* partial, fr_t* out, cudaStream_t st) {
   int bx = grid_for(h, kThreads, 64);
-  cross_ip_kernel<<<bx, kThreads, 0, st>>>(a, b, h, partial);
-  LB_LAUNCH_CHECK();
-  reduce_partials_kernel<<<2, kThreads, 0, st>>>(partial, bx, out);
-  LB_LAUNCH_CHECK();
+  launch(cross_ip_kernel, bx, kThreads, 0, st, a, b, h, partial);
+  launch(reduce_partials_kernel, 2, kThreads, 0, st, partial, bx, out);
 }
 __global__ void __launch_bounds__(kThreads)
     expand_weights_kernel(const fr_t* w, fr_t* w_out, size_t n_in, fr_t u, fr_t uinv) {
@@ -1489,8 +1439,7 @@ __global__ void __launch_bounds__(kThreads)
   }
 }
 void launch_expand_weights(const fr_t* w, fr_t* w_out, size_t n_in, const fr_t& u, const fr_t& uinv, cudaStream_t st) {
-  expand_weights_kernel<<<grid_for(n_in), kThreads, 0, st>>>(w, w_out, n_in, u, uinv);
-  LB_LAUNCH_CHECK();
+  launch(expand_weights_kernel, grid_for(n_in), kThreads, 0, st, w, w_out, n_in, u, uinv);
 }
 // Round with current vector length m (half h = m/2) over n original generators, weights w[t], t < n/m.
 // Global column j = t*m + pos:   sL[j] = a[pos-h] * w[t] for pos >= h (else 0),
@@ -1519,8 +1468,7 @@ __global__ void __launch_bounds__(kThreads)
 }
 void launch_bullet_scalars(const fr_t* a, const fr_t* w, size_t n_loc, size_t m, int G, int g, int a_rep, fr_t* sL,
                            fr_t* sR, cudaStream_t st) {
-  bullet_scalars_kernel<<<grid_for(n_loc), kThreads, 0, st>>>(a, w, n_loc, m, G, g, a_rep, sL, sR);
-  LB_LAUNCH_CHECK();
+  launch(bullet_scalars_kernel, grid_for(n_loc), kThreads, 0, st, a, w, n_loc, m, G, g, a_rep, sL, sR);
 }
 // Two MSM rows over the n + 2 generators (G_0..G_{n-1}, Q, h) in canonical form:
 //   row 0 = (k * v[0..n), t00, t01)    row 1 = (0 .. 0, t10, t11)
@@ -1543,16 +1491,14 @@ __global__ void __launch_bounds__(kThreads)
 }
 void launch_two_row_scalars(const fr_t* v, int scale, const fr_t& k, const fr_t& t00, const fr_t& t01, const fr_t& t10,
                             const fr_t& t11, size_t n, fr_t* out, cudaStream_t st) {
-  two_row_scalars_kernel<<<grid_for(n + 2), kThreads, 0, st>>>(v, scale, k, t00, t01, t10, t11, n, out);
-  LB_LAUNCH_CHECK();
+  launch(two_row_scalars_kernel, grid_for(n + 2), kThreads, 0, st, v, scale, k, t00, t01, t10, t11, n, out);
 }
 __global__ void __launch_bounds__(kThreads) scale_kernel(const fr_t* in, fr_t* out, size_t n, fr_t k) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
     st_fr(out + i, fr_mul(ld_fr(in + i), k));
 }
 void launch_scale(const fr_t* in, fr_t* out, size_t n, const fr_t& k, cudaStream_t st) {
-  scale_kernel<<<grid_for(n), kThreads, 0, st>>>(in, out, n, k);
-  LB_LAUNCH_CHECK();
+  launch(scale_kernel, grid_for(n), kThreads, 0, st, in, out, n, k);
 }
 
 }  // namespace lb

@@ -27,8 +27,6 @@
 
 namespace lb {
 
-std::atomic<unsigned long long> g_launches{0};
-
 // ---------------------------------------------------------------------------------------------- context
 __global__ void publish_kernel(const uint32_t* src, int nwords, uint32_t* mapped, uint32_t seq) {
   for (int i = threadIdx.x; i < nwords; i += blockDim.x) mapped[i] = src[i];
@@ -41,8 +39,7 @@ __global__ void publish_kernel(const uint32_t* src, int nwords, uint32_t* mapped
 }
 void Ctx::d2h_small(void* dst, const void* src, size_t bytes) {
   const uint32_t seq = ++mapped_seq;
-  publish_kernel<<<1, 128, 0, st>>>((const uint32_t*)src, (int)((bytes + 3) / 4), d_mapped, seq);
-  g_launches += 1;
+  launch(publish_kernel, 1, 128, 0, st, (const uint32_t*)src, (int)((bytes + 3) / 4), d_mapped, seq);
   wait_flag(seq);
   memcpy(dst, (const void*)h_mapped, bytes);
 }
@@ -269,7 +266,6 @@ static FrVec to_frvec(const std::vector<fr_t>& v, size_t off, size_t n) {
 // eq(r) table on the device (eq_poly.rs:21-38)
 static void eq_evals_dev(Ctx* c, const std::vector<fr_t>& r, size_t off, size_t ell, fr_t* out) {
   launch_eq_evals(to_frvec(r, off, ell), (int)ell, out, c->d_eq_scratch, c->st);
-  g_launches += ell <= 11 ? 1 : (ell <= 22 ? 3 : 5);
 }
 
 // ---------------------------------------------------------------------------------------------- generators
@@ -288,7 +284,6 @@ static void gens_build_tables(Ctx* c, Gens* g, const uint64_t* stream_affine, si
   LB_CUDA_CHECK(cudaMemcpyAsync(g->d_bases_ark.p, stream_affine, n_points * 64, cudaMemcpyHostToDevice, c->st));
   g->d_table.alloc(c, (size_t)kMsmFullWindows * n_points);
   launch_build_table(g->d_bases_ark.p, n_points, g->d_table.p, n_points, kMsmFullWindows, c->st);
-  g_launches += kMsmFullWindows;
   {
     size_t nd = widest_R + 2;
     const char* off = getenv("LASSO_B200_NO_MULTIPLES");
@@ -305,7 +300,6 @@ static void gens_build_tables(Ctx* c, Gens* g, const uint64_t* stream_affine, si
       g->n_direct = nd;
       g->d_multiples.alloc(c, (size_t)kMsmFullWindows * nd * 128);
       launch_build_multiples(g->d_table.p, n_points, nd, kMsmFullWindows, g->d_multiples.p, c->st);
-      g_launches += 1;
       const char* cap = getenv("LASSO_B200_TABLE_GB");
       const double cap_gb = cap ? atof(cap) : 64.0;
       const size_t ncols16 = (nd - 2) / G;  // this rank's columns: generators j * G + rank
@@ -314,11 +308,9 @@ static void gens_build_tables(Ctx* c, Gens* g, const uint64_t* stream_affine, si
         g->n_direct16 = ncols16;
         g->d_multiples16.alloc(c, ncols16 * 32768);
         launch_build_multiples16(g->d_table.p, g->d_multiples.p, nd, ncols16, G, gr, g->d_multiples16.p, c->st);
-        g_launches += 1;
         g->d_centre.alloc(c, 32);
         for (size_t k = 0; ((size_t)1 << k) <= ncols16 && k < 32; k++) {  // one constant per power-of-two (local) row length
           launch_centre_constant(g->d_multiples16.p, 1 << k, g->d_centre.p + k, c->st);
-          g_launches += 1;
         }
       }
     }
@@ -371,9 +363,7 @@ __global__ void publish_fr_kernel(const fr_t* src, int count, PubDst pub) {
 static Finalize reduce_to_host_begin(Ctx* c, const fr_t* d_buf, int count) {
   if (count > kPubElems) throw std::runtime_error("message larger than a publication region");
   Finalize f = c->fin_begin(true);
-  publish_fr_kernel<<<1, 128, 0, c->st>>>(d_buf, count, f.pub);
-  LB_LAUNCH_CHECK();
-  g_launches += 1;
+  launch(publish_fr_kernel, 1, 128, 0, c->st, d_buf, count, f.pub);
   return f;
 }
 static void reduce_to_host(Ctx* c, const fr_t* d_buf, int count, fr_t* h_out) {
@@ -393,7 +383,6 @@ static void eq_evals_shard(Ctx* c, const std::vector<fr_t>& r, size_t off, size_
     k = fr_mul(k, bit ? rj : fr_sub(fr_one(), rj));
   }
   launch_scale(out, out, (size_t)1 << (ell - lg), k, c->st);
-  g_launches += 1;
 }
 
 // ---------------------------------------------------------------------------------------------- MSM helpers
@@ -411,7 +400,6 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
     DBuf<uint32_t> comp(c, (size_t)nrows * 8);
     launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, 1, 0, part.p, nullptr, comp.p,
                     nullptr, c->st);
-    g_launches += 2;
     c->d2h(out.data(), comp.p, out.size());
     return out;
   }
@@ -420,13 +408,11 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
   uint32_t* mine = raw.p + (size_t)G * nrows * 32;  // scratch slot for this rank's partials
   launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, G, gr, part.p, nullptr, nullptr,
                   G == 1 ? raw.p : mine, c->st);
-  g_launches += 2;
   if (G > 1) comm_allgather(c, mine, raw.p, (size_t)nrows * 128);
   if (few) {
     uint32_t xyzt[8 * 32];
     if (G > 1) {
       launch_sum_raw_points(raw.p, G, nrows, mine, nullptr, nullptr, c->st);
-      g_launches += 1;
       c->d2h(xyzt, mine, (size_t)nrows * 128);
     } else {
       c->d2h(xyzt, raw.p, (size_t)nrows * 128);
@@ -438,7 +424,6 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
   }
   DBuf<uint32_t> comp(c, (size_t)nrows * 8);
   launch_sum_raw_points(raw.p, G, nrows, nullptr, comp.p, nullptr, c->st);
-  g_launches += 1;
   c->d2h(out.data(), comp.p, out.size());
   return out;
 }
@@ -447,7 +432,6 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
 static std::vector<uint8_t> msm_rows_fr(Ctx* c, const Gens& g, const fr_t* d_scal_mont, int nrows, int ncols) {
   DBuf<fr_t> canon(c, (size_t)nrows * ncols);
   launch_canonicalize(d_scal_mont, canon.p, (size_t)nrows * ncols, c->d_flag, c->st);
-  g_launches += 1;
   return msm_rows(c, g, canon.p, 8, (size_t)ncols, nrows, ncols, kMsmFullWindows, true);
 }
 
@@ -473,7 +457,6 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
     if (G == 1) {  // normalised on the device
       launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr,
                                  comp.p, nullptr, c->st);
-      g_launches += 2;
     } else {  // this rank's columns of every row -> partial points -> gather-then-add over the ranks
       DBuf<uint32_t> raw(c, (size_t)(G + 1) * L * 32);
       uint32_t* mine = raw.p + (size_t)G * L * 32;
@@ -481,7 +464,6 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
                                  part.p, nullptr, nullptr, mine, c->st);
       comm_allgather(c, mine, raw.p, L * 128);
       launch_sum_raw_points(raw.p, G, (int)L, nullptr, comp.p, nullptr, c->st);
-      g_launches += 3;
       c->d2h(out.data(), comp.p, out.size());
       return out;
     }
@@ -502,7 +484,6 @@ static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_
   if (!(g.d_multiples.p && R + 2 <= g.n_direct)) {
     DBuf<fr_t> canon(c, L * R_loc);
     launch_canonicalize(d_vals_loc, canon.p, L * R_loc, c->d_flag, c->st);
-    g_launches += 1;
     return msm_rows(c, g, canon.p, 8, R_loc, (int)L, (int)R_loc, kMsmFullWindows, false);
   }
   // rows as direct sums over the 8-bit digit-multiples tables: one table entry per non-zero signed digit
@@ -513,7 +494,6 @@ static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_
   if (G == 1) {
     launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, comp.p,
                               nullptr, c->st);
-    g_launches += 2;
   } else {  // this rank's columns of every row -> partial points -> gather-then-add over the ranks
     DBuf<uint32_t> raw(c, (size_t)(G + 1) * L * 32);
     uint32_t* mine = raw.p + (size_t)G * L * 32;
@@ -521,7 +501,6 @@ static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_
                               nullptr, nullptr, mine, c->st);
     comm_allgather(c, mine, raw.p, L * 128);
     launch_sum_raw_points(raw.p, G, (int)L, nullptr, comp.p, nullptr, c->st);
-    g_launches += 3;
   }
   c->d2h(out.data(), comp.p, out.size());
   return out;
@@ -579,11 +558,10 @@ static void densify_on_device(Ctx* c, Dense* d, size_t n, const DzIndices& idx, 
   DBuf<uint32_t> scratch(c, densify_scratch_words(s, (int)C, d->log_m));
   if (nl > 2 * C * s_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_l_u32.p + 2 * C * s_loc, 0, (nl - 2 * C * s_loc) * 4, c->st));
   if (nm > C * m_loc) LB_CUDA_CHECK(cudaMemsetAsync(d->d_m_u32.p + C * m_loc, 0, (nm - C * m_loc) * 4, c->st));
-  g_launches += launch_densify(idx, check, n, s, (int)C, d->log_m, (int)G, (int)gr, scratch.p, d->d_l_u32.p, s_loc,
-                               d->d_l_u32.p + C * s_loc, s_loc, d->d_m_u32.p, m_loc, c->st);
+  launch_densify(idx, check, n, s, (int)C, d->log_m, (int)G, (int)gr, scratch.p, d->d_l_u32.p, s_loc,
+                 d->d_l_u32.p + C * s_loc, s_loc, d->d_m_u32.p, m_loc, c->st);
   launch_from_u32(d->d_l_u32.p, d->d_l_fr.p, nl, c->st);  // DensePolynomial::from_usize + merge
   launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
-  g_launches += 2;
 }
 
 Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m, int* err) {
@@ -751,7 +729,6 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
   LB_CUDA_CHECK(cudaMemcpyAsync(d->d_m_u32.p, m_host, nm * 4, cudaMemcpyHostToDevice, c->st));
   launch_from_u32(d->d_l_u32.p, d->d_l_fr.p, nl, c->st);  // DensePolynomial::from_usize + merge
   launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
-  g_launches += 2;
   c->sync();
   return d.release();
 }
@@ -908,7 +885,6 @@ static SumcheckProof prove_arbitrary(Ctx* c, const Strategy& S, fr_t* base, size
   auto flush_bind = [&]() {
     if (!pending) return;
     launch_bind_top(base, stride, npolys, len, r_pending, c->st);
-    g_launches += 1;
     pending = false;
   };
   for (;;) {
@@ -933,7 +909,6 @@ static SumcheckProof prove_arbitrary(Ctx* c, const Strategy& S, fr_t* base, size
       }
       c->fin_wait(f, evals.data(), npts);
     }
-    g_launches += 1;
     std::vector<fr_t> coeffs = unipoly_from_evals(evals);
     unipoly_append(coeffs, transcript);
     fr_t r_j = transcript.challenge_scalar("challenge_nextround");
@@ -983,7 +958,6 @@ static void build_trees(Ctx* c, std::vector<std::vector<Circuit*>>& groups, cons
       if (pend.size() >= (size_t)kPubRegions) throw std::runtime_error("too many product-tree batches in flight");
       Finalize f = c->fin_begin(G > 1);
       launch_product_trees(tp, nt, sizes[gi] / (size_t)G, 0, G == 1 ? 2 : 1, f, c->st);
-      g_launches += product_trees_launches(sizes[gi] / (size_t)G);
       pend.push_back({f, gi, t0, nt});
     }
   }
@@ -1126,7 +1100,6 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
       if (!have_evals) {  // first round of a phase; later rounds come out of the fused bind+eval kernel
         fz = c->fin_begin(sharded);
         launch_sumcheck_eval_cubic_comb(dA, dB, Ccur, ncirc, cur / 2, cf, stored_scaled ? 0 : 1, fz, c->st);
-        g_launches += 1;
       }
       if (inv_coeff.empty()) {  // 1 / coeff_k by Montgomery's trick, overlapping the kernel just launched
         inv_coeff.resize(ncirc);
@@ -1163,12 +1136,10 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
         dAB = slot_AB(1);
         on_caller = false;
         have_evals = false;
-        g_launches += 1;
         if (half > 1) {
           std::swap(Ccur, Cnext);
           fz = c->fin_begin();
           launch_sumcheck_eval_cubic_comb(dA, dB, Ccur, ncirc, half / 2, cf, 1, fz, c->st);
-          g_launches += 1;
           have_evals = true;
         }
       } else if (half > 1) {
@@ -1176,20 +1147,17 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
         fz = c->fin_begin(sharded);
         launch_sumcheck_bind_eval_cubic_comb(dA, dB, Ccur, Cnext, ncirc, half, r_j, cf, stored_scaled ? 0 : 1, fz, c->st);
         stored_scaled = true;
-        g_launches += 1;
         std::swap(Ccur, Cnext);
         have_evals = true;
       } else if (!sharded) {
         // last round: bind the 2*ncirc heads and publish them (the layer's claims); eq is not needed any more
         fz = c->fin_begin();
         launch_bind_heads(dAB, 2 * ncirc, r_j, fz, c->st);
-        g_launches += 1;
         have_evals = false;
         heads_published = true;
       } else {
         launch_bind_top_ptrs(dAB, 2 * ncirc, half, r_j, c->st);
         launch_bind_top(Ccur, 0, 1, half, r_j, c->st);
-        g_launches += 2;
         have_evals = false;
       }
       auto tp3 = std::chrono::steady_clock::now();
@@ -1239,7 +1207,8 @@ static void ser_gpa(ByteWriter& w, const GPAProof& p) {
 }
 
 // A caller's circuit: layer 1 from the caller's buffer, then the library's tree from N/2 down.  N = 2: the top layer is
-// the caller's two elements.  Launches: 1 + product_trees_launches(N/2), or the one read-back for N = 2.
+// the caller's two elements.  Launches: layer 1, one per tree layer above 4096 elements and the tree's tail kernel, or
+// the one read-back for N = 2.
 Circuit* gp_circuit_create(Ctx* c, const Poly& p, fr_t* product) {
   std::unique_ptr<Circuit> ci(new Circuit());
   ci->N = p.len;
@@ -1255,7 +1224,6 @@ Circuit* gp_circuit_create(Ctx* c, const Poly& p, fr_t* product) {
     tp.p[0] = ci->tree.p;
     const Finalize f = c->fin_begin();
     launch_product_trees(tp, 1, p.len / 2, 0, 2, f, c->st);
-    g_launches += 1 + product_trees_launches(p.len / 2);
     c->fin_wait(f, top, 2);
   }
   *product = fr_mul(top[0], top[1]);
@@ -1334,7 +1302,6 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     launch_bound_u32(Z.u32, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
   else
     launch_bound_fr(Z.fr, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
-  g_launches += 2;
   if (G > 1) comm_gather_vector(c, a_loc.p, n_loc, a_gath.p, a.p);
 
   // ---- DotProductProofLog::prove
@@ -1353,9 +1320,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
   DBuf<fr_t> W0(c, n), W1(c, n), sLR(c, 2 * (n + 2));
   fr_t* W = W0.p;   // weights of the unfolded generators (indexed by the HIGH column bits)
   fr_t* Wn = W1.p;
-  set_elems_kernel<<<1, 32, 0, c->st>>>(W, fr_one(), fr_zero());
-  LB_LAUNCH_CHECK();
-  g_launches += 1;
+  launch(set_elems_kernel, 1, 32, 0, c->st, W, fr_one(), fr_zero());
   fr_t* sL = sLR.p;
   fr_t* sR = sLR.p + (n + 2);
   fr_t* av = a.p;  // current a / b vectors
@@ -1381,12 +1346,10 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     launch_two_row_scalars(av, 0, fr_one(), fr_zero(), fr_zero(), Zr, fr_zero(), n, sLR.p, c->st);
     const PubDst pd_c = c->pub_begin(false);
     launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd_c, c->st);
-    g_launches += 2;
     // a_vec of the transcript = canonical bytes of b; the copy is waited for only when it is appended
     launch_canonicalize(bv, canon.p, n, c->d_flag, c->st);
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, canon.p, n * 32, cudaMemcpyDeviceToHost, c->st));
     LB_CUDA_CHECK(cudaEventRecord(c->ev_aux, c->st));
-    g_launches += 2;
     fr_t u = fr_one(), u_inv = fr_one();
     int fold = 0;
     size_t m = n;  // vector length entering the round (after the fold with the previous challenge)
@@ -1396,7 +1359,6 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
       pd_round = c->pub_begin(false);
       launch_bullet_fused(g.d_multiples.p, g.n_direct, av, bv, W, an, bn, Wn, n, m, fold, u, u_inv, v1[round], v2[round],
                           part_f.p, c->d_partial, c->d_flag + 4, pd_round, c->st);
-      g_launches += 1;
       if (fold) {
         std::swap(av, an);
         std::swap(bv, bn);
@@ -1429,7 +1391,6 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     if (fold) {  // the last challenge: a, b -> one element each, weights -> n (bullet.rs:127-134)
       launch_fold_ab(av, bv, 1, u, u_inv, c->st);
       launch_expand_weights(W, Wn, n / 2, u, u_inv, c->st);
-      g_launches += 2;
       std::swap(W, Wn);
     }
   } else {
@@ -1442,16 +1403,13 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
       transcript.append_point_compressed("Cx", Cx.data());
       // (0 .. 0, y, 0) on (G_0 .. G_{n-1}, Q, h)
       launch_fill_zero(sL, n, c->st);
-      set_elems_kernel<<<1, 32, 0, c->st>>>(sL + n, Zr, fr_zero());
-      LB_LAUNCH_CHECK();
-      g_launches += 1;
+      launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, Zr, fr_zero());
       std::vector<uint8_t> Cy = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
       transcript.append_point_compressed("Cy", Cy.data());
       memcpy(out.Cy, Cy.data(), 32);
       // append_scalars(b"a", a_vec): canonical bytes straight from the device
       DBuf<fr_t> canon(c, n);
       launch_canonicalize(b.p, canon.p, n, c->d_flag, c->st);
-      g_launches += 1;
       std::vector<uint8_t> bytes(n * 32);
       c->d2h(bytes.data(), canon.p, bytes.size());
       transcript.append_scalars_bytes("a", bytes.data(), n);
@@ -1461,11 +1419,8 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     for (size_t round = 0; m != 1; round++) {
       const size_t h = m / 2;
       launch_cross_inner_products(av, bv, h, c->d_partial, c->d_small, c->st);  // c_L, c_R (bullet.rs:78-79)
-      g_launches += 2;
       launch_bullet_scalars(av, W, n, m, 1, 0, 0, sL, sR, c->st);
-      set_tail_kernel<<<1, 32, 0, c->st>>>(sL + n, sR + n, c->d_small, v1[round], v2[round]);
-      LB_LAUNCH_CHECK();
-      g_launches += 2;
+      launch(set_tail_kernel, 1, 32, 0, c->st, sL + n, sR + n, c->d_small, v1[round], v2[round]);
       std::vector<uint8_t> LR = msm_rows_fr(c, g, sLR.p, 2, (int)(n + 2));
       transcript.append_point_compressed("L", LR.data());
       transcript.append_point_compressed("R", LR.data() + 32);
@@ -1473,7 +1428,6 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
       fr_t u_inv = fr_inv(u);
       launch_fold_ab(av, bv, h, u, u_inv, c->st);  // bullet.rs:127-130 (scalars only; G stays unfolded)
       launch_expand_weights(W, Wn, nw_count, u, u_inv, c->st);
-      g_launches += 2;
       std::swap(W, Wn);
       nw_count *= 2;
       blind_fin = fr_add(blind_fin, fr_add(fr_mul(fr_mul(v1[round], u), u), fr_mul(fr_mul(v2[round], u_inv), u_inv)));
@@ -1493,7 +1447,6 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd, c->st);
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, av, 32, cudaMemcpyDeviceToHost, c->st));
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 32, bv, 32, cudaMemcpyDeviceToHost, c->st));
-    g_launches += 3;
     uint32_t xyz[48];
     c->wait_points(pd, 2, xyz);
     h64::compress_xyz_pair(xyz, xyz + 24, out.delta, out.beta);
@@ -1508,17 +1461,13 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     memcpy(ab, c->h_pin, 64);
     // delta = d * g_hat + r_delta * h with g_hat = sum_j W[j] G_j  (dot_product.rs:219-227)
     launch_scale(W, sL, n, d, c->st);
-    set_elems_kernel<<<1, 32, 0, c->st>>>(sL + n, fr_zero(), r_delta);
-    LB_LAUNCH_CHECK();
-    g_launches += 2;
+    launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, fr_zero(), r_delta);
     std::vector<uint8_t> delta = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
     memcpy(out.delta, delta.data(), 32);
     transcript.append_point_compressed("delta", out.delta);
     // beta = d * Q + r_beta * h  (dot_product.rs:229-230)
     launch_fill_zero(sL, n, c->st);
-    set_elems_kernel<<<1, 32, 0, c->st>>>(sL + n, d, r_beta);
-    LB_LAUNCH_CHECK();
-    g_launches += 1;
+    launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, d, r_beta);
     std::vector<uint8_t> beta = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
     memcpy(out.beta, beta.data(), 32);
     transcript.append_point_compressed("beta", out.beta);
@@ -1590,10 +1539,8 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     SpanTimer sp(c, "Subtables.new");
     if (!custom) {
       launch_materialize_subtables(S, tables_fr_buf.p, tables_u32_buf.p, c->st);
-      g_launches += 1;
     }
     launch_gather_lookup_polys(S, tables_fr, tables_u32, dense.nz(), s_loc, E.p, s_loc, E_u32.p, c->st);
-    g_launches += 1;
     if (nd_loc > alpha * s_loc) {
       launch_fill_zero(E.p + alpha * s_loc, nd_loc - alpha * s_loc, c->st);
       if (E_u32.p) LB_CUDA_CHECK(cudaMemsetAsync(E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
@@ -1624,7 +1571,6 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     LB_CUDA_CHECK(cudaMemcpyAsync(Wk.p, E.p, alpha * s_loc * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
     eq_evals_shard(c, r, 0, log_s, Wk.p + alpha * s_loc);
     launch_sumcheck_claim(S, Wk.p, s_loc, s_loc, c->d_partial, c->d_small, c->st);  // subtables/mod.rs:186-216
-    g_launches += 2;
     fr_t claimed_eval;
     const Finalize fclaim = reduce_to_host_begin(c, c->d_small, 1);
     absorb_comm_E();  // transcript order unchanged: the commitment, then the claim
@@ -1641,7 +1587,6 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     SpanTimer sp(c, "CombinedEval.prove");
     eq_evals_shard(c, r_z, 0, log_s, eqtab.p);
     multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
-    g_launches += 2;
     reduce_to_host(c, c->d_small, (int)alpha, eval_derefs.data());
     w.arr_fr(eval_derefs);
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
@@ -1674,7 +1619,6 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
                                  fin[i]->tree.p, c->st);
       launch_gp_fingerprints_ops(dense.dim(j), E.p + i * s_loc, dense.read(j), s_loc, gamma, tau, rd[i]->tree.p,
                                  wr[i]->tree.p, c->st);
-      g_launches += 2;
     }
     // all trees of a size at once + the top layers straight to the host
     std::vector<std::vector<fr_t>> tops(2);  // [0]: init_i, final_i interleaved; [1]: read_i, write_i interleaved
@@ -1730,7 +1674,6 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     eq_evals_shard(c, rand_ops, 0, rand_ops.size(), eqtab.p);
     multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
     launch_multi_dot_u32(dense.d_l_u32.p, s_loc, (int)(2 * C), eqtab.p, s_loc, c->d_partial + 65536, c->d_small + 64, c->st);
-    g_launches += 4;
     {
       std::vector<fr_t> tmp(64 + 2 * C);
       reduce_to_host(c, c->d_small, (int)tmp.size(), tmp.data());
@@ -1746,7 +1689,6 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
                     "joint_claim_eval", rand_ops, transcript, tape);
     eq_evals_shard(c, rand_mem, 0, rand_mem.size(), eqtab.p);
     launch_multi_dot_u32(dense.d_m_u32.p, M_loc, (int)C, eqtab.p, M_loc, c->d_partial, c->d_small, c->st);
-    g_launches += 2;
     reduce_to_host(c, c->d_small, (int)C, eval_final.data());
     std::vector<fr_t> evals_ops = eval_dim;
     evals_ops.insert(evals_ops.end(), eval_read.begin(), eval_read.end());
@@ -1805,7 +1747,6 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
     LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, Z, len * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
     launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, len, p->d_fr.p, flags.p, c->st);
   }
-  g_launches += 1;
   unsigned f[2];
   c->d2h(f, flags.p, sizeof f);
   if (f[0]) {
@@ -1818,7 +1759,6 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
   if (p->bits <= 32) {
     p->d_u32.alloc(c, len);
     launch_poly_mirror_u32(p->d_fr.p, len, p->d_u32.p, c->st);
-    g_launches += 1;
   }
   return p.release();
 }
@@ -1836,7 +1776,6 @@ fr_t poly_evaluate(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
   DBuf<fr_t> eq(c, p.len);
   eq_evals_dev(c, r, 0, p.nv, eq.p);
   multi_dot_src(poly_src(p), p.len, 1, eq.p, p.len, c->d_partial, c->d_small, c->st);
-  g_launches += 2;
   fr_t out;
   c->d2h(&out, c->d_small, sizeof out);
   return out;
@@ -1912,7 +1851,6 @@ std::vector<fr_t> poly_evaluate_batch(Ctx* c, const Poly* const* polys, int k, c
     }
     if (!m) continue;
     launch_multi_dot_ptrs(in, m, form == 0, eq.p, n, c->d_partial, c->d_small + (order.size() - m), c->st);
-    g_launches += 2;
   }
   std::vector<fr_t> got(k), out(k);
   c->d2h(got.data(), c->d_small, k * sizeof(fr_t));
@@ -1968,7 +1906,6 @@ Poly* poly_create_comb(Ctx* c, const Comb& g, const Poly* const* polys, int k) {
   CombPtrs in{};
   for (int j = 0; j < k; j++) in.p[j] = polys[j]->d_fr.p;
   launch_comb_map(dev.pg, in, p->len, p->d_fr.p, c->st);
-  g_launches += 1;
   return p.release();
 }
 // prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first evaluates the
@@ -2001,14 +1938,10 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
     const Finalize f = c->fin_begin();
     if (j == 0) {
       launch_sumcheck_eval_comb(pg, src, len / 2, f, c->st);
-      g_launches += 1;
     } else {  // bind the previous challenge (caller buffers -> workspace, then in place) and evaluate
-      if (!unfused && launch_sumcheck_bind_eval_comb(pg, src, dst, len / 4, r_prev, f, 0, c->st)) {
-        g_launches += 1;
-      } else {
+      if (unfused || !launch_sumcheck_bind_eval_comb(pg, src, dst, len / 4, r_prev, f, 0, c->st)) {
         launch_bind_comb(src, dst, k, len / 2, r_prev, c->st);
         launch_sumcheck_eval_comb(pg, dst, len / 4, f, c->st);
-        g_launches += 2;
       }
       src = dst;
       len /= 2;
@@ -2024,7 +1957,6 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
   out.final_evals.resize(k);
   const Finalize f = c->fin_begin();
   launch_final_comb(src, k, len / 2, r_prev, f, c->st);
-  g_launches += 1;
   c->fin_wait(f, out.final_evals.data(), k);
   out.proof = std::move(w.b);
   return out;

@@ -15,8 +15,6 @@
 
 namespace lb {
 
-extern std::atomic<unsigned long long> g_launches;  // kernels launched by this process (bench.py's gpu_launches)
-
 struct Ctx {
   int device = 0;
   cudaStream_t st = nullptr;
@@ -64,6 +62,7 @@ struct Ctx {
   unsigned long long* h_pub = nullptr;
   unsigned long long* d_pub_reader[kPubMaxReaders] = {};
   uint32_t pub_seq = 0;
+  uint32_t pub_ring[2] = {0, 0};  // next region of messages to this process only [0] and to every process [1]
   static constexpr size_t kPubBytes = (size_t)kPubMaxReaders * kPubRegions * kPubElems * kPubSlotWords * 8;  // 1 MiB
   cudaEvent_t ev_aux = nullptr;  // marks a device->host copy that overlaps later launches on the same stream
   cudaEvent_t ev_caller = nullptr;  // densify_device: the caller's stream up to the call (the index matrix is ready)
@@ -87,9 +86,12 @@ struct Ctx {
     p.all = 0;
     for (int i = 0; i < kPubMaxReaders; i++) p.dst[i] = nullptr;
     const uint32_t seq = pub_seq++;
-    p.region = (int)(seq % kPubRegions);
-    p.tag = 1 + seq % kPubTagMod;
     p.all = (all && world > 1) ? 1 : 0;
+    // A peer reads this writer's message to every process before it launches its next one, so in a peer's buffer a
+    // region is free again two such messages later.  Messages to this process only take no peer with them: were they
+    // to advance the same ring, a writer running ahead through them would reuse a region a peer has not read yet.
+    p.region = (int)(pub_ring[p.all]++ % kPubRegions);
+    p.tag = 1 + seq % kPubTagMod;
     const size_t off = ((size_t)rank * kPubRegions + p.region) * kPubElems * kPubSlotWords;
     if (p.all) {
       for (int r = 0; r < world; r++) p.dst[p.ndst++] = d_pub_reader[r] + off;

@@ -52,14 +52,13 @@ void KH_ARITH_LAUNCH(int op, size_t n, const uint32_t* a, const uint32_t* b, con
   const unsigned quad_blocks = (unsigned)((4 * n + 127) / 128);
   switch (op) {
 #define KH_ARITH_THREAD_CASE(name) \
-  case OP_##name: arith_thread_kernel<OP_##name><<<(unsigned)blocks, 128, 0, st>>>(n, a, b, k, out); break;
+  case OP_##name: lb::launch(arith_thread_kernel<OP_##name>, (unsigned)blocks, 128, 0, st, n, a, b, k, out); break;
     KH_ARITH_THREAD_OPS(KH_ARITH_THREAD_CASE)
 #undef KH_ARITH_THREAD_CASE
 #define KH_ARITH_QUAD_CASE(name) \
-  case OP_##name: arith_quad_kernel<OP_##name><<<quad_blocks, 128, 0, st>>>(n, a, b, out); break;
+  case OP_##name: lb::launch(arith_quad_kernel<OP_##name>, quad_blocks, 128, 0, st, n, a, b, out); break;
     KH_ARITH_QUAD_OPS(KH_ARITH_QUAD_CASE)
 #undef KH_ARITH_QUAD_CASE
     default: throw std::runtime_error("kh_arith: unknown operation");
   }
-  LB_LAUNCH_CHECK();
 }
