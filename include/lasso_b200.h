@@ -316,6 +316,43 @@ int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*,
  * variable: 2^r_len evaluations, r_len <= 28 (LASSO_ERR_LENGTH), each coordinate a canonical residue (LASSO_ERR_VALUE). */
 int lasso_poly_create_eq(lasso_ctx*, const uint64_t* r, size_t r_len, lasso_poly** out);
 
+/* ---------------------------------------------------------------- lookups inside a caller's protocol
+ *
+ * SparsePolynomialEvaluationProof::prove (lasso/surge.rs:118-211) on the caller's transcript and tape, both advanced in
+ * place: the reference's signature prove(dense, r, gens, transcript, random_tape) one to one.  lasso_prove is this call on
+ * Transcript::new(transcript_label) and a fresh tape, with the same bytes.  proof_out receives the ark-serialize
+ * (compressed) proof, whose size is fixed by the strategy, s, log_m and the generators (*proof_len receives it, also when
+ * proof_cap is too small); claimed_eval_out (may be NULL) PrimarySumcheck::claimed_evaluation, the sum over k of
+ * eq(r, k) combine_lookups(E_0(k), ..).  Collective on a sharded context like lasso_prove: every rank passes its own
+ * transcript and tape in the same state, and every rank's handles end in the same state.
+ * Errors, each returned before any launch and before the transcript or the tape is touched: LASSO_ERR_STRATEGY for
+ * the strategies lasso_prove / lasso_prove_custom reject (LT with C > 8 included), a strategy of another context, or
+ * (C, log_m) that differ from the dense's; LASSO_ERR_LENGTH for r_len != log2(s), proof_cap too small, or a null
+ * transcript, tape or proof_len; LASSO_ERR_GENS for generators of another context or built for another
+ * (c, s, num_memories, log_m); LASSO_ERR_VALUE for a coordinate of r that is not a canonical residue.  The proof's
+ * working memory is reserved in the context's pool before the first transcript write.  LASSO_ERR_MULTISET, as the
+ * reference's panic, can only be raised after the transcript and the tape have moved. */
+int lasso_prove_transcript(lasso_ctx*, int strategy, int log_R, lasso_dense*, const uint64_t* r, size_t r_len,
+                           const lasso_gens*, lasso_transcript* transcript, lasso_random_tape* random_tape,
+                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]);
+int lasso_prove_custom_transcript(lasso_ctx*, const lasso_strategy*, lasso_dense*, const uint64_t* r, size_t r_len,
+                                  const lasso_gens*, lasso_transcript* transcript, lasso_random_tape* random_tape,
+                                  uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]);
+/* SparsePolynomialCommitment::append_to_transcript (lasso/surge.rs:70-82) of lasso_commit's output bytes: both
+ * PolyCommitments with their begin / end markers, then s, log_m and m as u64.  Host only: no context.  LASSO_ERR_LENGTH
+ * when the bytes do not parse as that struct (a count beyond the bytes, missing or trailing bytes); LASSO_ERR_VALUE for a
+ * point that does not decompress; nothing is absorbed in either case. */
+int lasso_transcript_append_sparse_commitment(lasso_transcript*, const uint8_t* bytes, size_t len);
+/* The lookup outputs v[k] = combine_lookups(T_sub(0)[dim_usize(0)[k]], ..) for k < s, padded lookups included (their
+ * indices are 0, densified.rs:37), as a polynomial of log2(s) variables.  Its MLE at r is the claimed evaluation of a
+ * proof at r, so a caller can commit to v (lasso_poly_commit) and open it at r (lasso_poly_eval_prove) to tie the proof
+ * to its own commitments.  One pass over the indices on the GPU; built-in entries are computed from the index, custom
+ * ones read from the strategy's tables.  When every value is below 2^32, v has the u32 mirror (the 16-bit commitment
+ * path).  LASSO_ERR_STRATEGY for the strategies lasso_prove rejects, a strategy of another context or other (C, log_m),
+ * and on a sharded context; LASSO_ERR_LENGTH for a null output. */
+int lasso_dense_outputs(lasso_ctx*, int strategy, int log_R, const lasso_dense*, lasso_poly** out);
+int lasso_dense_outputs_custom(lasso_ctx*, const lasso_strategy*, const lasso_dense*, lasso_poly** out);
+
 /* ---------------------------------------------------------------- many polynomials per call
  *
  * DensePolynomial::merge (poly/dense_mlpoly.rs:251-261): a new polynomial holding the evaluations of polys[0..n_polys) one

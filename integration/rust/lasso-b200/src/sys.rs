@@ -19,6 +19,10 @@ pub struct lasso_msm_job {
     _p: [u8; 0],
 }
 #[repr(C)]
+pub struct lasso_strategy {
+    _p: [u8; 0],
+}
+#[repr(C)]
 pub struct lasso_transcript {
     _p: [u8; 0],
 }
@@ -138,6 +142,21 @@ extern "C" {
                                      evals: *const u64, n_evals: usize, r: *const u64, r_len: usize,
                                      transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
                                      proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize) -> c_int;
+    // lookups inside a caller's protocol (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_prove_transcript(ctx: *mut lasso_ctx, strategy: c_int, log_r: c_int, dense: *mut lasso_dense, r: *const u64,
+                                  r_len: usize, gens: *const lasso_gens, transcript: *mut lasso_transcript,
+                                  random_tape: *mut lasso_random_tape, proof_out: *mut u8, proof_cap: usize,
+                                  proof_len: *mut usize, claimed_eval_out: *mut u64) -> c_int;
+    pub fn lasso_prove_custom_transcript(ctx: *mut lasso_ctx, s: *const lasso_strategy, dense: *mut lasso_dense,
+                                         r: *const u64, r_len: usize, gens: *const lasso_gens,
+                                         transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
+                                         proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize,
+                                         claimed_eval_out: *mut u64) -> c_int;
+    pub fn lasso_transcript_append_sparse_commitment(t: *mut lasso_transcript, bytes: *const u8, len: usize) -> c_int;
+    pub fn lasso_dense_outputs(ctx: *mut lasso_ctx, strategy: c_int, log_r: c_int, dense: *const lasso_dense,
+                               out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_dense_outputs_custom(ctx: *mut lasso_ctx, s: *const lasso_strategy, dense: *const lasso_dense,
+                                      out: *mut *mut lasso_poly) -> c_int;
     // sumchecks over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
     pub fn lasso_comb_create(n_inputs: c_int, program: *const i32, n_ops: c_int, constants: *const u64, n_constants: c_int,
                              degree: c_int, out: *mut *mut lasso_comb) -> c_int;

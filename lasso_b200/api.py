@@ -583,6 +583,19 @@ class DensifiedRepresentation:
         _chk(lib().lasso_commit(self.ctx._h, self._h, gens._h, _p(out), C.c_size_t(cap), C.byref(n)))
         return bytes(out[: n.value])
 
+    def outputs(self, strategy):
+        """The lookup outputs v[k] = combine_lookups(E_0[k], ..) for k < s (padded lookups included) as a
+        DensePolynomial of log2(s) variables on the context's GPU.  Its MLE at r is the claimed evaluation of a proof
+        at r: commit to v and open it there to tie the proof to the caller's commitments."""
+        h = C.c_void_p()
+        if isinstance(strategy, CustomStrategy):
+            if strategy._h is None:
+                raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
+            _chk(lib().lasso_dense_outputs_custom(self.ctx._h, strategy._h, self._h, C.byref(h)))
+        else:
+            _chk(lib().lasso_dense_outputs(self.ctx._h, strategy.kind, strategy.log_r, self._h, C.byref(h)))
+        return DensePolynomial._wrap(self.ctx, h)
+
     def __del__(self):
         try:
             if self._h and self.ctx._h:
@@ -592,13 +605,28 @@ class DensifiedRepresentation:
 
 
 class SparsePolynomialEvaluationProof:
-    """src/lasso/surge.rs:92-211.  `.bytes` is the ark-serialize (compressed) encoding of the proof."""
+    """src/lasso/surge.rs:92-211.  `.bytes` is the ark-serialize (compressed) encoding of the proof.  On the label path
+    `.challenges` holds every challenge drawn; on a caller's transcript it is None and `.claimed_evaluation` holds the
+    primary sumcheck's claim (4 limbs)."""
 
-    def __init__(self, data, challenges):
-        self.bytes, self.challenges = data, challenges
+    def __init__(self, data, challenges, claimed_evaluation=None):
+        self.bytes, self.challenges, self.claimed_evaluation = data, challenges, claimed_evaluation
 
     @classmethod
-    def prove(cls, ctx, strategy, dense, r, gens, transcript_label=b"example", tape_label=b"proof", tape_seed=None):
+    def prove(cls, ctx, strategy, dense, r, gens, transcript_label=None, tape_label=None, tape_seed=None,
+              transcript=None, random_tape=None):
+        """Without transcript / random_tape: on Transcript::new(transcript_label or b"example") and a tape
+        RandomTape::new(tape_label or b"proof") seeded with tape_seed (zero by default).  With both: on the caller's
+        Transcript and RandomTape, advanced in place; no label or seed may then be given."""
+        if transcript is not None or random_tape is not None:
+            if transcript is None or random_tape is None:
+                raise LassoError(LASSO_ERR_LENGTH, "pass both a transcript and a random_tape, or neither")
+            if transcript_label is not None or tape_label is not None or tape_seed is not None:
+                raise LassoError(LASSO_ERR_LENGTH, "labels and tape_seed belong to the label path, not to a caller's "
+                                                   "transcript and random_tape")
+            return cls._prove_transcript(ctx, strategy, dense, r, gens, transcript, random_tape)
+        transcript_label = b"example" if transcript_label is None else transcript_label
+        tape_label = b"proof" if tape_label is None else tape_label
         r = _fr(r).reshape(-1, 4)
         seed = _fr(tape_seed if tape_seed is not None else np.zeros(4, dtype=np.uint64))
         cap = 1 << 22
@@ -614,6 +642,23 @@ class SparsePolynomialEvaluationProof:
         else:
             _chk(lib().lasso_prove(ctx._h, strategy.kind, strategy.log_r, *tail))
         return cls(bytes(out[: n.value]), chal[: nch.value].copy())
+
+    @classmethod
+    def _prove_transcript(cls, ctx, strategy, dense, r, gens, transcript, random_tape):
+        r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+        cap = 1 << 22
+        out = ctx._buf("proof", cap, np.uint8)
+        claim = np.zeros(4, dtype=np.uint64)
+        n = C.c_size_t(0)
+        tail = (dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, transcript._h, random_tape._h, _p(out),
+                C.c_size_t(cap), C.byref(n), _p(claim))
+        if isinstance(strategy, CustomStrategy):
+            if strategy._h is None:
+                raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
+            _chk(lib().lasso_prove_custom_transcript(ctx._h, strategy._h, *tail))
+        else:
+            _chk(lib().lasso_prove_transcript(ctx._h, strategy.kind, strategy.log_r, *tail))
+        return cls(bytes(out[: n.value]), None, claim)
 
 
 # ------------------------------------------------------------------ dense polynomials on a caller's transcript
@@ -685,6 +730,12 @@ class Transcript:
         """PolyCommitment::append_to_transcript (src/poly/dense_mlpoly.rs:281-289) of DensePolynomial.commit's bytes"""
         b = bytes(commitment)
         _chk(lib().lasso_transcript_append_poly_commitment(self._h, _label(label), b, C.c_size_t(len(b))))
+
+    def append_sparse_commitment(self, commitment):
+        """SparsePolynomialCommitment::append_to_transcript (src/lasso/surge.rs:70-82) of
+        DensifiedRepresentation.commit's bytes"""
+        b = bytes(commitment)
+        _chk(lib().lasso_transcript_append_sparse_commitment(self._h, b, C.c_size_t(len(b))))
 
     def challenge_scalar(self, label):
         out = np.zeros(4, dtype=np.uint64)

@@ -2,6 +2,7 @@
 // point states the reference item it replaces in the header.
 #include "../../include/lasso_b200.h"
 
+#include "host_fq64.hpp"
 #include "program_check.hpp"
 #include "prover.cuh"
 
@@ -772,6 +773,106 @@ int lasso_prove_custom(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, co
   LB_CATCH
 }
 
+// ---- lookups inside a caller's protocol
+static bool load_scalars(const uint64_t* s, size_t n, std::vector<fr_t>& out);
+static int poly_ctx_check(lasso_ctx* h);
+// The strategy of a built-in kind (strategy, log_R) or a custom one (s), checked against the context and the dense:
+// "" = usable, else the reason (LASSO_ERR_STRATEGY)
+static std::string strategy_for(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
+                                Strategy& S) {
+  if (!d) return "null densified representation";
+  if (s) {
+    if (s->c != h->c) return "strategy was created on another context";
+    if ((size_t)s->cs.C != d->d->C || (size_t)s->cs.log_m != d->d->log_m)
+      return "strategy (C, log_m) differ from the densified representation";
+    S = s->S();
+    return "";
+  }
+  S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
+  if (!S.valid()) return "unsupported strategy parameters";
+  if (!S.provable())
+    return "prove: " + std::to_string(2 * S.num_memories()) + " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)";
+  return "";
+}
+static int prove_transcript(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
+                            const lasso_gens* g, lasso_transcript* transcript, lasso_random_tape* tape, uint8_t* proof_out,
+                            size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
+  const Dense& dense = *d->d;
+  if (!transcript || !tape || !proof_len) return fail(LASSO_ERR_LENGTH, "prove: null transcript, random tape or proof_len");
+  if (r_len != log2_exact_or_ceil(dense.s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");  // surge.rs:131
+  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "prove: null point");
+  // the generators lasso_gens_create built for this (c, s, num_memories, log_m) (surge.rs:32-58)
+  const size_t alpha = (size_t)S.num_memories();
+  if (!g || g->g->ctx != h->c) return fail(LASSO_ERR_GENS, "prove: null generators, or generators of another context");
+  const Gens& gg = *g->g;
+  if (gg.c != dense.C || next_pow2(gg.s) != dense.s || gg.num_memories != alpha || gg.log_m != dense.log_m ||
+      gg.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || gg.nv_l != dense.nv_l || gg.nv_m != dense.nv_m)
+    return fail(LASSO_ERR_GENS, "prove: generators built for another (c, s, num_memories, log_m)");
+  const size_t need = proof_bytes(S, dense, gg);
+  *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "prove: output buffer too small");
+  std::vector<fr_t> rv;
+  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "prove: a coordinate of r is not a canonical residue");
+  auto t0 = std::chrono::steady_clock::now();
+  fr_t claimed;
+  std::vector<uint8_t> b;
+  try {
+    b = prove(h->c, S, *d->d, rv, gg, transcript->t, tape->t, &claimed);
+  } catch (const std::runtime_error& e) {
+    if (std::string(e.what()).find("multiset") != std::string::npos) return fail(LASSO_ERR_MULTISET, e.what());
+    throw;
+  }
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (b.size() != need) return fail(-1, "prove: unexpected proof size");
+  memcpy(proof_out, b.data(), b.size());
+  if (claimed_eval_out) memcpy(claimed_eval_out, claimed.v, 32);
+  return 0;
+}
+int lasso_prove_transcript(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
+                           const lasso_gens* g, lasso_transcript* transcript, lasso_random_tape* random_tape,
+                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
+  LB_TRY_CTX(h)
+  Strategy S{};
+  const std::string why = strategy_for(h, strategy, log_R, nullptr, d, S);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, why);
+  return prove_transcript(h, S, d, r, r_len, g, transcript, random_tape, proof_out, proof_cap, proof_len, claimed_eval_out);
+  LB_CATCH
+}
+int lasso_prove_custom_transcript(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, const uint64_t* r, size_t r_len,
+                                  const lasso_gens* g, lasso_transcript* transcript, lasso_random_tape* random_tape,
+                                  uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
+  LB_TRY_CTX(h)
+  if (!s) return fail(LASSO_ERR_STRATEGY, "null strategy");
+  Strategy S{};
+  const std::string why = strategy_for(h, 0, 0, s, d, S);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, why);
+  return prove_transcript(h, S, d, r, r_len, g, transcript, random_tape, proof_out, proof_cap, proof_len, claimed_eval_out);
+  LB_CATCH
+}
+static int dense_outputs_checked(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
+                                 lasso_poly** out) {
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!out) return fail(LASSO_ERR_LENGTH, "outputs: null output");
+  Strategy S{};
+  const std::string why = strategy_for(h, strategy, log_R, s, d, S);
+  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "outputs: " + why);
+  *out = new lasso_poly{dense_outputs(h->c, S, *d->d)};
+  return 0;
+}
+int lasso_dense_outputs(lasso_ctx* h, int strategy, int log_R, const lasso_dense* d, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return dense_outputs_checked(h, strategy, log_R, nullptr, d, out);
+  LB_CATCH
+}
+int lasso_dense_outputs_custom(lasso_ctx* h, const lasso_strategy* s, const lasso_dense* d, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (!s) return fail(LASSO_ERR_STRATEGY, "outputs: null strategy");
+  return dense_outputs_checked(h, 0, 0, s, d, out);
+  LB_CATCH
+}
+
 // ---- transcripts and random tapes (host only: no context, no device)
 #define LB_TRY_T(t) \
   try {             \
@@ -853,6 +954,42 @@ int lasso_transcript_append_poly_commitment(lasso_transcript* t, const char* lab
   t->t.append_message(label, std::string("poly_commitment_begin"));
   for (uint64_t i = 0; i < n; i++) t->t.append_point_compressed("poly_commitment_share", bytes + 8 + 32 * i);
   t->t.append_message(label, std::string("poly_commitment_end"));
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_sparse_commitment(lasso_transcript* t, const uint8_t* bytes, size_t len) {
+  LB_TRY_T(t)
+  if (!bytes && len) return fail(LASSO_ERR_LENGTH, "sparse commitment: null bytes");
+  // lasso_commit's bytes: two (u64 count, 32 bytes per point) vectors, then s, log_m, m
+  size_t at = 0, begin[2], count[2];
+  for (int v = 0; v < 2; v++) {
+    uint64_t n = 0;
+    if (len - at < 8) return fail(LASSO_ERR_LENGTH, "sparse commitment: shorter than its counts");
+    memcpy(&n, bytes + at, 8);
+    at += 8;
+    if (n > (len - at) / 32) return fail(LASSO_ERR_LENGTH, "sparse commitment: a count exceeds the bytes");
+    begin[v] = at;
+    count[v] = n;
+    at += 32 * n;
+  }
+  if (len - at != 24) return fail(LASSO_ERR_LENGTH, "sparse commitment: not followed by exactly s, log_m, m");
+  for (int v = 0; v < 2; v++)
+    for (size_t i = 0; i < count[v]; i++)
+      if (!h64::decompresses(bytes + begin[v] + 32 * i))
+        return fail(LASSO_ERR_VALUE, "sparse commitment: a point does not decompress");
+  // SparsePolynomialCommitment::append_to_transcript (surge.rs:70-82)
+  static const char* const labels[2] = {"l_variate_polys_commitment", "log_m_variate_polys_commitment"};
+  for (int v = 0; v < 2; v++) {
+    t->t.append_message(labels[v], std::string("poly_commitment_begin"));
+    for (size_t i = 0; i < count[v]; i++) t->t.append_point_compressed("poly_commitment_share", bytes + begin[v] + 32 * i);
+    t->t.append_message(labels[v], std::string("poly_commitment_end"));
+  }
+  static const char* const fields[3] = {"s", "log_m", "m"};
+  for (int k = 0; k < 3; k++) {
+    uint64_t x;
+    memcpy(&x, bytes + at + 8 * k, 8);
+    t->t.append_u64(fields[k], x);
+  }
   return 0;
   LB_CATCH
 }

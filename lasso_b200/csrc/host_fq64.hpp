@@ -103,6 +103,45 @@ inline fe canonical(const fe& a) {
   for (int i = 0; i < 4; i++) r.v[i] = ge ? s[i] : t[i];
   return r;
 }
+// Whether a 32-byte ark-serialize compressed point decompresses (get_point_from_y_unchecked): y below q, and
+// x^2 = (y^2 - 1) / (d y^2 + 1) a square (Euler's criterion), d = -121665/121666.  Not a subgroup check.
+inline bool decompresses(const uint8_t in[32]) {
+  static const uint64_t kQm1[4] = {0xffffffffffffffecULL, 0xffffffffffffffffULL, 0xffffffffffffffffULL, 0x7fffffffffffffffULL};
+  static const fe kD = {{0x75eb4dca135978a3ULL, 0x00700a4d4141d8abULL, 0x8cc740797779e898ULL, 0x52036cee2b6ffe73ULL}};
+  fe y;
+  memcpy(y.v, in, 32);
+  y.v[3] &= 0x7fffffffffffffffULL;
+  for (int i = 3; i >= 0; i--) {  // y < q = (q - 1) + 1
+    if (y.v[i] != kQm1[i]) {
+      if (y.v[i] > kQm1[i]) return false;
+      break;
+    }
+    if (i == 0) return false;
+  }
+  auto add = [](const fe& a, const uint64_t* b) {  // a, b < 2^255: the sum fits 256 bits
+    fe r;
+    u128 c = 0;
+    for (int i = 0; i < 4; i++) {
+      c += (u128)a.v[i] + b[i];
+      r.v[i] = (uint64_t)c;
+      c >>= 64;
+    }
+    return canonical(r);
+  };
+  const uint64_t one[4] = {1, 0, 0, 0};
+  const fe y2 = canonical(mul(y, y));
+  const fe num = add(y2, kQm1), den = add(canonical(mul(kD, y2)), one);
+  if (!(den.v[0] | den.v[1] | den.v[2] | den.v[3])) return false;
+  const fe x2 = mul(num, inv(den));
+  fe e = {{1, 0, 0, 0}}, b = x2;  // x2^((q - 1) / 2), the exponent 2^254 - 10 taken bit by bit
+  static const uint64_t kE[4] = {0xfffffffffffffff6ULL, 0xffffffffffffffffULL, 0xffffffffffffffffULL, 0x3fffffffffffffffULL};
+  for (int i = 0; i < 256; i++) {
+    if ((kE[i / 64] >> (i % 64)) & 1) e = mul(e, b);
+    b = mul(b, b);
+  }
+  e = canonical(e);
+  return e.v[1] == 0 && e.v[2] == 0 && e.v[3] == 0 && e.v[0] <= 1;
+}
 // (X, Y, Z) internal limbs (3 x 8 u32) -> ark-serialize compressed point (32 bytes)
 inline void compress_xyz(const uint32_t* xyz, uint8_t out[32]) {
   fe X = from_limbs32(xyz), Y = from_limbs32(xyz + 8), Z = from_limbs32(xyz + 16);

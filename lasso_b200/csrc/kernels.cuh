@@ -165,6 +165,9 @@ void launch_materialize_subtables(const Strategy& S, fr_t* tables_fr, uint32_t* 
 void launch_gather_lookup_polys(const Strategy& S, const fr_t* tables_fr, const uint32_t* tables_u32,
                                 const uint32_t* nz, size_t s, fr_t* E_fr, size_t E_stride, uint32_t* E_u32,
                                 cudaStream_t st);
+// The lookup outputs out[k] = combine_lookups(T_sub(0)[nz_dim(0)[k]], ..) for k < s, one launch; *bits (zeroed by the
+// caller) receives the bit width of the widest value
+void launch_lookup_outputs(const Strategy& S, const uint32_t* nz, size_t s, fr_t* out, unsigned* bits, cudaStream_t st);
 // out[i] = F::from(in[i])  (dense_mlpoly.rs:263-269)
 void launch_from_u32(const uint32_t* in, fr_t* out, size_t n, cudaStream_t st);
 void launch_fill_zero(fr_t* out, size_t n, cudaStream_t st);

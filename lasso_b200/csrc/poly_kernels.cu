@@ -657,6 +657,8 @@ __global__ void __launch_bounds__(kCustomThreads)
     st_fr(out + i, custom_run(ops, pg.n_ops, consts, slots, [&](int k) { return ld_fr(in.p[k] + i); }));
 }
 
+__global__ void __launch_bounds__(kCustomThreads)
+    lookup_outputs_custom_kernel(CustomStrategy cs, const uint32_t* nz, size_t s, fr_t* out, unsigned* bits);
 // dynamic shared memory above the default 48 KiB needs an opt-in per kernel and device (at context creation): the
 // largest program's
 void poly_init_device() {
@@ -667,6 +669,8 @@ void poly_init_device() {
   const int bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 2);
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
   LB_CUDA_CHECK(cudaFuncSetAttribute(claim_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+  LB_CUDA_CHECK(cudaFuncSetAttribute(lookup_outputs_custom_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)custom_smem_bytes(cs, 0)));
   const int comb_bytes = (int)custom_smem_bytes(cs, kCustomMaxDegree + 1);
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
   LB_CUDA_CHECK(cudaFuncSetAttribute(sc_bind_eval_comb_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, comb_bytes));
@@ -1091,6 +1095,85 @@ void launch_gather_lookup_polys(const Strategy& S, const fr_t* tables_fr, const 
   }
   dim3 grid(grid_for(s, kThreads, kMaxBlocks / S.num_memories() + 1), S.num_memories());
   launch(gather_kernel, grid, kThreads, 0, st, map, S.log_m, tables_fr, tables_u32, nz, s, E_fr, E_stride, E_u32);
+}
+// The lookup outputs v[k] = combine_lookups(E_0[k], .., E_{alpha-1}[k]), E_i[k] = T_sub(i)[nz_dim(i)[k]], one lookup per
+// thread: its C indices in (4 C bytes), the Montgomery value out (32 bytes); E is never stored.  The bit width of the
+// widest value is reduced over the warp, then the CTA, and one atomic per CTA publishes it (as poly_ingest_kernel).
+__device__ __forceinline__ unsigned fr_bit_width(const fr_t& x) {
+  const fr_t c = fr_to_canonical(x);
+  unsigned b = 0;
+#pragma unroll
+  for (int l = 0; l < 8; l++)
+    if (c.v[l]) b = 32 * l + (32 - __clz(c.v[l]));
+  return b;
+}
+__device__ __forceinline__ void publish_max_bits(unsigned mb, unsigned* bits) {
+  __shared__ unsigned s_bits[32];
+  mb = __reduce_max_sync(0xffffffffu, mb);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) s_bits[warp] = mb;
+  __syncthreads();
+  if (warp == 0) {
+    unsigned v = lane < (int)(blockDim.x >> 5) ? s_bits[lane] : 0u;
+    v = __reduce_max_sync(0xffffffffu, v);
+    if (lane == 0 && v) atomicMax(bits, v);
+  }
+}
+// Built-in strategies: the subtable entries in closed form from the index (subtable_value), no table read.  The linear
+// strategies combine with the Horner form of claim_linear_kernel; LT with claim_lt_kernel's h = lt_k + eq_k h, over
+// integers since every entry is 0 or 1 and lt_k, eq_k are never both 1.
+__global__ void __launch_bounds__(kThreads)
+    lookup_outputs_kernel(int kind, int C, int log_m, int log_r, const uint32_t* nz, size_t s, fr_t* out, unsigned* bits) {
+  unsigned mb = 0;
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < s; k += (size_t)gridDim.x * blockDim.x) {
+    fr_t v;
+    if (kind == STRAT_LT) {  // memory 2i: LT of dimension i, memory 2i + 1: EQ of dimension i (lt.rs:16-30)
+      uint32_t h = 0;
+      for (int i = C - 1; i >= 0; i--) {
+        const uint32_t a = nz[(size_t)i * s + k];
+        h = subtable_value(kind, 0, a, log_m, log_r) + subtable_value(kind, 1, a, log_m, log_r) * h;
+      }
+      v = fr_from_u64(h);
+    } else {  // memory i: dimension i (range_check.rs:62-73 picks the subtable by position)
+      const int inc = kind == STRAT_RANGE ? log_m : log_m / 2;
+      auto entry = [&](int i) {
+        const int sub = kind != STRAT_RANGE ? 0 : (i * log_m > log_r ? 2 : ((i + 1) * log_m > log_r ? 1 : 0));
+        return fr_from_u64(subtable_value(kind, sub, nz[(size_t)i * s + k], log_m, log_r));
+      };
+      v = entry(C - 1);
+      for (int i = C - 2; i >= 0; i--) v = fr_add(fr_mul_pow2(v, inc), entry(i));
+    }
+    st_fr(out + k, v);
+    mb = max(mb, fr_bit_width(v));
+  }
+  publish_max_bits(mb, bits);
+}
+// Custom strategies: the uploaded tables (u32 when the strategy has them, else Montgomery), combined by custom_run with
+// the program staged in shared memory as claim_custom_kernel does
+__global__ void __launch_bounds__(kCustomThreads)
+    lookup_outputs_custom_kernel(CustomStrategy cs, const uint32_t* nz, size_t s, fr_t* out, unsigned* bits) {
+  CustomIns* ops;
+  fr_t* consts;
+  uint32_t* slots;
+  custom_stage(cs, ops, consts, slots);
+  unsigned mb = 0;
+  for (size_t k = (size_t)blockIdx.x * blockDim.x + threadIdx.x; k < s; k += (size_t)gridDim.x * blockDim.x) {
+    const fr_t v = custom_run(ops, cs.n_ops, consts, slots, [&](int i) {
+      const size_t t = ((size_t)cs.sub[i] << cs.log_m) + nz[(size_t)cs.dim[i] * s + k];
+      return cs.d_tables_u32 ? fr_from_u64(cs.d_tables_u32[t]) : ld_fr(cs.d_tables_fr + t);
+    });
+    st_fr(out + k, v);
+    mb = max(mb, fr_bit_width(v));
+  }
+  publish_max_bits(mb, bits);
+}
+void launch_lookup_outputs(const Strategy& S, const uint32_t* nz, size_t s, fr_t* out, unsigned* bits, cudaStream_t st) {
+  if (S.kind == STRAT_CUSTOM) {
+    const size_t smem = custom_smem_bytes(*S.custom, 0);
+    launch(lookup_outputs_custom_kernel, custom_grid(s, smem), kCustomThreads, smem, st, *S.custom, nz, s, out, bits);
+  } else {
+    launch(lookup_outputs_kernel, grid_for(s), kThreads, 0, st, S.kind, S.C, S.log_m, S.log_r, nz, s, out, bits);
+  }
 }
 __global__ void __launch_bounds__(kThreads) from_u32_kernel(const uint32_t* in, fr_t* out, size_t n) {
   for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)

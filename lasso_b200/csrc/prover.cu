@@ -1506,13 +1506,31 @@ static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, PolySrc Z, siz
 }
 
 // ---------------------------------------------------------------------------------------------- prove
+// The serialised size of a PolyEvalProof at nv variables: L_vec and R_vec of nv - nv/2 points, delta, beta, z1, z2
+static size_t dpl_bytes(size_t nv) { return 2 * (8 + 32 * (nv - nv / 2)) + 4 * 32; }
+// The serialised size of a BatchedGrandProductArgument over n circuits of v variables: layer j has j cubic rounds
+static size_t gpa_bytes(size_t n, size_t v) { return 8 + v * (24 + 64 * n) + 52 * v * (v - 1); }
+size_t proof_bytes(const Strategy& S, const Dense& dense, const Gens& g) {
+  const size_t alpha = (size_t)S.num_memories(), C = dense.C, log_s = log2_exact_or_ceil(dense.s);
+  return 8 + 32 * ((size_t)1 << (g.nv_d / 2))                        // comm_derefs
+         + 8 + log_s * (8 + 32 * (size_t)S.sumcheck_poly_degree())  // primary sumcheck
+         + 32 + 32 * alpha + dpl_bytes(g.nv_d)                      // claimed_evaluation, eval_derefs, proof_derefs
+         + 4 * 32 * alpha + gpa_bytes(2 * alpha, dense.log_m) + gpa_bytes(2 * alpha, log_s)  // product layer
+         + 32 * (3 * C + alpha) + dpl_bytes(g.nv_l) + dpl_bytes(g.nv_m) + dpl_bytes(g.nv_d);  // hash layer
+}
+
 std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
                            const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,
                            std::vector<fr_t>* challenges) {
-  SpanTimer sp_all(c, "SparsePoly.prove");
   Transcript transcript(transcript_label);
   transcript.trace = challenges;
   RandomTape tape(tape_label, tape_seed);
+  return prove(c, S, dense, r, g, transcript, tape, nullptr);
+}
+
+std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
+                           Transcript& transcript, RandomTape& tape, fr_t* claimed_evaluation) {
+  SpanTimer sp_all(c, "SparsePoly.prove");
   const int G = c->world, gr = c->rank;
   const size_t s = dense.s, C = dense.C, M = dense.m, alpha = (size_t)S.num_memories();
   const size_t s_loc = dense.s_loc, M_loc = dense.m_loc;
@@ -1520,10 +1538,24 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
   if ((size_t)S.C != C || (size_t)S.log_m != dense.log_m) throw std::runtime_error("strategy does not match the densified representation");
   if (g.nv_d != log2_exact_or_ceil(next_pow2(alpha * s)) || g.nv_l != dense.nv_l || g.nv_m != dense.nv_m)
     throw std::runtime_error("generators were built for different (c, s, num_memories, log_m)");
+  const size_t nv_d = g.nv_d, nd_loc = ((size_t)1 << nv_d) / G;
+  {
+    // The proof's device memory, in elements of this rank, is largest either in the primary sumcheck (E, its u32 copy,
+    // the alpha + 1 working copies) or in the product layer (E, its u32 copy, the eq table, four trees of 2N elements per
+    // memory, N = M for init / final and s for read / write), plus the built-in tables and an opening's vectors
+    // (16 R + L + 4096, as combined_eval_prove reserves) at the widest of the three openings.  Reserving that much in
+    // the context's pool, which keeps freed memory, makes a short device fail here, before the transcript or the tape
+    // has moved.
+    const size_t E_elems = nd_loc + nd_loc / 8 + 1;
+    const size_t primary = E_elems + (alpha + 1) * s_loc;
+    const size_t product = E_elems + std::max(s_loc, M_loc) + 4 * alpha * (M_loc + s_loc) + 4 * alpha * 2 * (size_t)G;
+    const size_t tables = S.kind == STRAT_CUSTOM ? 0 : (size_t)S.num_subtables() * M * 9 / 8 + 1;
+    const size_t nv = std::max(nv_d, std::max(g.nv_l, g.nv_m)), R = poly_R(nv);
+    DBuf<fr_t> reserve(c, std::max(primary, product) + tables + 16 * R + ((size_t)1 << nv) / R + 4096);
+  }
   transcript.append_protocol_name("Lasso SparsePolynomialEvaluationProof");
 
   // ---- Subtables::new (subtables/mod.rs:116-129): materialise (replicated, 2-6 MiB), gather, merge
-  const size_t nv_d = g.nv_d, nd_loc = ((size_t)1 << nv_d) / G;
   // a custom strategy's tables were uploaded when it was created: used in place
   const bool custom = S.kind == STRAT_CUSTOM;
   const int nsub = S.num_subtables();
@@ -1579,6 +1611,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     SumcheckProof primary = prove_arbitrary(c, S, Wk.p, s_loc, s_loc, transcript, r_z);
     ser_sumcheck(w, primary);
     w.fr(claimed_eval);
+    if (claimed_evaluation) *claimed_evaluation = claimed_eval;
   }
   // ---- eval_derefs = E_i(r_z) (surge.rs:175-176) and the combined opening (177-184)
   DBuf<fr_t> eqtab(c, std::max(s_loc, M_loc));
@@ -1759,6 +1792,24 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
   if (p->bits <= 32) {
     p->d_u32.alloc(c, len);
     launch_poly_mirror_u32(p->d_fr.p, len, p->d_u32.p, c->st);
+  }
+  return p.release();
+}
+// The lookup outputs in one pass over the indices (poly_kernels.cu), then the integer mirror as poly_create makes it
+Poly* dense_outputs(Ctx* c, const Strategy& S, const Dense& dense) {
+  SpanTimer sp(c, "DensifiedRepresentation.outputs");
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->len = dense.s;
+  p->nv = log2_exact_or_ceil(dense.s);
+  p->d_fr.alloc(c, p->len);
+  DBuf<unsigned> bits(c, 1);
+  LB_CUDA_CHECK(cudaMemsetAsync(bits.p, 0, sizeof(unsigned), c->st));
+  launch_lookup_outputs(S, dense.nz(), dense.s, p->d_fr.p, bits.p, c->st);
+  c->d2h(&p->bits, bits.p, sizeof(unsigned));
+  if (p->bits <= 32) {
+    p->d_u32.alloc(c, p->len);
+    launch_poly_mirror_u32(p->d_fr.p, p->len, p->d_u32.p, c->st);
   }
   return p.release();
 }

@@ -326,9 +326,21 @@ Dense* densify(Ctx*, const uint64_t* indices, size_t n_lookups, size_t C, size_t
 Dense* densify_device(Ctx*, const void* indices, size_t elem_bytes, size_t n_lookups, size_t C, size_t row_stride,
                       size_t col_stride, size_t log_m, cudaStream_t caller, int* err);
 std::vector<uint8_t> commit(Ctx*, const Dense&, const Gens&);
+// SparsePolynomialEvaluationProof::prove (surge.rs:118-211) on the caller's transcript and tape, advanced in place.
+// Throws before the first transcript write when S or g do not fit the dense; the working memory is reserved in the
+// context's pool before it too.  *claimed_evaluation (may be null): the primary sumcheck's claim.
+std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr_t>& r, const Gens&, Transcript&,
+                           RandomTape&, fr_t* claimed_evaluation);
+// the same on Transcript::new(transcript_label) and RandomTape::new(tape_label) seeded with tape_seed; challenges (may
+// be null) receives every challenge drawn
 std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr_t>& r, const Gens&,
                            const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,
                            std::vector<fr_t>* challenges);
+// the size of prove's output, fixed by the shapes (S and g fit dense)
+size_t proof_bytes(const Strategy& S, const Dense&, const Gens&);
+// The lookup outputs v[k] = combine_lookups(E_0[k], .., E_{alpha-1}[k]) for k < s as a new polynomial of log2(s)
+// variables, with a u32 mirror when every value is below 2^32.  Single-GPU contexts (the caller checks).
+Poly* dense_outputs(Ctx*, const Strategy& S, const Dense&);
 void sample_generators(const std::string& label, size_t count, uint64_t* out_affine);
 
 // dense polynomials of a caller (prover.cu): PolyCommitmentGens, DensePolynomial::{new, commit, evaluate},

@@ -10,7 +10,7 @@
 //   HashLayerProof::verify                           memory_checking.rs:462-523
 //   Subtables::new, compute_sumcheck_claim           subtables/mod.rs:116-129, 186-216
 // evaluate_subtable_mle of a custom table is its dense MLE (DensePolynomial::evaluate, point[0] the MSB).
-#include "../oracle/lasso.hpp"
+#include "../oracle_dense/sparse_bytes.hpp"
 
 using namespace oracle;
 
@@ -292,6 +292,50 @@ int prove_all(const CustomStrategy& S, const uint64_t* indices, size_t n, const 
   }
 }
 
+// The same proof on a caller's transcript and tape (oracle_dense's Transcript / RandomTape objects): densify, commit
+// (comm_out: the serialised commitment), prove at r.  Returns the proof's length, 0 on error; claim_out = the claimed
+// evaluation.
+size_t prove_transcript(const CustomStrategy& S, const uint64_t* indices, size_t n, const uint64_t* r, const uint64_t* gens,
+                        size_t n_gens, void* transcript, void* tape, uint8_t* out, size_t cap, uint8_t* comm_out,
+                        size_t comm_cap, uint64_t* claim_out) {
+  try {
+    const size_t C = S.C, log_m = S.log_m, alpha = S.num_memories();
+    std::vector<std::vector<size_t>> idx(n, std::vector<size_t>(C));
+    for (size_t j = 0; j < n; j++)
+      for (size_t i = 0; i < C; i++) idx[j][i] = indices[j * C + i];
+    std::vector<Affine> stream(n_gens);
+    for (size_t i = 0; i < n_gens; i++) stream[i] = ldaff(gens + 8 * i);
+    DensifiedRepresentation dense = DensifiedRepresentation::from_lookup_indices(idx, C, log_m);
+    if (n_gens < SparsePolyCommitmentGens::needs_points(C, dense.s, alpha, log_m)) return 0;
+    SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, dense.s, alpha, log_m, stream);
+    const std::vector<uint8_t> cb = serialize_commitment(densified_commit(dense, pg));
+    const SparsePolynomialEvaluationProof proof =
+        prove(S, dense, ldvec(r, ark_log2(dense.s)), pg, *(Transcript*)transcript, *(RandomTape*)tape);
+    const std::vector<uint8_t> pb = serialize_proof(proof);
+    if (pb.size() > cap || cb.size() > comm_cap) return 0;
+    memcpy(out, pb.data(), pb.size());
+    memcpy(comm_out, cb.data(), cb.size());
+    stfr(claim_out, proof.claimed_evaluation);
+    return pb.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orc_custom_prove_transcript: %s\n", e.what());
+    return 0;
+  }
+}
+// verify of serialised proof and commitment bytes on a caller's transcript: 0 accepted, 1 rejected, 2 the bytes do not
+// parse or the generator stream is too short
+int verify_transcript(const CustomStrategy& S, const uint64_t* gens, size_t n_gens, const uint8_t* comm, size_t comm_len,
+                      const uint8_t* proof, size_t proof_len, const uint64_t* r, void* transcript) {
+  SparsePolynomialCommitment c;
+  SparsePolynomialEvaluationProof p;
+  if (!read_sparse_commitment(comm, comm_len, c) || !read_sparse_proof(proof, proof_len, S.num_memories(), S.C, p)) return 2;
+  if (n_gens < SparsePolyCommitmentGens::needs_points(S.C, c.s, S.num_memories(), S.log_m)) return 2;
+  std::vector<Affine> stream(n_gens);
+  for (size_t i = 0; i < n_gens; i++) stream[i] = ldaff(gens + 8 * i);
+  SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(S.C, c.s, S.num_memories(), S.log_m, stream);
+  return verify(p, S, c, ldvec(r, ark_log2(c.s)), pg, *(Transcript*)transcript) ? 0 : 1;
+}
+
 }  // namespace
 
 #define ORC_CUSTOM_ARGS                                                                                             \
@@ -344,6 +388,28 @@ int orc_custom_prove_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* indices, size_t n, c
                         uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
   return prove_all(ORC_CUSTOM_FR, indices, n, r, gens, n_gens, tape_seed, flags, proof_out, proof_cap, proof_len,
                    commit_out, commit_cap, commit_len, challenges_out, challenges_cap, n_challenges);
+}
+
+// prove_transcript / verify_transcript above, tables as u32 and as Fr
+size_t orc_custom_prove_transcript(ORC_CUSTOM_ARGS, const uint64_t* indices, size_t n, const uint64_t* r,
+                                   const uint64_t* gens, size_t n_gens, void* transcript, void* tape, uint8_t* out,
+                                   size_t cap, uint8_t* comm_out, size_t comm_cap, uint64_t* claim_out) {
+  return prove_transcript(ORC_CUSTOM, indices, n, r, gens, n_gens, transcript, tape, out, cap, comm_out, comm_cap, claim_out);
+}
+int orc_custom_verify_transcript(ORC_CUSTOM_ARGS, const uint64_t* gens, size_t n_gens, const uint8_t* comm, size_t comm_len,
+                                 const uint8_t* proof, size_t proof_len, const uint64_t* r, void* transcript) {
+  return verify_transcript(ORC_CUSTOM, gens, n_gens, comm, comm_len, proof, proof_len, r, transcript);
+}
+size_t orc_custom_prove_transcript_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* indices, size_t n, const uint64_t* r,
+                                      const uint64_t* gens, size_t n_gens, void* transcript, void* tape, uint8_t* out,
+                                      size_t cap, uint8_t* comm_out, size_t comm_cap, uint64_t* claim_out) {
+  return prove_transcript(ORC_CUSTOM_FR, indices, n, r, gens, n_gens, transcript, tape, out, cap, comm_out, comm_cap,
+                          claim_out);
+}
+int orc_custom_verify_transcript_fr(ORC_CUSTOM_ARGS_FR, const uint64_t* gens, size_t n_gens, const uint8_t* comm,
+                                    size_t comm_len, const uint8_t* proof, size_t proof_len, const uint64_t* r,
+                                    void* transcript) {
+  return verify_transcript(ORC_CUSTOM_FR, gens, n_gens, comm, comm_len, proof, proof_len, r, transcript);
 }
 
 }  // extern "C"

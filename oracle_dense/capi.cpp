@@ -6,7 +6,7 @@
 // only inside its own round trips; this file puts C entry points on the same code that take and return what the
 // library takes and returns: serialised bytes, an explicit generator stream, and transcript / tape objects that live
 // across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof.
-#include "../oracle/lasso.hpp"
+#include "sparse_bytes.hpp"
 
 using namespace oracle;
 
@@ -23,12 +23,6 @@ std::vector<Affine> ldstream(const uint64_t* p, size_t n) {
   std::vector<Affine> s(n);
   for (size_t i = 0; i < n; i++) s[i] = Affine{Fq::from_raw(p + 8 * i), Fq::from_raw(p + 8 * i + 4)};
   return s;
-}
-bool ldpoint(const uint8_t* in, Point& out) {
-  Affine a;
-  if (!decompress(in, a)) return false;
-  out = Point::from_affine(a);
-  return true;
 }
 void put_u64(std::vector<uint8_t>& b, uint64_t v) {
   for (int i = 0; i < 8; i++) b.push_back((uint8_t)(v >> (8 * i)));
@@ -64,48 +58,6 @@ std::vector<uint8_t> ser_proof(const PolyEvalProof& p) {
   put_fr(b, d.z2);
   return b;
 }
-struct Reader {
-  const uint8_t* p;
-  size_t n, at = 0;
-  bool ok = true;
-  const uint8_t* take(size_t k) {
-    if (!ok || n - at < k) {
-      ok = false;
-      return nullptr;
-    }
-    at += k;
-    return p + at - k;
-  }
-  uint64_t u64() {
-    const uint8_t* b = take(8);
-    uint64_t v = 0;
-    if (b) memcpy(&v, b, 8);
-    return v;
-  }
-  Point point() {
-    const uint8_t* b = take(32);
-    Point q = Point::zero();
-    if (b && !ldpoint(b, q)) ok = false;
-    return q;
-  }
-  std::vector<Point> points() {
-    const uint64_t k = u64();
-    std::vector<Point> v;
-    if (k > (n - at) / 32) ok = false;
-    for (uint64_t i = 0; ok && i < k; i++) v.push_back(point());
-    return v;
-  }
-  Fr fr() {  // ark rejects a non-canonical encoding
-    const uint8_t* b = take(32);
-    if (!b) return Fr::zero();
-    Fr f = Fr::from_bytes32_mod_order(b);
-    uint8_t back[32];
-    f.to_bytes(back);
-    if (memcmp(back, b, 32)) ok = false;
-    return f;
-  }
-};
-
 // A combining function as lasso_comb_create takes it: 3 ints {op, a, b} per instruction, slots 0..n-1 the inputs,
 // instruction j writes slot n + j, the last slot is g; op: 0 a + b, 1 a - b, 2 a * b, 3 a * K[b], 4 a + K[b].
 // Interpreted directly, SSA slot by SSA slot (no slot allocation).  Taken as given: the GPU library checks it.
@@ -464,6 +416,56 @@ int orcd_combined_eval_verify(const uint64_t* stream, size_t n_points, size_t nv
   p.proof_table_eval.proof.z2 = rp.fr();
   if (!rp.ok || rp.at != proof_len) return 2;
   return p.verify(ldvec(r, r_len), ldvec(evals, n_evals), gens, c, *(Transcript*)transcript) ? 0 : 1;
+}
+
+// ---- SparsePolynomialEvaluationProof on a caller's transcript and tape (surge.rs:70-82, 118-271), built-in strategies
+// SparsePolynomialCommitment::append_to_transcript of lasso_commit-shaped bytes: 0 absorbed, 1 they do not parse (nothing
+// is absorbed then)
+int orcd_sparse_append_commitment(void* t, const uint8_t* bytes, size_t len) {
+  SparsePolynomialCommitment c;
+  if (!read_sparse_commitment(bytes, len, c)) return 1;
+  append_sparse_commitment(c, *(Transcript*)t);
+  return 0;
+}
+// Densify n x C indices, commit (comm_out: serialize_commitment's bytes, comm_cap) and prove at r on a caller's
+// transcript and tape: returns the proof's length (0 on error); claim_out = the claimed evaluation
+size_t orcd_sparse_prove(int kind, size_t C, size_t log_m, size_t log_r, const uint64_t* indices, size_t n, const uint64_t* r,
+                         const uint64_t* stream, size_t n_points, void* transcript, void* tape, uint8_t* out, size_t cap,
+                         uint8_t* comm_out, size_t comm_cap, uint64_t* claim_out) {
+  try {
+    const Strategy S{kind, C, log_m, log_r};
+    std::vector<std::vector<size_t>> idx(n, std::vector<size_t>(C));
+    for (size_t j = 0; j < n; j++)
+      for (size_t i = 0; i < C; i++) idx[j][i] = indices[j * C + i];
+    DensifiedRepresentation dense = DensifiedRepresentation::from_lookup_indices(idx, C, log_m);
+    if (n_points < SparsePolyCommitmentGens::needs_points(C, dense.s, S.num_memories(), log_m)) return 0;
+    SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, dense.s, S.num_memories(), log_m, ldstream(stream, n_points));
+    const std::vector<uint8_t> cb = serialize_commitment(densified_commit(dense, pg));
+    const SparsePolynomialEvaluationProof p = SparsePolynomialEvaluationProof::prove(
+        S, dense, ldvec(r, ark_log2(dense.s)), pg, *(Transcript*)transcript, *(RandomTape*)tape);
+    const std::vector<uint8_t> b = serialize_proof(p);
+    if (b.size() > cap || cb.size() > comm_cap) return 0;
+    memcpy(out, b.data(), b.size());
+    memcpy(comm_out, cb.data(), cb.size());
+    stfr(claim_out, p.claimed_evaluation);
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_sparse_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// SparsePolynomialEvaluationProof::verify of serialised bytes against serialised commitment bytes, on a caller's
+// transcript: 0 accepted, 1 rejected, 2 the bytes do not parse or the generator stream is too short
+int orcd_sparse_verify(int kind, size_t C, size_t log_m, size_t log_r, const uint64_t* stream, size_t n_points,
+                       const uint8_t* comm, size_t comm_len, const uint8_t* proof, size_t proof_len, const uint64_t* r,
+                       void* transcript) {
+  const Strategy S{kind, C, log_m, log_r};
+  SparsePolynomialCommitment c;
+  SparsePolynomialEvaluationProof p;
+  if (!read_sparse_commitment(comm, comm_len, c) || !read_sparse_proof(proof, proof_len, S.num_memories(), C, p)) return 2;
+  if (n_points < SparsePolyCommitmentGens::needs_points(C, c.s, S.num_memories(), log_m)) return 2;
+  SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, c.s, S.num_memories(), log_m, ldstream(stream, n_points));
+  return p.verify(S, c, ldvec(r, ark_log2(c.s)), pg, *(Transcript*)transcript) ? 0 : 1;
 }
 
 }  // extern "C"
