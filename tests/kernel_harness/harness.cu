@@ -13,6 +13,7 @@ using namespace lb;
 using kh::ck;
 using kh::fr_of;
 using kh::guarded;
+using kh::KhTables;
 using kh::make_fin;
 using kh::Pub;
 using kh::Scope;
@@ -21,10 +22,6 @@ using kh::Scope;
 // Built once per test module with the library's launchers (launch_build_table, launch_build_multiples, optionally
 // launch_build_multiples16 for ncols16 local columns, column jl <-> generator jl * col_mul + col_add) and kept on the
 // device until kh_tables_destroy: rebuilding ~1 GB per launch under test would dominate the suite.
-struct KhTables {
-  size_t npts = 0, ncols16 = 0;
-  pt_niels *T = nullptr, *M = nullptr, *M16 = nullptr;
-};
 
 extern "C" {
 

@@ -1,6 +1,6 @@
-// Test harness plumbing shared by its translation units (harness.cu, harness_comb.cu, arith.cu, harness_fr.cu): error
-// codes, the per-call device allocation scope, the publication region of the launchers that publish, and the wrapper
-// that turns exceptions into return codes.
+// Test harness plumbing shared by its translation units (harness.cu, harness_comb.cu, harness_msm.cu, arith.cu,
+// harness_fr.cu): error codes, the per-call device allocation scope, the publication region of the launchers that
+// publish, the generator tables, and the wrapper that turns exceptions into return codes.
 // Return codes: 0 ok, -1 a launcher threw (std::runtime_error), -2 a CUDA error, -3 a publication slot did not carry
 // the message's tag, -4 bad arguments, -5 a repeated launch published different values (harness_comb.cu).
 #pragma once
@@ -105,6 +105,13 @@ struct Pub {
     for (size_t i = (size_t)v0 * lb::kPubSlotWords; i < (size_t)(v0 + count) * lb::kPubSlotWords; i++)
       if (h[i] != 0) throw HarnessError{-3};
   }
+};
+
+// window + digit-multiples tables of a generator set (kh_tables_create, harness.cu).  The device arrays belong to the
+// process's primary context, so every harness library loaded into the process can use them.
+struct KhTables {
+  size_t npts = 0, ncols16 = 0;
+  lb::pt_niels *T = nullptr, *M = nullptr, *M16 = nullptr;
 };
 
 inline lb::Finalize make_fin(Scope& s, const Pub& p, size_t partial_elems) {

@@ -5,14 +5,8 @@
 
 using namespace lb;
 using kh::guarded;
+using kh::KhTables;  // created by kh_tables_create (harness.cu, libkernel_harness.so)
 using kh::Scope;
-
-// the tables of kh_tables_create (harness.cu, libkernel_harness.so): the same layout; the device arrays belong to the
-// process's primary context, so they are valid here too
-struct KhTables {
-  size_t npts = 0, ncols16 = 0;
-  pt_niels *T = nullptr, *M = nullptr, *M16 = nullptr;
-};
 
 extern "C" {
 

@@ -36,6 +36,10 @@ def lib():
         L.kh_bullet_fused.argtypes = [V, V, V, V, S, S, I, V, V, V, V, V, V, V, V]
         L.kh_msm_rows_direct_u32.argtypes = [V, V, I, I, I, I, I, I, V]
         L.kh_msm_large.argtypes = [V, S, V, S, I, V, V, V]
+        L.kh_msm_rows.argtypes = [V, I, V, I, S, I, I, I, I, I, V, V, V]
+        L.kh_sum_raw_points.argtypes = [V, I, I, V, V, V]
+        L.kh_canonicalize.argtypes = [V, S, C.c_uint, V, V]
+        L.kh_msm_rows_direct_raw.argtypes = [V, I, V, I, I, I, I, I, I, V, V]
         L.kh_comb_program.argtypes = [I, V, I, V, I, I, V, V]
         L.kh_comb_eval.argtypes = [I, V, I, V, I, I, V, V, S, I, V]
         L.kh_comb_bind_eval.argtypes = [I, V, I, V, I, I, V, V, S, V, S, I, I, V, V, V]
