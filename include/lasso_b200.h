@@ -299,8 +299,9 @@ int lasso_poly_create_device(lasso_ctx*, const uint64_t* Z, size_t len, size_t r
                              lasso_poly** out);
 size_t lasso_poly_num_vars(const lasso_poly*);
 void lasso_poly_destroy(lasso_poly*);
-/* DensePolynomial::commit (poly/dense_mlpoly.rs:152-181) without blinds -> PolyCommitment { C: Vec<G> } serialised
- * with ark-serialize (compressed): a u64 count L = 2^(num_vars/2), then 32 bytes per row.  *out_len receives the size
+/* DensePolynomial::commit (poly/dense_mlpoly.rs:152-181) without blinds (with them: lasso_poly_commit_hiding) ->
+ * PolyCommitment { C: Vec<G> } serialised with ark-serialize (compressed): a u64 count L = 2^(num_vars/2), then 32
+ * bytes per row.  *out_len receives the size
  * (also when cap is too small: LASSO_ERR_LENGTH).  LASSO_ERR_GENS when the generators' R differs from the
  * polynomial's (poly/commitments.rs:85). */
 int lasso_poly_commit(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, uint8_t* out, size_t cap, size_t* out_len);
@@ -312,6 +313,25 @@ int lasso_poly_evaluate(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t
 int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, const uint64_t* r, size_t r_len,
                           const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* random_tape,
                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]);
+/* Hiding commitments and openings (single-GPU contexts, like every lasso_poly_* call).
+ * lasso_poly_commit_hiding is DensePolynomial::commit(gens, Some(random_tape)) (poly/dense_mlpoly.rs:152-181): it draws
+ * L = 2^(num_vars/2) blinds from the tape as random_vector("poly_blinds", L), writes the hiding PolyCommitment (row i is
+ * <row_i, G> + blinds[i] * h; same format and size as lasso_poly_commit) to out and the L blinds (L x 4 Montgomery limbs)
+ * to blinds_out, which has room for blinds_cap of them.
+ * lasso_poly_eval_prove_hiding is PolyEvalProof::prove(poly, blinds_opt, r, Zr, blind_Zr_opt, ...)
+ * (poly/dense_mlpoly.rs:301-359): blinds (n_blinds == L, the commitment's blinds) or None (n_blinds == 0); blind_Zr
+ * or None (NULL).  Same proof size as lasso_poly_eval_prove; C_Zr_out (may be null) is Zr * Q + blind_Zr * h.  With no
+ * blinds and no blind_Zr it is lasso_poly_eval_prove, byte for byte.
+ * Both check everything before any launch and before the tape or the transcript moves: LASSO_ERR_LENGTH for out / cap
+ * or blinds_out / blinds_cap too small (*out_len / *proof_len receive the size needed), a null tape or transcript, or
+ * n_blinds other than 0 or L; LASSO_ERR_VALUE for a blind, blind_Zr, Zr or coordinate of r that is not a canonical
+ * residue; LASSO_ERR_GENS and LASSO_ERR_STRATEGY as lasso_poly_commit / lasso_poly_eval_prove. */
+int lasso_poly_commit_hiding(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, lasso_random_tape*,
+                             uint8_t* out, size_t cap, size_t* out_len, uint64_t* blinds_out, size_t blinds_cap);
+int lasso_poly_eval_prove_hiding(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, const uint64_t* blinds,
+                                 size_t n_blinds, const uint64_t* r, size_t r_len, const uint64_t Zr[4],
+                                 const uint64_t blind_Zr[4], lasso_transcript*, lasso_random_tape*, uint8_t* proof_out,
+                                 size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]);
 /* EqPolynomial::new(r).evals() (poly/eq_poly.rs:21-38) as a polynomial of the context, r[0] the most significant
  * variable: 2^r_len evaluations, r_len <= 28 (LASSO_ERR_LENGTH), each coordinate a canonical residue (LASSO_ERR_VALUE). */
 int lasso_poly_create_eq(lasso_ctx*, const uint64_t* r, size_t r_len, lasso_poly** out);

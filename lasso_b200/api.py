@@ -913,6 +913,18 @@ class DensePolynomial:
         _chk(lib().lasso_poly_commit(self.ctx._h, self._h, gens._h, _p(out), C.c_size_t(cap), C.byref(n)))
         return bytes(out[: n.value])
 
+    def commit_hiding(self, gens, random_tape):
+        """DensePolynomial::commit with Some(random_tape): draws L = 2^(num_vars // 2) blinds as
+        random_vector("poly_blinds", L) and commits row i with blind i on h -> (the ark-serialize bytes of
+        PolyCommitment, the blinds as an (L, 4) uint64 array of Montgomery limbs).  Advances random_tape in place."""
+        L = 1 << (self.num_vars // 2)
+        out = np.zeros(8 + 32 * L, dtype=np.uint8)
+        blinds = np.zeros((L, 4), dtype=np.uint64)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_poly_commit_hiding(self.ctx._h, self._h, gens._h, random_tape._h, _p(out), C.c_size_t(out.shape[0]),
+                                            C.byref(n), _p(blinds), C.c_size_t(L)))
+        return bytes(out[: n.value]), blinds
+
     def evaluate(self, r):
         r = _limbs(r, what="r")
         out = np.zeros(4, dtype=np.uint64)
@@ -935,16 +947,25 @@ class PolyEvalProof:
         self.bytes, self.C_Zr = data, C_Zr
 
     @classmethod
-    def prove(cls, ctx, poly, r, Zr, gens, transcript, random_tape):
-        """advances transcript and random_tape in place"""
+    def prove(cls, ctx, poly, r, Zr, gens, transcript, random_tape, *, blinds=None, blind_Zr=None):
+        """advances transcript and random_tape in place.  blinds: the (L, 4) row blinds commit_hiding returned (None:
+        the commitment was not hiding); blind_Zr: the blind of C_Zr = Zr Q + blind_Zr h (None: zero)"""
         r = _limbs(r, what="r")
         Zr = _limbs(Zr, 1, "Zr")
         cap = 2 * (8 + 32 * 32) + 4 * 32
         out = np.zeros(cap, dtype=np.uint8)
         czr = np.zeros(32, dtype=np.uint8)
         n = C.c_size_t(0)
-        _chk(lib().lasso_poly_eval_prove(ctx._h, poly._h, gens._h, _p(r), C.c_size_t(r.shape[0]), _p(Zr), transcript._h,
-                                         random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
+        if blinds is None and blind_Zr is None:
+            _chk(lib().lasso_poly_eval_prove(ctx._h, poly._h, gens._h, _p(r), C.c_size_t(r.shape[0]), _p(Zr), transcript._h,
+                                             random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
+        else:
+            bl = None if blinds is None else _limbs(blinds, what="blinds")
+            bz = None if blind_Zr is None else _limbs(blind_Zr, 1, "blind_Zr")
+            _chk(lib().lasso_poly_eval_prove_hiding(
+                ctx._h, poly._h, gens._h, None if bl is None else _p(bl), C.c_size_t(0 if bl is None else bl.shape[0]),
+                _p(r), C.c_size_t(r.shape[0]), _p(Zr), None if bz is None else _p(bz), transcript._h, random_tape._h,
+                _p(out), C.c_size_t(cap), C.byref(n), _p(czr)))
         return cls(bytes(out[: n.value]), czr.tobytes())
 
 

@@ -1117,6 +1117,25 @@ int lasso_poly_commit(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* 
   return 0;
   LB_CATCH
 }
+int lasso_poly_commit_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, lasso_random_tape* tape,
+                             uint8_t* out, size_t cap, size_t* out_len, uint64_t* blinds_out, size_t blinds_cap) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, g)) return rc;
+  if (!g) return fail(LASSO_ERR_GENS, "poly commit: null generators");
+  if (!tape) return fail(LASSO_ERR_LENGTH, "poly commit: null random tape");
+  const size_t L = (size_t)1 << (p->p->nv / 2), need = 8 + 32 * L;
+  if (out_len) *out_len = need;
+  if (!out || cap < need) return fail(LASSO_ERR_LENGTH, "poly commit: output buffer too small");
+  if (!blinds_out || blinds_cap < L) return fail(LASSO_ERR_LENGTH, "poly commit: room for fewer blinds than rows");
+  auto t0 = std::chrono::steady_clock::now();
+  const std::vector<fr_t> blinds = tape->t.random_vector("poly_blinds", L);  // dense_mlpoly.rs:165-170
+  const std::vector<uint8_t> b = poly_commit_hiding(h->c, *p->p, *g->g, blinds);
+  h->c->t_commit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  memcpy(out, b.data(), b.size());
+  for (size_t i = 0; i < L; i++) memcpy(blinds_out + 4 * i, blinds[i].v, 32);
+  return 0;
+  LB_CATCH
+}
 static int load_point(const Poly& p, const uint64_t* r, size_t r_len, std::vector<fr_t>& rv) {
   if (r_len != p.nv) return fail(LASSO_ERR_LENGTH, "poly: r.len() != num_vars");
   if (r_len && !r) return fail(LASSO_ERR_LENGTH, "poly: null point");
@@ -1136,20 +1155,32 @@ int lasso_poly_evaluate(lasso_ctx* h, const lasso_poly* p, const uint64_t* r, si
 int lasso_poly_eval_prove(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, const uint64_t* r, size_t r_len,
                           const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* tape,
                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]) {
+  return lasso_poly_eval_prove_hiding(h, p, g, nullptr, 0, r, r_len, Zr, nullptr, transcript, tape, proof_out, proof_cap,
+                                      proof_len, C_Zr_out);
+}
+int lasso_poly_eval_prove_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, const uint64_t* blinds,
+                                 size_t n_blinds, const uint64_t* r, size_t r_len, const uint64_t Zr[4],
+                                 const uint64_t blind_Zr[4], lasso_transcript* transcript, lasso_random_tape* tape,
+                                 uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]) {
   LB_TRY_CTX(h)
   if (const int rc = poly_use_check(h, p, g)) return rc;
   if (!g) return fail(LASSO_ERR_GENS, "poly eval proof: null generators");
   if (!transcript || !tape) return fail(LASSO_ERR_LENGTH, "poly eval proof: null transcript or random tape");
-  std::vector<fr_t> rv, zr;
+  if (n_blinds != 0 && (n_blinds != ((size_t)1 << (p->p->nv / 2)) || !blinds))
+    return fail(LASSO_ERR_LENGTH, "poly eval proof: n_blinds must be 0 (no blinds) or the commitment's row count");
+  std::vector<fr_t> rv, zr, bl, bzr(1, fr_zero());
   if (const int rc = load_point(*p->p, r, r_len, rv)) return rc;
   if (!load_scalars(Zr, 1, zr)) return fail(LASSO_ERR_VALUE, "poly eval proof: Zr is not a canonical residue");
+  if (!load_scalars(blinds, n_blinds, bl)) return fail(LASSO_ERR_VALUE, "poly eval proof: a blind is not a canonical residue");
+  if (blind_Zr && !load_scalars(blind_Zr, 1, bzr))
+    return fail(LASSO_ERR_VALUE, "poly eval proof: blind_Zr is not a canonical residue");
   // the proof's size is fixed by num_vars: L_vec and R_vec of log2(R) points, delta, beta, z1, z2
   const size_t lg = p->p->nv - p->p->nv / 2, need = 2 * (8 + 32 * lg) + 4 * 32;
   if (proof_len) *proof_len = need;
   if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "poly eval proof: output buffer too small");
   auto t0 = std::chrono::steady_clock::now();
   uint8_t czr[32];
-  const std::vector<uint8_t> b = poly_eval_prove(h->c, *p->p, *g->g, rv, zr[0], transcript->t, tape->t, czr);
+  const std::vector<uint8_t> b = poly_eval_prove(h->c, *p->p, *g->g, rv, zr[0], transcript->t, tape->t, czr, bl, bzr[0]);
   h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
   if (b.size() != need) return fail(-1, "poly eval proof: unexpected proof size");
   memcpy(proof_out, b.data(), b.size());

@@ -64,6 +64,12 @@ void launch_msm_rows_direct_u32(const pt_niels* M, size_t npts, const pt_niels* 
 void launch_msm_rows_direct_fr(const pt_niels* M, size_t npts, const fr_t* scalars, size_t row_stride, int nrows, int ncols,
                                int nw, int col_mul, int col_add, pt_ext* partials, fq_t* out_ext, uint32_t* out_comp,
                                uint32_t* out_raw, cudaStream_t st);
+// Hiding row commitments C_i = R_i + blinds[i] * h: raw = nrows x 128 B un-normalised R_i (the out_raw of a row
+// launcher), blinds = nrows Montgomery Fr elements, Mh = the 8-bit multiples of h alone: entry (w, d) at
+// Mh[w * wstride + d - 1] (a column of launch_build_multiples' M: wstride = 128 * npts; a table built for h: 128).
+// out_comp = nrows x 32 B compressed, as launch_sum_raw_points writes them.
+void launch_row_blinds(const pt_niels* Mh, size_t wstride, const fr_t* blinds, const uint32_t* raw, int nrows,
+                       uint32_t* out_comp, cudaStream_t st);
 void msm_init_device();
 
 // ---- one large variable-base MSM (msm_large.cu): the reference's Pippenger with a large window, buckets in HBM

@@ -1066,6 +1066,55 @@ void launch_msm_rows_direct_fr(const pt_niels* M, size_t npts, const fr_t* scala
     launch(normalize_rows_kernel, (nrows + 31) / 32, 32, 0, st, partials, nrows, out_ext, out_comp);
 }
 
+// The blind term of hiding row commitments (commitments.rs:84-93 with a blind): C_i = R_i + blind_i * h.  One warp per
+// row; lane w takes signed 8-bit digit w of the canonical blind by the offset recoding of msm_rows_direct_fr_kernel
+// over all 32 windows (b = v + sum_w 128 * 2^(8w) has no carry out of the top byte since v < l < 2^253), fetches
+// +-Mh[w][|d| - 1] (the identity for d = 0), the warp adds its 32 points by shuffles, and lane 0 adds R_i, normalises
+// and writes the compressed point.
+__global__ void __launch_bounds__(256)
+    row_blinds_kernel(const pt_niels* Mh, size_t wstride, const fr_t* blinds, const uint32_t* raw, int nrows,
+                      uint32_t* out_comp) {
+  const int lane = threadIdx.x & 31;
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= nrows) return;  // uniform per warp
+  const fr_t v = fr_to_canonical(ld_fr(blinds + row));
+  const MsmDigits<8> dg(v.v);
+  uint32_t limb = 0;
+#pragma unroll
+  for (int l = 0; l < 8; l++) limb = (l == (lane >> 2)) ? dg.b[l] : limb;  // no dynamic register indexing
+  const int d = (int)((limb >> (8 * (lane & 3))) & 0xff) - 128;
+  pt_ext acc = pt_identity();
+  if (d != 0) {
+    const pt_niels n = ld_niels(Mh + (size_t)lane * wstride + ((d < 0 ? -d : d) - 1));
+    acc = pt_from_niels(d < 0 ? niels_neg(n) : n);
+  }
+#pragma unroll 1
+  for (int s = 16; s >= 1; s >>= 1) acc = pt_add(acc, shfl_down_pt(acc, s));
+  if (lane == 0) {
+    const uint32_t* p = raw + (size_t)row * 32;
+    pt_ext r;
+#pragma unroll
+    for (int l = 0; l < 8; l++) {
+      r.X.v[l] = p[l];
+      r.Y.v[l] = p[8 + l];
+      r.Z.v[l] = p[16 + l];
+      r.T.v[l] = p[24 + l];
+    }
+    acc = pt_add(acc, r);
+    fq_t x, y;
+    pt_to_affine_canonical(acc, x, y);
+    uint32_t c[8];
+    pt_compress_canonical(x, y, c);
+#pragma unroll
+    for (int l = 0; l < 8; l++) out_comp[(size_t)row * 8 + l] = c[l];
+  }
+}
+void launch_row_blinds(const pt_niels* Mh, size_t wstride, const fr_t* blinds, const uint32_t* raw, int nrows,
+                       uint32_t* out_comp, cudaStream_t st) {
+  if (nrows <= 0) return;
+  launch(row_blinds_kernel, (nrows + 7) / 8, 256, 0, st, Mh, wstride, blinds, raw, nrows, out_comp);
+}
+
 // Launch geometry.  wpc = windows per CTA (all of them over a shifted table), ngroups = window groups,
 // chunk_cols = columns per CTA: at most MSM_CHUNK list entries (columns x windows) per CTA; with only a few
 // rows (Bulletproofs rounds) the columns are split further so that about one CTA per SM exists.

@@ -389,13 +389,19 @@ static void eq_evals_shard(Ctx* c, const std::vector<fr_t>& r, size_t off, size_
 // Row-MSMs over the generator table with the bucket kernels.  Column-sharded (replicated == false, G > 1): `d_scal`
 // holds this rank's columns (ncols per row, local column c' = generator c'*G + rank), the per-row partial points
 // of every rank are all-gathered and added ("bucket-sum reduce" = gather-then-add).  Replicated: every rank
-// passes the same full rows and computes the same points, no exchange.  Returns nrows compressed points.
+// passes the same full rows and computes the same points, no exchange.  Returns nrows compressed points; with raw_out
+// (single GPU) the rows go un-normalised to raw_out instead and nothing is returned (hiding commitments).
 static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, int limbs, size_t row_stride, int nrows,
-                                     int ncols, int nw, bool replicated) {
+                                     int ncols, int nw, bool replicated, uint32_t* raw_out = nullptr) {
   const int G = replicated ? 1 : c->world, gr = replicated ? 0 : c->rank;
+  DBuf<pt_ext> part(c, msm_partials_count(nrows, ncols, nw));
+  if (raw_out) {
+    launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, 1, 0, part.p, nullptr, nullptr,
+                    raw_out, c->st);
+    return {};
+  }
   std::vector<uint8_t> out((size_t)nrows * 32);
   const bool few = nrows <= 8;
-  DBuf<pt_ext> part(c, msm_partials_count(nrows, ncols, nw));
   if (G == 1 && !few) {  // the common single-GPU commit: normalise on the device
     DBuf<uint32_t> comp(c, (size_t)nrows * 8);
     launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, 1, 0, part.p, nullptr, comp.p,
@@ -436,8 +442,10 @@ static std::vector<uint8_t> msm_rows_fr(Ctx* c, const Gens& g, const fr_t* d_sca
 }
 
 // DensePolynomial::commit (dense_mlpoly.rs:152-181) for an integer-valued polynomial of 2^nv entries viewed as
-// L x R; this rank holds, for every row, the R/G columns congruent to its rank (= its low-bit shard of the array)
-static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_vals_loc, size_t nv, unsigned max_bits) {
+// L x R; this rank holds, for every row, the R/G columns congruent to its rank (= its low-bit shard of the array).
+// raw (single GPU): the rows un-normalised, for the blind term of a hiding commitment; nothing is returned then.
+static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_vals_loc, size_t nv, unsigned max_bits,
+                                       uint32_t* raw = nullptr) {
   size_t L = (size_t)1 << (nv / 2), R = (size_t)1 << (nv - nv / 2);
   if (R + 2 > g.n_points) throw std::runtime_error("generator stream too short for this polynomial");
   int nw = msm_windows_for_bits(max_bits);
@@ -446,14 +454,19 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
   size_t R_loc = loc(c, R);
   if (g.d_multiples.p && R + 2 <= g.n_direct && L > 8) {
     // rows as direct sums over the digit-multiples tables (msm_kernels.cu): one table entry per committed integer
-    std::vector<uint8_t> out(L * 32);
     DBuf<pt_ext> part(c, L);
-    DBuf<uint32_t> comp(c, L * 8);
     const bool wide = R_loc <= g.n_direct16;
     size_t lg_rloc = 0;
     while (((size_t)1 << lg_rloc) < R_loc) lg_rloc++;
     const pt_niels* m16 = wide ? g.d_multiples16.p : nullptr;
     const pt_ext* k16 = wide ? g.d_centre.p + lg_rloc : nullptr;
+    if (raw) {
+      launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr,
+                                 nullptr, raw, c->st);
+      return {};
+    }
+    std::vector<uint8_t> out(L * 32);
+    DBuf<uint32_t> comp(c, L * 8);
     if (G == 1) {  // normalised on the device
       launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr,
                                  comp.p, nullptr, c->st);
@@ -470,13 +483,14 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
     c->d2h(out.data(), comp.p, out.size());
     return out;
   }
-  return msm_rows(c, g, d_vals_loc, 1, R_loc, (int)L, (int)R_loc, nw, false);
+  return msm_rows(c, g, d_vals_loc, 1, R_loc, (int)L, (int)R_loc, nw, false, raw);
 }
 
 // The same commitment of a field-valued polynomial (Montgomery, shard as commit_u32) whose entries have at most
 // max_bits bits.  No sign folding: v is committed as the canonical integer it is, so an entry l - k costs the full
 // width (folding it to -k is exact only in the prime-order subgroup, and the generators are the caller's).
-static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_loc, size_t nv, unsigned max_bits) {
+static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_loc, size_t nv, unsigned max_bits,
+                                      uint32_t* raw = nullptr) {
   size_t L = (size_t)1 << (nv / 2), R = (size_t)1 << (nv - nv / 2);
   if (R + 2 > g.n_points) throw std::runtime_error("generator stream too short for this polynomial");
   const int G = c->world;
@@ -484,12 +498,17 @@ static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_
   if (!(g.d_multiples.p && R + 2 <= g.n_direct)) {
     DBuf<fr_t> canon(c, L * R_loc);
     launch_canonicalize(d_vals_loc, canon.p, L * R_loc, c->d_flag, c->st);
-    return msm_rows(c, g, canon.p, 8, R_loc, (int)L, (int)R_loc, kMsmFullWindows, false);
+    return msm_rows(c, g, canon.p, 8, R_loc, (int)L, (int)R_loc, kMsmFullWindows, false, raw);
   }
   // rows as direct sums over the 8-bit digit-multiples tables: one table entry per non-zero signed digit
   const int nw = msm_windows_for_bits(max_bits);
-  std::vector<uint8_t> out(L * 32);
   DBuf<pt_ext> part(c, L);
+  if (raw) {
+    launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, nullptr,
+                              raw, c->st);
+    return {};
+  }
+  std::vector<uint8_t> out(L * 32);
   DBuf<uint32_t> comp(c, L * 8);
   if (G == 1) {
     launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, comp.p,
@@ -514,8 +533,9 @@ struct PolySrc {
   PolySrc(const uint32_t* u) : u32(u), fr(nullptr) {}
   PolySrc(const uint32_t* u, const fr_t* f) : u32(u), fr(f) {}
 };
-static std::vector<uint8_t> commit_src(Ctx* c, const Gens& g, PolySrc Z, size_t nv, unsigned max_bits) {
-  return Z.u32 ? commit_u32(c, g, Z.u32, nv, max_bits) : commit_fr(c, g, Z.fr, nv, max_bits);
+static std::vector<uint8_t> commit_src(Ctx* c, const Gens& g, PolySrc Z, size_t nv, unsigned max_bits,
+                                       uint32_t* raw = nullptr) {
+  return Z.u32 ? commit_u32(c, g, Z.u32, nv, max_bits, raw) : commit_fr(c, g, Z.fr, nv, max_bits, raw);
 }
 static void multi_dot_src(PolySrc Z, size_t stride, int npolys, const fr_t* eq, size_t n, fr_t* partial, fr_t* out,
                           cudaStream_t st) {
@@ -1272,6 +1292,11 @@ __global__ void set_elems_kernel(fr_t* dst, fr_t a, fr_t b) {
   dst[0] = a;
   dst[1] = b;
 }
+// *dst <- *src, made canonical for the rows of launch_msm_direct (canonical != 0)
+__global__ void set_from_device_kernel(fr_t* dst, const fr_t* src, int canonical) {
+  if (threadIdx.x || blockIdx.x) return;
+  *dst = canonical ? fr_to_canonical(*src) : *src;
+}
 
 // PolyEvalProof::prove (dense_mlpoly.rs:301-359) -> DotProductProofLog::prove (dot_product.rs:166-249)
 // -> BulletReductionProof::prove (bullet.rs:40-154).  Z: this rank's shard of a polynomial of 2^nv elements, i.e. for
@@ -1280,9 +1305,12 @@ __global__ void set_elems_kernel(fr_t* dst, fr_t a, fr_t b) {
 // there on the opening runs REPLICATED on every rank — its vectors are only R = 2^(nv - nv/2) long and every round
 // is latency-bound, so splitting its two-row MSMs would add an exchange per round and save nothing.  Every rank
 // computes the same points and the same transcript.
+// Hiding openings (single GPU): blinds = the commitment's L_size row blinds (empty: None, all zero), blind_Zr the blind
+// of Cy = Zr * Q + blind_Zr * h (dense_mlpoly.rs:325-344).  Absent / zero blinds give the unblinded proof's launches.
 static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z, size_t nv,
                                                const std::vector<fr_t>& r, const fr_t& Zr, Transcript& transcript,
-                                               RandomTape& tape) {
+                                               RandomTape& tape, const std::vector<fr_t>& blinds = {},
+                                               const fr_t& blind_Zr = fr_zero()) {
   SpanTimer sp(c, "DensePolyEval.prove");
   transcript.append_protocol_name("polynomial evaluation proof");
   if (r.size() != nv) throw std::runtime_error("PolyEvalProof: r.len() != num_vars");
@@ -1303,6 +1331,14 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
   else
     launch_bound_fr(Z.fr, Lvec.p, L_size, n_loc, c->d_partial, G > 1 ? a_loc.p : a.p, c->st);
   if (G > 1) comm_gather_vector(c, a_loc.p, n_loc, a_gath.p, a.p);
+  // blind_x = LZ_blind = <L, blinds> (dense_mlpoly.rs:325-344) stays on the device until the read-back of x_hat, a_hat
+  const bool blinded = !blinds.empty();
+  DBuf<fr_t> d_blinds(c, blinded ? L_size : 0), blind_x(c, blinded ? 1 : 0);
+  if (blinded) {
+    if (blinds.size() != L_size) throw std::runtime_error("PolyEvalProof: one blind per row");
+    LB_CUDA_CHECK(cudaMemcpyAsync(d_blinds.p, blinds.data(), L_size * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+    launch_multi_dot_fr(d_blinds.p, L_size, 1, Lvec.p, L_size, c->d_partial, blind_x.p, c->st);
+  }
 
   // ---- DotProductProofLog::prove
   sp1.reset(new SpanTimer(c, "PE.2 Cx,Cy,append a"));
@@ -1316,7 +1352,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
   // table pipeline below: needs the multiples table of the generators 0 .. n+1
   const bool fast = n * 32 <= c->h_pin_bytes && g.d_multiples.p && n + 2 <= g.n_direct;
   // ---- BulletReductionProof::prove with unfolded generators (see file header)
-  fr_t blind_fin = fr_zero();  // blind_Gamma = blind_x + blind_y = 0
+  fr_t blind_fin = blind_Zr;  // blind_Gamma = blind_x + blind_y; blind_x joins at the read-back of x_hat
   DBuf<fr_t> W0(c, n), W1(c, n), sLR(c, 2 * (n + 2));
   fr_t* W = W0.p;   // weights of the unfolded generators (indexed by the HIGH column bits)
   fr_t* Wn = W1.p;
@@ -1343,7 +1379,8 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     fr_t *an = a_alt.p, *bn = b_alt.p;
     DBuf<pt_ext> part(c, 2 * (size_t)msm_direct_chunks((int)(n + 2), 1));
     DBuf<fr_t> canon(c, n);
-    launch_two_row_scalars(av, 0, fr_one(), fr_zero(), fr_zero(), Zr, fr_zero(), n, sLR.p, c->st);
+    launch_two_row_scalars(av, 0, fr_one(), fr_zero(), fr_zero(), Zr, blind_Zr, n, sLR.p, c->st);
+    if (blinded) launch(set_from_device_kernel, 1, 32, 0, c->st, sLR.p + n + 1, (const fr_t*)blind_x.p, 1);  // Cx on h
     const PubDst pd_c = c->pub_begin(false);
     launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd_c, c->st);
     // a_vec of the transcript = canonical bytes of b; the copy is waited for only when it is appended
@@ -1398,12 +1435,20 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     // kernel per step
     DBuf<fr_t> two(c, 4);
     {
-      // Cx = batch_commit(x_vec, blind_x = 0) ; Cy = y*Q + 0*h
-      std::vector<uint8_t> Cx = msm_rows_fr(c, g, a.p, 1, (int)n);
+      // Cx = batch_commit(x_vec, blind_x) ; Cy = y*Q + blind_Zr*h
+      std::vector<uint8_t> Cx;
+      if (blinded) {  // (x_vec, 0, blind_x) on (G_0 .. G_{n-1}, Q, h)
+        LB_CUDA_CHECK(cudaMemcpyAsync(sL, a.p, n * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+        launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, fr_zero(), fr_zero());
+        launch(set_from_device_kernel, 1, 32, 0, c->st, sL + n + 1, (const fr_t*)blind_x.p, 0);
+        Cx = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
+      } else {
+        Cx = msm_rows_fr(c, g, a.p, 1, (int)n);
+      }
       transcript.append_point_compressed("Cx", Cx.data());
-      // (0 .. 0, y, 0) on (G_0 .. G_{n-1}, Q, h)
+      // (0 .. 0, y, blind_Zr) on (G_0 .. G_{n-1}, Q, h)
       launch_fill_zero(sL, n, c->st);
-      launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, Zr, fr_zero());
+      launch(set_elems_kernel, 1, 32, 0, c->st, sL + n, Zr, blind_Zr);
       std::vector<uint8_t> Cy = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
       transcript.append_point_compressed("Cy", Cy.data());
       memcpy(out.Cy, Cy.data(), 32);
@@ -1447,6 +1492,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     launch_msm_direct(g.d_multiples.p, g.n_direct, (const uint32_t*)sLR.p, (int)(n + 2), part.p, pd, c->st);
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, av, 32, cudaMemcpyDeviceToHost, c->st));
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 32, bv, 32, cudaMemcpyDeviceToHost, c->st));
+    if (blinded) LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 64, blind_x.p, 32, cudaMemcpyDeviceToHost, c->st));
     uint32_t xyz[48];
     c->wait_points(pd, 2, xyz);
     h64::compress_xyz_pair(xyz, xyz + 24, out.delta, out.beta);
@@ -1457,6 +1503,7 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
   } else {
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin, av, 32, cudaMemcpyDeviceToHost, c->st));
     LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 32, bv, 32, cudaMemcpyDeviceToHost, c->st));
+    if (blinded) LB_CUDA_CHECK(cudaMemcpyAsync(c->h_pin + 64, blind_x.p, 32, cudaMemcpyDeviceToHost, c->st));
     c->sync();
     memcpy(ab, c->h_pin, 64);
     // delta = d * g_hat + r_delta * h with g_hat = sum_j W[j] G_j  (dot_product.rs:219-227)
@@ -1471,6 +1518,11 @@ static DotProductProofLogBytes prove_poly_eval(Ctx* c, const Gens& g, PolySrc Z,
     std::vector<uint8_t> beta = msm_rows_fr(c, g, sL, 1, (int)(n + 2));
     memcpy(out.beta, beta.data(), 32);
     transcript.append_point_compressed("beta", out.beta);
+  }
+  if (blinded) {
+    fr_t bx;
+    memcpy(&bx, c->h_pin + 64, 32);
+    blind_fin = fr_add(blind_fin, bx);
   }
   fr_t x_hat = ab[0], a_hat = ab[1], rhat_Gamma = blind_fin;
   fr_t y_hat = fr_mul(x_hat, a_hat);
@@ -1831,10 +1883,39 @@ fr_t poly_evaluate(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
   c->d2h(&out, c->d_small, sizeof out);
   return out;
 }
-// PolyEvalProof::prove (dense_mlpoly.rs:301-359, no blinds) on the caller's transcript and tape
+// DensePolynomial::commit with Some(random_tape) (dense_mlpoly.rs:152-181): C_i = <row_i, G> + blinds[i] h.  The rows
+// come un-normalised from the launchers poly_commit uses; launch_row_blinds adds the blind terms and normalises.
+std::vector<uint8_t> poly_commit_hiding(Ctx* c, const Poly& p, const Gens& g, const std::vector<fr_t>& blinds) {
+  SpanTimer sp(c, "DensePolynomial.commit_hiding");
+  const size_t L = (size_t)1 << (p.nv / 2), R = poly_R(p.nv);
+  if (blinds.size() != L) throw std::runtime_error("hiding commitment: one blind per row");
+  DBuf<uint32_t> raw(c, L * 32), comp(c, L * 8);
+  DBuf<fr_t> d_blinds(c, L);
+  LB_CUDA_CHECK(cudaMemcpyAsync(d_blinds.p, blinds.data(), L * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+  commit_src(c, g, poly_src(p), p.nv, std::max(p.bits, 1u), raw.p);
+  // the multiples of h = stream[R + 1]: its column of the 8-bit multiples table, else its 32 x 128 built for this call
+  // from the window table (the same points, so the same bytes)
+  DBuf<pt_niels> mh;
+  const pt_niels* Mh = g.d_multiples.p + (R + 1) * 128;
+  size_t wstride = g.n_direct * 128;
+  if (!(g.d_multiples.p && R + 2 <= g.n_direct)) {
+    mh.alloc(c, (size_t)kMsmFullWindows * 128);
+    launch_build_multiples(g.d_table.p + R + 1, g.n_points, 1, kMsmFullWindows, mh.p, c->st);
+    Mh = mh.p;
+    wstride = 128;
+  }
+  launch_row_blinds(Mh, wstride, d_blinds.p, raw.p, (int)L, comp.p, c->st);
+  std::vector<uint8_t> pts(L * 32);
+  c->d2h(pts.data(), comp.p, pts.size());
+  ByteWriter w;
+  w.vec_pts(pts);
+  return w.b;
+}
+// PolyEvalProof::prove (dense_mlpoly.rs:301-359) on the caller's transcript and tape; blinds empty: None
 std::vector<uint8_t> poly_eval_prove(Ctx* c, const Poly& p, const Gens& g, const std::vector<fr_t>& r, const fr_t& Zr,
-                                     Transcript& transcript, RandomTape& tape, uint8_t C_Zr[32]) {
-  const DotProductProofLogBytes proof = prove_poly_eval(c, g, poly_src(p), p.nv, r, Zr, transcript, tape);
+                                     Transcript& transcript, RandomTape& tape, uint8_t C_Zr[32],
+                                     const std::vector<fr_t>& blinds, const fr_t& blind_Zr) {
+  const DotProductProofLogBytes proof = prove_poly_eval(c, g, poly_src(p), p.nv, r, Zr, transcript, tape, blinds, blind_Zr);
   c->sync();
   memcpy(C_Zr, proof.Cy, 32);
   ByteWriter w;

@@ -354,10 +354,14 @@ Gens* poly_gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, siz
 // (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory
 Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err);
 std::vector<uint8_t> poly_commit(Ctx*, const Poly&, const Gens&);  // serialised PolyCommitment
+// the hiding PolyCommitment of the same size: row i is committed with blinds[i] on h (blinds.size() == L)
+std::vector<uint8_t> poly_commit_hiding(Ctx*, const Poly&, const Gens&, const std::vector<fr_t>& blinds);
 fr_t poly_evaluate(Ctx*, const Poly&, const std::vector<fr_t>& r);
-// serialised PolyEvalProof; C_Zr receives the compressed commitment to Zr the reference returns alongside it
+// serialised PolyEvalProof; C_Zr receives the compressed commitment to Zr the reference returns alongside it,
+// Zr * Q + blind_Zr * h.  blinds: the commitment's L row blinds, or empty for None (zero blinds)
 std::vector<uint8_t> poly_eval_prove(Ctx*, const Poly&, const Gens&, const std::vector<fr_t>& r, const fr_t& Zr,
-                                     Transcript&, RandomTape&, uint8_t C_Zr[32]);
+                                     Transcript&, RandomTape&, uint8_t C_Zr[32], const std::vector<fr_t>& blinds = {},
+                                     const fr_t& blind_Zr = fr_zero());
 // EqPolynomial::new(r).evals() (eq_poly.rs:21-38) as a full-width polynomial (no u32 mirror); r.size() <= 28
 Poly* poly_create_eq(Ctx*, const std::vector<fr_t>& r);
 // DensePolynomial::merge (dense_mlpoly.rs:251-261) of k >= 1 polynomials (the caller checks the merged length): a new

@@ -5,7 +5,8 @@
 // DensePolynomial::commit / evaluate, PolyEvalProof::prove / verify_plain, ProofTranscript, RandomTape) but drives them
 // only inside its own round trips; this file puts C entry points on the same code that take and return what the
 // library takes and returns: serialised bytes, an explicit generator stream, and transcript / tape objects that live
-// across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof.
+// across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof and the hiding forms
+// of DensePolynomial::commit / PolyEvalProof::prove (blinds on h), which oracle/ leaves out.
 #include "sparse_bytes.hpp"
 
 using namespace oracle;
@@ -58,6 +59,47 @@ std::vector<uint8_t> ser_proof(const PolyEvalProof& p) {
   put_fr(b, d.z2);
   return b;
 }
+// PolyEvalProof { proof } of serialised bytes; false when they do not parse
+bool read_poly_eval_proof(const uint8_t* proof, size_t proof_len, PolyEvalProof& p) {
+  Reader rp{proof, proof_len};
+  p.proof.bullet_reduction_proof.L_vec = rp.points();
+  p.proof.bullet_reduction_proof.R_vec = rp.points();
+  p.proof.delta = rp.point();
+  p.proof.beta = rp.point();
+  p.proof.z1 = rp.fr();
+  p.proof.z2 = rp.fr();
+  return rp.ok && rp.at == proof_len;
+}
+// The hiding forms of DensePolynomial::commit and PolyEvalProof::prove, restated beside the unblinded ones of oracle/:
+// commit (dense_mlpoly.rs:152-181): row i is batch_commit(row_i, blinds[i]) = <row_i, G> + blinds[i] h
+PolyCommitment commit_hiding(const DensePolynomial& poly, const PolyCommitmentGens& gens, const std::vector<Fr>& blinds) {
+  size_t lv, rv;
+  EqPolynomial::compute_factored_lens(poly.num_vars, lv, rv);
+  const size_t L_size = pow2(lv), R_size = pow2(rv);
+  if (blinds.size() != L_size) throw std::runtime_error("commit_hiding: one blind per row");
+  PolyCommitment pc;
+  pc.C.resize(L_size);
+#pragma omp parallel for schedule(dynamic, 1)
+  for (size_t i = 0; i < L_size; i++) pc.C[i] = batch_commit(&poly.Z[R_size * i], R_size, blinds[i], gens.gens.gens_n);
+  return pc;
+}
+// prove (dense_mlpoly.rs:301-359) with Some(blinds) (empty: None, all zero) and blind_Zr: LZ_blind = <L, blinds> is
+// the dot-product proof's blind_x, blind_Zr its blind_y; C_Zr = Zr Q + blind_Zr h is returned alongside
+PolyEvalProof prove_hiding(const DensePolynomial& poly, const std::vector<Fr>& blinds, const std::vector<Fr>& r,
+                           const Fr& Zr, const Fr& blind_Zr, const PolyCommitmentGens& gens, Transcript& transcript,
+                           RandomTape& tape, Point& C_Zr) {
+  transcript.append_protocol_name("polynomial evaluation proof");
+  std::vector<Fr> L, R;
+  EqPolynomial(r).compute_factored_evals(L, R);
+  if (!blinds.empty() && blinds.size() != L.size()) throw std::runtime_error("prove_hiding: one blind per row");
+  Fr LZ_blind = Fr::zero();
+  for (size_t i = 0; i < blinds.size(); i++) LZ_blind += L[i] * blinds[i];
+  Point Cx;
+  PolyEvalProof out;
+  out.proof = DotProductProofLog::prove(gens.gens, transcript, tape, poly.bound(L), LZ_blind, R, Zr, blind_Zr, Cx, C_Zr);
+  return out;
+}
+
 // A combining function as lasso_comb_create takes it: 3 ints {op, a, b} per instruction, slots 0..n-1 the inputs,
 // instruction j writes slot n + j, the last slot is g; op: 0 a + b, 1 a - b, 2 a * b, 3 a * K[b], 4 a + K[b].
 // Interpreted directly, SSA slot by SSA slot (no slot allocation).  Taken as given: the GPU library checks it.
@@ -208,16 +250,72 @@ int orcd_poly_verify(const uint64_t* stream, size_t n_points, size_t nv, const u
   PolyCommitment c;
   c.C = rc.points();
   if (!rc.ok || rc.at != comm_len || c.C.size() != pow2(l)) return 2;
-  Reader rp{proof, proof_len};
   PolyEvalProof p;
-  p.proof.bullet_reduction_proof.L_vec = rp.points();
-  p.proof.bullet_reduction_proof.R_vec = rp.points();
-  p.proof.delta = rp.point();
-  p.proof.beta = rp.point();
-  p.proof.z1 = rp.fr();
-  p.proof.z2 = rp.fr();
-  if (!rp.ok || rp.at != proof_len) return 2;
+  if (!read_poly_eval_proof(proof, proof_len, p)) return 2;
   return p.verify_plain(gens, *(Transcript*)transcript, ldvec(r, nv), ldfr(Zr), c) ? 0 : 1;
+}
+// The hiding commitment: with a tape (non-null) its L = 2^(nv/2) blinds are drawn as random_vector("poly_blinds", L)
+// and written to blinds (L x 4 limbs); without one, blinds holds them.  Returns the commitment's length, 0 on error.
+size_t orcd_poly_commit_hiding(const uint64_t* Z, size_t n, const uint64_t* stream, size_t n_points, void* tape,
+                               uint64_t* blinds, uint8_t* out, size_t cap) {
+  try {
+    DensePolynomial poly(ldvec(Z, n));
+    size_t l, r;
+    EqPolynomial::compute_factored_lens(poly.num_vars, l, r);
+    if (n_points < pow2(r) + 2) return 0;
+    PolyCommitmentGens gens = PolyCommitmentGens::make(poly.num_vars, ldstream(stream, n_points));
+    std::vector<Fr> bl = tape ? ((RandomTape*)tape)->random_vector("poly_blinds", pow2(l)) : ldvec(blinds, pow2(l));
+    for (size_t i = 0; i < bl.size(); i++) stfr(blinds + 4 * i, bl[i]);
+    std::vector<uint8_t> b = ser_commitment(commit_hiding(poly, gens, bl));
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_poly_commit_hiding: %s\n", e.what());
+    return 0;
+  }
+}
+// PolyEvalProof::prove with blinds (n_blinds == 0: None) and blind_Zr (null: None) on a caller's transcript and tape:
+// returns the proof's length (0 on error); C_Zr_out = the compressed Zr * Q + blind_Zr * h
+size_t orcd_poly_prove_hiding(const uint64_t* Z, size_t n, const uint64_t* blinds, size_t n_blinds, const uint64_t* r,
+                              const uint64_t* Zr, const uint64_t* blind_Zr, const uint64_t* stream, size_t n_points,
+                              void* transcript, void* tape, uint8_t* out, size_t cap, uint8_t* C_Zr_out) {
+  try {
+    DensePolynomial poly(ldvec(Z, n));
+    size_t l, rr;
+    EqPolynomial::compute_factored_lens(poly.num_vars, l, rr);
+    if (n_points < pow2(rr) + 2) return 0;
+    PolyCommitmentGens gens = PolyCommitmentGens::make(poly.num_vars, ldstream(stream, n_points));
+    Point C_Zr;
+    PolyEvalProof proof = prove_hiding(poly, ldvec(blinds, n_blinds), ldvec(r, poly.num_vars), ldfr(Zr),
+                                       blind_Zr ? ldfr(blind_Zr) : Fr::zero(), gens, *(Transcript*)transcript,
+                                       *(RandomTape*)tape, C_Zr);
+    C_Zr.compress(C_Zr_out);
+    std::vector<uint8_t> b = ser_proof(proof);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_poly_prove_hiding: %s\n", e.what());
+    return 0;
+  }
+}
+// PolyEvalProof::verify (dense_mlpoly.rs:361-386) of serialised bytes against a compressed C_Zr: 0 accepted,
+// 1 rejected, 2 the commitment, the proof or C_Zr does not parse
+int orcd_poly_verify_czr(const uint64_t* stream, size_t n_points, size_t nv, const uint8_t* comm, size_t comm_len,
+                         const uint8_t* proof, size_t proof_len, const uint64_t* r, const uint8_t* C_Zr, void* transcript) {
+  size_t l, rr;
+  EqPolynomial::compute_factored_lens(nv, l, rr);
+  if (n_points < pow2(rr) + 2) return 2;
+  PolyCommitmentGens gens = PolyCommitmentGens::make(nv, ldstream(stream, n_points));
+  Reader rc{comm, comm_len};
+  PolyCommitment c;
+  c.C = rc.points();
+  if (!rc.ok || rc.at != comm_len || c.C.size() != pow2(l)) return 2;
+  PolyEvalProof p;
+  Point czr;
+  if (!read_poly_eval_proof(proof, proof_len, p) || !ldpoint(C_Zr, czr)) return 2;
+  return p.verify(gens, *(Transcript*)transcript, ldvec(r, nv), czr, c) ? 0 : 1;
 }
 
 // ---- SumcheckInstanceProof (subprotocols/sumcheck.rs)

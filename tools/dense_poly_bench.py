@@ -5,7 +5,10 @@ Each call is timed with the host clock around the library call; every call ends 
 of the ingest, the commitment's points, Z(r), the proof's last message).  W warm-ups, then the median and range of N
 runs.  Every commitment and proof is checked against tests/golden/dense_poly.json.  Also prints the card's name and
 power limit, and (--cpu) the CPU oracle's commit and prove at 2^20 with 8 threads for comparison.
-usage: python tools/dense_poly_bench.py [--warmup W] [--reps N] [--cases a,b] [--cpu] [--out FILE.json]"""
+--hiding adds a leg per case: the plain commit + prove and the hiding ones (DensePolynomial.commit_hiding, the proof
+with blinds and blind_Zr) alternating on one polynomial, hiding results checked against
+tests/golden/dense_poly_hiding.json where it has the case, with the launches of each call.
+usage: python tools/dense_poly_bench.py [--warmup W] [--reps N] [--cases a,b] [--cpu] [--hiding] [--out FILE.json]"""
 import argparse
 import hashlib
 import json
@@ -90,6 +93,45 @@ def run_case(ctx, name, warmup, reps, gold):
     return out
 
 
+def run_hiding(ctx, name, warmup, reps, gold):
+    """plain and hiding commit + prove alternating on one polynomial (host input)"""
+    nv, Z, r, seed = dc.inputs(name)
+    stream = np.ascontiguousarray(ol.generators(dc.n_generators(nv)))
+    gens = lb.PolyCommitmentGens.new(ctx, b"gens_sparse_poly", nv, stream=stream)
+    p = lb.DensePolynomial(ctx, Z)
+    Zr = p.evaluate(r)
+    times = {k: {"commit": [], "prove": []} for k in ("plain", "hiding")}
+    launches = {k: {} for k in times}
+    match = True
+    for i in range(warmup + reps):
+        for k in ("plain", "hiding"):
+            tape = lb.RandomTape(dc.TAPE_LABEL, seed)
+            l0, t0 = ctx.launches, time.perf_counter()
+            if k == "plain":
+                comm = p.commit(gens)
+            else:
+                comm, blinds = p.commit_hiding(gens, tape)
+            tc, l1 = ms_since(t0), ctx.launches
+            tr = lb.Transcript(dc.TRANSCRIPT_LABEL)
+            tr.append_poly_commitment(dc.COMMIT_LABEL, comm)
+            kw = {} if k == "plain" else {"blinds": blinds, "blind_Zr": tape.random_scalar(b"blind_Zr")}
+            t0 = time.perf_counter()
+            proof = lb.PolyEvalProof.prove(ctx, p, r, Zr, gens, tr, tape, **kw)
+            tp = ms_since(t0)
+            launches[k] = {"commit": l1 - l0, "prove": ctx.launches - l1}
+            if k == "hiding" and gold:
+                match &= (hashlib.sha256(comm).hexdigest() == gold["commitment_sha256"]
+                          and hashlib.sha256(proof.bytes).hexdigest() == gold["proof_sha256"])
+            if i >= warmup:
+                times[k]["commit"].append(tc)
+                times[k]["prove"].append(tp)
+    out = {"num_vars": nv, "values": dc.CASES[name][1], "hiding_golden_match": bool(match) if gold else None}
+    for k in times:
+        out[k] = {s: stats(v) for s, v in times[k].items()}
+        out[k]["launches"] = launches[k]
+    return out
+
+
 def cpu_oracle(reps):
     """the CPU oracle (the restatement of the reference, OpenMP) at 2^20 with 8 threads: commit and prove"""
     ol.lib().orc_set_num_threads(8)
@@ -117,6 +159,7 @@ def main():
     ap.add_argument("--cases", default=",".join(CASES))
     ap.add_argument("--cpu", action="store_true")
     ap.add_argument("--cpu-reps", type=int, default=3)
+    ap.add_argument("--hiding", action="store_true")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     gold = json.load(open(os.path.join(ROOT, "tests", "golden", "dense_poly.json")))["cases"]
@@ -126,6 +169,12 @@ def main():
     for name in a.cases.split(","):
         doc["cases"][name] = run_case(ctx, name, a.warmup, a.reps, gold[name])
         print(name, json.dumps(doc["cases"][name]), flush=True)
+    if a.hiding:
+        gold_h = json.load(open(os.path.join(ROOT, "tests", "golden", "dense_poly_hiding.json")))["cases"]
+        doc["hiding"] = {}
+        for name in a.cases.split(","):
+            doc["hiding"][name] = run_hiding(ctx, name, a.warmup, a.reps, gold_h.get(name))
+            print("hiding", name, json.dumps(doc["hiding"][name]), flush=True)
     if a.cpu:
         doc["cpu_oracle"] = cpu_oracle(a.cpu_reps)
         print("cpu_oracle", json.dumps(doc["cpu_oracle"]), flush=True)
