@@ -275,7 +275,20 @@ int lasso_random_tape_random_vector(lasso_random_tape*, const char* label, size_
  * G_0..G_{R-1} = stream[0..R), Q = stream[R], h = stream[R+1] (poly/commitments.rs:21-44, dot_product.rs:146-149).
  * Its own type: it cannot be passed to lasso_commit or lasso_prove.  Builds the same device tables a lasso_gens of the
  * same R builds (window table, digit-multiples tables; LASSO_B200_NO_MULTIPLES and LASSO_B200_TABLE_GB apply): about
- * 14 GB of HBM at R = 2^12.  LASSO_ERR_GENS when n_points < R + 2, LASSO_ERR_LENGTH when num_vars > 28. */
+ * 14 GB of HBM at R = 2^12.  LASSO_ERR_GENS when n_points < R + 2, LASSO_ERR_LENGTH when num_vars > 28.
+ *
+ * Sharded contexts (lasso_ctx_init_comm over G ranks): the lasso_poly_* calls below, lasso_poly_gens_create and
+ * lasso_combined_eval_prove are COLLECTIVE, like lasso_commit and lasso_prove: every rank calls them in the same order
+ * with the same arguments (the same kind of pointer too: host or device), device inputs on its own GPU, transcripts and
+ * tapes in the same state.  Every rank returns the same bytes, values and error code, and its handles end in the same
+ * state; the outputs are those of a single-GPU context, byte for byte.  A polynomial is held as its low-bit shard (rank
+ * g holds evaluations i * G + g: the R/G columns congruent to g of every row), so on G ranks a polynomial, or the
+ * generators, of num_vars variables needs R = 2^(num_vars - num_vars/2) >= G, i.e. num_vars >= 2 log2(G) - 1:
+ * otherwise LASSO_ERR_LENGTH before any launch (lasso_poly_gens_create, lasso_poly_create[_device], lasso_poly_create_eq,
+ * lasso_poly_create_comb).  Commitments make one all-gather of the row partials; evaluations add the ranks' partial
+ * values in one message to every process; openings gather L.Z and run the Bulletproofs rounds replicated.
+ * lasso_sumcheck_prove, lasso_gp_circuit_create, lasso_gp_prove and lasso_dense_outputs[_custom] are not available on a
+ * sharded context (LASSO_ERR_STRATEGY). */
 typedef struct lasso_poly_gens lasso_poly_gens;
 typedef struct lasso_poly lasso_poly;
 size_t lasso_poly_gens_points_needed(size_t num_vars); /* R + 2 */
@@ -293,7 +306,10 @@ void lasso_poly_gens_destroy(lasso_poly_gens*);
  * first and the last row must be device memory of the context's device, otherwise LASSO_ERR_POINTER before any launch;
  * the rows are read after the work enqueued on `stream` (NULL = the legacy default stream) before the call, and later
  * work on `stream` is ordered after those reads.  The library keeps its own copy: the caller may free Z on return.
- * Not available on a sharded context (LASSO_ERR_STRATEGY). */
+ * On a sharded context every rank passes the WHOLE polynomial, as lasso_densify takes the whole index matrix, and reads
+ * only its rows i * G + g (host rows are staged and uploaded by each rank, 1/G of the PCIe bytes); the ranks agree on the
+ * verdict and on the widest value in one exchange, so a non-canonical evaluation in any rank's rows gives
+ * LASSO_ERR_VALUE on every rank, and the context stays usable for the next collective call. */
 int lasso_poly_create(lasso_ctx*, const uint64_t* Z, size_t len, lasso_poly** out);
 int lasso_poly_create_device(lasso_ctx*, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
                              lasso_poly** out);
@@ -313,7 +329,8 @@ int lasso_poly_evaluate(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t
 int lasso_poly_eval_prove(lasso_ctx*, const lasso_poly*, const lasso_poly_gens*, const uint64_t* r, size_t r_len,
                           const uint64_t Zr[4], lasso_transcript* transcript, lasso_random_tape* random_tape,
                           uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint8_t C_Zr_out[32]);
-/* Hiding commitments and openings (single-GPU contexts, like every lasso_poly_* call).
+/* Hiding commitments and openings (collective on a sharded context, like every lasso_poly_* call: every rank draws the
+ * same blinds from its tape and returns the same bytes).
  * lasso_poly_commit_hiding is DensePolynomial::commit(gens, Some(random_tape)) (poly/dense_mlpoly.rs:152-181): it draws
  * L = 2^(num_vars/2) blinds from the tape as random_vector("poly_blinds", L), writes the hiding PolyCommitment (row i is
  * <row_i, G> + blinds[i] * h; same format and size as lasso_poly_commit) to out and the L blinds (L x 4 Montgomery limbs)
@@ -380,7 +397,8 @@ int lasso_dense_outputs_custom(lasso_ctx*, const lasso_strategy*, const lasso_de
  * modified, and the result owns its own copy, so they may be destroyed afterwards.  It has a u32 mirror (is committed and
  * opened through the 16-bit tables) iff every input has one, i.e. iff every value is an integer below 2^32.  Copies only:
  * no kernel is launched.  Errors, before any copy: LASSO_ERR_LENGTH for n_polys == 0, a null array or output, or more
- * than 2^28 evaluations after padding; LASSO_ERR_STRATEGY for a polynomial of another context or a sharded context. */
+ * than 2^28 evaluations after padding; LASSO_ERR_STRATEGY for a polynomial of another context.  Sharded: every input's
+ * length is a multiple of G, so each rank concatenates its shards of the inputs, with no exchange. */
 int lasso_poly_create_merge(lasso_ctx*, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out);
 /* DensePolynomial::evaluate (poly/dense_mlpoly.rs:229-235) of n_polys polynomials of one num_vars at one point r: out
  * receives n_polys x 4 limbs, P_j(r) at out + 4 j.  One eq table serves every polynomial, and the dot kernel reads each of
@@ -388,7 +406,7 @@ int lasso_poly_create_merge(lasso_ctx*, const lasso_poly* const* polys, size_t n
  * and the per-input block partials of one launch fill at most 8 x 528 elements of the context's scratch.  Integer and
  * full-width polynomials may be mixed.  Errors, before any launch: LASSO_ERR_LENGTH for different num_vars,
  * r_len != num_vars, n_polys outside 1..64, or a null array or output; LASSO_ERR_VALUE for a non-canonical coordinate;
- * LASSO_ERR_STRATEGY for a polynomial of another context or a sharded context. */
+ * LASSO_ERR_STRATEGY for a polynomial of another context.  Collective on a sharded context. */
 int lasso_poly_evaluate_batch(lasso_ctx*, const lasso_poly* const* polys, size_t n_polys, const uint64_t* r, size_t r_len,
                               uint64_t* out);
 /* CombinedTableEvalProof::prove (subtables/mod.rs:229-313) without blinds: opens the merged polynomial `combined` at r for
@@ -405,8 +423,8 @@ int lasso_poly_evaluate_batch(lasso_ctx*, const lasso_poly* const* polys, size_t
  * Errors, each returned before any launch and before the transcript or the tape is touched: LASSO_ERR_LENGTH for
  * num_vars != r_len + log2(next_pow2(n_evals)), n_evals == 0, a too small proof_cap, or a null transcript, tape, evals or
  * output; LASSO_ERR_GENS for generators whose R differs from the polynomial's; LASSO_ERR_VALUE for a non-canonical eval or
- * coordinate; LASSO_ERR_STRATEGY for another context or a sharded context.  The opening's working memory is reserved in
- * the context's memory pool before the first transcript write. */
+ * coordinate; LASSO_ERR_STRATEGY for another context.  The opening's working memory is reserved in the context's memory
+ * pool before the first transcript write.  Collective on a sharded context. */
 int lasso_combined_eval_prove(lasso_ctx*, const lasso_poly* combined, const lasso_poly_gens*, const uint64_t* evals,
                               size_t n_evals, const uint64_t* r, size_t r_len, lasso_transcript*, lasso_random_tape*,
                               uint8_t* proof_out, size_t proof_cap, size_t* proof_len);
@@ -443,8 +461,9 @@ int lasso_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* const*
  * h(a, v, t) = t gamma^2 + v gamma + a - tau of offline memory checking (lasso/memory_checking.rs:251-252).  g's
  * declared degree is not used.  The result is a full-width polynomial like lasso_poly_create_eq (committed through the
  * Fr windows): it can be committed, evaluated, opened, summed over or made a grand-product circuit.  Errors, before any
- * launch: LASSO_ERR_STRATEGY for n_polys != n_inputs, a polynomial of another context or a sharded context;
- * LASSO_ERR_LENGTH for polynomials of different num_vars or a null output. */
+ * launch: LASSO_ERR_STRATEGY for n_polys != n_inputs or a polynomial of another context; LASSO_ERR_LENGTH for
+ * polynomials of different num_vars or a null output.  Collective on a sharded context: element-wise, each rank maps its
+ * own shards, with no exchange. */
 int lasso_poly_create_comb(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
                            lasso_poly** out);
 

@@ -789,7 +789,8 @@ def poly_gens_points_needed(num_vars):
 
 
 class PolyCommitmentGens:
-    """src/poly/dense_mlpoly.rs:31-45: G_0..G_{R-1}, Q, h from one generator stream"""
+    """src/poly/dense_mlpoly.rs:31-45: G_0..G_{R-1}, Q, h from one generator stream (collective on a sharded context,
+    where R >= G)"""
 
     def __init__(self, ctx, handle, stream, num_vars):
         self.ctx, self._h, self.stream, self.num_vars = ctx, handle, stream, num_vars
@@ -843,7 +844,11 @@ def _poly_handles(polys):
 class DensePolynomial:
     """DensePolynomial<Fr> (src/poly/dense_mlpoly.rs:13-235), resident on ctx's GPU.  Z: the 2^num_vars evaluations as
     an (n, 4) uint64 numpy array of Montgomery limbs, or a torch CUDA tensor (int64 or uint64, limbs contiguous, any row
-    stride) read in the order of torch's current stream.  The library keeps its own copy."""
+    stride) read in the order of torch's current stream.  The library keeps its own copy.
+    On a sharded context (Context.init_comm) creating, committing, evaluating and opening are collective: every rank
+    passes the WHOLE polynomial (of the same kind, host or CUDA on its own GPU) and the same arguments, keeps only its
+    low-bit shard, and gets the single-GPU bytes and values.  There a polynomial needs 2^(num_vars - num_vars // 2) >= G
+    (LASSO_ERR_LENGTH otherwise); sumchecks, grand products and DensifiedRepresentation.outputs stay single-GPU."""
 
     def __init__(self, ctx, Z):
         kind, src, row_stride = _poly_source(Z)
@@ -949,7 +954,8 @@ class PolyEvalProof:
     @classmethod
     def prove(cls, ctx, poly, r, Zr, gens, transcript, random_tape, *, blinds=None, blind_Zr=None):
         """advances transcript and random_tape in place.  blinds: the (L, 4) row blinds commit_hiding returned (None:
-        the commitment was not hiding); blind_Zr: the blind of C_Zr = Zr Q + blind_Zr h (None: zero)"""
+        the commitment was not hiding); blind_Zr: the blind of C_Zr = Zr Q + blind_Zr h (None: zero).  Collective on a
+        sharded context: every rank's transcript and tape in the same state, every rank gets the same proof."""
         r = _limbs(r, what="r")
         Zr = _limbs(Zr, 1, "Zr")
         cap = 2 * (8 + 32 * 32) + 4 * 32
@@ -986,7 +992,7 @@ class CombinedTableEvalProof:
     def prove(cls, ctx, combined, evals, r, gens, transcript, random_tape):
         """CombinedTableEvalProof::prove over `combined` for the claims `evals` at r (combined.num_vars == len(r) +
         log2(next_pow2(len(evals)))), on the caller's transcript and tape, advanced in place.  The claims are not checked:
-        a wrong one gives a proof the verifier rejects."""
+        a wrong one gives a proof the verifier rejects.  Collective on a sharded context, like PolyEvalProof.prove."""
         evals = _limbs(evals, what="evals")
         r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
         cap = cls.proof_len(combined.num_vars)

@@ -1033,8 +1033,16 @@ int lasso_random_tape_random_vector(lasso_random_tape* t, const char* label, siz
 }
 
 // ---- dense polynomials of the caller
+// Commitments, evaluations and openings are collective on a sharded context; the sumchecks, grand products and lookup
+// outputs are not available there.
 static int poly_ctx_check(lasso_ctx* h) {
-  if (h->c->world > 1) return fail(LASSO_ERR_STRATEGY, "dense polynomials are not available on a sharded context");
+  if (h->c->world > 1) return fail(LASSO_ERR_STRATEGY, "not available on a sharded context");
+  return 0;
+}
+// a sharded context holds every row's columns on G ranks: R = poly_R(num_vars) >= G
+static int poly_size_check(lasso_ctx* h, size_t num_vars) {
+  if (!poly_fits(num_vars, h->c->world))
+    return fail(LASSO_ERR_LENGTH, "poly: on a sharded context of G ranks, 2^(num_vars - num_vars/2) >= G");
   return 0;
 }
 size_t lasso_poly_gens_points_needed(size_t num_vars) { return poly_R(num_vars) + 2; }
@@ -1042,9 +1050,9 @@ int lasso_poly_gens_create(lasso_ctx* h, const uint64_t* stream_affine, size_t n
                            lasso_poly_gens** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!out || !stream_affine) return fail(LASSO_ERR_GENS, "poly gens: null stream or output");
   if (num_vars > 28) return fail(LASSO_ERR_LENGTH, "poly gens: num_vars <= 28");
+  if (const int rc = poly_size_check(h, num_vars)) return rc;
   if (n_points < poly_R(num_vars) + 2) return fail(LASSO_ERR_GENS, "poly gens: stream shorter than lasso_poly_gens_points_needed()");
   Gens* g = poly_gens_create(h->c, stream_affine, n_points, num_vars);
   *out = new lasso_poly_gens{g, num_vars};
@@ -1060,10 +1068,10 @@ void lasso_poly_gens_destroy(lasso_poly_gens* g) {
 static int poly_new(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, bool device, void* stream,
                     lasso_poly** out) {
   if (out) *out = nullptr;
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!out) return fail(LASSO_ERR_LENGTH, "poly: null output");
   if (!is_pow2(len)) return fail(LASSO_ERR_NOT_POW2, "poly: the length must be a power of two (dense_mlpoly.rs:63-66)");
   if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly: at most 2^28 evaluations");
+  if (const int rc = poly_size_check(h, log2_exact_or_ceil(len))) return rc;
   if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly: row_stride must be at least 4 u64");
   if (!device && !Z) return fail(LASSO_ERR_POINTER, "poly: null evaluations");
   int err = 0;
@@ -1093,7 +1101,6 @@ void lasso_poly_destroy(lasso_poly* p) {
 }
 // the checks every use of a polynomial shares: same context, and the generators' R equals the polynomial's
 static int poly_use_check(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g) {
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!p || p->p->ctx != h->c) return fail(LASSO_ERR_STRATEGY, "poly: created on another context");
   if (g) {
     if (g->g->ctx != h->c) return fail(LASSO_ERR_GENS, "poly gens: created on another context");
@@ -1191,9 +1198,9 @@ int lasso_poly_eval_prove_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_
 int lasso_poly_create_eq(lasso_ctx* h, const uint64_t* r, size_t r_len, lasso_poly** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!out) return fail(LASSO_ERR_LENGTH, "eq poly: null output");
   if (r_len > 28) return fail(LASSO_ERR_LENGTH, "eq poly: at most 28 variables (2^28 evaluations)");
+  if (const int rc = poly_size_check(h, r_len)) return rc;
   if (r_len && !r) return fail(LASSO_ERR_LENGTH, "eq poly: null point");
   std::vector<fr_t> rv;
   if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "eq poly: a coordinate of r is not a canonical residue");
@@ -1206,7 +1213,6 @@ int lasso_poly_create_eq(lasso_ctx* h, const uint64_t* r, size_t r_len, lasso_po
 int lasso_poly_create_merge(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!polys || n_polys == 0 || !out) return fail(LASSO_ERR_LENGTH, "merge: no polynomials, or a null output");
   for (size_t j = 0; j < n_polys; j++)
     if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
@@ -1224,7 +1230,6 @@ int lasso_poly_create_merge(lasso_ctx* h, const lasso_poly* const* polys, size_t
 int lasso_poly_evaluate_batch(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, const uint64_t* r,
                               size_t r_len, uint64_t* out) {
   LB_TRY_CTX(h)
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!polys || n_polys == 0 || n_polys > (size_t)kDotMaxPolys || !out)
     return fail(LASSO_ERR_LENGTH, "evaluate batch: 1..64 polynomials and an output");
   for (size_t j = 0; j < n_polys; j++)
@@ -1326,7 +1331,6 @@ int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* 
                            lasso_poly** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
-  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!g) return fail(LASSO_ERR_STRATEGY, "comb poly: null combining function");
   if (!polys || n_polys != (size_t)g->g.n_inputs)
     return fail(LASSO_ERR_STRATEGY, "comb poly: " + std::to_string(n_polys) + " polynomials for a combining function of " +
@@ -1335,6 +1339,7 @@ int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* 
     if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
   for (size_t j = 1; j < n_polys; j++)
     if (polys[j]->p->nv != polys[0]->p->nv) return fail(LASSO_ERR_LENGTH, "comb poly: the polynomials have different num_vars");
+  if (const int rc = poly_size_check(h, polys[0]->p->nv)) return rc;
   if (!out) return fail(LASSO_ERR_LENGTH, "comb poly: null output");
   std::vector<const Poly*> ps(n_polys);
   for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
@@ -1347,6 +1352,7 @@ int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* 
 int lasso_gp_circuit_create(lasso_ctx* h, const lasso_poly* p, lasso_gp_circuit** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (const int rc = poly_use_check(h, p, nullptr)) return rc;
   if (!out) return fail(LASSO_ERR_LENGTH, "grand product circuit: null output");
   if (p->p->nv < 1 || p->p->nv > 28)

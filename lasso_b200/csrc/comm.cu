@@ -272,7 +272,6 @@ static void comm_init_impl(Ctx* c, Xchg* x, const uint8_t id_bytes[128], int ran
   c->h_pub_owned = false;
   c->h_pub = (unsigned long long*)((uint8_t*)x->seg[rank] + kSegHeaderBytes);
   for (int r = 0; r < world; r++) c->d_pub_reader[r] = readers[r];
-  c->pub_seq = 0;
   c->pub_ring[0] = c->pub_ring[1] = 0;
 }
 

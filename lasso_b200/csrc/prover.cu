@@ -390,12 +390,13 @@ static void eq_evals_shard(Ctx* c, const std::vector<fr_t>& r, size_t off, size_
 // holds this rank's columns (ncols per row, local column c' = generator c'*G + rank), the per-row partial points
 // of every rank are all-gathered and added ("bucket-sum reduce" = gather-then-add).  Replicated: every rank
 // passes the same full rows and computes the same points, no exchange.  Returns nrows compressed points; with raw_out
-// (single GPU) the rows go un-normalised to raw_out instead and nothing is returned (hiding commitments).
+// the rows go un-normalised to raw_out instead (the sums over the ranks when column-sharded) and nothing is returned
+// (hiding commitments).  Column-sharded, every path makes one all-gather of nrows x 128 B.
 static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, int limbs, size_t row_stride, int nrows,
                                      int ncols, int nw, bool replicated, uint32_t* raw_out = nullptr) {
   const int G = replicated ? 1 : c->world, gr = replicated ? 0 : c->rank;
   DBuf<pt_ext> part(c, msm_partials_count(nrows, ncols, nw));
-  if (raw_out) {
+  if (raw_out && G == 1) {
     launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, 1, 0, part.p, nullptr, nullptr,
                     raw_out, c->st);
     return {};
@@ -415,6 +416,10 @@ static std::vector<uint8_t> msm_rows(Ctx* c, const Gens& g, const void* d_scal, 
   launch_msm_rows(g.d_table.p, g.n_points, 1, d_scal, limbs, row_stride, nrows, ncols, nw, G, gr, part.p, nullptr, nullptr,
                   G == 1 ? raw.p : mine, c->st);
   if (G > 1) comm_allgather(c, mine, raw.p, (size_t)nrows * 128);
+  if (raw_out) {
+    launch_sum_raw_points(raw.p, G, nrows, raw_out, nullptr, nullptr, c->st);
+    return {};
+  }
   if (few) {
     uint32_t xyzt[8 * 32];
     if (G > 1) {
@@ -443,7 +448,9 @@ static std::vector<uint8_t> msm_rows_fr(Ctx* c, const Gens& g, const fr_t* d_sca
 
 // DensePolynomial::commit (dense_mlpoly.rs:152-181) for an integer-valued polynomial of 2^nv entries viewed as
 // L x R; this rank holds, for every row, the R/G columns congruent to its rank (= its low-bit shard of the array).
-// raw (single GPU): the rows un-normalised, for the blind term of a hiding commitment; nothing is returned then.
+// raw: the whole rows un-normalised (summed over the ranks), for the blind term of a hiding commitment; nothing is
+// returned then.  Sharded, every path makes exactly one all-gather of the L x 128 B row partials, whichever tables
+// this rank's GPU holds.
 static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_vals_loc, size_t nv, unsigned max_bits,
                                        uint32_t* raw = nullptr) {
   size_t L = (size_t)1 << (nv / 2), R = (size_t)1 << (nv - nv / 2);
@@ -460,26 +467,20 @@ static std::vector<uint8_t> commit_u32(Ctx* c, const Gens& g, const uint32_t* d_
     while (((size_t)1 << lg_rloc) < R_loc) lg_rloc++;
     const pt_niels* m16 = wide ? g.d_multiples16.p : nullptr;
     const pt_ext* k16 = wide ? g.d_centre.p + lg_rloc : nullptr;
-    if (raw) {
+    DBuf<uint32_t> comp(c, raw ? 0 : L * 8);
+    if (G == 1) {  // normalised on the device, or the raw rows
       launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr,
-                                 nullptr, raw, c->st);
-      return {};
-    }
-    std::vector<uint8_t> out(L * 32);
-    DBuf<uint32_t> comp(c, L * 8);
-    if (G == 1) {  // normalised on the device
-      launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr,
-                                 comp.p, nullptr, c->st);
+                                 comp.p, raw, c->st);
     } else {  // this rank's columns of every row -> partial points -> gather-then-add over the ranks
-      DBuf<uint32_t> raw(c, (size_t)(G + 1) * L * 32);
-      uint32_t* mine = raw.p + (size_t)G * L * 32;
+      DBuf<uint32_t> all(c, (size_t)(G + 1) * L * 32);
+      uint32_t* mine = all.p + (size_t)G * L * 32;
       launch_msm_rows_direct_u32(g.d_multiples.p, g.n_direct, m16, k16, d_vals_loc, R_loc, (int)L, (int)R_loc, nw, G, c->rank,
                                  part.p, nullptr, nullptr, mine, c->st);
-      comm_allgather(c, mine, raw.p, L * 128);
-      launch_sum_raw_points(raw.p, G, (int)L, nullptr, comp.p, nullptr, c->st);
-      c->d2h(out.data(), comp.p, out.size());
-      return out;
+      comm_allgather(c, mine, all.p, L * 128);
+      launch_sum_raw_points(all.p, G, (int)L, raw, comp.p, nullptr, c->st);
     }
+    if (raw) return {};
+    std::vector<uint8_t> out(L * 32);
     c->d2h(out.data(), comp.p, out.size());
     return out;
   }
@@ -503,24 +504,20 @@ static std::vector<uint8_t> commit_fr(Ctx* c, const Gens& g, const fr_t* d_vals_
   // rows as direct sums over the 8-bit digit-multiples tables: one table entry per non-zero signed digit
   const int nw = msm_windows_for_bits(max_bits);
   DBuf<pt_ext> part(c, L);
-  if (raw) {
-    launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, nullptr,
-                              raw, c->st);
-    return {};
-  }
-  std::vector<uint8_t> out(L * 32);
-  DBuf<uint32_t> comp(c, L * 8);
+  DBuf<uint32_t> comp(c, raw ? 0 : L * 8);
   if (G == 1) {
     launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R, (int)L, (int)R, nw, 1, 0, part.p, nullptr, comp.p,
-                              nullptr, c->st);
+                              raw, c->st);
   } else {  // this rank's columns of every row -> partial points -> gather-then-add over the ranks
-    DBuf<uint32_t> raw(c, (size_t)(G + 1) * L * 32);
-    uint32_t* mine = raw.p + (size_t)G * L * 32;
+    DBuf<uint32_t> all(c, (size_t)(G + 1) * L * 32);
+    uint32_t* mine = all.p + (size_t)G * L * 32;
     launch_msm_rows_direct_fr(g.d_multiples.p, g.n_direct, d_vals_loc, R_loc, (int)L, (int)R_loc, nw, G, c->rank, part.p,
                               nullptr, nullptr, mine, c->st);
-    comm_allgather(c, mine, raw.p, L * 128);
-    launch_sum_raw_points(raw.p, G, (int)L, nullptr, comp.p, nullptr, c->st);
+    comm_allgather(c, mine, all.p, L * 128);
+    launch_sum_raw_points(all.p, G, (int)L, raw, comp.p, nullptr, c->st);
   }
+  if (raw) return {};
+  std::vector<uint8_t> out(L * 32);
   c->d2h(out.data(), comp.p, out.size());
   return out;
 }
@@ -1800,10 +1797,15 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
 // ---------------------------------------------------------------------------------------------- dense polynomials
 // DensePolynomial::new (dense_mlpoly.rs:62-71) from the caller's evaluations.  Both sources go through the same ingest
 // kernel: host rows are first uploaded into the polynomial's own buffer and checked there in place.  The caller checks
-// len (a power of two, at most 2^28) and row_stride (>= 4).
+// len (a power of two, at most 2^28, poly_fits) and row_stride (>= 4).
+// Sharded: every rank is given the whole polynomial and reads only its rows i*G + rank.  Host rows are staged into pinned
+// memory and uploaded in one copy (1/G of the PCIe bytes); device rows are read by the ingest kernel at base rank and
+// stride G rows.  The verdict and the widest value are then agreed in one message to every process, so that every rank
+// fails together, or makes the same u32-mirror decision.
 Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err) {
   SpanTimer sp(c, "DensePolynomial.new");
   *err = 0;
+  const size_t G = (size_t)c->world, gr = (size_t)c->rank;
   if (device) {  // the first and the last row must both lie in device memory of this GPU
     size_t last = 0;
     const bool wraps = __builtin_mul_overflow(len - 1, row_stride, &last) || __builtin_add_overflow(last, (size_t)3, &last) ||
@@ -1816,8 +1818,10 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
   std::unique_ptr<Poly> p(new Poly());
   p->ctx = c;
   p->len = len;
+  p->len_loc = loc(c, len);
   p->nv = log2_exact_or_ceil(len);
-  p->d_fr.alloc(c, len);
+  const size_t n = p->len_loc;
+  p->d_fr.alloc(c, n);
   DBuf<unsigned> flags(c, 2);
   LB_CUDA_CHECK(cudaMemsetAsync(flags.p, 0, 2 * sizeof(unsigned), c->st));
   if (device) {
@@ -1825,15 +1829,37 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
     // work on `caller` (a caching allocator freeing the tensor, say) comes after the last read of them
     LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
     LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
-    launch_poly_ingest(Z, row_stride, len, p->d_fr.p, flags.p, c->st);
+    launch_poly_ingest(Z + gr * row_stride, G * row_stride, n, p->d_fr.p, flags.p, c->st);
     LB_CUDA_CHECK(cudaEventRecord(c->ev_aux, c->st));
     LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
-  } else {
+  } else if (G == 1) {
     LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, Z, len * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
     launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, len, p->d_fr.p, flags.p, c->st);
+  } else {
+    if (c->stage_busy) {  // the previous call's upload may still be reading the staging buffer
+      LB_CUDA_CHECK(cudaEventSynchronize(c->ev_stage));
+      c->stage_busy = false;
+    }
+    uint64_t* stage = reinterpret_cast<uint64_t*>(c->stage(n * 8));
+    for (size_t i = 0; i < n; i++) memcpy(stage + 4 * i, Z + 4 * (i * G + gr), 32);
+    LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, stage, n * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+    LB_CUDA_CHECK(cudaEventRecord(c->ev_stage, c->st));
+    c->stage_busy = true;
+    launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, n, p->d_fr.p, flags.p, c->st);
   }
   unsigned f[2];
   c->d2h(f, flags.p, sizeof f);
+  if (G > 1) {
+    // element 0: the non-canonical flags, summed (non-zero iff any rank saw one); element 1 + g: rank g's widest value
+    std::vector<fr_t> mine(1 + G, fr_zero()), all(1 + G);
+    mine[0].v[0] = f[0] ? 1u : 0u;
+    mine[1 + gr].v[0] = f[1];
+    c->h2d(c->d_small, mine.data(), mine.size() * sizeof(fr_t));
+    reduce_to_host(c, c->d_small, (int)(1 + G), all.data());
+    f[0] = fr_is_zero(all[0]) ? 0u : 1u;
+    f[1] = 0;
+    for (size_t r = 0; r < G; r++) f[1] = std::max(f[1], all[1 + r].v[0]);
+  }
   if (f[0]) {
     *err = 8;
     return nullptr;
@@ -1842,8 +1868,8 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
   // integer values: the u32 mirror feeds commit_u32 / bound_u32 / multi_dot_u32, which give the same bytes as the
   // Montgomery forms (lasso_strategy_create_fr sets the same precedent)
   if (p->bits <= 32) {
-    p->d_u32.alloc(c, len);
-    launch_poly_mirror_u32(p->d_fr.p, len, p->d_u32.p, c->st);
+    p->d_u32.alloc(c, n);
+    launch_poly_mirror_u32(p->d_fr.p, n, p->d_u32.p, c->st);
   }
   return p.release();
 }
@@ -1852,7 +1878,7 @@ Poly* dense_outputs(Ctx* c, const Strategy& S, const Dense& dense) {
   SpanTimer sp(c, "DensifiedRepresentation.outputs");
   std::unique_ptr<Poly> p(new Poly());
   p->ctx = c;
-  p->len = dense.s;
+  p->len = p->len_loc = dense.s;
   p->nv = log2_exact_or_ceil(dense.s);
   p->d_fr.alloc(c, p->len);
   DBuf<unsigned> bits(c, 1);
@@ -1873,18 +1899,23 @@ std::vector<uint8_t> poly_commit(Ctx* c, const Poly& p, const Gens& g) {
   w.vec_pts(commit_src(c, g, poly_src(p), p.nv, std::max(p.bits, 1u)));
   return w.b;
 }
-// DensePolynomial::evaluate (dense_mlpoly.rs:229-235): <Z, eq(r)>
+// DensePolynomial::evaluate (dense_mlpoly.rs:229-235): <Z, eq(r)>; sharded: this rank's shard of eq, and the ranks'
+// partial dots summed in one message to every process
 fr_t poly_evaluate(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
   SpanTimer sp(c, "DensePolynomial.evaluate");
-  DBuf<fr_t> eq(c, p.len);
-  eq_evals_dev(c, r, 0, p.nv, eq.p);
-  multi_dot_src(poly_src(p), p.len, 1, eq.p, p.len, c->d_partial, c->d_small, c->st);
+  DBuf<fr_t> eq(c, p.len_loc);
+  eq_evals_shard(c, r, 0, p.nv, eq.p);
+  multi_dot_src(poly_src(p), p.len_loc, 1, eq.p, p.len_loc, c->d_partial, c->d_small, c->st);
   fr_t out;
-  c->d2h(&out, c->d_small, sizeof out);
+  if (c->world > 1)
+    reduce_to_host(c, c->d_small, 1, &out);
+  else
+    c->d2h(&out, c->d_small, sizeof out);
   return out;
 }
 // DensePolynomial::commit with Some(random_tape) (dense_mlpoly.rs:152-181): C_i = <row_i, G> + blinds[i] h.  The rows
-// come un-normalised from the launchers poly_commit uses; launch_row_blinds adds the blind terms and normalises.
+// come un-normalised from the launchers poly_commit uses (sharded: summed over the ranks, so every rank holds the
+// whole rows); launch_row_blinds adds the blind terms and normalises, replicated on every rank.
 std::vector<uint8_t> poly_commit_hiding(Ctx* c, const Poly& p, const Gens& g, const std::vector<fr_t>& blinds) {
   SpanTimer sp(c, "DensePolynomial.commit_hiding");
   const size_t L = (size_t)1 << (p.nv / 2), R = poly_R(p.nv);
@@ -1927,13 +1958,16 @@ Poly* poly_create_eq(Ctx* c, const std::vector<fr_t>& r) {
   p->ctx = c;
   p->nv = r.size();
   p->len = (size_t)1 << p->nv;
+  p->len_loc = loc(c, p->len);
   p->bits = 253;  // the width of l: eq values are committed through the Fr windows
-  p->d_fr.alloc(c, p->len);
-  eq_evals_dev(c, r, 0, p->nv, p->d_fr.p);
+  p->d_fr.alloc(c, p->len_loc);
+  eq_evals_shard(c, r, 0, p->nv, p->d_fr.p);
   return p.release();
 }
 // DensePolynomial::merge (dense_mlpoly.rs:251-261): the inputs' evaluations one after another, zero-padded to a power of
 // two.  Copies only, no kernel: one device-to-device copy per input and form, a memset per form for the padding.
+// Sharded: every input's length is a multiple of G, so every input starts at a multiple of G and this rank's shard of
+// the merged polynomial is its shards of the inputs one after another, then its share of the padding: no exchange.
 Poly* poly_merge(Ctx* c, const Poly* const* polys, int k) {
   size_t total = 0;
   unsigned bits = 0;
@@ -1946,31 +1980,33 @@ Poly* poly_merge(Ctx* c, const Poly* const* polys, int k) {
   std::unique_ptr<Poly> p(new Poly());
   p->ctx = c;
   p->len = next_pow2(total);
+  p->len_loc = loc(c, p->len);
   p->nv = log2_exact_or_ceil(p->len);
   p->bits = bits;  // the padding is zero: the widest value is an input's
-  p->d_fr.alloc(c, p->len);
-  if (mirror) p->d_u32.alloc(c, p->len);
+  p->d_fr.alloc(c, p->len_loc);
+  if (mirror) p->d_u32.alloc(c, p->len_loc);
   size_t at = 0;
   for (int j = 0; j < k; j++) {
-    const size_t n = polys[j]->len;
+    const size_t n = polys[j]->len_loc;
     LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p + at, polys[j]->d_fr.p, n * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
     if (mirror)
       LB_CUDA_CHECK(cudaMemcpyAsync(p->d_u32.p + at, polys[j]->d_u32.p, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c->st));
     at += n;
   }
-  if (p->len > total) {  // zero is all-zero limbs in Montgomery form too
-    LB_CUDA_CHECK(cudaMemsetAsync(p->d_fr.p + total, 0, (p->len - total) * sizeof(fr_t), c->st));
-    if (mirror) LB_CUDA_CHECK(cudaMemsetAsync(p->d_u32.p + total, 0, (p->len - total) * sizeof(uint32_t), c->st));
+  if (p->len_loc > at) {  // zero is all-zero limbs in Montgomery form too
+    LB_CUDA_CHECK(cudaMemsetAsync(p->d_fr.p + at, 0, (p->len_loc - at) * sizeof(fr_t), c->st));
+    if (mirror) LB_CUDA_CHECK(cudaMemsetAsync(p->d_u32.p + at, 0, (p->len_loc - at) * sizeof(uint32_t), c->st));
   }
   return p.release();
 }
 // P_j(r) for k polynomials of one num_vars over ONE eq table: the integer inputs through their u32 mirrors and the others
-// through their Montgomery forms, one pointer-table dot launch (+ its reduction) per form present
+// through their Montgomery forms, one pointer-table dot launch (+ its reduction) per form present.  Sharded: over this
+// rank's shards, and the k partial values of every rank summed in one message to every process.
 std::vector<fr_t> poly_evaluate_batch(Ctx* c, const Poly* const* polys, int k, const std::vector<fr_t>& r) {
   SpanTimer sp(c, "DensePolynomial.evaluate_batch");
-  const size_t n = polys[0]->len;
+  const size_t n = polys[0]->len_loc;
   DBuf<fr_t> eq(c, n);
-  eq_evals_dev(c, r, 0, polys[0]->nv, eq.p);
+  eq_evals_shard(c, r, 0, polys[0]->nv, eq.p);
   std::vector<int> order;  // the inputs in the order their values land in d_small: integer ones first
   for (int form = 0; form < 2; form++) {
     DotPtrs in{};
@@ -1985,7 +2021,10 @@ std::vector<fr_t> poly_evaluate_batch(Ctx* c, const Poly* const* polys, int k, c
     launch_multi_dot_ptrs(in, m, form == 0, eq.p, n, c->d_partial, c->d_small + (order.size() - m), c->st);
   }
   std::vector<fr_t> got(k), out(k);
-  c->d2h(got.data(), c->d_small, k * sizeof(fr_t));
+  if (c->world > 1)
+    reduce_to_host(c, c->d_small, k, got.data());
+  else
+    c->d2h(got.data(), c->d_small, k * sizeof(fr_t));
   for (int i = 0; i < k; i++) out[order[i]] = got[i];
   return out;
 }
@@ -2031,13 +2070,14 @@ Poly* poly_create_comb(Ctx* c, const Comb& g, const Poly* const* polys, int k) {
   p->ctx = c;
   p->nv = polys[0]->nv;
   p->len = polys[0]->len;
+  p->len_loc = polys[0]->len_loc;  // element-wise: sharded, every rank maps its own shards
   p->bits = 253;  // committed through the Fr windows, as an eq polynomial
-  p->d_fr.alloc(c, p->len);
+  p->d_fr.alloc(c, p->len_loc);
   CombDev dev;
   comb_upload(c, g, dev);
   CombPtrs in{};
   for (int j = 0; j < k; j++) in.p[j] = polys[j]->d_fr.p;
-  launch_comb_map(dev.pg, in, p->len, p->d_fr.p, c->st);
+  launch_comb_map(dev.pg, in, p->len_loc, p->d_fr.p, c->st);
   return p.release();
 }
 // prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first evaluates the

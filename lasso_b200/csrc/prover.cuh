@@ -61,8 +61,10 @@ struct Ctx {
   // own, plain cudaHostAlloc; world > 1: shared pinned host segments mapped by every process, comm.cu)
   unsigned long long* h_pub = nullptr;
   unsigned long long* d_pub_reader[kPubMaxReaders] = {};
-  uint32_t pub_seq = 0;
-  uint32_t pub_ring[2] = {0, 0};  // next region of messages to this process only [0] and to every process [1]
+  // messages so far to this process only [0] and to every process [1]: the next region of each ring, and its tag.
+  // Each ring counts its own messages, so that a rank's private messages (their number may depend on the tables
+  // its GPU holds) never shift the tags of the messages every rank of a sharded context exchanges.
+  uint32_t pub_ring[2] = {0, 0};
   static constexpr size_t kPubBytes = (size_t)kPubMaxReaders * kPubRegions * kPubElems * kPubSlotWords * 8;  // 1 MiB
   cudaEvent_t ev_aux = nullptr;  // marks a device->host copy that overlaps later launches on the same stream
   cudaEvent_t ev_caller = nullptr;  // densify_device: the caller's stream up to the call (the index matrix is ready)
@@ -85,12 +87,12 @@ struct Ctx {
     p.region = 0;
     p.all = 0;
     for (int i = 0; i < kPubMaxReaders; i++) p.dst[i] = nullptr;
-    const uint32_t seq = pub_seq++;
     p.all = (all && world > 1) ? 1 : 0;
     // A peer reads this writer's message to every process before it launches its next one, so in a peer's buffer a
     // region is free again two such messages later.  Messages to this process only take no peer with them: were they
     // to advance the same ring, a writer running ahead through them would reuse a region a peer has not read yet.
-    p.region = (int)(pub_ring[p.all]++ % kPubRegions);
+    const uint32_t seq = pub_ring[p.all]++;
+    p.region = (int)(seq % kPubRegions);
     p.tag = 1 + seq % kPubTagMod;
     const size_t off = ((size_t)rank * kPubRegions + p.region) * kPubElems * kPubSlotWords;
     if (p.all) {
@@ -237,9 +239,12 @@ struct Dense {
 
 // DensePolynomial<Fr> (poly/dense_mlpoly.rs:13-18) of a caller, device resident: the library's own copy of its
 // evaluations, checked canonical on the way in (dense_poly_kernels.cu)
+// On a sharded context every rank holds its low-bit shard, as Dense does: element i' is global element i'*G + rank, so
+// for every one of the L rows the R/G columns congruent to the rank (poly_R(nv) >= G, poly_fits).
 struct Poly {
   Ctx* ctx = nullptr;
-  size_t len = 0, nv = 0;
+  size_t len = 0, nv = 0;  // the whole polynomial
+  size_t len_loc = 0;      // this rank's share, len / G: the length of d_fr and d_u32
   unsigned bits = 0;     // bit width of the widest value as an integer (0: the zero polynomial)
   DBuf<fr_t> d_fr;       // Montgomery form
   DBuf<uint32_t> d_u32;  // the same values as integers when bits <= 32 (commit_u32 / bound_u32), else empty
@@ -344,14 +349,19 @@ Poly* dense_outputs(Ctx*, const Strategy& S, const Dense&);
 void sample_generators(const std::string& label, size_t count, uint64_t* out_affine);
 
 // dense polynomials of a caller (prover.cu): PolyCommitmentGens, DensePolynomial::{new, commit, evaluate},
-// PolyEvalProof::prove.  Single-GPU contexts only.
+// PolyEvalProof::prove.  On a sharded context the calls are collective: every rank calls them with the same arguments
+// and gets the same results.  The sumchecks and grand products below are single-GPU only.
 static constexpr size_t kPolyMaxLen = (size_t)1 << 28;
 inline size_t poly_R(size_t num_vars) { return (size_t)1 << (num_vars - num_vars / 2); }
+// a polynomial of num_vars variables can be held on `world` ranks: every rank has at least one column of every row,
+// R = 2^(num_vars - num_vars/2) >= world, i.e. num_vars >= 2 log2(world) - 1
+inline bool poly_fits(size_t num_vars, int world) { return poly_R(num_vars) >= (size_t)world; }
 // PolyCommitmentGens::new (dense_mlpoly.rs:38-45) from an explicit stream: G_0..G_{R-1}, Q = stream[R], h = stream[R+1];
 // nullptr when n_points < R + 2
 Gens* poly_gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t num_vars);
 // Z: len rows of 4 u64 Montgomery limbs, row_stride u64 apart; host memory, or device memory of the context's GPU
-// (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory
+// (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory.
+// Sharded: every rank passes the whole polynomial and reads its rows; the verdict and the width are agreed by all ranks.
 Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err);
 std::vector<uint8_t> poly_commit(Ctx*, const Poly&, const Gens&);  // serialised PolyCommitment
 // the hiding PolyCommitment of the same size: row i is committed with blinds[i] on h (blinds.size() == L)
