@@ -31,6 +31,7 @@ int kh_tables_create(const uint64_t* gens_affine, size_t npts, size_t ncols16, s
   int rc = guarded([&] {
     Scope s;
     t->npts = npts;
+    t->nd = npts;
     t->ncols16 = ncols16;
     ck(cudaMalloc(&t->T, (size_t)kMsmFullWindows * npts * sizeof(pt_niels)));
     ck(cudaMalloc(&t->M, (size_t)kMsmFullWindows * npts * 128 * sizeof(pt_niels)));
@@ -57,6 +58,7 @@ void kh_tables_destroy(KhTables* t) {
   cudaFree(t->T);
   cudaFree(t->M);
   cudaFree(t->M16);
+  cudaFree(t->K16);
   delete t;
 }
 

@@ -107,11 +107,15 @@ struct Pub {
   }
 };
 
-// window + digit-multiples tables of a generator set (kh_tables_create, harness.cu).  The device arrays belong to the
-// process's primary context, so every harness library loaded into the process can use them.
+// window + digit-multiples tables of a generator set (kh_tables_create, harness.cu; kh_tables_build, harness_setup.cu).
+// The device arrays belong to the process's primary context, so every harness library loaded into the process can use
+// them.  T has npts points per window; M covers the first nd of them (nd == npts unless built by kh_tables_build);
+// K16[k] = the centring constant of 2^k local columns, for every 2^k <= ncols16 (kh_tables_build only).
 struct KhTables {
   size_t npts = 0, ncols16 = 0;
   lb::pt_niels *T = nullptr, *M = nullptr, *M16 = nullptr;
+  size_t nd = 0, nk16 = 0;
+  lb::pt_ext* K16 = nullptr;
 };
 
 inline lb::Finalize make_fin(Scope& s, const Pub& p, size_t partial_elems) {

@@ -51,6 +51,9 @@ def lib():
         L.kh_poly_ingest.argtypes = [V, S, S, V, V]
         L.kh_poly_mirror_u32.argtypes = [V, S, V]
         L.kh_eq_evals.argtypes = [I, V, V, S, V, V]
+        L.kh_densify.argtypes = [V, I, S, S, S, S, I, S, I, I, I, V, S, V, S, V, S, V]
+        L.kh_tables_build.argtypes = [V, S, S, S, S, S, C.POINTER(C.c_void_p)]
+        L.kh_table_entries.argtypes = [V, I, V, S, V]
         L.kh_arith.argtypes = [I, I, S, V, V, V, V]
         L.kh_arith_op_name.argtypes = [I]
         L.kh_arith_op_name.restype = C.c_char_p
@@ -88,6 +91,20 @@ class Tables:
         call("kh_tables_create", g.ctypes.data, g.shape[0], ncols16, col_mul, col_add, C.byref(h))
         self.h = h
         self.npts = g.shape[0]
+
+    @classmethod
+    def as_prover(cls, gens_affine, nd, ncols16=0, col_mul=1, col_add=0):
+        """the tables as a proof builds them (kh_tables_build): M over the first nd generators of a T over all of them,
+        and with ncols16 the 16-bit multiples of columns jl * col_mul + col_add and their centring constants"""
+        import numpy as np
+
+        t = cls.__new__(cls)
+        g = np.ascontiguousarray(gens_affine, dtype=np.uint64)
+        h = C.c_void_p()
+        call("kh_tables_build", g.ctypes.data, g.shape[0], nd, ncols16, col_mul, col_add, C.byref(h))
+        t.h = h
+        t.npts = g.shape[0]
+        return t
 
     def close(self):
         if self.h:

@@ -70,6 +70,8 @@ SHAPES = [
     (1, 1, 1, False), (1, 16, 20, False), (3, 3, 7, False), (3, 8, 1, False), (5000, 3, 7, True), (5000, 16, 20, True),
     (2**15 - 1, 4, 16, False), (2**15 - 1, 1, 20, False), (2**15 - 1, 8, 7, False), (2**20, 4, 20, False),
     (2**20, 8, 1, False), (2**20, 1, 16, False),
+    # the largest log_m a strategy accepts, and the largest the densified shape does (four radix passes)
+    (3000, 2, 24, False), (5, 1, 28, False),
 ]
 
 
