@@ -287,8 +287,8 @@ int lasso_random_tape_random_vector(lasso_random_tape*, const char* label, size_
  * otherwise LASSO_ERR_LENGTH before any launch (lasso_poly_gens_create, lasso_poly_create[_device], lasso_poly_create_eq,
  * lasso_poly_create_comb).  Commitments make one all-gather of the row partials; evaluations add the ranks' partial
  * values in one message to every process; openings gather L.Z and run the Bulletproofs rounds replicated.
- * lasso_sumcheck_prove, lasso_gp_circuit_create, lasso_gp_prove and lasso_dense_outputs[_custom] are not available on a
- * sharded context (LASSO_ERR_STRATEGY). */
+ * lasso_sumcheck_prove_cubic_batched is collective too.  lasso_sumcheck_prove, lasso_gp_circuit_create, lasso_gp_prove
+ * and lasso_dense_outputs[_custom] are not available on a sharded context (LASSO_ERR_STRATEGY). */
 typedef struct lasso_poly_gens lasso_poly_gens;
 typedef struct lasso_poly lasso_poly;
 size_t lasso_poly_gens_points_needed(size_t num_vars); /* R + 2 */
@@ -457,6 +457,28 @@ void lasso_comb_destroy(lasso_comb*);
 int lasso_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
                          size_t num_rounds, lasso_transcript*, uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
                          uint64_t* r_out, uint64_t* final_evals_out, uint64_t claim_out[4]);
+/* SumcheckInstanceProof::prove_cubic_batched (subprotocols/sumcheck.rs:26-135): num_rounds rounds of the sumcheck of
+ * claim = sum_x C(x) * sum_k coeffs[k] * A[k](x) * B[k](x) over 1 <= n <= 32 pairs, top variable first, on the
+ * caller's transcript, which is advanced in place.  Round j appends the cubic through [e0, e - e0, e2, e3], e starting
+ * at the caller's claim, which is not checked (as in the reference: a wrong claim gives a proof the verifier rejects).
+ * The caller's polynomials are NOT modified, and the same polynomial may appear several times (A[k] == B[j], A[k] == C).
+ * Any canonical coefficients are accepted, zero included.
+ *  - proof_out: the ark-serialize bytes of SumcheckInstanceProof, 8 + 104 * num_rounds bytes (*proof_len receives the
+ *    size, also when proof_cap is too small);
+ *  - r_out: the num_rounds challenges;
+ *  - claims_A_out, claims_B_out (n values each) and claim_C_out: element 0 of every polynomial after the binds, i.e. its
+ *    evaluation at (r || 0..0), and at r when num_rounds == num_vars.
+ * Errors, each returned before any launch and before the transcript is touched: LASSO_ERR_STRATEGY for n outside 1..32
+ * or a polynomial of another context; LASSO_ERR_LENGTH for polynomials of different num_vars, num_rounds outside
+ * 1..num_vars, proof_cap too small, or a null transcript, input or output; LASSO_ERR_VALUE for a non-canonical
+ * coefficient or claim.  The working memory ((2 n + 1) x 2^(num_vars-1) elements at most) is allocated before the first
+ * transcript write.  Collective on a sharded context: every rank sums its shards, the ranks add their round sums, the
+ * last rounds run replicated on every rank, and every rank returns the bytes, r and values of a single-GPU context. */
+int lasso_sumcheck_prove_cubic_batched(lasso_ctx*, const lasso_poly* const* A, const lasso_poly* const* B, size_t n,
+                                       const lasso_poly* C, const uint64_t* coeffs, const uint64_t claim[4],
+                                       size_t num_rounds, lasso_transcript*, uint8_t* proof_out, size_t proof_cap,
+                                       size_t* proof_len, uint64_t* r_out, uint64_t* claims_A_out,
+                                       uint64_t* claims_B_out, uint64_t claim_C_out[4]);
 /* Q(x) = g(polys[0](x), .., polys[n_polys-1](x)) at every point of the hypercube, e.g. the fingerprints
  * h(a, v, t) = t gamma^2 + v gamma + a - tau of offline memory checking (lasso/memory_checking.rs:251-252).  g's
  * declared degree is not used.  The result is a full-width polynomial like lasso_poly_create_eq (committed through the

@@ -167,6 +167,12 @@ extern "C" {
                                 -> c_int;
     pub fn lasso_poly_create_comb(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly,
                                   n_polys: usize, out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_sumcheck_prove_cubic_batched(ctx: *mut lasso_ctx, a: *const *const lasso_poly, b: *const *const lasso_poly,
+                                              n: usize, c: *const lasso_poly, coeffs: *const u64, claim: *const u64,
+                                              num_rounds: usize, transcript: *mut lasso_transcript, proof_out: *mut u8,
+                                              proof_cap: usize, proof_len: *mut usize, r_out: *mut u64,
+                                              claims_a_out: *mut u64, claims_b_out: *mut u64, claim_c_out: *mut u64)
+                                              -> c_int;
     // grand products over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
     pub fn lasso_gp_circuit_create(ctx: *mut lasso_ctx, poly: *const lasso_poly, out: *mut *mut lasso_gp_circuit) -> c_int;
     pub fn lasso_gp_circuit_evaluate(c: *const lasso_gp_circuit, out: *mut u64) -> c_int;

@@ -1071,6 +1071,33 @@ class SumcheckInstanceProof:
                                         transcript._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin), _p(claim)))
         return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim)
 
+    @classmethod
+    def prove_cubic_batched(cls, ctx, A, B, C_poly, coeffs, claim, transcript, num_rounds=None):
+        """prove_cubic_batched of claim = sum_x C(x) sum_k coeffs[k] A[k](x) B[k](x) over 1..32 pairs of DensePolynomials
+        of ctx and C_poly, all of one num_vars, on the caller's transcript, advanced in place; the claim is not checked.
+        The polynomials are not modified, and the same one may appear several times.  num_rounds=None: num_vars.
+        `.final_evals` is (2n + 1, 4): A_0.., B_0.., C at (r || 0..0); `.claim` is the caller's claim.  Collective on a
+        sharded context."""
+        A, B = list(A), list(B)
+        if len(A) != len(B):
+            raise LassoError(LASSO_ERR_STRATEGY, "prove_cubic_batched: %d A polynomials and %d B" % (len(A), len(B)))
+        n = len(A)
+        if num_rounds is None:
+            num_rounds = C_poly.num_vars
+        num_rounds = int(num_rounds)
+        coeffs = _limbs(coeffs, n, what="coeffs") if n else np.zeros((1, 4), dtype=np.uint64)
+        claim = _limbs(claim, 1, what="claim")
+        cap = 8 + max(num_rounds, 0) * 104
+        out = np.zeros(cap, dtype=np.uint8)
+        r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
+        fin = np.zeros((2 * n + 1, 4), dtype=np.uint64)
+        ln = C.c_size_t(0)
+        _chk(lib().lasso_sumcheck_prove_cubic_batched(
+            ctx._h, _poly_handles(A), _poly_handles(B), C.c_size_t(n), C_poly._h, _p(coeffs), _p(claim),
+            C.c_size_t(num_rounds), transcript._h, _p(out), C.c_size_t(cap), C.byref(ln), _p(r), _p(fin[:n] if n else fin),
+            _p(fin[n:2 * n] if n else fin), _p(fin[2 * n:])))
+        return cls(bytes(out[: ln.value]), r[:num_rounds], fin, claim.reshape(4).copy())
+
 
 # ------------------------------------------------------------------ grand products over a caller's polynomials
 class GrandProductCircuit:

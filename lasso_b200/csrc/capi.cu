@@ -1327,6 +1327,52 @@ int lasso_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly* co
   return 0;
   LB_CATCH
 }
+int lasso_sumcheck_prove_cubic_batched(lasso_ctx* h, const lasso_poly* const* A, const lasso_poly* const* B, size_t n,
+                                       const lasso_poly* C, const uint64_t* coeffs, const uint64_t claim[4],
+                                       size_t num_rounds, lasso_transcript* transcript, uint8_t* proof_out,
+                                       size_t proof_cap, size_t* proof_len, uint64_t* r_out, uint64_t* claims_A_out,
+                                       uint64_t* claims_B_out, uint64_t claim_C_out[4]) {
+  LB_TRY_CTX(h)
+  if (n < 1 || n > 32) return fail(LASSO_ERR_STRATEGY, "cubic sumcheck: 1 <= n <= 32 pairs");
+  if (!A || !B) return fail(LASSO_ERR_STRATEGY, "cubic sumcheck: null polynomial array");
+  for (size_t k = 0; k < n; k++) {
+    if (const int rc = poly_use_check(h, A[k], nullptr)) return rc;
+    if (const int rc = poly_use_check(h, B[k], nullptr)) return rc;
+  }
+  if (const int rc = poly_use_check(h, C, nullptr)) return rc;
+  const size_t nv = C->p->nv;
+  for (size_t k = 0; k < n; k++)
+    if (A[k]->p->nv != nv || B[k]->p->nv != nv)
+      return fail(LASSO_ERR_LENGTH, "cubic sumcheck: the polynomials have different num_vars");
+  if (num_rounds < 1 || num_rounds > nv) return fail(LASSO_ERR_LENGTH, "cubic sumcheck: num_rounds must be in 1..num_vars");
+  // SumcheckInstanceProof of a cubic: a u64 count, then per round a u64 length and 3 coefficients
+  const size_t need = 8 + num_rounds * (8 + 32 * 3);
+  if (proof_len) *proof_len = need;
+  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "cubic sumcheck: output buffer too small");
+  if (!transcript || !coeffs || !claim || !r_out || !claims_A_out || !claims_B_out || !claim_C_out)
+    return fail(LASSO_ERR_LENGTH, "cubic sumcheck: null transcript, input or output");
+  std::vector<fr_t> cv, e;
+  if (!load_scalars(coeffs, n, cv)) return fail(LASSO_ERR_VALUE, "cubic sumcheck: a coefficient is not a canonical residue");
+  if (!load_scalars(claim, 1, e)) return fail(LASSO_ERR_VALUE, "cubic sumcheck: the claim is not a canonical residue");
+  std::vector<const Poly*> pa(n), pb(n);
+  for (size_t k = 0; k < n; k++) {
+    pa[k] = A[k]->p;
+    pb[k] = B[k]->p;
+  }
+  auto t0 = std::chrono::steady_clock::now();
+  const CubicOut o = cubic_prove(h->c, pa.data(), pb.data(), (int)n, *C->p, cv, e[0], num_rounds, transcript->t);
+  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  if (o.proof.size() != need) return fail(-1, "cubic sumcheck: unexpected proof size");
+  memcpy(proof_out, o.proof.data(), need);
+  for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
+  for (size_t k = 0; k < n; k++) {
+    memcpy(claims_A_out + 4 * k, o.finals[k].v, 32);
+    memcpy(claims_B_out + 4 * k, o.finals[n + k].v, 32);
+  }
+  memcpy(claim_C_out, o.finals[2 * n].v, 32);
+  return 0;
+  LB_CATCH
+}
 int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* const* polys, size_t n_polys,
                            lasso_poly** out) {
   LB_TRY_CTX(h)

@@ -216,6 +216,10 @@ void launch_product_trees(const TreePtrs& trees, int ntrees, size_t N, int slot0
 void launch_product_layer1(const fr_t* P, fr_t* out, size_t half, cudaStream_t st);
 // x_k[0] <- x_k[0] + r (x_k[1] - x_k[0]) for the n arrays x_k = d_AB[k]; results also published (Finalize)
 void launch_bind_heads(fr_t* const* d_AB, int n, const fr_t& r, const Finalize& fin, cudaStream_t st);
+// publishes x[0] + r (x[half] - x[0]) for the n arrays x = d_AB[k] and then for C (n + 1 values, n < 1024), writing
+// nothing; publish = false publishes zeros instead (the ranks of a sharded context that do not hold element 0)
+void launch_cubic_finals(fr_t* const* d_AB, int n, const fr_t* C, size_t half, const fr_t& r, bool publish,
+                         const Finalize& fin, cudaStream_t st);
 // elementwise helpers for the Bulletproofs scalar folds (bullet.rs:125-130)
 // a[i] <- a[i]*u + uinv*a[i+h];  b[i] <- b[i]*uinv + u*b[i+h]
 void launch_fold_ab(fr_t* a, fr_t* b, size_t h, const fr_t& u, const fr_t& uinv, cudaStream_t st);

@@ -1483,6 +1483,19 @@ __global__ void bind_heads_kernel(fr_t* const* AB, int n, fr_t r, Finalize fin) 
 void launch_bind_heads(fr_t* const* d_AB, int n, const fr_t& r, const Finalize& fin, cudaStream_t st) {
   launch(bind_heads_kernel, 1, (n + 31) / 32 * 32, 0, st, d_AB, n, r, fin);
 }
+// after the last round of a caller's batched cubic sumcheck: element 0 of every array bound with r, read only,
+// x[0] + r (x[half] - x[0]) for x = AB[0..n) and then C; published as n + 1 values (zeros when publish == 0)
+__global__ void cubic_finals_kernel(fr_t* const* AB, int n, const fr_t* C, size_t half, fr_t r, int publish, Finalize fin) {
+  const int k = threadIdx.x;
+  if (k > n) return;
+  const fr_t* x = k < n ? AB[k] : C;
+  const fr_t lo = ld_fr(x), hi = ld_fr(x + half);
+  finalize_publish(fin, k, publish ? fr_add(lo, fr_mul(r, fr_sub(hi, lo))) : fr_zero());
+}
+void launch_cubic_finals(fr_t* const* d_AB, int n, const fr_t* C, size_t half, const fr_t& r, bool publish,
+                         const Finalize& fin, cudaStream_t st) {
+  launch(cubic_finals_kernel, 1, (n + 32) / 32 * 32, 0, st, d_AB, n, C, half, r, publish ? 1 : 0, fin);
+}
 
 // ---- Bulletproofs scalar-side helpers (bullet.rs:73-134) ----
 __global__ void __launch_bounds__(kThreads) fold_ab_kernel(fr_t* a, fr_t* b, size_t h, fr_t u, fr_t uinv) {

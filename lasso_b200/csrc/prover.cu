@@ -1008,7 +1008,138 @@ struct LayerProof {
 };
 typedef std::vector<LayerProof> GPAProof;
 
-// BatchedGrandProductArgument::prove (grand_product.rs:100-201) with prove_cubic_batched (sumcheck.rs:26-135)
+// One batched cubic sumcheck (sumcheck.rs:26-135): rounds of  sum_x C(x) sum_k coeff_k A_k(x) B_k(x)  over n pairs,
+// top variable first.  Every pointer table lists [A_0..A_{n-1} | B_0..B_{n-1} | A_0,B_0,A_1,B_1,..] (4n entries).  The
+// kernels fold the batching coefficients in (poly_kernels.cu K3): the first fused bind stores coeff_k * A_k, and a
+// round message is the 3 combined values of sumcheck.rs:95-97.
+struct CubicArrays {
+  int n = 0;
+  size_t cur = 0;  // the length of every array on this rank
+  // low-bit shards of a sharded context: every rank sums its shards and the ranks' sums are added; at one element per
+  // rank the G-element remainders are gathered into `tail` (table tail_tab) and the last rounds run replicated
+  bool sharded = false;
+  fr_t* const* first = nullptr;  // the arrays the first round reads
+  fr_t* C = nullptr;             // C for the first round
+  fr_t* Cw[2] = {nullptr, nullptr};  // the buffers C is bound into, alternately: the first bind writes Cw[0]
+  // read-only arrays (a caller's): the first bind goes out of place, bind_src -> bind_dst ([A.. | B.. | C], 2n + 1
+  // entries each, C into Cw[0]), and `bound` lists the arrays after it.  Null: the arrays are bound in place.
+  fr_t* const* bind_src = nullptr;
+  fr_t* const* bind_dst = nullptr;
+  fr_t* const* bound = nullptr;
+  fr_t* const* tail_tab = nullptr;
+  fr_t* tail = nullptr;  // (2n + 1) x G: A_0, B_0, A_1, .., C
+};
+// The arrays after the last round: its challenge r is not bound in yet.  Their length is cur (on this rank).
+struct CubicEnd {
+  fr_t* const* tab;
+  fr_t* C;
+  size_t cur;
+  bool on_src, sharded, stored_scaled;  // on_src: still the read-only arrays; stored_scaled: A_k holds coeff_k A_k
+  fr_t r;
+};
+// num_rounds rounds from the claim e on the transcript: appends the compressed round polynomials to proof and the
+// challenges to r; inv_coeff receives 1 / coeff_k (computed while the first kernel runs) when num_rounds >= 1.
+// Launches: one evaluation, then per later round one fused bind + evaluation, or for the first bind of read-only
+// arrays an out-of-place bind and an evaluation; sharded, the last local round's bind (two launches) and the
+// remainders' exchange (comm_gather_heads) come before the replicated evaluation.
+static CubicEnd cubic_rounds(Ctx* c, const CubicArrays& a, const CubicCoeffs& cf, const std::vector<fr_t>& coeff_vec,
+                             fr_t e, size_t num_rounds, Transcript& transcript, SumcheckProof& proof,
+                             std::vector<fr_t>& r, std::vector<fr_t>& inv_coeff) {
+  const int n = a.n;
+  auto A_of = [](fr_t* const* t) { return t; };
+  auto B_of = [n](fr_t* const* t) { return t + n; };
+  auto AB_of = [n](fr_t* const* t) { return t + 2 * n; };
+  auto other = [&a](const fr_t* x) { return x == a.Cw[0] ? a.Cw[1] : a.Cw[0]; };
+  CubicEnd end{a.first, a.C, a.cur, a.bind_src != nullptr, a.sharded, false, fr_zero()};
+  fr_t* const*& tab = end.tab;
+  fr_t*& Ccur = end.C;
+  size_t& cur = end.cur;
+  bool& sharded = end.sharded;
+  bool have_evals = false;
+  std::vector<fr_t> ev(3);
+  Finalize fz{};
+  for (size_t j = 0; j < num_rounds; j++) {
+    if (sharded && cur == 1) {  // all-gather the G-element remainders; the tail rounds run replicated
+      comm_gather_heads(c, AB_of(tab), nullptr, 0, 2 * n, Ccur, a.tail);  // A_k, B_k and C in one exchange
+      tab = a.tail_tab;
+      Ccur = a.tail + (size_t)2 * n * c->world;
+      cur = (size_t)c->world;
+      sharded = end.on_src = have_evals = false;
+    }
+    if (!have_evals) {  // first round of a phase; later rounds come out of the fused bind+eval kernel
+      fz = c->fin_begin(sharded);
+      launch_sumcheck_eval_cubic_comb(A_of(tab), B_of(tab), Ccur, n, cur / 2, cf, end.stored_scaled ? 0 : 1, fz, c->st);
+    }
+    if (inv_coeff.empty()) {  // 1 / coeff_k by Montgomery's trick, overlapping the kernel just launched
+      inv_coeff.resize(n);
+      std::vector<fr_t> pre(n);
+      fr_t acc = fr_one();
+      for (int k = 0; k < n; k++) {
+        pre[k] = acc;
+        acc = fr_mul(acc, coeff_vec[k]);
+      }
+      if (fr_eq(acc, fr_zero())) throw std::runtime_error("zero batching coefficient");
+      fr_t ainv = fr_inv(acc);
+      for (int k = n; k-- > 0;) {
+        inv_coeff[k] = fr_mul(ainv, pre[k]);
+        ainv = fr_mul(ainv, coeff_vec[k]);
+      }
+    }
+    const size_t half = cur / 2;
+    auto tp0 = std::chrono::steady_clock::now();
+    c->fin_wait(fz, ev.data(), 3);  // sharded: the three sums of every rank, added here
+    auto tp1 = std::chrono::steady_clock::now();
+    const fr_t c0 = ev[0], c2 = ev[1], c3 = ev[2];  // already combined over the pairs (sumcheck.rs:95-97)
+    std::vector<fr_t> evals = {c0, fr_sub(e, c0), c2, c3};  // eval(1) = e - eval(0), sumcheck.rs:99-104
+    std::vector<fr_t> coeffs = unipoly_from_evals(evals);
+    unipoly_append(coeffs, transcript);
+    const fr_t r_j = transcript.challenge_scalar("challenge_nextround");
+    r.push_back(r_j);
+    auto tp2 = std::chrono::steady_clock::now();
+    e = unipoly_evaluate(coeffs, r_j);
+    proof.push_back(unipoly_compress(coeffs));
+    if (j + 1 == num_rounds) {  // the caller binds the last challenge into what it needs
+      end.r = r_j;
+      return end;
+    }
+    if (end.on_src) {
+      // bind A_k, B_k and C out of place, unscaled; then evaluate the next round there
+      launch_bind_ptrs(a.bind_src, a.bind_dst, 2 * n + 1, half, r_j, c->st);
+      tab = a.bound;
+      Ccur = a.Cw[0];
+      end.on_src = false;
+      have_evals = false;
+      if (half > 1) {
+        fz = c->fin_begin(sharded);
+        launch_sumcheck_eval_cubic_comb(A_of(tab), B_of(tab), Ccur, n, half / 2, cf, 1, fz, c->st);
+        have_evals = true;
+      }
+    } else if (half > 1) {
+      // bind with r_j and evaluate the next round in one pass (sumcheck.rs:116-120 + 63-89)
+      fz = c->fin_begin(sharded);
+      fr_t* Cnext = other(Ccur);
+      launch_sumcheck_bind_eval_cubic_comb(A_of(tab), B_of(tab), Ccur, Cnext, n, half, r_j, cf,
+                                           end.stored_scaled ? 0 : 1, fz, c->st);
+      end.stored_scaled = true;
+      Ccur = Cnext;
+      have_evals = true;
+    } else {  // sharded, one pair per rank left: bind in place, and the next round gathers the remainders
+      launch_bind_top_ptrs(AB_of(tab), 2 * n, half, r_j, c->st);
+      launch_bind_top(Ccur, 0, 1, half, r_j, c->st);
+      have_evals = false;
+    }
+    auto tp3 = std::chrono::steady_clock::now();
+    if (c->span_sync) {  // where a round goes: waiting for the device, host glue, launch call
+      c->spans["Cubic.round wait"] += std::chrono::duration<double, std::milli>(tp1 - tp0).count();
+      c->spans["Cubic.round host"] += std::chrono::duration<double, std::milli>(tp2 - tp1).count();
+      c->spans["Cubic.round launch"] += std::chrono::duration<double, std::milli>(tp3 - tp2).count();
+    }
+    cur = half;
+  }
+  return end;
+}
+
+// BatchedGrandProductArgument::prove (grand_product.rs:100-201): one cubic_rounds per layer, C = eq(rand)
 static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<fr_t> claims_to_verify,
                           Transcript& transcript, std::vector<fr_t>& rand_out) {
   SpanTimer sp(c, "BatchedGrandProductArgument.prove");
@@ -1029,12 +1160,11 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
   DBuf<fr_t> tail(c, (size_t)(2 * ncirc + 1) * G);  // replicated remainders of A_k, B_k, C (G elements each)
   std::vector<fr_t> rand;
   if (ncirc > 32) throw std::runtime_error("more than 32 circuits in one batched grand product");
-  std::vector<fr_t> ev(3), fin((size_t)2 * ncirc);
+  std::vector<fr_t> fin((size_t)2 * ncirc);
   // per slot: [A_0..A_{n-1} | B_0..B_{n-1} | A_0,B_0,A_1,B_1,...]
   std::vector<fr_t*> table(d_ptrs.n);
-  auto slot_A = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc; };
-  auto slot_B = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc + ncirc; };
-  auto slot_AB = [&](size_t slot) { return d_ptrs.p + slot * 4 * ncirc + 2 * ncirc; };
+  auto slot = [&](size_t s) { return d_ptrs.p + s * 4 * ncirc; };
+  auto slot_AB = [&](size_t s) { return d_ptrs.p + s * 4 * ncirc + 2 * ncirc; };
   fr_t* const* bind_src = d_ptrs.p + nslots * 4 * ncirc;
   fr_t* const* bind_dst = bind_src + nbind;
   if (ext) {
@@ -1053,33 +1183,30 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
     replicated_layer = G > 1 && !circuits[0]->layer_is_sharded(layer_id);
     return replicated_layer ? len_g / 2 : len_g / 2 / (size_t)G;  // |A| = |B| = |C| on this rank
   };
-  for (size_t slot = 0; slot < nslots; slot++) {
+  for (size_t s = 0; s < nslots; s++) {
     for (int k = 0; k < ncirc; k++) {
       fr_t *pa, *pb;
-      if (slot == num_layers) {
+      if (s == num_layers) {
         pa = tail.p + (size_t)(2 * k) * G;
         pb = tail.p + (size_t)(2 * k + 1) * G;
       } else {
         bool rep;
-        size_t cur0 = layer_cur(slot, rep);
-        pa = rep ? circuits[k]->layer_rep(slot) : circuits[k]->layer_local(slot);
+        size_t cur0 = layer_cur(s, rep);
+        pa = rep ? circuits[k]->layer_rep(s) : circuits[k]->layer_local(s);
         pb = pa + cur0;
       }
-      table[slot * 4 * ncirc + k] = pa;
-      table[slot * 4 * ncirc + ncirc + k] = pb;
-      table[slot * 4 * ncirc + 2 * ncirc + 2 * k] = pa;
-      table[slot * 4 * ncirc + 2 * ncirc + 2 * k + 1] = pb;
+      table[s * 4 * ncirc + k] = pa;
+      table[s * 4 * ncirc + ncirc + k] = pb;
+      table[s * 4 * ncirc + 2 * ncirc + 2 * k] = pa;
+      table[s * 4 * ncirc + 2 * ncirc + 2 * k + 1] = pb;
     }
   }
   LB_CUDA_CHECK(cudaMemcpyAsync(d_ptrs.p, table.data(), table.size() * sizeof(fr_t*), cudaMemcpyHostToDevice, c->st));
   c->sync();
   for (size_t layer_id = num_layers; layer_id-- > 0;) {
     bool replicated_layer;
-    size_t cur = layer_cur(layer_id, replicated_layer);
-    bool sharded = G > 1 && !replicated_layer;
-    fr_t* const* dA = slot_A(layer_id);
-    fr_t* const* dB = slot_B(layer_id);
-    fr_t* const* dAB = slot_AB(layer_id);
+    const size_t cur = layer_cur(layer_id, replicated_layer);
+    const bool sharded = G > 1 && !replicated_layer;
     // poly_C = eq(rand), grand_product.rs:122
     if (sharded)
       eq_evals_shard(c, rand, 0, rand.size(), eqbuf.p);
@@ -1088,114 +1215,43 @@ static GPAProof prove_gpa(Ctx* c, std::vector<Circuit*>& circuits, std::vector<f
     std::vector<fr_t> coeff_vec = transcript.challenge_vector("rand_coeffs_next_layer", ncirc);
     fr_t e = fr_zero();
     for (int k = 0; k < ncirc; k++) e = fr_add(e, fr_mul(claims_to_verify[k], coeff_vec[k]));
-    // The kernels fold the batching coefficients in (poly_kernels.cu): the first bind of the layer stores
-    // coeff_k * A_k, a round message is the 3 combined values of sumcheck.rs:95-97.
     CubicCoeffs cf;
     for (int k = 0; k < ncirc; k++) cf.v[k] = coeff_vec[k];
-    bool stored_scaled = false;
-    std::vector<fr_t> inv_coeff;  // computed while the first kernel of the layer runs
-    LayerProof lp;
-    std::vector<fr_t> rand_prod;
-    fr_t* Ccur = eqbuf.p;
-    fr_t* Cnext = eqbuf2.p;
-    bool have_evals = false, heads_published = false;
-    bool on_caller = ext && layer_id == 0;  // dA, dB still point at the caller's buffers: nothing may write them
-    Finalize fz = c->fin_begin();
-    for (;;) {
-      if (sharded && cur == 1) {  // all-gather the G-element remainders; the tail rounds run replicated
-        comm_gather_heads(c, dAB, nullptr, 0, 2 * ncirc, Ccur, tail.p);  // A_k, B_k and eq in one exchange
-        dA = slot_A(num_layers);
-        dB = slot_B(num_layers);
-        dAB = slot_AB(num_layers);
-        Ccur = tail.p + (size_t)2 * ncirc * G;
-        Cnext = eqbuf2.p;
-        cur = (size_t)G;
-        sharded = false;
-        have_evals = false;
-      }
-      if (cur <= 1) break;
-      if (!have_evals) {  // first round of a phase; later rounds come out of the fused bind+eval kernel
-        fz = c->fin_begin(sharded);
-        launch_sumcheck_eval_cubic_comb(dA, dB, Ccur, ncirc, cur / 2, cf, stored_scaled ? 0 : 1, fz, c->st);
-      }
-      if (inv_coeff.empty()) {  // 1 / coeff_k by Montgomery's trick, overlapping the kernel just launched
-        inv_coeff.resize(ncirc);
-        std::vector<fr_t> pre(ncirc);
-        fr_t acc = fr_one();
-        for (int k = 0; k < ncirc; k++) {
-          pre[k] = acc;
-          acc = fr_mul(acc, coeff_vec[k]);
-        }
-        if (fr_eq(acc, fr_zero())) throw std::runtime_error("zero batching coefficient");
-        fr_t ainv = fr_inv(acc);
-        for (int k = ncirc; k-- > 0;) {
-          inv_coeff[k] = fr_mul(ainv, pre[k]);
-          ainv = fr_mul(ainv, coeff_vec[k]);
-        }
-      }
-      size_t half = cur / 2;
-      auto tp0 = std::chrono::steady_clock::now();
-      c->fin_wait(fz, ev.data(), 3);  // sharded: the three sums of every rank, added here
-      auto tp1 = std::chrono::steady_clock::now();
-      const fr_t c0 = ev[0], c2 = ev[1], c3 = ev[2];  // already combined over the circuits (sumcheck.rs:95-97)
-      std::vector<fr_t> evals = {c0, fr_sub(e, c0), c2, c3};  // eval(1) = e - eval(0), sumcheck.rs:99-104
-      std::vector<fr_t> coeffs = unipoly_from_evals(evals);
-      unipoly_append(coeffs, transcript);
-      fr_t r_j = transcript.challenge_scalar("challenge_nextround");
-      rand_prod.push_back(r_j);
-      auto tp2 = std::chrono::steady_clock::now();
-      if (on_caller) {
-        // bind A_k, B_k (and eq, unless this is the last round) out of place into layer 1's storage, unscaled; then
-        // evaluate the next round there, or read the heads with pack_heads below
-        launch_bind_ptrs(bind_src, bind_dst, half > 1 ? (int)nbind : 2 * ncirc, half, r_j, c->st);
-        dA = slot_A(1);
-        dB = slot_B(1);
-        dAB = slot_AB(1);
-        on_caller = false;
-        have_evals = false;
-        if (half > 1) {
-          std::swap(Ccur, Cnext);
-          fz = c->fin_begin();
-          launch_sumcheck_eval_cubic_comb(dA, dB, Ccur, ncirc, half / 2, cf, 1, fz, c->st);
-          have_evals = true;
-        }
-      } else if (half > 1) {
-        // bind with r_j and evaluate the next round in one pass (sumcheck.rs:116-120 + 63-89)
-        fz = c->fin_begin(sharded);
-        launch_sumcheck_bind_eval_cubic_comb(dA, dB, Ccur, Cnext, ncirc, half, r_j, cf, stored_scaled ? 0 : 1, fz, c->st);
-        stored_scaled = true;
-        std::swap(Ccur, Cnext);
-        have_evals = true;
-      } else if (!sharded) {
-        // last round: bind the 2*ncirc heads and publish them (the layer's claims); eq is not needed any more
-        fz = c->fin_begin();
-        launch_bind_heads(dAB, 2 * ncirc, r_j, fz, c->st);
-        have_evals = false;
-        heads_published = true;
-      } else {
-        launch_bind_top_ptrs(dAB, 2 * ncirc, half, r_j, c->st);
-        launch_bind_top(Ccur, 0, 1, half, r_j, c->st);
-        have_evals = false;
-      }
-      auto tp3 = std::chrono::steady_clock::now();
-      if (c->span_sync) {  // where a grand-product round goes: waiting for the device, host glue, launch call
-        c->spans["GPA.round wait"] += std::chrono::duration<double, std::milli>(tp1 - tp0).count();
-        c->spans["GPA.round host"] += std::chrono::duration<double, std::milli>(tp2 - tp1).count();
-        c->spans["GPA.round launch"] += std::chrono::duration<double, std::milli>(tp3 - tp2).count();
-      }
-      e = unipoly_evaluate(coeffs, r_j);
-      lp.proof.push_back(unipoly_compress(coeffs));
-      cur = half;
+    CubicArrays arr;
+    arr.n = ncirc;
+    arr.cur = cur;
+    arr.sharded = sharded;
+    arr.first = slot(layer_id);
+    arr.C = eqbuf.p;
+    arr.Cw[0] = eqbuf2.p;
+    arr.Cw[1] = eqbuf.p;
+    if (ext && layer_id == 0) {  // the caller's buffers: nothing may write them
+      arr.bind_src = bind_src;
+      arr.bind_dst = bind_dst;
+      arr.bound = slot(1);
     }
-    // claims_prod = (A_k[0], B_k[0]): published by the last round's kernel, or packed on the device + one transfer
-    if (heads_published) {
+    arr.tail_tab = slot(num_layers);
+    arr.tail = tail.p;
+    const size_t num_rounds = (size_t)__builtin_ctzll(circuits[0]->layer_len_global(layer_id) / 2);
+    LayerProof lp;
+    std::vector<fr_t> rand_prod, inv_coeff;
+    const CubicEnd end = cubic_rounds(c, arr, cf, coeff_vec, e, num_rounds, transcript, lp.proof, rand_prod, inv_coeff);
+    // claims_prod = (A_k[0], B_k[0]) after the last bind: published by bind_heads, or packed on the device + one transfer
+    if (num_rounds && !end.on_src) {
+      const Finalize fz = c->fin_begin();
+      launch_bind_heads(end.tab + 2 * ncirc, 2 * ncirc, end.r, fz, c->st);  // eq is not needed any more
       c->fin_wait(fz, fin.data(), 2 * ncirc);
     } else {
-      pack_heads(c, dAB, nullptr, 0, 2 * ncirc, c->d_small + 1024);
+      fr_t* const* heads = slot_AB(layer_id);
+      if (num_rounds) {  // a caller's layer 0 of two elements per array: bound out of place into layer 1's storage
+        launch_bind_ptrs(bind_src, bind_dst, 2 * ncirc, 1, end.r, c->st);
+        heads = slot_AB(1);
+      }
+      pack_heads(c, heads, nullptr, 0, 2 * ncirc, c->d_small + 1024);
       c->d2h(fin.data(), c->d_small + 1024, fin.size() * sizeof(fr_t));
     }
     for (int k = 0; k < ncirc; k++) {  // the left arrays carry coeff_k once a bind has stored them
-      lp.claims_prod_left.push_back(stored_scaled ? fr_mul(fin[2 * k], inv_coeff[k]) : fin[2 * k]);
+      lp.claims_prod_left.push_back(end.stored_scaled ? fr_mul(fin[2 * k], inv_coeff[k]) : fin[2 * k]);
       lp.claims_prod_right.push_back(fin[2 * k + 1]);
     }
     for (int k = 0; k < ncirc; k++) {
@@ -2130,6 +2186,126 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
   const Finalize f = c->fin_begin();
   launch_final_comb(src, k, len / 2, r_prev, f, c->st);
   c->fin_wait(f, out.final_evals.data(), k);
+  out.proof = std::move(w.b);
+  return out;
+}
+
+// prove_cubic_batched over a caller's polynomials.  The pairs with a non-zero coefficient go through cubic_rounds on
+// the caller's buffers (read only): the first bind writes a workspace, later rounds bind there in place.  A pair with
+// coeff_k = 0 adds nothing to any round (and coeff_k A_k cannot give A_k back): its finals, and C's when every
+// coefficient is zero, are batched evaluations at (r || 0..0), element 0 after the binds.
+CubicOut cubic_prove(Ctx* c, const Poly* const* A, const Poly* const* B, int n, const Poly& C,
+                     const std::vector<fr_t>& coeffs, const fr_t& claim, size_t num_rounds, Transcript& transcript) {
+  SpanTimer sp(c, "Sumcheck.prove_cubic_batched");
+  const int G = c->world;
+  const size_t len = C.len_loc;  // on this rank
+  std::vector<int> act, idle;    // pairs with a non-zero / zero coefficient
+  for (int k = 0; k < n; k++) (fr_eq(coeffs[k], fr_zero()) ? idle : act).push_back(k);
+  const int m = (int)act.size();
+  const size_t nbind = 2 * (size_t)m + 1, h = std::max<size_t>(len / 2, 1);
+  // every allocation before the first transcript write: a failure leaves the caller's transcript as it was
+  DBuf<fr_t*> d_ptrs;
+  DBuf<fr_t> ws, cw, tail;
+  CubicArrays a;
+  if (m) {
+    // tables: the caller's arrays, the workspace's, the tail's (4m each), then bind_src and bind_dst (2m + 1 each)
+    d_ptrs.alloc(c, 12 * (size_t)m + 2 * nbind);
+    if (num_rounds >= 2) ws.alloc(c, 2 * (size_t)m * h);
+    const size_t cw0 = std::max<size_t>(len / 2, (size_t)G), cw1 = std::max<size_t>(len / 4, (size_t)G);
+    cw.alloc(c, cw0 + cw1);
+    if (G > 1) tail.alloc(c, nbind * G);
+    std::vector<fr_t*> table(d_ptrs.n, nullptr);
+    auto fill = [&](size_t at, auto pa, auto pb) {
+      for (int k = 0; k < m; k++) {
+        table[at + k] = table[at + 2 * m + 2 * k] = pa(k);
+        table[at + m + k] = table[at + 2 * m + 2 * k + 1] = pb(k);
+      }
+    };
+    fill(0, [&](int k) { return A[act[k]]->d_fr.p; }, [&](int k) { return B[act[k]]->d_fr.p; });
+    if (ws.p) fill(4 * (size_t)m, [&](int k) { return ws.p + k * h; }, [&](int k) { return ws.p + (m + k) * h; });
+    if (tail.p)
+      fill(8 * (size_t)m, [&](int k) { return tail.p + (size_t)(2 * k) * G; },
+           [&](int k) { return tail.p + (size_t)(2 * k + 1) * G; });
+    fr_t** src = table.data() + 12 * (size_t)m;
+    fr_t** dst = src + nbind;
+    for (int k = 0; k < 2 * m; k++) {
+      src[k] = table[k];
+      dst[k] = table[4 * (size_t)m + k];
+    }
+    src[2 * m] = C.d_fr.p;
+    dst[2 * m] = cw.p;
+    c->h2d(d_ptrs.p, table.data(), table.size() * sizeof(fr_t*));
+    a.n = m;
+    a.cur = len;
+    a.sharded = G > 1;
+    a.first = d_ptrs.p;
+    a.C = C.d_fr.p;
+    a.Cw[0] = cw.p;
+    a.Cw[1] = cw.p + cw0;
+    a.bind_src = d_ptrs.p + 12 * (size_t)m;
+    a.bind_dst = a.bind_src + nbind;
+    a.bound = d_ptrs.p + 4 * (size_t)m;
+    a.tail_tab = d_ptrs.p + 8 * (size_t)m;
+    a.tail = tail.p;
+  }
+  if (!idle.empty() || !m) {  // reserve the batched evaluations' eq table in the context's pool
+    DBuf<fr_t> reserve(c, len);
+  }
+  SumcheckProof proof;
+  CubicOut out;
+  std::vector<fr_t> inv_coeff;
+  CubicEnd end{};
+  if (m) {
+    CubicCoeffs cf;
+    std::vector<fr_t> cv(m);
+    for (int k = 0; k < m; k++) cf.v[k] = cv[k] = coeffs[act[k]];
+    end = cubic_rounds(c, a, cf, cv, claim, num_rounds, transcript, proof, out.r, inv_coeff);
+  } else {  // every round polynomial is e(1 - x) (sumcheck.rs:95-104 with all sums zero): no device work
+    fr_t e = claim;
+    for (size_t j = 0; j < num_rounds; j++) {
+      const std::vector<fr_t> coeffs_j = unipoly_from_evals({fr_zero(), e, fr_zero(), fr_zero()});
+      unipoly_append(coeffs_j, transcript);
+      const fr_t r_j = transcript.challenge_scalar("challenge_nextround");
+      out.r.push_back(r_j);
+      e = unipoly_evaluate(coeffs_j, r_j);
+      proof.push_back(unipoly_compress(coeffs_j));
+    }
+  }
+  out.finals.assign(2 * (size_t)n + 1, fr_zero());
+  if (m) {  // sharded with rounds left over: element 0 is rank 0's, and the other ranks publish zeros into the sum
+    std::vector<fr_t> fin(nbind);
+    const Finalize f = c->fin_begin(end.sharded);
+    launch_cubic_finals(end.tab + 2 * m, 2 * m, end.C, end.cur / 2, end.r, !end.sharded || c->rank == 0, f, c->st);
+    c->fin_wait(f, fin.data(), (int)nbind);
+    for (int k = 0; k < m; k++) {  // the A arrays carry coeff_k once a fused bind has stored them
+      out.finals[act[k]] = end.stored_scaled ? fr_mul(fin[2 * k], inv_coeff[k]) : fin[2 * k];
+      out.finals[n + act[k]] = fin[2 * k + 1];
+    }
+    out.finals[2 * n] = fin[2 * m];
+  }
+  if (!idle.empty() || !m) {
+    std::vector<const Poly*> ps;
+    std::vector<size_t> at;
+    for (int k : idle) {
+      ps.push_back(A[k]);
+      at.push_back(k);
+      ps.push_back(B[k]);
+      at.push_back(n + k);
+    }
+    if (!m) {
+      ps.push_back(&C);
+      at.push_back(2 * n);
+    }
+    std::vector<fr_t> point(out.r);
+    point.resize(C.nv, fr_zero());
+    for (size_t i = 0; i < ps.size(); i += kDotMaxPolys) {
+      const int cnt = (int)std::min<size_t>(kDotMaxPolys, ps.size() - i);
+      const std::vector<fr_t> v = poly_evaluate_batch(c, ps.data() + i, cnt, point);
+      for (int j = 0; j < cnt; j++) out.finals[at[i + j]] = v[j];
+    }
+  }
+  ByteWriter w;
+  ser_sumcheck(w, proof);
   out.proof = std::move(w.b);
   return out;
 }

@@ -350,7 +350,8 @@ void sample_generators(const std::string& label, size_t count, uint64_t* out_aff
 
 // dense polynomials of a caller (prover.cu): PolyCommitmentGens, DensePolynomial::{new, commit, evaluate},
 // PolyEvalProof::prove.  On a sharded context the calls are collective: every rank calls them with the same arguments
-// and gets the same results.  The sumchecks and grand products below are single-GPU only.
+// and gets the same results.  cubic_prove is collective too; the other sumchecks and the grand products below are
+// single-GPU only.
 static constexpr size_t kPolyMaxLen = (size_t)1 << 28;
 inline size_t poly_R(size_t num_vars) { return (size_t)1 << (num_vars - num_vars / 2); }
 // a polynomial of num_vars variables can be held on `world` ranks: every rank has at least one column of every row,
@@ -403,6 +404,16 @@ SumcheckOut sumcheck_prove(Ctx*, const Comb& g, const Poly* const* polys, int k,
 // Q(x) = g(polys[0](x), .., polys[k-1](x)) at every point, k == g.n_inputs, all of one num_vars (the caller checks): a
 // full-width polynomial like poly_create_eq
 Poly* poly_create_comb(Ctx*, const Comb& g, const Poly* const* polys, int k);
+struct CubicOut {
+  std::vector<uint8_t> proof;  // ark-serialize (compressed) SumcheckInstanceProof
+  std::vector<fr_t> r, finals;  // finals: A_0(..), .., A_{n-1}, B_0, .., B_{n-1}, C at (r || 0..0)
+};
+// SumcheckInstanceProof::prove_cubic_batched (sumcheck.rs:26-135) of claim = sum_x C(x) sum_k coeffs[k] A[k](x) B[k](x)
+// over 1 <= n <= 32 pairs and C, all of one num_vars, 1 <= num_rounds <= num_vars (the caller checks).  The polynomials
+// are not modified: the first bind writes a workspace, allocated before the transcript is touched.  Collective on a
+// sharded context.
+CubicOut cubic_prove(Ctx*, const Poly* const* A, const Poly* const* B, int n, const Poly& C,
+                     const std::vector<fr_t>& coeffs, const fr_t& claim, size_t num_rounds, Transcript&);
 
 // grand products over a caller's polynomials (single GPU)
 // GrandProductCircuit::new (grand_product.rs:38-58) with p as layer 0 (p.nv >= 1; p is only read and must outlive the

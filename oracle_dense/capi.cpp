@@ -372,6 +372,43 @@ int orcd_sumcheck_verify(const uint8_t* bytes, size_t n, const uint64_t* claim, 
   for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
   return 0;
 }
+// SumcheckInstanceProof::prove_cubic_batched (sumcheck.rs:26-135) on copies of n pairs (A, B: n x len elements each,
+// row-major) and C, with the caller's claim and coefficients, on a caller's transcript.  out: the serialised proof
+// (returns its length, 0 on error); r_out: num_rounds challenges; finals_out: A_0.., B_0.., C after the binds (2n + 1).
+size_t orcd_cubic_prove(const uint64_t* A, const uint64_t* B, size_t n, const uint64_t* Cz, size_t len, const uint64_t* coeffs,
+                        const uint64_t* claim, size_t num_rounds, void* transcript, uint8_t* out, size_t cap, uint64_t* r_out,
+                        uint64_t* finals_out) {
+  try {
+    std::vector<DensePolynomial> pa, pb;
+    for (size_t k = 0; k < n; k++) {
+      pa.emplace_back(ldvec(A + 4 * len * k, len));
+      pb.emplace_back(ldvec(B + 4 * len * k, len));
+    }
+    DensePolynomial pc(ldvec(Cz, len));
+    std::vector<DensePolynomial*> va, vb;
+    for (size_t k = 0; k < n; k++) {
+      va.push_back(&pa[k]);
+      vb.push_back(&pb[k]);
+    }
+    std::vector<Fr> r, fa, fb;
+    Fr fc;
+    SumcheckInstanceProof proof = SumcheckInstanceProof::prove_cubic_batched(
+        ldfr(claim), num_rounds, va, vb, pc, ldvec(coeffs, n), *(Transcript*)transcript, r, fa, fb, fc);
+    std::vector<uint8_t> b = ser_sumcheck(proof);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+    for (size_t k = 0; k < n; k++) {
+      stfr(finals_out + 4 * k, fa[k]);
+      stfr(finals_out + 4 * (n + k), fb[k]);
+    }
+    stfr(finals_out + 8 * n, fc);
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_cubic_prove: %s\n", e.what());
+    return 0;
+  }
+}
 // out[i] = g(polys[0][i], .., polys[k-1][i]) (k x len Montgomery elements, row-major), the program interpreted on the host
 void orcd_comb_map(const uint64_t* polys, size_t k, size_t len, const int32_t* prog, size_t n_ops, const uint64_t* K, size_t n_k,
                    uint64_t* out) {
