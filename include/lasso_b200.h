@@ -353,6 +353,44 @@ int lasso_poly_eval_prove_hiding(lasso_ctx*, const lasso_poly*, const lasso_poly
  * variable: 2^r_len evaluations, r_len <= 28 (LASSO_ERR_LENGTH), each coordinate a canonical residue (LASSO_ERR_VALUE). */
 int lasso_poly_create_eq(lasso_ctx*, const uint64_t* r, size_t r_len, lasso_poly** out);
 
+/* ---------------------------------------------------------------- deriving polynomials and reading them back
+ *
+ * None of these calls modifies its input.  Each result is a new polynomial with storage of its own (a grand-product
+ * circuit may hold the input as its layer 0), to be destroyed with lasso_poly_destroy.  Collective on a sharded context
+ * like every lasso_poly_* call: every rank passes the same arguments and gets the single-GPU result.  Every error is
+ * returned before any launch, exchange or allocation: LASSO_ERR_LENGTH for a null pointer, k outside 1..num_vars, a
+ * result that a sharded context cannot hold (2^(nv - nv/2) >= G for the result's nv), cap too small, or more than 2^28
+ * evaluations after padding; LASSO_ERR_VALUE for a coordinate of r or an evaluation that is not a canonical residue
+ * (an evaluation is found by the ingest pass, as in lasso_poly_create); LASSO_ERR_STRATEGY for a polynomial of another
+ * context; LASSO_ERR_POINTER for device memory of another GPU.
+ *
+ * lasso_poly_bind_top: k calls of DensePolynomial::bound_poly_var_top (poly/dense_mlpoly.rs:209-216), r[0] first:
+ * P(r_0, .., r_{k-1}, x), num_vars - k variables.  Up to 8 variables per pass over the data (the first pass reads the
+ * 4-byte integer form of a polynomial whose values are below 2^32), so a sumcheck stopped after k rounds continues on
+ * the result without a host round trip.
+ * lasso_poly_bind_bot: k calls of bound_poly_var_bot (:218-225) in the order given, r[0] binding the lowest variable:
+ * P(x, r_{k-1}, .., r_0).  The reference's own callers pass their challenges last first (subtables/mod.rs:256): to get
+ * their result, pass r reversed.
+ * Both results are full width: committed through the Fr windows, like lasso_poly_create_eq.
+ * lasso_poly_split: split(idx) (:101-107): lo = Z[0..idx), hi = Z[idx..2 idx); idx a power of two with 2 idx <= len.
+ * Both keep the parent's width (the 16-bit commitment path when its values are below 2^32).
+ * lasso_poly_create_padded[_device]: DensePolynomial::new_padded (:75-87): len evaluations of any length (the forms and
+ * rules of lasso_poly_create / lasso_poly_create_device), zero-padded up to the next power of two.  As in the
+ * reference, whose utils::is_power_of_two(0) is false, len = 0 gives the polynomial of one zero evaluation (num_vars 0).
+ * lasso_poly_read: the 2^num_vars evaluations in natural order, 4 Montgomery limbs each (the layout lasso_poly_create
+ * takes), into out, which has room for cap of them.  lasso_poly_read_device writes them into DEVICE memory of the
+ * context's GPU, row i at dst + i * row_stride (row_stride in u64, >= 4), as a copy on `stream` (NULL = the legacy
+ * default stream) ordered after the library's work on the polynomial.  Sharded: every rank receives the whole
+ * polynomial. */
+int lasso_poly_bind_top(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t k, lasso_poly** out);
+int lasso_poly_bind_bot(lasso_ctx*, const lasso_poly*, const uint64_t* r, size_t k, lasso_poly** out);
+int lasso_poly_split(lasso_ctx*, const lasso_poly*, size_t idx, lasso_poly** lo_out, lasso_poly** hi_out);
+int lasso_poly_create_padded(lasso_ctx*, const uint64_t* Z, size_t len, lasso_poly** out);
+int lasso_poly_create_padded_device(lasso_ctx*, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
+                                    lasso_poly** out);
+int lasso_poly_read(lasso_ctx*, const lasso_poly*, uint64_t* out, size_t cap);
+int lasso_poly_read_device(lasso_ctx*, const lasso_poly*, uint64_t* dst, size_t row_stride, void* stream);
+
 /* ---------------------------------------------------------------- lookups inside a caller's protocol
  *
  * SparsePolynomialEvaluationProof::prove (lasso/surge.rs:118-211) on the caller's transcript and tape, both advanced in

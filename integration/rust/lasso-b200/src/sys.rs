@@ -133,6 +133,19 @@ extern "C" {
                                  random_tape: *mut lasso_random_tape, proof_out: *mut u8, proof_cap: usize,
                                  proof_len: *mut usize, c_zr_out: *mut u8) -> c_int;
     pub fn lasso_poly_create_eq(ctx: *mut lasso_ctx, r: *const u64, r_len: usize, out: *mut *mut lasso_poly) -> c_int;
+    // deriving polynomials and reading them back (raw declarations only; not compiled: no cargo was available)
+    pub fn lasso_poly_bind_top(ctx: *mut lasso_ctx, p: *const lasso_poly, r: *const u64, k: usize,
+                               out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_bind_bot(ctx: *mut lasso_ctx, p: *const lasso_poly, r: *const u64, k: usize,
+                               out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_split(ctx: *mut lasso_ctx, p: *const lasso_poly, idx: usize, lo_out: *mut *mut lasso_poly,
+                            hi_out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_create_padded(ctx: *mut lasso_ctx, z: *const u64, len: usize, out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_create_padded_device(ctx: *mut lasso_ctx, z: *const u64, len: usize, row_stride: usize,
+                                           stream: *mut c_void, out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_poly_read(ctx: *mut lasso_ctx, p: *const lasso_poly, out: *mut u64, cap: usize) -> c_int;
+    pub fn lasso_poly_read_device(ctx: *mut lasso_ctx, p: *const lasso_poly, dst: *mut u64, row_stride: usize,
+                                  stream: *mut c_void) -> c_int;
     // many polynomials per call (raw declarations only; not compiled: no cargo was available)
     pub fn lasso_poly_create_merge(ctx: *mut lasso_ctx, polys: *const *const lasso_poly, n_polys: usize,
                                    out: *mut *mut lasso_poly) -> c_int;

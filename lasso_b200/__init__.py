@@ -16,6 +16,9 @@ and, for a caller that composes Lasso into a larger protocol, its own dense poly
     DensePolynomial.eq(ctx, r)                                           src/poly/eq_poly.rs:21
     DensePolynomial.merge(ctx, polys)                                    src/poly/dense_mlpoly.rs:251
     DensePolynomial.evaluate_batch(ctx, polys, r)                        (DensePolynomial::evaluate of many, one eq table)
+    DensePolynomial.new_padded(ctx, Z), .split(idx)                      src/poly/dense_mlpoly.rs:75, 101
+    p.bound_top(r) / .bound_bot(r): new polynomials, p unchanged         src/poly/dense_mlpoly.rs:209, 218
+    p.to_numpy() / .to_tensor() / .copy_to(tensor)                       (the evaluations Z, read back)
     CombinedTableEvalProof.prove(ctx, combined, evals, r, gens, transcript, random_tape)   src/subtables/mod.rs:284
     SumcheckInstanceProof.prove_arbitrary(ctx, polys, Comb(fn, k), transcript)   src/subprotocols/sumcheck.rs:149
     DensePolynomial.from_comb(ctx, comb, polys)                          (pointwise g(P_0, .., P_{k-1}))

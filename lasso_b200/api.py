@@ -847,8 +847,10 @@ class DensePolynomial:
     stride) read in the order of torch's current stream.  The library keeps its own copy.
     On a sharded context (Context.init_comm) creating, committing, evaluating and opening are collective: every rank
     passes the WHOLE polynomial (of the same kind, host or CUDA on its own GPU) and the same arguments, keeps only its
-    low-bit shard, and gets the single-GPU bytes and values.  There a polynomial needs 2^(num_vars - num_vars // 2) >= G
-    (LASSO_ERR_LENGTH otherwise); sumchecks, grand products and DensifiedRepresentation.outputs stay single-GPU."""
+    low-bit shard, and gets the single-GPU bytes and values.  The same holds for prove_cubic_batched and for deriving and
+    reading back polynomials (bound_top, bound_bot, split, new_padded, to_numpy, to_tensor, copy_to).  There a
+    polynomial needs 2^(num_vars - num_vars // 2) >= G (LASSO_ERR_LENGTH otherwise); prove_arbitrary, grand products and
+    DensifiedRepresentation.outputs stay single-GPU."""
 
     def __init__(self, ctx, Z):
         kind, src, row_stride = _poly_source(Z)
@@ -935,6 +937,75 @@ class DensePolynomial:
         out = np.zeros(4, dtype=np.uint64)
         _chk(lib().lasso_poly_evaluate(self.ctx._h, self._h, _p(r), C.c_size_t(r.shape[0]), _p(out)))
         return out
+
+    @classmethod
+    def new_padded(cls, ctx, Z):
+        """DensePolynomial::new_padded (src/poly/dense_mlpoly.rs:75-87): Z of any length (the forms __init__ takes),
+        zero-padded up to the next power of two; an empty Z gives the polynomial of one zero evaluation"""
+        kind, src, row_stride = _poly_source(Z)
+        h = C.c_void_p()
+        if kind == "device":
+            torch = sys.modules["torch"]
+            stream = torch.cuda.current_stream(src.device).cuda_stream
+            _chk(lib().lasso_poly_create_padded_device(ctx._h, C.c_void_p(src.data_ptr()), C.c_size_t(src.shape[0]),
+                                                       C.c_size_t(row_stride), C.c_void_p(stream), C.byref(h)))
+        else:
+            _chk(lib().lasso_poly_create_padded(ctx._h, _p(src), C.c_size_t(src.shape[0]), C.byref(h)))
+        return cls._wrap(ctx, h)
+
+    def _bound(self, fn, r):
+        r = _limbs(np.asarray(r).reshape(-1, 4), what="r")
+        h = C.c_void_p()
+        _chk(fn(self.ctx._h, self._h, _p(r), C.c_size_t(r.shape[0]), C.byref(h)))
+        return DensePolynomial._wrap(self.ctx, h)
+
+    def bound_top(self, r):
+        """bound_poly_var_top (dense_mlpoly.rs:209-216) with r[0], r[1], .. in turn, r a (k, 4) or (4,) array: a NEW
+        polynomial P(r_0, .., r_{k-1}, x); self is unchanged (the reference binds in place)"""
+        return self._bound(lib().lasso_poly_bind_top, r)
+
+    def bound_bot(self, r):
+        """bound_poly_var_bot (dense_mlpoly.rs:218-225) with r[0], r[1], .. in turn, r[0] binding the lowest variable:
+        a NEW polynomial P(x, r_{k-1}, .., r_0); self is unchanged.  Callers of the reference that bind their challenges
+        last first (subtables/mod.rs:256) pass r[::-1]."""
+        return self._bound(lib().lasso_poly_bind_bot, r)
+
+    def split(self, idx=None):
+        """split(idx) (dense_mlpoly.rs:101-107) -> (Z[:idx], Z[idx:2 idx]) as new polynomials; idx a power of two with
+        2 idx <= len, None for len / 2"""
+        idx = (1 << self.num_vars) // 2 if idx is None else int(idx)
+        lo, hi = C.c_void_p(), C.c_void_p()
+        _chk(lib().lasso_poly_split(self.ctx._h, self._h, C.c_size_t(idx), C.byref(lo), C.byref(hi)))
+        return DensePolynomial._wrap(self.ctx, lo), DensePolynomial._wrap(self.ctx, hi)
+
+    def to_numpy(self):
+        """the 2^num_vars evaluations as an (n, 4) uint64 array of Montgomery limbs (the layout __init__ takes)"""
+        out = np.zeros((1 << self.num_vars, 4), dtype=np.uint64)
+        _chk(lib().lasso_poly_read(self.ctx._h, self._h, _p(out), C.c_size_t(out.shape[0])))
+        return out
+
+    def copy_to(self, tensor):
+        """writes the evaluations into an (n, 4) int64 / uint64 CUDA tensor on ctx's GPU (limbs contiguous, any row
+        stride), in the order of torch's current stream; returns the tensor"""
+        kind, dst, row_stride = _poly_source(tensor)
+        if kind != "device":
+            raise LassoError(LASSO_ERR_POINTER, "copy_to takes a CUDA tensor")
+        if dst.shape[0] != 1 << self.num_vars:
+            raise LassoError(LASSO_ERR_LENGTH, "copy_to: the tensor has %d rows, the polynomial %d evaluations"
+                             % (dst.shape[0], 1 << self.num_vars))
+        torch = sys.modules["torch"]
+        stream = torch.cuda.current_stream(dst.device).cuda_stream
+        _chk(lib().lasso_poly_read_device(self.ctx._h, self._h, C.c_void_p(dst.data_ptr()), C.c_size_t(row_stride),
+                                          C.c_void_p(stream)))
+        return tensor
+
+    def to_tensor(self, device=None):
+        """the evaluations as a new (n, 4) int64 CUDA tensor (default: torch's current device), written in the order
+        of torch's current stream"""
+        import torch
+
+        t = torch.empty((1 << self.num_vars, 4), dtype=torch.int64, device=device if device is not None else "cuda")
+        return self.copy_to(t)
 
     def __del__(self):
         try:

@@ -1209,6 +1209,88 @@ int lasso_poly_create_eq(lasso_ctx* h, const uint64_t* r, size_t r_len, lasso_po
   LB_CATCH
 }
 
+// ---- transforms of a caller's polynomial: binds, split, padding, read-back
+static int poly_bind(lasso_ctx* h, const lasso_poly* p, const uint64_t* r, size_t k, lasso_poly** out, bool top) {
+  if (out) *out = nullptr;
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  if (!out || !r) return fail(LASSO_ERR_LENGTH, "poly bind: null point or output");
+  if (k < 1 || k > p->p->nv) return fail(LASSO_ERR_LENGTH, "poly bind: k must be in 1..num_vars");
+  if (const int rc = poly_size_check(h, p->p->nv - k)) return rc;
+  std::vector<fr_t> rv;
+  if (!load_scalars(r, k, rv)) return fail(LASSO_ERR_VALUE, "poly bind: a coordinate of r is not a canonical residue");
+  *out = new lasso_poly{top ? poly_bind_top(h->c, *p->p, rv) : poly_bind_bot(h->c, *p->p, rv)};
+  return 0;
+}
+int lasso_poly_bind_top(lasso_ctx* h, const lasso_poly* p, const uint64_t* r, size_t k, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_bind(h, p, r, k, out, true);
+  LB_CATCH
+}
+int lasso_poly_bind_bot(lasso_ctx* h, const lasso_poly* p, const uint64_t* r, size_t k, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_bind(h, p, r, k, out, false);
+  LB_CATCH
+}
+int lasso_poly_split(lasso_ctx* h, const lasso_poly* p, size_t idx, lasso_poly** lo_out, lasso_poly** hi_out) {
+  LB_TRY_CTX(h)
+  if (lo_out) *lo_out = nullptr;
+  if (hi_out) *hi_out = nullptr;
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  if (!lo_out || !hi_out) return fail(LASSO_ERR_LENGTH, "poly split: null output");
+  if (!is_pow2(idx) || idx > p->p->len / 2) return fail(LASSO_ERR_LENGTH, "poly split: idx must be a power of two, 2 idx <= len");
+  if (const int rc = poly_size_check(h, log2_exact_or_ceil(idx))) return rc;
+  Poly *lo = nullptr, *hi = nullptr;
+  poly_split(h->c, *p->p, idx, &lo, &hi);
+  *lo_out = new lasso_poly{lo};
+  *hi_out = new lasso_poly{hi};
+  return 0;
+  LB_CATCH
+}
+static int poly_new_padded(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, bool device, void* stream,
+                           lasso_poly** out) {
+  if (out) *out = nullptr;
+  if (!out || (len && !Z)) return fail(LASSO_ERR_LENGTH, "poly padded: null evaluations or output");
+  if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly padded: at most 2^28 evaluations after padding");
+  const size_t full = next_pow2(std::max<size_t>(len, 1));
+  if (const int rc = poly_size_check(h, log2_exact_or_ceil(full))) return rc;
+  if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly padded: row_stride must be at least 4 u64");
+  int err = 0;
+  Poly* p = poly_create(h->c, Z, len, row_stride, device, static_cast<cudaStream_t>(stream), &err);
+  if (err == 7) return fail(LASSO_ERR_POINTER, "poly padded: the evaluations are not device memory of the context's GPU");
+  if (err == 8) return fail(LASSO_ERR_VALUE, "poly padded: an evaluation is not a canonical Montgomery residue");
+  *out = new lasso_poly{p};
+  return 0;
+}
+int lasso_poly_create_padded(lasso_ctx* h, const uint64_t* Z, size_t len, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_new_padded(h, Z, len, 4, false, nullptr, out);
+  LB_CATCH
+}
+int lasso_poly_create_padded_device(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
+                                    lasso_poly** out) {
+  LB_TRY_CTX(h)
+  return poly_new_padded(h, Z, len, row_stride, true, stream, out);
+  LB_CATCH
+}
+int lasso_poly_read(lasso_ctx* h, const lasso_poly* p, uint64_t* out, size_t cap) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  if (!out || cap < p->p->len) return fail(LASSO_ERR_LENGTH, "poly read: room for fewer evaluations than the polynomial has");
+  poly_read(h->c, *p->p, out);
+  return 0;
+  LB_CATCH
+}
+int lasso_poly_read_device(lasso_ctx* h, const lasso_poly* p, uint64_t* dst, size_t row_stride, void* stream) {
+  LB_TRY_CTX(h)
+  if (const int rc = poly_use_check(h, p, nullptr)) return rc;
+  if (!dst) return fail(LASSO_ERR_LENGTH, "poly read: null destination");
+  if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly read: row_stride must be at least 4 u64");
+  if (poly_read_device(h->c, *p->p, dst, row_stride, static_cast<cudaStream_t>(stream)) == 7)
+    return fail(LASSO_ERR_POINTER, "poly read: the destination is not device memory of the context's GPU");
+  return 0;
+  LB_CATCH
+}
+
 // ---- many polynomials per call: merge, batched evaluation, one combined opening
 int lasso_poly_create_merge(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out) {
   LB_TRY_CTX(h)

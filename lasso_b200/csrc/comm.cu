@@ -369,6 +369,70 @@ void comm_allgather(Ctx* c, const void* d_send, void* d_recv, size_t bytes_per_r
   }
 }
 
+// The scatter form of xchg_push_kernel: elements [off, off + n_per) of the columns owned by peer p (vec[j G + p]) go to
+// slot `rank` of peer p's exchange buffer only, so each rank sends (G - 1) / G of its vector instead of G times it.
+__global__ void __launch_bounds__(256) xchg_scatter_kernel(const fr_t* vec, size_t off, size_t n_per, PeerPtrs peers, int world,
+                                                           unsigned* counter, PubDst marker, uint32_t seq) {
+  const size_t n = n_per * world;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const size_t p = i / n_per, j = i - p * n_per;
+    st_fr(reinterpret_cast<fr_t*>(peers.p[p]) + j, ld_fr(vec + (off + j) * world + p));
+  }
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    __threadfence_system();
+    if (atomicAdd(counter, 1u) == gridDim.x - 1) {
+      *counter = 0;
+      __threadfence_system();
+      uint32_t one[8] = {seq, 0, 0, 0, 0, 0, 0, 0};
+      pub_store(marker, 0, one);
+    }
+  }
+}
+// out[j] = sum_w src[w * wstride + j * estride], j < n
+__global__ void __launch_bounds__(256) sum_columns_kernel(const fr_t* src, size_t wstride, size_t estride, int world, size_t n,
+                                                          fr_t* out) {
+  for (size_t j = (size_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (size_t)gridDim.x * blockDim.x) {
+    fr_t acc = ld_fr(src + j * estride);
+    for (int w = 1; w < world; w++) acc = fr_add(acc, ld_fr(src + (size_t)w * wstride + j * estride));
+    st_fr(out + j, acc);
+  }
+}
+static unsigned grid_256(size_t n) { return (unsigned)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, 4 * (size_t)kNumSMs)); }
+// every rank holds a vector of m elements (m a multiple of G); d_out (m / G elements) <- this rank's low-bit shard of
+// the sum of the G vectors: d_out[j] = sum_g vec_g[j G + rank].  One scatter per 64K output elements and an add;
+// LASSO_B200_XCHG=nccl: an all-gather of the whole vectors and the same add.
+void comm_sum_shard(Ctx* c, const fr_t* d_vec, size_t m, fr_t* d_out) {
+  const size_t G = (size_t)c->world, n_out = m / G;
+  if (G == 1) {
+    LB_CUDA_CHECK(cudaMemcpyAsync(d_out, d_vec, m * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+    return;
+  }
+  Xchg* x = xc(c);
+  if (x->nccl_comm) {
+    DBuf<fr_t> all(c, m * G);
+    comm_allgather(c, d_vec, all.p, m * sizeof(fr_t));
+    launch(sum_columns_kernel, grid_256(n_out), 256, 0, c->st, all.p + c->rank, m, G, c->world, n_out, d_out);
+    return;
+  }
+  const size_t slot = kXchgSlotBytes / sizeof(fr_t);
+  for (size_t off = 0; off < n_out; off += slot) {
+    const size_t chunk = std::min(slot, n_out - off);
+    const uint32_t seq = ++x->xseq;
+    const size_t par = seq & 1;
+    PeerPtrs peers;
+    for (int r = 0; r < c->world; r++) peers.p[r] = (uint4*)(x->xbuf[r] + (par * kPubMaxReaders + c->rank) * kXchgSlotBytes);
+    const PubDst marker = c->pub_begin(true);
+    launch(xchg_scatter_kernel, std::min<unsigned>(grid_256(chunk * G), kNumSMs), 256, 0, c->st, d_vec, off, chunk, peers,
+           c->world, c->d_flag + 8, marker, seq);
+    uint32_t got[8];
+    for (int w = 0; w < c->world; w++) c->pub_wait_raw(marker, w, 1, got);  // every rank's columns have landed here
+    const fr_t* recv = reinterpret_cast<const fr_t*>(x->xbuf[c->rank] + par * kPubMaxReaders * kXchgSlotBytes);
+    launch(sum_columns_kernel, grid_256(chunk), 256, 0, c->st, recv, slot, (size_t)1, c->world, chunk, d_out + off);
+  }
+}
+
 // tail hand-over: every rank holds ONE element of each of npolys polynomials (local length 1), optionally one
 // more (`extra`, the shared eq polynomial of a grand-product layer) as polynomial number npolys;
 // afterwards out[k*G + g] = rank g's element of polynomial k, on every rank (global index = g).

@@ -112,6 +112,37 @@ __device__ __forceinline__ void block_sum_fr(fr_t (&v)[NV], fr_t* scratch) {
   __syncthreads();
 }
 
+// A sum of products (Montgomery field element) x (32-bit integer) carried as a plain 320-bit integer and reduced once
+// (poly_kernels.cu K7, dense_poly_kernels.cu): an element stored as a*R mod l times z sums to the Montgomery form of
+// sum a z.
+struct wide_t {
+  uint32_t v[10];
+};
+__device__ __forceinline__ void wide_zero(wide_t& a) {
+#pragma unroll
+  for (int l = 0; l < 10; l++) a.v[l] = 0;
+}
+__device__ __forceinline__ void wide_mad(wide_t& acc, const fr_t& a, uint32_t z) {  // acc += a * z
+  uint64_t carry = 0;
+#pragma unroll
+  for (int l = 0; l < 8; l++) {
+    const uint64_t t = (uint64_t)a.v[l] * z + acc.v[l] + carry;
+    acc.v[l] = (uint32_t)t;
+    carry = t >> 32;
+  }
+  const uint64_t t = (uint64_t)acc.v[8] + carry;
+  acc.v[8] = (uint32_t)t;
+  acc.v[9] += (uint32_t)(t >> 32);
+}
+// X mod l for X < 2^320, as a field element: X = X_lo + 2^256 * X_hi;  X_lo mod l through two Montgomery products
+// (x -> x*R -> x), X_hi * 2^256 mod l = the Montgomery form of the 64-bit integer X_hi
+__device__ __forceinline__ fr_t wide_reduce(const wide_t& a) {
+  fr_t lo;
+#pragma unroll
+  for (int l = 0; l < 8; l++) lo.v[l] = a.v[l];
+  const fr_t lo_mod = fr_to_canonical(fr_from_raw_int(lo));
+  return fr_add(lo_mod, fr_from_u64((uint64_t)a.v[8] | ((uint64_t)a.v[9] << 32)));
+}
 // ---- single-launch reduction + publication of a round message ---------------------------------------------
 // Every CTA stores its partial sums, takes a ticket, and the LAST CTA to finish adds the partials of all
 // values and writes the results straight into mapped pinned host memory the host is spinning on.  One kernel per sumcheck round instead of eval + reduce + copy: the rounds of the

@@ -239,6 +239,22 @@ void launch_scale(const fr_t* in, fr_t* out, size_t n, const fr_t& k, cudaStream
 void launch_poly_ingest(const uint64_t* src, size_t row_stride, size_t n, fr_t* dst, unsigned* flags, cudaStream_t st);
 // out[i] <- the integer value of in[i] (every value below 2^32)
 void launch_poly_mirror_u32(const fr_t* in, size_t n, uint32_t* out, cudaStream_t st);
+// One pass of a multi-variable bind: t <= kBindPassVars variables with the weights scale * eq(r, b), r[0] on the most
+// significant bit of b (omr[j] = 1 - r[j]).  t == 0 (bottom only) scales.
+static constexpr int kBindPassVars = 8;
+struct BindPass {
+  int t;
+  fr_t scale;
+  fr_t r[kBindPassVars], omr[kBindPassVars];
+};
+// out[i] = sum_b w[b] P[b (n >> t) + i] for i < n >> t: P the Montgomery form (in_u32 null) or the u32 mirror
+void launch_bind_top_multi(const fr_t* in_fr, const uint32_t* in_u32, size_t n, const BindPass& pt, fr_t* out,
+                           cudaStream_t st);
+// out[i] = sum_b w[b] P[i 2^t + b] for i < n >> t
+void launch_bind_bot_multi(const fr_t* in, size_t n, const BindPass& pt, fr_t* out, cudaStream_t st);
+// out[j] = j % period == phase ? weight * in[j / period] : 0 for j < m (a sharded bottom bind of fewer than lg G variables)
+void launch_bind_bot_spread(const fr_t* in, size_t m, size_t period, size_t phase, const fr_t& weight, fr_t* out,
+                            cudaStream_t st);
 
 // ---- densify on the GPU (densify_kernels.cu; densified.rs:33-56): stable LSD radix sort by address ----
 void densify_init_device();

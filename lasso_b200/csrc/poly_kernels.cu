@@ -1193,34 +1193,7 @@ void launch_fill_zero(fr_t* out, size_t n, cudaStream_t st) {
 // times a 32-bit integer is 8 IMAD.WIDE instead of a ~235-instruction Montgomery product, and the sum can be carried
 // as a plain 320-bit integer (X = sum_j L_j * z_j < 2^288 * #terms) and reduced ONCE: L_j is stored as L_j*R mod l, so
 // X mod l is already the Montgomery form of the result.  Reads 4 B per element instead of 32 B.
-struct wide_t {
-  uint32_t v[10];
-};
-__device__ __forceinline__ void wide_zero(wide_t& a) {
-#pragma unroll
-  for (int l = 0; l < 10; l++) a.v[l] = 0;
-}
-__device__ __forceinline__ void wide_mad(wide_t& acc, const fr_t& a, uint32_t z) {  // acc += a * z
-  uint64_t carry = 0;
-#pragma unroll
-  for (int l = 0; l < 8; l++) {
-    const uint64_t t = (uint64_t)a.v[l] * z + acc.v[l] + carry;
-    acc.v[l] = (uint32_t)t;
-    carry = t >> 32;
-  }
-  const uint64_t t = (uint64_t)acc.v[8] + carry;
-  acc.v[8] = (uint32_t)t;
-  acc.v[9] += (uint32_t)(t >> 32);
-}
-// X mod l for X < 2^320, as a field element: X = X_lo + 2^256 * X_hi;  X_lo mod l through two Montgomery products
-// (x -> x*R -> x), X_hi * 2^256 mod l = the Montgomery form of the 64-bit integer X_hi
-__device__ __forceinline__ fr_t wide_reduce(const wide_t& a) {
-  fr_t lo;
-#pragma unroll
-  for (int l = 0; l < 8; l++) lo.v[l] = a.v[l];
-  const fr_t lo_mod = fr_to_canonical(fr_from_raw_int(lo));
-  return fr_add(lo_mod, fr_from_u64((uint64_t)a.v[8] | ((uint64_t)a.v[9] << 32)));
-}
+// wide_t, wide_mad, wide_reduce: common.cuh
 // LZ[i] = sum_j L[j] z[j*R + i]: thread = column (coalesced across the warp), rows split into chunks over blockIdx.y
 // (<= 2^20 rows per chunk), a second pass sums the chunk partials
 static constexpr int kBoundChunks = 64;

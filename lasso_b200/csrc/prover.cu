@@ -1851,9 +1851,17 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
 }
 
 // ---------------------------------------------------------------------------------------------- dense polynomials
+// the first and the last of `rows` rows of 4 u64, row_stride u64 apart, lie in device memory of the context's GPU
+static bool rows_on_device(const Ctx* c, const uint64_t* Z, size_t rows, size_t row_stride) {
+  size_t last = 0;
+  const bool wraps = __builtin_mul_overflow(rows - 1, row_stride, &last) || __builtin_add_overflow(last, (size_t)3, &last) ||
+                     __builtin_mul_overflow(last, sizeof(uint64_t), &last) || (uintptr_t)Z > UINTPTR_MAX - last;
+  return Z && !wraps && device_memory_of(c, Z) && device_memory_of(c, (const char*)Z + last);
+}
 // DensePolynomial::new (dense_mlpoly.rs:62-71) from the caller's evaluations.  Both sources go through the same ingest
-// kernel: host rows are first uploaded into the polynomial's own buffer and checked there in place.  The caller checks
-// len (a power of two, at most 2^28, poly_fits) and row_stride (>= 4).
+// kernel: host rows are first uploaded into the polynomial's own buffer and checked there in place.  A len that is not a
+// power of two is zero-padded up to the next one (new_padded; len 0 gives one zero).  The caller checks the padded
+// length (at most 2^28, poly_fits) and row_stride (>= 4).
 // Sharded: every rank is given the whole polynomial and reads only its rows i*G + rank.  Host rows are staged into pinned
 // memory and uploaded in one copy (1/G of the PCIe bytes); device rows are read by the ingest kernel at base rank and
 // stride G rows.  The verdict and the widest value are then agreed in one message to every process, so that every rank
@@ -1862,22 +1870,19 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
   SpanTimer sp(c, "DensePolynomial.new");
   *err = 0;
   const size_t G = (size_t)c->world, gr = (size_t)c->rank;
-  if (device) {  // the first and the last row must both lie in device memory of this GPU
-    size_t last = 0;
-    const bool wraps = __builtin_mul_overflow(len - 1, row_stride, &last) || __builtin_add_overflow(last, (size_t)3, &last) ||
-                       __builtin_mul_overflow(last, sizeof(uint64_t), &last) || (uintptr_t)Z > UINTPTR_MAX - last;
-    if (!Z || wraps || !device_memory_of(c, Z) || !device_memory_of(c, (const char*)Z + last)) {
-      *err = 7;
-      return nullptr;
-    }
+  if (device && len && !rows_on_device(c, Z, len, row_stride)) {
+    *err = 7;
+    return nullptr;
   }
   std::unique_ptr<Poly> p(new Poly());
   p->ctx = c;
-  p->len = len;
-  p->len_loc = loc(c, len);
-  p->nv = log2_exact_or_ceil(len);
+  p->len = next_pow2(std::max<size_t>(len, 1));  // new_padded (dense_mlpoly.rs:75-87): len itself when a power of two
+  p->len_loc = loc(c, p->len);
+  p->nv = log2_exact_or_ceil(p->len);
   const size_t n = p->len_loc;
+  const size_t own = len > gr ? (len - gr + G - 1) / G : 0;  // this rank's given rows i*G + rank < len; the rest is padding
   p->d_fr.alloc(c, n);
+  if (own < n) LB_CUDA_CHECK(cudaMemsetAsync(p->d_fr.p + own, 0, (n - own) * sizeof(fr_t), c->st));
   DBuf<unsigned> flags(c, 2);
   LB_CUDA_CHECK(cudaMemsetAsync(flags.p, 0, 2 * sizeof(unsigned), c->st));
   if (device) {
@@ -1885,23 +1890,23 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
     // work on `caller` (a caching allocator freeing the tensor, say) comes after the last read of them
     LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
     LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
-    launch_poly_ingest(Z + gr * row_stride, G * row_stride, n, p->d_fr.p, flags.p, c->st);
+    launch_poly_ingest(Z + gr * row_stride, G * row_stride, own, p->d_fr.p, flags.p, c->st);
     LB_CUDA_CHECK(cudaEventRecord(c->ev_aux, c->st));
     LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
   } else if (G == 1) {
-    LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, Z, len * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+    if (len) LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, Z, len * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
     launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, len, p->d_fr.p, flags.p, c->st);
   } else {
     if (c->stage_busy) {  // the previous call's upload may still be reading the staging buffer
       LB_CUDA_CHECK(cudaEventSynchronize(c->ev_stage));
       c->stage_busy = false;
     }
-    uint64_t* stage = reinterpret_cast<uint64_t*>(c->stage(n * 8));
-    for (size_t i = 0; i < n; i++) memcpy(stage + 4 * i, Z + 4 * (i * G + gr), 32);
-    LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, stage, n * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
+    uint64_t* stage = reinterpret_cast<uint64_t*>(c->stage(std::max<size_t>(own, 1) * 8));
+    for (size_t i = 0; i < own; i++) memcpy(stage + 4 * i, Z + 4 * (i * G + gr), 32);
+    if (own) LB_CUDA_CHECK(cudaMemcpyAsync(p->d_fr.p, stage, own * sizeof(fr_t), cudaMemcpyHostToDevice, c->st));
     LB_CUDA_CHECK(cudaEventRecord(c->ev_stage, c->st));
     c->stage_busy = true;
-    launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, n, p->d_fr.p, flags.p, c->st);
+    launch_poly_ingest(reinterpret_cast<const uint64_t*>(p->d_fr.p), 4, own, p->d_fr.p, flags.p, c->st);
   }
   unsigned f[2];
   c->d2h(f, flags.p, sizeof f);
@@ -2103,6 +2108,142 @@ std::vector<uint8_t> combined_eval_prove(Ctx* c, const Poly& p, const Gens& g, c
   ByteWriter w;
   ser_dpl(w, proof);
   return w.b;
+}
+
+// ---- transforms of a caller's polynomial (DESIGN §3.14): new polynomials with storage of their own, the input is only read
+static Poly* poly_shell(Ctx* c, size_t nv, unsigned bits) {
+  std::unique_ptr<Poly> p(new Poly());
+  p->ctx = c;
+  p->nv = nv;
+  p->len = (size_t)1 << nv;
+  p->len_loc = loc(c, p->len);
+  p->bits = bits;
+  p->d_fr.alloc(c, p->len_loc);
+  return p.release();
+}
+// the weights of one pass: r[0..t) with r[0] on the most significant bit, all times scale
+static BindPass bind_pass(const fr_t* r, int t, const fr_t& scale) {
+  BindPass b{};
+  b.t = t;
+  b.scale = scale;
+  for (int j = 0; j < t; j++) {
+    b.r[j] = r[j];
+    b.omr[j] = fr_sub(fr_one(), r[j]);
+  }
+  return b;
+}
+// bound_poly_var_top (dense_mlpoly.rs:209-216) with r[0], r[1], .. in turn: passes of up to 8 variables, each on an
+// array 256 times smaller than the one before; the first reads the u32 mirror when there is one.  Sharded: local, as
+// the pairs (i, i + n/2) of every bind have the same low bits.
+Poly* poly_bind_top(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
+  SpanTimer sp(c, "DensePolynomial.bound_top");
+  const size_t k = r.size();
+  std::unique_ptr<Poly> q(poly_shell(c, p.nv - k, 253));
+  const fr_t* in_fr = p.d_fr.p;
+  const uint32_t* in_u32 = p.d_u32.p;
+  size_t n = p.len_loc;
+  std::vector<DBuf<fr_t>> tmp;
+  for (size_t done = 0; done < k;) {
+    const int t = (int)std::min<size_t>(kBindPassVars, k - done);
+    fr_t* out = q->d_fr.p;
+    if (done + t < k) {
+      tmp.emplace_back(c, n >> t);
+      out = tmp.back().p;
+    }
+    launch_bind_top_multi(in_fr, in_u32, n, bind_pass(r.data() + done, t, fr_one()), out, c->st);
+    in_fr = out;
+    in_u32 = nullptr;
+    n >>= t;
+    done += t;
+  }
+  return q.release();
+}
+// bottom passes over r[from..to) of a local array of n elements into out (n >> (to - from) elements), the first pass
+// scaled; a pass binds the lowest variables left, r[from] the lowest.  from == to: out = scale * in.
+static void bind_bot_passes(Ctx* c, const fr_t* in, size_t n, const std::vector<fr_t>& r, size_t from, size_t to,
+                            fr_t scale, fr_t* out) {
+  std::vector<DBuf<fr_t>> tmp;
+  size_t done = from;
+  do {
+    const int t = (int)std::min<size_t>(kBindPassVars, to - done);
+    std::vector<fr_t> rev(t);  // the pass's weights take their first challenge on the most significant bit
+    for (int j = 0; j < t; j++) rev[j] = r[done + t - 1 - j];
+    fr_t* dst = out;
+    if (done + t < to) {
+      tmp.emplace_back(c, n >> t);
+      dst = tmp.back().p;
+    }
+    launch_bind_bot_multi(in, n, bind_pass(rev.data(), t, scale), dst, c->st);
+    scale = fr_one();
+    in = dst;
+    n >>= t;
+    done += t;
+  } while (done < to);
+}
+// bound_poly_var_bot (dense_mlpoly.rs:218-225) with r[0], r[1], .. in turn: r[0] binds the lowest variable.  Sharded
+// over G = 2^s ranks the lowest s index bits are the rank, so the bound variables span ranks: every rank writes its
+// partial sums for all n/2^k outputs (its s lowest challenges fold into one weight), and comm_sum_shard hands every
+// output's G partials to its owner, which adds them.
+Poly* poly_bind_bot(Ctx* c, const Poly& p, const std::vector<fr_t>& r) {
+  SpanTimer sp(c, "DensePolynomial.bound_bot");
+  const size_t k = r.size(), s = (size_t)c->lg_world, G = (size_t)c->world, g = (size_t)c->rank;
+  std::unique_ptr<Poly> q(poly_shell(c, p.nv - k, 253));
+  if (G == 1) {
+    bind_bot_passes(c, p.d_fr.p, p.len_loc, r, 0, k, fr_one(), q->d_fr.p);
+    return q.release();
+  }
+  const size_t m = p.len >> k;
+  fr_t weight = fr_one();  // eq of the rank's low bits with the challenges that bind them
+  for (size_t j = 0; j < std::min(k, s); j++) weight = fr_mul(weight, (g >> j) & 1 ? r[j] : fr_sub(fr_one(), r[j]));
+  DBuf<fr_t> partial(c, m);
+  if (k >= s)
+    bind_bot_passes(c, p.d_fr.p, p.len_loc, r, s, k, weight, partial.p);
+  else
+    launch_bind_bot_spread(p.d_fr.p, m, G >> k, g >> k, weight, partial.p, c->st);
+  comm_sum_shard(c, partial.p, m, q->d_fr.p);
+  return q.release();
+}
+// split (dense_mlpoly.rs:101-107): Z[..idx] and Z[idx..2 idx], copies of the parent's forms.  Sharded: the first idx/G and
+// the next idx/G elements of every shard.
+void poly_split(Ctx* c, const Poly& p, size_t idx, Poly** lo, Poly** hi) {
+  std::unique_ptr<Poly> h[2];
+  for (int half = 0; half < 2; half++) {
+    h[half].reset(poly_shell(c, log2_exact_or_ceil(idx), p.bits));
+    const size_t n = h[half]->len_loc;
+    LB_CUDA_CHECK(cudaMemcpyAsync(h[half]->d_fr.p, p.d_fr.p + half * n, n * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+    if (p.d_u32.p) {
+      h[half]->d_u32.alloc(c, n);
+      LB_CUDA_CHECK(cudaMemcpyAsync(h[half]->d_u32.p, p.d_u32.p + half * n, n * sizeof(uint32_t), cudaMemcpyDeviceToDevice, c->st));
+    }
+  }
+  *lo = h[0].release();
+  *hi = h[1].release();
+}
+// Z: the 2^nv evaluations in natural order on this device (sharded: gathered), in c->st order; `all` owns the gather
+static const fr_t* poly_whole(Ctx* c, const Poly& p, DBuf<fr_t>& all) {
+  if (c->world == 1) return p.d_fr.p;
+  DBuf<fr_t> scratch(c, p.len);
+  all.alloc(c, p.len);
+  comm_gather_vector(c, p.d_fr.p, p.len_loc, scratch.p, all.p);
+  return all.p;
+}
+void poly_read(Ctx* c, const Poly& p, uint64_t* out) {
+  DBuf<fr_t> all;
+  c->d2h(out, poly_whole(c, p, all), p.len * sizeof(fr_t));
+}
+int poly_read_device(Ctx* c, const Poly& p, uint64_t* dst, size_t row_stride, cudaStream_t caller) {
+  if (!rows_on_device(c, dst, p.len, row_stride)) return 7;
+  DBuf<fr_t> all;
+  const fr_t* src = poly_whole(c, p, all);
+  // the copy runs on the caller's stream after the polynomial is ready, and the library's later work (freeing the
+  // gathered copy or the polynomial) after the copy
+  LB_CUDA_CHECK(cudaEventRecord(c->ev_aux, c->st));
+  LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
+  LB_CUDA_CHECK(cudaMemcpy2DAsync(dst, row_stride * sizeof(uint64_t), src, sizeof(fr_t), sizeof(fr_t), p.len,
+                                  cudaMemcpyDeviceToDevice, caller));
+  LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
+  LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
+  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------- caller sumchecks

@@ -362,6 +362,7 @@ inline bool poly_fits(size_t num_vars, int world) { return poly_R(num_vars) >= (
 Gens* poly_gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t num_vars);
 // Z: len rows of 4 u64 Montgomery limbs, row_stride u64 apart; host memory, or device memory of the context's GPU
 // (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory.
+// Any len: zero-padded to next_pow2(max(len, 1)) evaluations (DensePolynomial::new_padded, dense_mlpoly.rs:75-87).
 // Sharded: every rank passes the whole polynomial and reads its rows; the verdict and the width are agreed by all ranks.
 Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err);
 std::vector<uint8_t> poly_commit(Ctx*, const Poly&, const Gens&);  // serialised PolyCommitment
@@ -384,6 +385,19 @@ std::vector<fr_t> poly_evaluate_batch(Ctx*, const Poly* const* polys, int k, con
 // (challenges || r); p.nv == r.size() + log2(next_pow2(evals.size())) (the caller checks)
 std::vector<uint8_t> combined_eval_prove(Ctx*, const Poly& p, const Gens& g, const std::vector<fr_t>& evals,
                                          const std::vector<fr_t>& r, Transcript&, RandomTape&);
+
+// Transforms (DESIGN §3.14): new full-width polynomials, or copies, with storage of their own; the input is only read.
+// Collective on a sharded context.  The caller checks 1 <= r.size() <= nv and poly_fits of the result.
+// bound_poly_var_top with r[0], r[1], .. in turn (dense_mlpoly.rs:209-216)
+Poly* poly_bind_top(Ctx*, const Poly&, const std::vector<fr_t>& r);
+// bound_poly_var_bot with r[0], r[1], .. in turn (dense_mlpoly.rs:218-225): r[0] binds the lowest variable
+Poly* poly_bind_bot(Ctx*, const Poly&, const std::vector<fr_t>& r);
+// split(idx) (dense_mlpoly.rs:101-107), idx a power of two, 2 idx <= len: the parent's bits and u32 mirror, halved
+void poly_split(Ctx*, const Poly&, size_t idx, Poly** lo, Poly** hi);
+// the len evaluations in natural order, 4 Montgomery limbs each: to host memory, or (poly_read_device) to device
+// memory of the context's GPU, row i at dst + i * row_stride, in the order of `caller`; 7: dst is not such memory
+void poly_read(Ctx*, const Poly&, uint64_t* out);
+int poly_read_device(Ctx*, const Poly&, uint64_t* dst, size_t row_stride, cudaStream_t caller);
 
 // A combining function g(x_0..x_{n_inputs-1}) of SumcheckInstanceProof::prove_arbitrary: a checked program (capi.cu)
 // with its slots allocated, and the declared combined_degree.  Host only.
@@ -434,6 +448,8 @@ void comm_destroy(Ctx*);
 void comm_allgather(Ctx*, const void* d_send, void* d_recv, size_t bytes_per_rank);
 // every rank holds the low-bit shard (n_loc elements) of a vector; d_out <- the whole vector (n_loc * G), on every rank
 void comm_gather_vector(Ctx*, const fr_t* d_shard, size_t n_loc, fr_t* d_scratch, fr_t* d_out);
+// every rank holds a vector of m elements (a multiple of G); d_out (m / G) <- this rank's low-bit shard of their sum
+void comm_sum_shard(Ctx*, const fr_t* d_vec, size_t m, fr_t* d_out);
 // every rank holds one element per polynomial (ptrs[k][0], or base[k*stride] when ptrs == null);
 // d_out[k*G + g] <- rank g's element of polynomial k
 // `extra` (may be null): one more single-element polynomial, gathered as polynomial number npolys

@@ -603,4 +603,33 @@ int orcd_sparse_verify(int kind, size_t C, size_t log_m, size_t log_r, const uin
   return p.verify(S, c, ldvec(r, ark_log2(c.s)), pg, *(Transcript*)transcript) ? 0 : 1;
 }
 
+
+// ---- polynomials derived from a caller's: k sequential calls of the oracle's bound_poly_var_top / bound_poly_var_bot
+// (dense_mlpoly.rs:209-225), r[0] first; split (dense_mlpoly.rs:101-107) as the two copies it makes; new_padded
+// (dense_mlpoly.rs:75-87).  out receives the result's evaluations in natural order.
+void orcd_poly_bind_top(const uint64_t* Z, size_t len, const uint64_t* r, size_t k, uint64_t* out) {
+  DensePolynomial p(ldvec(Z, len));
+  for (size_t j = 0; j < k; j++) p.bound_poly_var_top(ldfr(r + 4 * j));
+  for (size_t i = 0; i < p.len; i++) stfr(out + 4 * i, p[i]);
+}
+void orcd_poly_bind_bot(const uint64_t* Z, size_t len, const uint64_t* r, size_t k, uint64_t* out) {
+  DensePolynomial p(ldvec(Z, len));
+  for (size_t j = 0; j < k; j++) p.bound_poly_var_bot(ldfr(r + 4 * j));
+  for (size_t i = 0; i < p.len; i++) stfr(out + 4 * i, p[i]);
+}
+void orcd_poly_split(const uint64_t* Z, size_t len, size_t idx, uint64_t* lo, uint64_t* hi) {
+  const DensePolynomial p(ldvec(Z, len));
+  const DensePolynomial a(std::vector<Fr>(p.Z.begin(), p.Z.begin() + idx)), b(std::vector<Fr>(p.Z.begin() + idx, p.Z.begin() + 2 * idx));
+  for (size_t i = 0; i < idx; i++) {
+    stfr(lo + 4 * i, a[i]);
+    stfr(hi + 4 * i, b[i]);
+  }
+}
+// -> the padded length; out has room for it
+size_t orcd_poly_new_padded(const uint64_t* Z, size_t len, uint64_t* out) {
+  const DensePolynomial p = DensePolynomial::new_padded(ldvec(Z, len));
+  for (size_t i = 0; i < p.len; i++) stfr(out + 4 * i, p[i]);
+  return p.len;
+}
+
 }  // extern "C"
