@@ -185,9 +185,15 @@ int lasso_commit(lasso_ctx*, const lasso_dense*, const lasso_gens*, uint8_t* out
  * tape_label / tape_seed: RandomTape::new(b"proof") seeded with an explicit scalar (the reference draws it
  * from ark_std::test_rng()).  proof_out receives the ark-serialize (compressed) bytes of the proof struct.
  * challenges_out (optional) receives every Fiat-Shamir challenge in order (4 limbs each).
- * LASSO_ERR_STRATEGY, before any launch, for the parameters lasso_sumcheck_round_arbitrary rejects and for LT with
- * C > 8: its 2C memories make 4C grand-product circuits, above the 32 that one batched grand product holds.  The
- * per-loop entry points above accept LT up to C = 16. */
+ * This is lasso_prove_transcript (below) on a transcript and a tape made from the labels and the seed: the same
+ * bytes, and the same errors, each returned before any launch.  LASSO_ERR_STRATEGY for the parameters
+ * lasso_sumcheck_round_arbitrary rejects and for LT with C > 8: its 2C memories make 4C grand-product circuits,
+ * above the 32 that one batched grand product holds.  The per-loop entry points above accept LT up to C = 16.
+ * LASSO_ERR_LENGTH for r_len != log2(s), a null label, tape seed or proof_len, or proof_cap too small (*proof_len
+ * receives the size the proof needs); LASSO_ERR_GENS for generators built for another (c, s, num_memories, log_m),
+ * or of another context unless both are single-GPU contexts of one device (such contexts may share one generator
+ * set: its tables are only read); LASSO_ERR_VALUE for a coordinate of r or a tape seed that is not a canonical
+ * residue. */
 int lasso_prove(lasso_ctx*, int strategy, int log_R, lasso_dense*, const uint64_t* r, size_t r_len,
                 const lasso_gens*, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
                 uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
@@ -234,7 +240,7 @@ void lasso_strategy_destroy(lasso_strategy*);
 int lasso_sumcheck_round_custom(lasso_ctx*, const lasso_strategy*, const uint64_t* const* polys, size_t len,
                                 uint64_t* evals_out);
 /* lasso_prove with a custom strategy: the same semantics, outputs, errors and collectiveness.  LASSO_ERR_STRATEGY
- * when the strategy's (C, log_m) differ from the densified representation's. */
+ * for a null strategy, one of another context, or one whose (C, log_m) differ from the densified representation's. */
 int lasso_prove_custom(lasso_ctx*, const lasso_strategy*, lasso_dense*, const uint64_t* r, size_t r_len,
                        const lasso_gens*, const char* transcript_label, const char* tape_label,
                        const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,

@@ -624,41 +624,37 @@ class SparsePolynomialEvaluationProof:
             if transcript_label is not None or tape_label is not None or tape_seed is not None:
                 raise LassoError(LASSO_ERR_LENGTH, "labels and tape_seed belong to the label path, not to a caller's "
                                                    "transcript and random_tape")
-            return cls._prove_transcript(ctx, strategy, dense, r, gens, transcript, random_tape)
+            r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+            claim = np.zeros(4, dtype=np.uint64)
+            data = cls._call(ctx, strategy, True, dense, r, gens, (transcript._h, random_tape._h), (_p(claim),))
+            return cls(data, None, claim)
         transcript_label = b"example" if transcript_label is None else transcript_label
         tape_label = b"proof" if tape_label is None else tape_label
         r = _fr(r).reshape(-1, 4)
         seed = _fr(tape_seed if tape_seed is not None else np.zeros(4, dtype=np.uint64))
-        cap = 1 << 22
-        out = ctx._buf("proof", cap, np.uint8)
         chal = ctx._buf("challenges", (1 << 14, 4), np.uint64)
-        n, nch = C.c_size_t(0), C.c_size_t(0)
-        tail = (dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, transcript_label, tape_label, _p(seed), _p(out),
-                C.c_size_t(cap), C.byref(n), _p(chal), C.c_size_t(chal.shape[0]), C.byref(nch))
+        nch = C.c_size_t(0)
+        data = cls._call(ctx, strategy, False, dense, r, gens, (transcript_label, tape_label, _p(seed)),
+                         (_p(chal), C.c_size_t(chal.shape[0]), C.byref(nch)))
+        return cls(data, chal[: nch.value].copy())
+
+    @staticmethod
+    def _call(ctx, strategy, on_transcript, dense, r, gens, inputs, outputs):
+        """lasso_prove[_custom][_transcript] into ctx's proof buffer -> the proof bytes.  inputs: the transcript's
+        arguments, between the generators and the proof buffer; outputs: the arguments after proof_len."""
+        L = lib()
         if isinstance(strategy, CustomStrategy):
             if strategy._h is None:
                 raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
-            _chk(lib().lasso_prove_custom(ctx._h, strategy._h, *tail))
+            fn, head = (L.lasso_prove_custom_transcript if on_transcript else L.lasso_prove_custom), (strategy._h,)
         else:
-            _chk(lib().lasso_prove(ctx._h, strategy.kind, strategy.log_r, *tail))
-        return cls(bytes(out[: n.value]), chal[: nch.value].copy())
-
-    @classmethod
-    def _prove_transcript(cls, ctx, strategy, dense, r, gens, transcript, random_tape):
-        r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
+            fn, head = (L.lasso_prove_transcript if on_transcript else L.lasso_prove), (strategy.kind, strategy.log_r)
         cap = 1 << 22
         out = ctx._buf("proof", cap, np.uint8)
-        claim = np.zeros(4, dtype=np.uint64)
         n = C.c_size_t(0)
-        tail = (dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, transcript._h, random_tape._h, _p(out),
-                C.c_size_t(cap), C.byref(n), _p(claim))
-        if isinstance(strategy, CustomStrategy):
-            if strategy._h is None:
-                raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
-            _chk(lib().lasso_prove_custom_transcript(ctx._h, strategy._h, *tail))
-        else:
-            _chk(lib().lasso_prove_transcript(ctx._h, strategy.kind, strategy.log_r, *tail))
-        return cls(bytes(out[: n.value]), None, claim)
+        _chk(fn(ctx._h, *head, dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, *inputs, _p(out), C.c_size_t(cap),
+                C.byref(n), *outputs))
+        return bytes(out[: n.value])
 
 
 # ------------------------------------------------------------------ dense polynomials on a caller's transcript
@@ -832,13 +828,34 @@ def _poly_source(Z):
     return "host", np.ascontiguousarray(a), 4
 
 
-def _poly_handles(polys):
-    """a C array of the lasso_poly handles of DensePolynomials (at least one slot)"""
-    polys = list(polys)
-    arr = (C.c_void_p * max(len(polys), 1))()
-    for i, p in enumerate(polys):
-        arr[i] = p._h.value
+def _handles(objs):
+    """a C array of the handles `_h` of library objects (at least one slot)"""
+    objs = list(objs)
+    arr = (C.c_void_p * max(len(objs), 1))()
+    for i, o in enumerate(objs):
+        arr[i] = o._h.value
     return arr
+
+
+_poly_handles = _handles  # the earlier name, still imported by callers that build their own lasso_poly arrays
+
+
+def _poly_rows(ctx, Z, padded):
+    """a new lasso_poly of Z, in the forms DensePolynomial takes: host rows, or a CUDA tensor read in the order of
+    torch's current stream.  padded: new_padded, of any length."""
+    kind, src, row_stride = _poly_source(Z)
+    h = C.c_void_p()
+    L = lib()
+    if kind == "device":
+        torch = sys.modules["torch"]
+        stream = torch.cuda.current_stream(src.device).cuda_stream
+        fn = L.lasso_poly_create_padded_device if padded else L.lasso_poly_create_device
+        _chk(fn(ctx._h, C.c_void_p(src.data_ptr()), C.c_size_t(src.shape[0]), C.c_size_t(row_stride),
+                C.c_void_p(stream), C.byref(h)))
+    else:
+        fn = L.lasso_poly_create_padded if padded else L.lasso_poly_create
+        _chk(fn(ctx._h, _p(src), C.c_size_t(src.shape[0]), C.byref(h)))
+    return h
 
 
 class DensePolynomial:
@@ -853,15 +870,7 @@ class DensePolynomial:
     DensifiedRepresentation.outputs stay single-GPU."""
 
     def __init__(self, ctx, Z):
-        kind, src, row_stride = _poly_source(Z)
-        h = C.c_void_p()
-        if kind == "device":
-            torch = sys.modules["torch"]
-            stream = torch.cuda.current_stream(src.device).cuda_stream
-            _chk(lib().lasso_poly_create_device(ctx._h, C.c_void_p(src.data_ptr()), C.c_size_t(src.shape[0]),
-                                                C.c_size_t(row_stride), C.c_void_p(stream), C.byref(h)))
-        else:
-            _chk(lib().lasso_poly_create(ctx._h, _p(src), C.c_size_t(src.shape[0]), C.byref(h)))
+        h = _poly_rows(ctx, Z, False)
         self.ctx, self._h = ctx, h
         self.num_vars = int(lib().lasso_poly_num_vars(h))
 
@@ -885,11 +894,8 @@ class DensePolynomial:
         """Q(x) = comb(P_0(x), .., P_{k-1}(x)) at every point of the hypercube, on ctx's GPU (comb.degree is not used),
         e.g. the fingerprints t gamma^2 + v gamma + a - tau of offline memory checking"""
         polys = list(polys)
-        arr = (C.c_void_p * max(len(polys), 1))()
-        for i, p in enumerate(polys):
-            arr[i] = p._h.value
         h = C.c_void_p()
-        _chk(lib().lasso_poly_create_comb(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.byref(h)))
+        _chk(lib().lasso_poly_create_comb(ctx._h, comb._h, _handles(polys), C.c_size_t(len(polys)), C.byref(h)))
         return cls._wrap(ctx, h)
 
     @classmethod
@@ -899,17 +905,17 @@ class DensePolynomial:
         dropped).  Integer-valued iff every input is."""
         polys = list(polys)
         h = C.c_void_p()
-        _chk(lib().lasso_poly_create_merge(ctx._h, _poly_handles(polys), C.c_size_t(len(polys)), C.byref(h)))
+        _chk(lib().lasso_poly_create_merge(ctx._h, _handles(polys), C.c_size_t(len(polys)), C.byref(h)))
         return cls._wrap(ctx, h)
 
     @staticmethod
     def evaluate_batch(ctx, polys, r):
         """P_j(r) for 1..64 DensePolynomials of one num_vars, over one eq table -> (n, 4) uint64 Montgomery limbs"""
         polys = list(polys)
-        arr = _poly_handles(polys)
         r = _limbs(r, what="r") if len(r) else np.zeros((0, 4), dtype=np.uint64)
         out = np.zeros((max(len(polys), 1), 4), dtype=np.uint64)
-        _chk(lib().lasso_poly_evaluate_batch(ctx._h, arr, C.c_size_t(len(polys)), _p(r), C.c_size_t(r.shape[0]), _p(out)))
+        _chk(lib().lasso_poly_evaluate_batch(ctx._h, _handles(polys), C.c_size_t(len(polys)), _p(r),
+                                             C.c_size_t(r.shape[0]), _p(out)))
         return out[: len(polys)]
 
     def commit(self, gens):
@@ -942,16 +948,7 @@ class DensePolynomial:
     def new_padded(cls, ctx, Z):
         """DensePolynomial::new_padded (src/poly/dense_mlpoly.rs:75-87): Z of any length (the forms __init__ takes),
         zero-padded up to the next power of two; an empty Z gives the polynomial of one zero evaluation"""
-        kind, src, row_stride = _poly_source(Z)
-        h = C.c_void_p()
-        if kind == "device":
-            torch = sys.modules["torch"]
-            stream = torch.cuda.current_stream(src.device).cuda_stream
-            _chk(lib().lasso_poly_create_padded_device(ctx._h, C.c_void_p(src.data_ptr()), C.c_size_t(src.shape[0]),
-                                                       C.c_size_t(row_stride), C.c_void_p(stream), C.byref(h)))
-        else:
-            _chk(lib().lasso_poly_create_padded(ctx._h, _p(src), C.c_size_t(src.shape[0]), C.byref(h)))
-        return cls._wrap(ctx, h)
+        return cls._wrap(ctx, _poly_rows(ctx, Z, True))
 
     def _bound(self, fn, r):
         r = _limbs(np.asarray(r).reshape(-1, 4), what="r")
@@ -1129,17 +1126,15 @@ class SumcheckInstanceProof:
         if num_rounds is None:
             num_rounds = polys[0].num_vars if polys else 0
         num_rounds = int(num_rounds)
-        arr = (C.c_void_p * max(len(polys), 1))()
-        for i, p in enumerate(polys):
-            arr[i] = p._h.value
         cap = 8 + max(num_rounds, 0) * (8 + 32 * comb.degree)
         out = np.zeros(cap, dtype=np.uint8)
         r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
         fin = np.zeros((max(len(polys), 1), 4), dtype=np.uint64)
         claim = np.zeros(4, dtype=np.uint64)
         n = C.c_size_t(0)
-        _chk(lib().lasso_sumcheck_prove(ctx._h, comb._h, arr, C.c_size_t(len(polys)), C.c_size_t(num_rounds),
-                                        transcript._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin), _p(claim)))
+        _chk(lib().lasso_sumcheck_prove(ctx._h, comb._h, _handles(polys), C.c_size_t(len(polys)),
+                                        C.c_size_t(num_rounds), transcript._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r),
+                                        _p(fin), _p(claim)))
         return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim)
 
     @classmethod
@@ -1164,7 +1159,7 @@ class SumcheckInstanceProof:
         fin = np.zeros((2 * n + 1, 4), dtype=np.uint64)
         ln = C.c_size_t(0)
         _chk(lib().lasso_sumcheck_prove_cubic_batched(
-            ctx._h, _poly_handles(A), _poly_handles(B), C.c_size_t(n), C_poly._h, _p(coeffs), _p(claim),
+            ctx._h, _handles(A), _handles(B), C.c_size_t(n), C_poly._h, _p(coeffs), _p(claim),
             C.c_size_t(num_rounds), transcript._h, _p(out), C.c_size_t(cap), C.byref(ln), _p(r), _p(fin[:n] if n else fin),
             _p(fin[n:2 * n] if n else fin), _p(fin[2 * n:])))
         return cls(bytes(out[: ln.value]), r[:num_rounds], fin, claim.reshape(4).copy())
@@ -1212,15 +1207,12 @@ class BatchedGrandProductArgument:
         """BatchedGrandProductArgument::prove over 1..32 GrandProductCircuits of one num_vars on the caller's transcript,
         advanced in place"""
         circuits = list(circuits)
-        arr = (C.c_void_p * max(len(circuits), 1))()
-        for i, c in enumerate(circuits):
-            arr[i] = c._h.value
         v = circuits[0].num_vars if circuits else 0
         cap = cls.proof_len(len(circuits), v)
         out = np.zeros(cap, dtype=np.uint8)
         r = np.zeros((max(v, 1), 4), dtype=np.uint64)
         claims = np.zeros((max(len(circuits), 1), 4), dtype=np.uint64)
         n = C.c_size_t(0)
-        _chk(lib().lasso_gp_prove(ctx._h, arr, C.c_size_t(len(circuits)), transcript._h, _p(out), C.c_size_t(cap),
-                                  C.byref(n), _p(r), _p(claims)))
+        _chk(lib().lasso_gp_prove(ctx._h, _handles(circuits), C.c_size_t(len(circuits)), transcript._h, _p(out),
+                                  C.c_size_t(cap), C.byref(n), _p(r), _p(claims)))
         return cls(bytes(out[: n.value]), r[:v], claims[: len(circuits)])

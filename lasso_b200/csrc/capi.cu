@@ -86,6 +86,9 @@ static int fail(int code, const std::string& msg) {
     LB_CUDA_CHECK(cudaSetDevice((h)->c->device));
 #define LB_CATCH                                  \
   }                                               \
+  catch (const LbError& e) {                      \
+    return fail(e.code, e.what());                \
+  }                                               \
   catch (const std::exception& e) {               \
     return fail(-1, e.what());                    \
   }
@@ -94,23 +97,51 @@ static bool is_pow2(size_t x) { return x && !(x & (x - 1)); }
 static constexpr size_t kMsmLargeMin = 1 << 14;  // below this the row kernels (c = 8, buckets in shared memory) win
 static Strategy mkS(int kind, int C, int log_M, int log_R) { return Strategy{kind, C, log_M, log_R}; }
 
-// Checks a custom strategy's descriptor (everything but the tables' contents) and fills cs with its shape, the degree
-// of g and the instructions with SSA slots mapped to physical slots.  "" = valid, else the reason.
-static std::string custom_check(int C, int log_m, int nsub, int alpha, const int* sub, const int* dim, const int32_t* prog,
-                                int n_ops, const uint64_t* consts, int n_consts, int degree, CustomStrategy& cs,
-                                std::vector<CustomIns>& ins) {
-  if (C < 1 || C > 16) return "C must be in 1..16";
-  if (log_m < 2 || log_m > 24) return "log_m must be in 2..24";
-  if (alpha < 1 || alpha > kCustomMaxMemories) return "num_memories must be in 1..16";
-  if (nsub < 1 || nsub > alpha) return "num_subtables must be in 1..num_memories";
-  if (!sub || !dim || !prog) return "null map or program";
+// The output tail of every proof and commitment.  out_room publishes the size the caller must provide and refuses a
+// null or short buffer; it runs before anything moves, so a refused call leaves transcripts and tapes as they were.
+// timed runs the producing call into one of the context's timers; out_copy checks the produced size and copies it out.
+static int out_room(const char* what, size_t need, const uint8_t* out, size_t cap, size_t* out_len) {
+  if (out_len) *out_len = need;
+  if (!out || cap < need) return fail(LASSO_ERR_LENGTH, std::string(what) + ": output buffer too small");
+  return 0;
+}
+template <class F>
+static auto timed(double& ms, F&& produce) {
+  const auto t0 = std::chrono::steady_clock::now();
+  auto out = produce();
+  ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  return out;
+}
+static int out_copy(const char* what, const std::vector<uint8_t>& b, size_t need, uint8_t* out) {
+  if (b.size() != need) return fail(-1, std::string(what) + ": unexpected proof size");
+  memcpy(out, b.data(), need);
+  return 0;
+}
+
+// Checks a custom strategy's descriptor and that its tables (of either kind) are there, but not their contents, and
+// fills cs with its shape, the degree of g and the instructions with SSA slots mapped to physical slots.  Nulls *out
+// first; every failure is LASSO_ERR_STRATEGY.
+template <class T>
+static int custom_check(int C, int log_m, int nsub, int alpha, const int* sub, const int* dim, const int32_t* prog,
+                        int n_ops, const uint64_t* consts, int n_consts, int degree, const T* const* tables,
+                        lasso_strategy** out, CustomStrategy& cs, std::vector<CustomIns>& ins) {
+  if (out) *out = nullptr;
+  auto bad = [](const std::string& why) { return fail(LASSO_ERR_STRATEGY, "strategy: " + why); };
+  if (C < 1 || C > 16) return bad("C must be in 1..16");
+  if (log_m < 2 || log_m > 24) return bad("log_m must be in 2..24");
+  if (alpha < 1 || alpha > kCustomMaxMemories) return bad("num_memories must be in 1..16");
+  if (nsub < 1 || nsub > alpha) return bad("num_subtables must be in 1..num_memories");
+  if (!sub || !dim || !prog) return bad("null map or program");
   for (int i = 0; i < alpha; i++) {
-    if (sub[i] < 0 || sub[i] >= nsub) return "memory_to_subtable_index out of range";
-    if (dim[i] < 0 || dim[i] >= C) return "memory_to_dimension_index out of range";
+    if (sub[i] < 0 || sub[i] >= nsub) return bad("memory_to_subtable_index out of range");
+    if (dim[i] < 0 || dim[i] >= C) return bad("memory_to_dimension_index out of range");
   }
   int n_slots = 0;
   const std::string why = program_check(alpha, prog, n_ops, consts, n_consts, degree, "g_poly_degree", ins, &n_slots);
-  if (!why.empty()) return why;
+  if (!why.empty()) return bad(why);
+  if (!out || !tables) return bad("null tables or output");
+  for (int k = 0; k < nsub; k++)
+    if (!tables[k]) return bad("null table");
   cs = CustomStrategy{};
   cs.C = C;
   cs.log_m = log_m;
@@ -124,7 +155,7 @@ static std::string custom_check(int C, int log_m, int nsub, int alpha, const int
     cs.sub[i] = sub[i];
     cs.dim[i] = dim[i];
   }
-  return "";
+  return 0;
 }
 
 extern "C" {
@@ -166,32 +197,29 @@ int lasso_ctx_bind_host_threads(lasso_ctx* h) {
   return bind_host_threads(h->c->device, &h->c->helper_mask, &h->c->have_helper_mask);
 }
 
-int lasso_bind_top(lasso_ctx* h, uint64_t* Z, size_t len, const uint64_t r[4]) {
-  LB_TRY_CTX(h)
-  if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "bind_top: len must be a power of two >= 2");
-  Ctx* c = h->c;
-  DBuf<fr_t> d(c, len);
+// one bound_poly_var_top / _bot of a host array: Z[0 .. len/2) receives the bound values
+static int bind_host(Ctx* c, uint64_t* Z, size_t len, const uint64_t r[4], bool top) {
+  if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "bind: len must be a power of two >= 2");
+  DBuf<fr_t> d(c, len), o(c, top ? 0 : len / 2);  // a top bind is in place
   LB_CUDA_CHECK(cudaMemcpyAsync(d.p, Z, len * 32, cudaMemcpyHostToDevice, c->st));
   fr_t rr;
   memcpy(rr.v, r, 32);
-  launch_bind_top(d.p, 0, 1, len / 2, rr, c->st);
-  LB_CUDA_CHECK(cudaMemcpyAsync(Z, d.p, (len / 2) * 32, cudaMemcpyDeviceToHost, c->st));
+  if (top)
+    launch_bind_top(d.p, 0, 1, len / 2, rr, c->st);
+  else
+    launch_bind_bot(d.p, o.p, len / 2, rr, c->st);
+  LB_CUDA_CHECK(cudaMemcpyAsync(Z, top ? d.p : o.p, (len / 2) * 32, cudaMemcpyDeviceToHost, c->st));
   c->sync();
   return 0;
+}
+int lasso_bind_top(lasso_ctx* h, uint64_t* Z, size_t len, const uint64_t r[4]) {
+  LB_TRY_CTX(h)
+  return bind_host(h->c, Z, len, r, true);
   LB_CATCH
 }
 int lasso_bind_bot(lasso_ctx* h, uint64_t* Z, size_t len, const uint64_t r[4]) {
   LB_TRY_CTX(h)
-  if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "bind_bot: len must be a power of two >= 2");
-  Ctx* c = h->c;
-  DBuf<fr_t> d(c, len), o(c, len / 2);
-  LB_CUDA_CHECK(cudaMemcpyAsync(d.p, Z, len * 32, cudaMemcpyHostToDevice, c->st));
-  fr_t rr;
-  memcpy(rr.v, r, 32);
-  launch_bind_bot(d.p, o.p, len / 2, rr, c->st);
-  LB_CUDA_CHECK(cudaMemcpyAsync(Z, o.p, (len / 2) * 32, cudaMemcpyDeviceToHost, c->st));
-  c->sync();
-  return 0;
+  return bind_host(h->c, Z, len, r, false);
   LB_CATCH
 }
 int lasso_eq_evals(lasso_ctx* h, const uint64_t* r, int ell, uint64_t* out) {
@@ -208,14 +236,10 @@ int lasso_eq_evals(lasso_ctx* h, const uint64_t* r, int ell, uint64_t* out) {
   return 0;
   LB_CATCH
 }
-int lasso_sumcheck_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M, int log_R,
-                                   const uint64_t* const* polys, size_t len, uint64_t* evals_out) {
-  LB_TRY_CTX(h)
-  Strategy S = mkS(strategy, C, log_M, log_R);
-  if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
+// one round of the primary sumcheck of a checked strategy: num_memories + 1 host arrays of len elements
+static int sumcheck_round(Ctx* c, const Strategy& S, const uint64_t* const* polys, size_t len, uint64_t* evals_out) {
   if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "len must be a power of two >= 2");
-  Ctx* c = h->c;
-  int np = S.num_memories() + 1, npts = S.sumcheck_poly_degree() + 1;
+  const int np = S.num_memories() + 1, npts = S.sumcheck_poly_degree() + 1;
   DBuf<fr_t> d(c, (size_t)np * len);
   for (int k = 0; k < np; k++)
     LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
@@ -223,6 +247,13 @@ int lasso_sumcheck_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M,
   launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
   c->fin_wait(f, (fr_t*)evals_out, npts);
   return 0;
+}
+int lasso_sumcheck_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M, int log_R,
+                                   const uint64_t* const* polys, size_t len, uint64_t* evals_out) {
+  LB_TRY_CTX(h)
+  Strategy S = mkS(strategy, C, log_M, log_R);
+  if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
+  return sumcheck_round(h->c, S, polys, len, evals_out);
   LB_CATCH
 }
 int lasso_sumcheck_bind_round_arbitrary(lasso_ctx* h, int strategy, int C, int log_M, int log_R, uint64_t* const* polys,
@@ -516,11 +547,7 @@ void lasso_gens_destroy(lasso_gens* g) {
 int lasso_densify(lasso_ctx* h, const uint64_t* indices, size_t n_lookups, size_t C, size_t log_m, lasso_dense** out) {
   LB_TRY_CTX(h)
   *out = nullptr;
-  auto t0 = std::chrono::steady_clock::now();
-  int err = 0;
-  Dense* d = densify(h->c, indices, n_lookups, C, log_m, &err);
-  if (!d) return fail(err == 3 ? LASSO_ERR_INDEX_RANGE : LASSO_ERR_STRATEGY, "densify: invalid input");
-  h->c->t_densify_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  Dense* d = timed(h->c->t_densify_ms, [&] { return densify(h->c, indices, n_lookups, C, log_m); });
   *out = new lasso_dense{d};
   return 0;
   LB_CATCH
@@ -529,14 +556,10 @@ int lasso_densify_device(lasso_ctx* h, const void* indices, size_t elem_bytes, s
                          size_t row_stride, size_t col_stride, size_t log_m, void* stream, lasso_dense** out) {
   LB_TRY_CTX(h)
   *out = nullptr;
-  auto t0 = std::chrono::steady_clock::now();
-  int err = 0;
-  Dense* d = densify_device(h->c, indices, elem_bytes, n_lookups, C, row_stride, col_stride, log_m,
-                            static_cast<cudaStream_t>(stream), &err);
-  if (err == 3) return fail(LASSO_ERR_INDEX_RANGE, "densify_device: an index is >= m");
-  if (err == 7) return fail(LASSO_ERR_POINTER, "densify_device: the indices are not device memory of the context's GPU");
-  if (!d) return fail(LASSO_ERR_STRATEGY, "densify_device: invalid input");
-  h->c->t_densify_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+  Dense* d = timed(h->c->t_densify_ms, [&] {
+    return densify_device(h->c, indices, elem_bytes, n_lookups, C, row_stride, col_stride, log_m,
+                          static_cast<cudaStream_t>(stream));
+  });
   *out = new lasso_dense{d};
   return 0;
   LB_CATCH
@@ -585,62 +608,9 @@ size_t lasso_dense_read(lasso_ctx* h, const lasso_dense* dd, int which, uint64_t
 
 int lasso_commit(lasso_ctx* h, const lasso_dense* d, const lasso_gens* g, uint8_t* out, size_t cap, size_t* out_len) {
   LB_TRY_CTX(h)
-  auto t0 = std::chrono::steady_clock::now();
-  std::vector<uint8_t> b = commit(h->c, *d->d, *g->g);
-  h->c->t_commit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  *out_len = b.size();
-  if (b.size() > cap) return fail(LASSO_ERR_LENGTH, "commit: output buffer too small");
-  memcpy(out, b.data(), b.size());
-  return 0;
-  LB_CATCH
-}
-
-}  // extern "C"
-
-// lasso_prove / lasso_prove_custom after the strategy has been checked
-static int prove_checked(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
-                         const lasso_gens* g, const char* transcript_label, const char* tape_label,
-                         const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
-                         uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
-  // assert_eq!(r.len(), log2(dense.s))  surge.rs:131
-  if (r_len != log2_exact_or_ceil(d->d->s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");
-  std::vector<fr_t> rv(r_len);
-  for (size_t i = 0; i < r_len; i++) memcpy(rv[i].v, r + 4 * i, 32);
-  fr_t seed;
-  memcpy(seed.v, tape_seed, 32);
-  std::vector<fr_t> trace;
-  auto t0 = std::chrono::steady_clock::now();
-  std::vector<uint8_t> b;
-  try {
-    b = prove(h->c, S, *d->d, rv, *g->g, transcript_label, tape_label, seed, &trace);
-  } catch (const std::runtime_error& e) {
-    if (std::string(e.what()).find("multiset") != std::string::npos) return fail(LASSO_ERR_MULTISET, e.what());
-    throw;
-  }
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  *proof_len = b.size();
-  if (n_challenges) *n_challenges = trace.size();
-  if (challenges_out)
-    for (size_t i = 0; i < trace.size() && i < challenges_cap; i++) memcpy(challenges_out + 4 * i, trace[i].v, 32);
-  if (b.size() > proof_cap) return fail(LASSO_ERR_LENGTH, "prove: output buffer too small");
-  memcpy(proof_out, b.data(), b.size());
-  return 0;
-}
-
-extern "C" {
-
-int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
-                const lasso_gens* g, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
-                uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
-                size_t challenges_cap, size_t* n_challenges) {
-  LB_TRY_CTX(h)
-  Strategy S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
-  if (!S.valid()) return fail(LASSO_ERR_STRATEGY, "unsupported strategy parameters");
-  if (!S.provable())
-    return fail(LASSO_ERR_STRATEGY, "prove: " + std::to_string(2 * S.num_memories()) +
-                                        " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)");
-  return prove_checked(h, S, d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
-                       challenges_out, challenges_cap, n_challenges);
+  const std::vector<uint8_t> b = timed(h->c->t_commit_ms, [&] { return commit(h->c, *d->d, *g->g); });
+  if (const int rc = out_room("commit", b.size(), out, cap, out_len)) return rc;
+  return out_copy("commit", b, b.size(), out);
   LB_CATCH
 }
 
@@ -681,15 +651,11 @@ int lasso_strategy_create(lasso_ctx* h, int C, int log_m, int num_subtables, con
                           int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
                           const int32_t* program, int n_ops, const uint64_t* constants, int n_constants, int g_degree,
                           lasso_strategy** out) {
-  if (out) *out = nullptr;
   CustomStrategy cs;
   std::vector<CustomIns> ins;
-  const std::string why = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
-                                       n_ops, constants, n_constants, g_degree, cs, ins);
-  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "strategy: " + why);
-  if (!out || !tables) return fail(LASSO_ERR_STRATEGY, "strategy: null tables or output");
-  for (int k = 0; k < num_subtables; k++)
-    if (!tables[k]) return fail(LASSO_ERR_STRATEGY, "strategy: null table");
+  if (const int rc = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
+                                  n_ops, constants, n_constants, g_degree, tables, out, cs, ins))
+    return rc;
   const size_t M = (size_t)1 << log_m;
   uint32_t mx = 0;
   for (int k = 0; k < num_subtables; k++)
@@ -703,15 +669,11 @@ int lasso_strategy_create_fr(lasso_ctx* h, int C, int log_m, int num_subtables, 
                              int num_memories, const int* mem_to_subtable, const int* mem_to_dimension,
                              const int32_t* program, int n_ops, const uint64_t* constants, int n_constants, int g_degree,
                              lasso_strategy** out) {
-  if (out) *out = nullptr;
   CustomStrategy cs;
   std::vector<CustomIns> ins;
-  const std::string why = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
-                                       n_ops, constants, n_constants, g_degree, cs, ins);
-  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "strategy: " + why);
-  if (!out || !tables) return fail(LASSO_ERR_STRATEGY, "strategy: null tables or output");
-  for (int k = 0; k < num_subtables; k++)
-    if (!tables[k]) return fail(LASSO_ERR_STRATEGY, "strategy: null table");
+  if (const int rc = custom_check(C, log_m, num_subtables, num_memories, mem_to_subtable, mem_to_dimension, program,
+                                  n_ops, constants, n_constants, g_degree, tables, out, cs, ins))
+    return rc;
   const size_t M = (size_t)1 << log_m;
   // canonical values: every entry a canonical Montgomery residue; the widest one fixes the commitment's windows
   std::vector<uint32_t> small((size_t)num_subtables * M);
@@ -747,17 +709,91 @@ int lasso_sumcheck_round_custom(lasso_ctx* h, const lasso_strategy* s, const uin
                                 uint64_t* evals_out) {
   LB_TRY_CTX(h)
   if (!s || s->c != h->c) return fail(LASSO_ERR_STRATEGY, "strategy was created on another context");
-  if (!is_pow2(len) || len < 2) return fail(LASSO_ERR_NOT_POW2, "len must be a power of two >= 2");
-  Ctx* c = h->c;
-  const Strategy S = s->S();
-  const int np = S.num_memories() + 1, npts = S.sumcheck_poly_degree() + 1;
-  DBuf<fr_t> d(c, (size_t)np * len);
-  for (int k = 0; k < np; k++)
-    LB_CUDA_CHECK(cudaMemcpyAsync(d.p + (size_t)k * len, polys[k], len * 32, cudaMemcpyHostToDevice, c->st));
-  const Finalize f = c->fin_begin();
-  launch_sumcheck_eval_arbitrary(S, d.p, len, len / 2, f, c->st);
-  c->fin_wait(f, (fr_t*)evals_out, npts);
+  return sumcheck_round(h->c, s->S(), polys, len, evals_out);
+  LB_CATCH
+}
+// ---- lookup proofs, on a caller's transcript and tape or on ones made from labels
+static bool load_scalars(const uint64_t* s, size_t n, std::vector<fr_t>& out);
+static int poly_ctx_check(lasso_ctx* h);
+// The strategy of a built-in kind (strategy, log_R) or a custom one (s), checked against the context and the dense;
+// every failure is LASSO_ERR_STRATEGY
+static int strategy_for(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
+                        Strategy& S) {
+  auto bad = [](const std::string& why) { return fail(LASSO_ERR_STRATEGY, why); };
+  if (!d) return bad("null densified representation");
+  if (s) {
+    if (s->c != h->c) return bad("strategy was created on another context");
+    if ((size_t)s->cs.C != d->d->C || (size_t)s->cs.log_m != d->d->log_m)
+      return bad("strategy (C, log_m) differ from the densified representation");
+    S = s->S();
+    return 0;
+  }
+  S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
+  if (!S.valid()) return bad("unsupported strategy parameters");
+  if (!S.provable())
+    return bad("prove: " + std::to_string(2 * S.num_memories()) +
+               " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)");
   return 0;
+}
+// shared_gens: generators of another single-GPU context on the same device will do (lasso_prove lets such contexts
+// share one set of read-only tables, many GB at 2^20 lookups); otherwise they must be the context's own
+static int prove_transcript(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
+                            const lasso_gens* g, bool shared_gens, lasso_transcript* transcript, lasso_random_tape* tape,
+                            uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
+  const Dense& dense = *d->d;
+  if (!transcript || !tape || !proof_len) return fail(LASSO_ERR_LENGTH, "prove: null transcript, random tape or proof_len");
+  if (r_len != log2_exact_or_ceil(dense.s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");  // surge.rs:131
+  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "prove: null point");
+  // the generators lasso_gens_create built for this (c, s, num_memories, log_m) (surge.rs:32-58)
+  const size_t alpha = (size_t)S.num_memories();
+  const Ctx* gc = g ? g->g->ctx : nullptr;
+  const bool shareable = shared_gens && gc && gc->device == h->c->device && gc->world == 1 && h->c->world == 1;
+  if (!g || (gc != h->c && !shareable))
+    return fail(LASSO_ERR_GENS, "prove: null generators, or generators of another context");
+  const Gens& gg = *g->g;
+  if (gg.c != dense.C || next_pow2(gg.s) != dense.s || gg.num_memories != alpha || gg.log_m != dense.log_m ||
+      gg.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || gg.nv_l != dense.nv_l || gg.nv_m != dense.nv_m)
+    return fail(LASSO_ERR_GENS, "prove: generators built for another (c, s, num_memories, log_m)");
+  const size_t need = proof_bytes(S, dense, gg);
+  if (const int rc = out_room("prove", need, proof_out, proof_cap, proof_len)) return rc;
+  std::vector<fr_t> rv;
+  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "prove: a coordinate of r is not a canonical residue");
+  fr_t claimed;
+  const std::vector<uint8_t> b =
+      timed(h->c->t_prove_ms, [&] { return prove(h->c, S, *d->d, rv, gg, transcript->t, tape->t, &claimed); });
+  if (const int rc = out_copy("prove", b, need, proof_out)) return rc;
+  if (claimed_eval_out) memcpy(claimed_eval_out, claimed.v, 32);
+  return 0;
+}
+// lasso_prove / lasso_prove_custom: prove_transcript on Transcript::new(transcript_label), which records every
+// challenge it draws, and on RandomTape::new(tape_label) seeded with tape_seed
+static int prove_labels(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
+                        const lasso_gens* g, const char* transcript_label, const char* tape_label,
+                        const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                        uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
+  if (!transcript_label || !tape_label || !tape_seed) return fail(LASSO_ERR_LENGTH, "prove: null label or tape seed");
+  std::vector<fr_t> seed, trace;
+  if (!load_scalars(tape_seed, 1, seed)) return fail(LASSO_ERR_VALUE, "prove: the tape seed is not a canonical residue");
+  lasso_transcript transcript{Transcript(transcript_label)};
+  transcript.t.trace = &trace;
+  lasso_random_tape tape{RandomTape(tape_label, seed[0])};
+  if (const int rc =
+          prove_transcript(h, S, d, r, r_len, g, true, &transcript, &tape, proof_out, proof_cap, proof_len, nullptr))
+    return rc;
+  if (n_challenges) *n_challenges = trace.size();
+  if (challenges_out)
+    for (size_t i = 0; i < trace.size() && i < challenges_cap; i++) memcpy(challenges_out + 4 * i, trace[i].v, 32);
+  return 0;
+}
+int lasso_prove(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
+                const lasso_gens* g, const char* transcript_label, const char* tape_label, const uint64_t tape_seed[4],
+                uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* challenges_out,
+                size_t challenges_cap, size_t* n_challenges) {
+  LB_TRY_CTX(h)
+  Strategy S{};
+  if (const int rc = strategy_for(h, strategy, log_R, nullptr, d, S)) return rc;
+  return prove_labels(h, S, d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
+                      challenges_out, challenges_cap, n_challenges);
   LB_CATCH
 }
 int lasso_prove_custom(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, const uint64_t* r, size_t r_len,
@@ -765,77 +801,21 @@ int lasso_prove_custom(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, co
                        const uint64_t tape_seed[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
                        uint64_t* challenges_out, size_t challenges_cap, size_t* n_challenges) {
   LB_TRY_CTX(h)
-  if (!s || s->c != h->c) return fail(LASSO_ERR_STRATEGY, "strategy was created on another context");
-  if ((size_t)s->cs.C != d->d->C || (size_t)s->cs.log_m != d->d->log_m)
-    return fail(LASSO_ERR_STRATEGY, "strategy (C, log_m) differ from the densified representation");
-  return prove_checked(h, s->S(), d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
-                       challenges_out, challenges_cap, n_challenges);
+  if (!s) return fail(LASSO_ERR_STRATEGY, "null strategy");
+  Strategy S{};
+  if (const int rc = strategy_for(h, 0, 0, s, d, S)) return rc;
+  return prove_labels(h, S, d, r, r_len, g, transcript_label, tape_label, tape_seed, proof_out, proof_cap, proof_len,
+                      challenges_out, challenges_cap, n_challenges);
   LB_CATCH
-}
-
-// ---- lookups inside a caller's protocol
-static bool load_scalars(const uint64_t* s, size_t n, std::vector<fr_t>& out);
-static int poly_ctx_check(lasso_ctx* h);
-// The strategy of a built-in kind (strategy, log_R) or a custom one (s), checked against the context and the dense:
-// "" = usable, else the reason (LASSO_ERR_STRATEGY)
-static std::string strategy_for(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
-                                Strategy& S) {
-  if (!d) return "null densified representation";
-  if (s) {
-    if (s->c != h->c) return "strategy was created on another context";
-    if ((size_t)s->cs.C != d->d->C || (size_t)s->cs.log_m != d->d->log_m)
-      return "strategy (C, log_m) differ from the densified representation";
-    S = s->S();
-    return "";
-  }
-  S = mkS(strategy, (int)d->d->C, (int)d->d->log_m, log_R);
-  if (!S.valid()) return "unsupported strategy parameters";
-  if (!S.provable())
-    return "prove: " + std::to_string(2 * S.num_memories()) + " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)";
-  return "";
-}
-static int prove_transcript(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
-                            const lasso_gens* g, lasso_transcript* transcript, lasso_random_tape* tape, uint8_t* proof_out,
-                            size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
-  const Dense& dense = *d->d;
-  if (!transcript || !tape || !proof_len) return fail(LASSO_ERR_LENGTH, "prove: null transcript, random tape or proof_len");
-  if (r_len != log2_exact_or_ceil(dense.s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");  // surge.rs:131
-  if (r_len && !r) return fail(LASSO_ERR_LENGTH, "prove: null point");
-  // the generators lasso_gens_create built for this (c, s, num_memories, log_m) (surge.rs:32-58)
-  const size_t alpha = (size_t)S.num_memories();
-  if (!g || g->g->ctx != h->c) return fail(LASSO_ERR_GENS, "prove: null generators, or generators of another context");
-  const Gens& gg = *g->g;
-  if (gg.c != dense.C || next_pow2(gg.s) != dense.s || gg.num_memories != alpha || gg.log_m != dense.log_m ||
-      gg.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || gg.nv_l != dense.nv_l || gg.nv_m != dense.nv_m)
-    return fail(LASSO_ERR_GENS, "prove: generators built for another (c, s, num_memories, log_m)");
-  const size_t need = proof_bytes(S, dense, gg);
-  *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "prove: output buffer too small");
-  std::vector<fr_t> rv;
-  if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "prove: a coordinate of r is not a canonical residue");
-  auto t0 = std::chrono::steady_clock::now();
-  fr_t claimed;
-  std::vector<uint8_t> b;
-  try {
-    b = prove(h->c, S, *d->d, rv, gg, transcript->t, tape->t, &claimed);
-  } catch (const std::runtime_error& e) {
-    if (std::string(e.what()).find("multiset") != std::string::npos) return fail(LASSO_ERR_MULTISET, e.what());
-    throw;
-  }
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (b.size() != need) return fail(-1, "prove: unexpected proof size");
-  memcpy(proof_out, b.data(), b.size());
-  if (claimed_eval_out) memcpy(claimed_eval_out, claimed.v, 32);
-  return 0;
 }
 int lasso_prove_transcript(lasso_ctx* h, int strategy, int log_R, lasso_dense* d, const uint64_t* r, size_t r_len,
                            const lasso_gens* g, lasso_transcript* transcript, lasso_random_tape* random_tape,
                            uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t claimed_eval_out[4]) {
   LB_TRY_CTX(h)
   Strategy S{};
-  const std::string why = strategy_for(h, strategy, log_R, nullptr, d, S);
-  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, why);
-  return prove_transcript(h, S, d, r, r_len, g, transcript, random_tape, proof_out, proof_cap, proof_len, claimed_eval_out);
+  if (const int rc = strategy_for(h, strategy, log_R, nullptr, d, S)) return rc;
+  return prove_transcript(h, S, d, r, r_len, g, false, transcript, random_tape, proof_out, proof_cap, proof_len,
+                          claimed_eval_out);
   LB_CATCH
 }
 int lasso_prove_custom_transcript(lasso_ctx* h, const lasso_strategy* s, lasso_dense* d, const uint64_t* r, size_t r_len,
@@ -844,9 +824,9 @@ int lasso_prove_custom_transcript(lasso_ctx* h, const lasso_strategy* s, lasso_d
   LB_TRY_CTX(h)
   if (!s) return fail(LASSO_ERR_STRATEGY, "null strategy");
   Strategy S{};
-  const std::string why = strategy_for(h, 0, 0, s, d, S);
-  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, why);
-  return prove_transcript(h, S, d, r, r_len, g, transcript, random_tape, proof_out, proof_cap, proof_len, claimed_eval_out);
+  if (const int rc = strategy_for(h, 0, 0, s, d, S)) return rc;
+  return prove_transcript(h, S, d, r, r_len, g, false, transcript, random_tape, proof_out, proof_cap, proof_len,
+                          claimed_eval_out);
   LB_CATCH
 }
 static int dense_outputs_checked(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
@@ -855,8 +835,7 @@ static int dense_outputs_checked(lasso_ctx* h, int strategy, int log_R, const la
   if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
   if (!out) return fail(LASSO_ERR_LENGTH, "outputs: null output");
   Strategy S{};
-  const std::string why = strategy_for(h, strategy, log_R, s, d, S);
-  if (!why.empty()) return fail(LASSO_ERR_STRATEGY, "outputs: " + why);
+  if (const int rc = strategy_for(h, strategy, log_R, s, d, S)) return rc;
   *out = new lasso_poly{dense_outputs(h->c, S, *d->d)};
   return 0;
 }
@@ -1065,31 +1044,29 @@ void lasso_poly_gens_destroy(lasso_poly_gens* g) {
   delete g->g;
   delete g;
 }
+// DensePolynomial::new of a power-of-two length, or (padded) new_padded of any length, from the caller's rows
 static int poly_new(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, bool device, void* stream,
-                    lasso_poly** out) {
+                    bool padded, lasso_poly** out) {
   if (out) *out = nullptr;
   if (!out) return fail(LASSO_ERR_LENGTH, "poly: null output");
-  if (!is_pow2(len)) return fail(LASSO_ERR_NOT_POW2, "poly: the length must be a power of two (dense_mlpoly.rs:63-66)");
-  if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly: at most 2^28 evaluations");
-  if (const int rc = poly_size_check(h, log2_exact_or_ceil(len))) return rc;
+  if (padded && len && !Z) return fail(LASSO_ERR_LENGTH, "poly padded: null evaluations");
+  if (!padded && !is_pow2(len)) return fail(LASSO_ERR_NOT_POW2, "poly: the length must be a power of two (dense_mlpoly.rs:63-66)");
+  if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly: at most 2^28 evaluations after padding");
+  if (const int rc = poly_size_check(h, log2_exact_or_ceil(next_pow2(std::max<size_t>(len, 1))))) return rc;
   if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly: row_stride must be at least 4 u64");
-  if (!device && !Z) return fail(LASSO_ERR_POINTER, "poly: null evaluations");
-  int err = 0;
-  Poly* p = poly_create(h->c, Z, len, row_stride, device, static_cast<cudaStream_t>(stream), &err);
-  if (err == 7) return fail(LASSO_ERR_POINTER, "poly: the evaluations are not device memory of the context's GPU");
-  if (err == 8) return fail(LASSO_ERR_VALUE, "poly: an evaluation is not a canonical Montgomery residue");
-  *out = new lasso_poly{p};
+  if (!device && len && !Z) return fail(LASSO_ERR_POINTER, "poly: null evaluations");
+  *out = new lasso_poly{poly_create(h->c, Z, len, row_stride, device, static_cast<cudaStream_t>(stream))};
   return 0;
 }
 int lasso_poly_create(lasso_ctx* h, const uint64_t* Z, size_t len, lasso_poly** out) {
   LB_TRY_CTX(h)
-  return poly_new(h, Z, len, 4, false, nullptr, out);
+  return poly_new(h, Z, len, 4, false, nullptr, false, out);
   LB_CATCH
 }
 int lasso_poly_create_device(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
                              lasso_poly** out) {
   LB_TRY_CTX(h)
-  return poly_new(h, Z, len, row_stride, true, stream, out);
+  return poly_new(h, Z, len, row_stride, true, stream, false, out);
   LB_CATCH
 }
 size_t lasso_poly_num_vars(const lasso_poly* p) { return p ? p->p->nv : 0; }
@@ -1114,14 +1091,10 @@ int lasso_poly_commit(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* 
   LB_TRY_CTX(h)
   if (const int rc = poly_use_check(h, p, g)) return rc;
   if (!g) return fail(LASSO_ERR_GENS, "poly commit: null generators");
-  const size_t need = 8 + 32 * ((size_t)1 << (p->p->nv / 2));
-  if (out_len) *out_len = need;
-  if (!out || cap < need) return fail(LASSO_ERR_LENGTH, "poly commit: output buffer too small");
-  auto t0 = std::chrono::steady_clock::now();
-  const std::vector<uint8_t> b = poly_commit(h->c, *p->p, *g->g);
-  h->c->t_commit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  memcpy(out, b.data(), b.size());
-  return 0;
+  const size_t need = poly_commitment_bytes(p->p->nv);
+  if (const int rc = out_room("poly commit", need, out, cap, out_len)) return rc;
+  const std::vector<uint8_t> b = timed(h->c->t_commit_ms, [&] { return poly_commit(h->c, *p->p, *g->g); });
+  return out_copy("poly commit", b, need, out);
   LB_CATCH
 }
 int lasso_poly_commit_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_poly_gens* g, lasso_random_tape* tape,
@@ -1130,15 +1103,15 @@ int lasso_poly_commit_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_poly
   if (const int rc = poly_use_check(h, p, g)) return rc;
   if (!g) return fail(LASSO_ERR_GENS, "poly commit: null generators");
   if (!tape) return fail(LASSO_ERR_LENGTH, "poly commit: null random tape");
-  const size_t L = (size_t)1 << (p->p->nv / 2), need = 8 + 32 * L;
-  if (out_len) *out_len = need;
-  if (!out || cap < need) return fail(LASSO_ERR_LENGTH, "poly commit: output buffer too small");
+  const size_t L = (size_t)1 << (p->p->nv / 2), need = poly_commitment_bytes(p->p->nv);
+  if (const int rc = out_room("poly commit", need, out, cap, out_len)) return rc;
   if (!blinds_out || blinds_cap < L) return fail(LASSO_ERR_LENGTH, "poly commit: room for fewer blinds than rows");
-  auto t0 = std::chrono::steady_clock::now();
-  const std::vector<fr_t> blinds = tape->t.random_vector("poly_blinds", L);  // dense_mlpoly.rs:165-170
-  const std::vector<uint8_t> b = poly_commit_hiding(h->c, *p->p, *g->g, blinds);
-  h->c->t_commit_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  memcpy(out, b.data(), b.size());
+  std::vector<fr_t> blinds;
+  const std::vector<uint8_t> b = timed(h->c->t_commit_ms, [&] {
+    blinds = tape->t.random_vector("poly_blinds", L);  // dense_mlpoly.rs:165-170
+    return poly_commit_hiding(h->c, *p->p, *g->g, blinds);
+  });
+  if (const int rc = out_copy("poly commit", b, need, out)) return rc;
   for (size_t i = 0; i < L; i++) memcpy(blinds_out + 4 * i, blinds[i].v, 32);
   return 0;
   LB_CATCH
@@ -1181,16 +1154,13 @@ int lasso_poly_eval_prove_hiding(lasso_ctx* h, const lasso_poly* p, const lasso_
   if (!load_scalars(blinds, n_blinds, bl)) return fail(LASSO_ERR_VALUE, "poly eval proof: a blind is not a canonical residue");
   if (blind_Zr && !load_scalars(blind_Zr, 1, bzr))
     return fail(LASSO_ERR_VALUE, "poly eval proof: blind_Zr is not a canonical residue");
-  // the proof's size is fixed by num_vars: L_vec and R_vec of log2(R) points, delta, beta, z1, z2
-  const size_t lg = p->p->nv - p->p->nv / 2, need = 2 * (8 + 32 * lg) + 4 * 32;
-  if (proof_len) *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "poly eval proof: output buffer too small");
-  auto t0 = std::chrono::steady_clock::now();
+  const size_t need = dpl_bytes(p->p->nv);
+  if (const int rc = out_room("poly eval proof", need, proof_out, proof_cap, proof_len)) return rc;
   uint8_t czr[32];
-  const std::vector<uint8_t> b = poly_eval_prove(h->c, *p->p, *g->g, rv, zr[0], transcript->t, tape->t, czr, bl, bzr[0]);
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (b.size() != need) return fail(-1, "poly eval proof: unexpected proof size");
-  memcpy(proof_out, b.data(), b.size());
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return poly_eval_prove(h->c, *p->p, *g->g, rv, zr[0], transcript->t, tape->t, czr, bl, bzr[0]);
+  });
+  if (const int rc = out_copy("poly eval proof", b, need, proof_out)) return rc;
   if (C_Zr_out) memcpy(C_Zr_out, czr, 32);
   return 0;
   LB_CATCH
@@ -1246,30 +1216,15 @@ int lasso_poly_split(lasso_ctx* h, const lasso_poly* p, size_t idx, lasso_poly**
   return 0;
   LB_CATCH
 }
-static int poly_new_padded(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, bool device, void* stream,
-                           lasso_poly** out) {
-  if (out) *out = nullptr;
-  if (!out || (len && !Z)) return fail(LASSO_ERR_LENGTH, "poly padded: null evaluations or output");
-  if (len > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "poly padded: at most 2^28 evaluations after padding");
-  const size_t full = next_pow2(std::max<size_t>(len, 1));
-  if (const int rc = poly_size_check(h, log2_exact_or_ceil(full))) return rc;
-  if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly padded: row_stride must be at least 4 u64");
-  int err = 0;
-  Poly* p = poly_create(h->c, Z, len, row_stride, device, static_cast<cudaStream_t>(stream), &err);
-  if (err == 7) return fail(LASSO_ERR_POINTER, "poly padded: the evaluations are not device memory of the context's GPU");
-  if (err == 8) return fail(LASSO_ERR_VALUE, "poly padded: an evaluation is not a canonical Montgomery residue");
-  *out = new lasso_poly{p};
-  return 0;
-}
 int lasso_poly_create_padded(lasso_ctx* h, const uint64_t* Z, size_t len, lasso_poly** out) {
   LB_TRY_CTX(h)
-  return poly_new_padded(h, Z, len, 4, false, nullptr, out);
+  return poly_new(h, Z, len, 4, false, nullptr, true, out);
   LB_CATCH
 }
 int lasso_poly_create_padded_device(lasso_ctx* h, const uint64_t* Z, size_t len, size_t row_stride, void* stream,
                                     lasso_poly** out) {
   LB_TRY_CTX(h)
-  return poly_new_padded(h, Z, len, row_stride, true, stream, out);
+  return poly_new(h, Z, len, row_stride, true, stream, true, out);
   LB_CATCH
 }
 int lasso_poly_read(lasso_ctx* h, const lasso_poly* p, uint64_t* out, size_t cap) {
@@ -1285,26 +1240,36 @@ int lasso_poly_read_device(lasso_ctx* h, const lasso_poly* p, uint64_t* dst, siz
   if (const int rc = poly_use_check(h, p, nullptr)) return rc;
   if (!dst) return fail(LASSO_ERR_LENGTH, "poly read: null destination");
   if (row_stride < 4) return fail(LASSO_ERR_LENGTH, "poly read: row_stride must be at least 4 u64");
-  if (poly_read_device(h->c, *p->p, dst, row_stride, static_cast<cudaStream_t>(stream)) == 7)
-    return fail(LASSO_ERR_POINTER, "poly read: the destination is not device memory of the context's GPU");
+  poly_read_device(h->c, *p->p, dst, row_stride, static_cast<cudaStream_t>(stream));
   return 0;
   LB_CATCH
 }
 
 // ---- many polynomials per call: merge, batched evaluation, one combined opening
+// The n polynomials of one call: each of this context (LASSO_ERR_STRATEGY), then, with same_nv, all of one num_vars
+// (LASSO_ERR_LENGTH).  ps receives them.
+static int poly_array(lasso_ctx* h, const char* what, const lasso_poly* const* polys, size_t n, bool same_nv,
+                      std::vector<const Poly*>& ps) {
+  for (size_t j = 0; j < n; j++)
+    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  for (size_t j = 1; same_nv && j < n; j++)
+    if (polys[j]->p->nv != polys[0]->p->nv)
+      return fail(LASSO_ERR_LENGTH, std::string(what) + ": the polynomials have different num_vars");
+  ps.resize(n);
+  for (size_t j = 0; j < n; j++) ps[j] = polys[j]->p;
+  return 0;
+}
 int lasso_poly_create_merge(lasso_ctx* h, const lasso_poly* const* polys, size_t n_polys, lasso_poly** out) {
   LB_TRY_CTX(h)
   if (out) *out = nullptr;
   if (!polys || n_polys == 0 || !out) return fail(LASSO_ERR_LENGTH, "merge: no polynomials, or a null output");
-  for (size_t j = 0; j < n_polys; j++)
-    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "merge", polys, n_polys, false, ps)) return rc;
   size_t total = 0;
-  for (size_t j = 0; j < n_polys; j++) {
-    total += polys[j]->p->len;  // each len <= 2^28: the running sum cannot wrap before it passes the limit
+  for (const Poly* p : ps) {
+    total += p->len;  // each len <= 2^28: the running sum cannot wrap before it passes the limit
     if (total > kPolyMaxLen) return fail(LASSO_ERR_LENGTH, "merge: at most 2^28 evaluations after padding");
   }
-  std::vector<const Poly*> ps(n_polys);
-  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
   *out = new lasso_poly{poly_merge(h->c, ps.data(), (int)n_polys)};
   return 0;
   LB_CATCH
@@ -1314,14 +1279,10 @@ int lasso_poly_evaluate_batch(lasso_ctx* h, const lasso_poly* const* polys, size
   LB_TRY_CTX(h)
   if (!polys || n_polys == 0 || n_polys > (size_t)kDotMaxPolys || !out)
     return fail(LASSO_ERR_LENGTH, "evaluate batch: 1..64 polynomials and an output");
-  for (size_t j = 0; j < n_polys; j++)
-    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
-  for (size_t j = 1; j < n_polys; j++)
-    if (polys[j]->p->nv != polys[0]->p->nv) return fail(LASSO_ERR_LENGTH, "evaluate batch: the polynomials have different num_vars");
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "evaluate batch", polys, n_polys, true, ps)) return rc;
   std::vector<fr_t> rv;
-  if (const int rc = load_point(*polys[0]->p, r, r_len, rv)) return rc;
-  std::vector<const Poly*> ps(n_polys);
-  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
+  if (const int rc = load_point(*ps[0], r, r_len, rv)) return rc;
   const std::vector<fr_t> v = poly_evaluate_batch(h->c, ps.data(), (int)n_polys, rv);
   for (size_t j = 0; j < n_polys; j++) memcpy(out + 4 * j, v[j].v, 32);
   return 0;
@@ -1339,20 +1300,16 @@ int lasso_combined_eval_prove(lasso_ctx* h, const lasso_poly* combined, const la
   const size_t nv = combined->p->nv;
   if (nv != r_len + log2_exact_or_ceil(next_pow2(n_evals)))
     return fail(LASSO_ERR_LENGTH, "combined eval proof: num_vars != r.len() + log2(next_pow2(n_evals))");
-  // the PolyEvalProof of lasso_poly_eval_prove at num_vars
-  const size_t lg = nv - nv / 2, need = 2 * (8 + 32 * lg) + 4 * 32;
-  if (proof_len) *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "combined eval proof: output buffer too small");
+  const size_t need = dpl_bytes(nv);  // the PolyEvalProof of lasso_poly_eval_prove at num_vars
+  if (const int rc = out_room("combined eval proof", need, proof_out, proof_cap, proof_len)) return rc;
   if (!transcript || !tape) return fail(LASSO_ERR_LENGTH, "combined eval proof: null transcript or random tape");
   std::vector<fr_t> ev, rv;
   if (!load_scalars(evals, n_evals, ev)) return fail(LASSO_ERR_VALUE, "combined eval proof: an eval is not a canonical residue");
   if (!load_scalars(r, r_len, rv)) return fail(LASSO_ERR_VALUE, "combined eval proof: a coordinate of r is not a canonical residue");
-  auto t0 = std::chrono::steady_clock::now();
-  const std::vector<uint8_t> b = combined_eval_prove(h->c, *combined->p, *g->g, ev, rv, transcript->t, tape->t);
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (b.size() != need) return fail(-1, "combined eval proof: unexpected proof size");
-  memcpy(proof_out, b.data(), b.size());
-  return 0;
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return combined_eval_prove(h->c, *combined->p, *g->g, ev, rv, transcript->t, tape->t);
+  });
+  return out_copy("combined eval proof", b, need, proof_out);
   LB_CATCH
 }
 
@@ -1385,24 +1342,16 @@ int lasso_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly* co
   if (!polys || n_polys != (size_t)g->g.n_inputs)
     return fail(LASSO_ERR_STRATEGY, "sumcheck: " + std::to_string(n_polys) + " polynomials for a combining function of " +
                                         std::to_string(g->g.n_inputs) + " inputs");
-  for (size_t j = 0; j < n_polys; j++)
-    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
-  const size_t nv = polys[0]->p->nv;
-  for (size_t j = 1; j < n_polys; j++)
-    if (polys[j]->p->nv != nv) return fail(LASSO_ERR_LENGTH, "sumcheck: the polynomials have different num_vars");
-  if (num_rounds < 1 || num_rounds > nv) return fail(LASSO_ERR_LENGTH, "sumcheck: num_rounds must be in 1..num_vars");
-  // SumcheckInstanceProof: a u64 count, then per round a u64 length and the degree coefficients except the linear one
-  const size_t need = 8 + num_rounds * (8 + 32 * (size_t)g->g.degree);
-  if (proof_len) *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "sumcheck: output buffer too small");
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "sumcheck", polys, n_polys, true, ps)) return rc;
+  if (num_rounds < 1 || num_rounds > ps[0]->nv) return fail(LASSO_ERR_LENGTH, "sumcheck: num_rounds must be in 1..num_vars");
+  const size_t need = sumcheck_bytes(num_rounds, (size_t)g->g.degree);
+  if (const int rc = out_room("sumcheck", need, proof_out, proof_cap, proof_len)) return rc;
   if (!transcript || !r_out || !final_evals_out) return fail(LASSO_ERR_LENGTH, "sumcheck: null transcript or output");
-  std::vector<const Poly*> ps(n_polys);
-  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
-  auto t0 = std::chrono::steady_clock::now();
-  const SumcheckOut o = sumcheck_prove(h->c, g->g, ps.data(), (int)n_polys, num_rounds, transcript->t);
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (o.proof.size() != need) return fail(-1, "sumcheck: unexpected proof size");
-  memcpy(proof_out, o.proof.data(), need);
+  const SumcheckOut o = timed(h->c->t_prove_ms, [&] {
+    return sumcheck_prove(h->c, g->g, ps.data(), (int)n_polys, num_rounds, transcript->t);
+  });
+  if (const int rc = out_copy("sumcheck", o.proof, need, proof_out)) return rc;
   for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
   for (size_t j = 0; j < n_polys; j++) memcpy(final_evals_out + 4 * j, o.final_evals[j].v, 32);
   if (claim_out) memcpy(claim_out, o.claim.v, 32);
@@ -1417,35 +1366,24 @@ int lasso_sumcheck_prove_cubic_batched(lasso_ctx* h, const lasso_poly* const* A,
   LB_TRY_CTX(h)
   if (n < 1 || n > 32) return fail(LASSO_ERR_STRATEGY, "cubic sumcheck: 1 <= n <= 32 pairs");
   if (!A || !B) return fail(LASSO_ERR_STRATEGY, "cubic sumcheck: null polynomial array");
-  for (size_t k = 0; k < n; k++) {
-    if (const int rc = poly_use_check(h, A[k], nullptr)) return rc;
-    if (const int rc = poly_use_check(h, B[k], nullptr)) return rc;
-  }
-  if (const int rc = poly_use_check(h, C, nullptr)) return rc;
-  const size_t nv = C->p->nv;
-  for (size_t k = 0; k < n; k++)
-    if (A[k]->p->nv != nv || B[k]->p->nv != nv)
-      return fail(LASSO_ERR_LENGTH, "cubic sumcheck: the polynomials have different num_vars");
-  if (num_rounds < 1 || num_rounds > nv) return fail(LASSO_ERR_LENGTH, "cubic sumcheck: num_rounds must be in 1..num_vars");
-  // SumcheckInstanceProof of a cubic: a u64 count, then per round a u64 length and 3 coefficients
-  const size_t need = 8 + num_rounds * (8 + 32 * 3);
-  if (proof_len) *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "cubic sumcheck: output buffer too small");
+  // A_0.., B_0.., C: one array for the checks
+  std::vector<const lasso_poly*> all(A, A + n);
+  all.insert(all.end(), B, B + n);
+  all.push_back(C);
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "cubic sumcheck", all.data(), all.size(), true, ps)) return rc;
+  if (num_rounds < 1 || num_rounds > ps[0]->nv) return fail(LASSO_ERR_LENGTH, "cubic sumcheck: num_rounds must be in 1..num_vars");
+  const size_t need = sumcheck_bytes(num_rounds, 3);
+  if (const int rc = out_room("cubic sumcheck", need, proof_out, proof_cap, proof_len)) return rc;
   if (!transcript || !coeffs || !claim || !r_out || !claims_A_out || !claims_B_out || !claim_C_out)
     return fail(LASSO_ERR_LENGTH, "cubic sumcheck: null transcript, input or output");
   std::vector<fr_t> cv, e;
   if (!load_scalars(coeffs, n, cv)) return fail(LASSO_ERR_VALUE, "cubic sumcheck: a coefficient is not a canonical residue");
   if (!load_scalars(claim, 1, e)) return fail(LASSO_ERR_VALUE, "cubic sumcheck: the claim is not a canonical residue");
-  std::vector<const Poly*> pa(n), pb(n);
-  for (size_t k = 0; k < n; k++) {
-    pa[k] = A[k]->p;
-    pb[k] = B[k]->p;
-  }
-  auto t0 = std::chrono::steady_clock::now();
-  const CubicOut o = cubic_prove(h->c, pa.data(), pb.data(), (int)n, *C->p, cv, e[0], num_rounds, transcript->t);
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (o.proof.size() != need) return fail(-1, "cubic sumcheck: unexpected proof size");
-  memcpy(proof_out, o.proof.data(), need);
+  const CubicOut o = timed(h->c->t_prove_ms, [&] {
+    return cubic_prove(h->c, ps.data(), ps.data() + n, (int)n, *ps[2 * n], cv, e[0], num_rounds, transcript->t);
+  });
+  if (const int rc = out_copy("cubic sumcheck", o.proof, need, proof_out)) return rc;
   for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
   for (size_t k = 0; k < n; k++) {
     memcpy(claims_A_out + 4 * k, o.finals[k].v, 32);
@@ -1463,14 +1401,10 @@ int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* 
   if (!polys || n_polys != (size_t)g->g.n_inputs)
     return fail(LASSO_ERR_STRATEGY, "comb poly: " + std::to_string(n_polys) + " polynomials for a combining function of " +
                                         std::to_string(g->g.n_inputs) + " inputs");
-  for (size_t j = 0; j < n_polys; j++)
-    if (const int rc = poly_use_check(h, polys[j], nullptr)) return rc;
-  for (size_t j = 1; j < n_polys; j++)
-    if (polys[j]->p->nv != polys[0]->p->nv) return fail(LASSO_ERR_LENGTH, "comb poly: the polynomials have different num_vars");
-  if (const int rc = poly_size_check(h, polys[0]->p->nv)) return rc;
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "comb poly", polys, n_polys, true, ps)) return rc;
+  if (const int rc = poly_size_check(h, ps[0]->nv)) return rc;
   if (!out) return fail(LASSO_ERR_LENGTH, "comb poly: null output");
-  std::vector<const Poly*> ps(n_polys);
-  for (size_t j = 0; j < n_polys; j++) ps[j] = polys[j]->p;
   *out = new lasso_poly{poly_create_comb(h->c, g->g, ps.data(), (int)n_polys)};
   return 0;
   LB_CATCH
@@ -1517,10 +1451,8 @@ int lasso_gp_prove(lasso_ctx* h, const lasso_gp_circuit* const* circuits, size_t
   const size_t v = circuits[0]->ci->num_layers;
   for (size_t k = 1; k < n; k++)
     if (circuits[k]->ci->num_layers != v) return fail(LASSO_ERR_LENGTH, "grand product: the circuits have different num_vars");
-  // per layer i < v: a sumcheck of i cubic rounds (8 + 8 + 104 i) and two vectors of n claims (2 (8 + 32 n))
-  const size_t need = 8 + v * (24 + 64 * n) + 52 * v * (v - 1);
-  if (proof_len) *proof_len = need;
-  if (!proof_out || proof_cap < need) return fail(LASSO_ERR_LENGTH, "grand product: output buffer too small");
+  const size_t need = gpa_bytes(n, v);
+  if (const int rc = out_room("grand product", need, proof_out, proof_cap, proof_len)) return rc;
   if (!transcript || !r_out || !claims_out) return fail(LASSO_ERR_LENGTH, "grand product: null transcript or output");
   std::vector<Circuit*> cs(n);
   std::vector<fr_t> products(n);
@@ -1529,11 +1461,8 @@ int lasso_gp_prove(lasso_ctx* h, const lasso_gp_circuit* const* circuits, size_t
     products[k] = circuits[k]->product;
     circuits[k]->proven = true;
   }
-  auto t0 = std::chrono::steady_clock::now();
-  const GrandProductOut o = gp_prove(h->c, cs, products, transcript->t);
-  h->c->t_prove_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
-  if (o.proof.size() != need) return fail(-1, "grand product: unexpected proof size");
-  memcpy(proof_out, o.proof.data(), need);
+  const GrandProductOut o = timed(h->c->t_prove_ms, [&] { return gp_prove(h->c, cs, products, transcript->t); });
+  if (const int rc = out_copy("grand product", o.proof, need, proof_out)) return rc;
   for (size_t j = 0; j < v; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
   for (size_t k = 0; k < n; k++) memcpy(claims_out + 4 * k, o.claims[k].v, 32);
   return 0;

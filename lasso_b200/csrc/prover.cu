@@ -581,14 +581,10 @@ static void densify_on_device(Ctx* c, Dense* d, size_t n, const DzIndices& idx, 
   launch_from_u32(d->d_m_u32.p, d->d_m_fr.p, nm, c->st);
 }
 
-Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m, int* err) {
+Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m) {
   SpanTimer sp(c, "Densify");
-  *err = 0;
   std::unique_ptr<Dense> d = dense_shape(c, n, C, log_m);
-  if (!d) {
-    *err = 4;
-    return nullptr;
-  }
+  if (!d) throw LbError(LASSO_ERR_STRATEGY, "densify: invalid input");
   const size_t G = (size_t)c->world, gr = (size_t)c->rank;
   const size_t s = d->s, m = d->m, s_loc = d->s_loc, m_loc = d->m_loc;
   const size_t nl = ((size_t)1 << d->nv_l) / G, nm = ((size_t)1 << d->nv_m) / G;  // local lengths
@@ -672,8 +668,7 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
         }
         if (any_bad) {
           c->sync();
-          *err = 3;
-          return nullptr;
+          throw LbError(LASSO_ERR_INDEX_RANGE, "densify: an index is >= m");
         }
         if (G > 1) comm_allgather(c, d_mine.p, d_idx.p, rows_per * C * sizeof(uint32_t));
       }
@@ -734,10 +729,7 @@ Dense* densify(Ctx* c, const uint64_t* indices, size_t n, size_t C, size_t log_m
     for (auto& t : th) t.join();
   }
   for (size_t i = 0; i < C; i++)
-    if (bad[i]) {
-      *err = 3;
-      return nullptr;
-    }
+    if (bad[i]) throw LbError(LASSO_ERR_INDEX_RANGE, "densify: an index is >= m");
   d->d_l_u32.alloc(c, nl);
   d->d_m_u32.alloc(c, nm);
   d->d_l_fr.alloc(c, nl);
@@ -761,23 +753,17 @@ static bool device_memory_of(const Ctx* c, const void* p) {
 // densify from an index matrix in device memory of the context's GPU (lasso_densify_device): no staging, the GPU sort
 // at every size, the range check in the extract kernel.  `caller`: the stream the matrix is ordered on.
 Dense* densify_device(Ctx* c, const void* indices, size_t elem_bytes, size_t n, size_t C, size_t row_stride,
-                      size_t col_stride, size_t log_m, cudaStream_t caller, int* err) {
+                      size_t col_stride, size_t log_m, cudaStream_t caller) {
   SpanTimer sp(c, "Densify");
-  *err = 0;
   std::unique_ptr<Dense> d = elem_bytes == 4 || elem_bytes == 8 ? dense_shape(c, n, C, log_m) : nullptr;
-  if (!d || !densify_gpu_supported(d->s, log_m)) {
-    *err = 4;
-    return nullptr;
-  }
+  if (!d || !densify_gpu_supported(d->s, log_m)) throw LbError(LASSO_ERR_STRATEGY, "densify_device: invalid input");
   // the first and the last entry must both lie in device memory of this GPU (host, pinned and other GPUs' memory fail)
   size_t last = 0, a = 0, b = 0;
   const bool wraps = __builtin_mul_overflow(n - 1, row_stride, &a) || __builtin_mul_overflow(C - 1, col_stride, &b) ||
                      __builtin_add_overflow(a, b, &last) || __builtin_mul_overflow(last, elem_bytes, &last) ||
                      (uintptr_t)indices > UINTPTR_MAX - last;
-  if (!indices || wraps || !device_memory_of(c, indices) || !device_memory_of(c, (const char*)indices + last)) {
-    *err = 7;
-    return nullptr;
-  }
+  if (!indices || wraps || !device_memory_of(c, indices) || !device_memory_of(c, (const char*)indices + last))
+    throw LbError(LASSO_ERR_POINTER, "densify_device: the indices are not device memory of the context's GPU");
   // the matrix is read only after the work the caller enqueued on `caller` before this call
   LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
   LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
@@ -787,10 +773,7 @@ Dense* densify_device(Ctx* c, const void* indices, size_t elem_bytes, size_t n, 
   // the caller's later work on `caller` (a caching allocator freeing the matrix, say) comes after the last read of it
   LB_CUDA_CHECK(cudaStreamWaitEvent(caller, c->ev_aux, 0));
   LB_CUDA_CHECK(cudaEventSynchronize(c->ev_aux));  // the verdict; the sort may still run
-  if (*h_bad) {
-    *err = 3;
-    return nullptr;
-  }
+  if (*h_bad) throw LbError(LASSO_ERR_INDEX_RANGE, "densify_device: an index is >= m");
   return d.release();
 }
 
@@ -1611,26 +1594,17 @@ static DotProductProofLogBytes prove_joint(Ctx* c, const Gens& g, PolySrc Z, siz
 }
 
 // ---------------------------------------------------------------------------------------------- prove
-// The serialised size of a PolyEvalProof at nv variables: L_vec and R_vec of nv - nv/2 points, delta, beta, z1, z2
-static size_t dpl_bytes(size_t nv) { return 2 * (8 + 32 * (nv - nv / 2)) + 4 * 32; }
-// The serialised size of a BatchedGrandProductArgument over n circuits of v variables: layer j has j cubic rounds
-static size_t gpa_bytes(size_t n, size_t v) { return 8 + v * (24 + 64 * n) + 52 * v * (v - 1); }
+size_t dpl_bytes(size_t nv) { return 2 * (8 + 32 * (nv - nv / 2)) + 4 * 32; }
+size_t gpa_bytes(size_t n, size_t v) { return 8 + v * (24 + 64 * n) + 52 * v * (v - 1); }
+size_t sumcheck_bytes(size_t rounds, size_t degree) { return 8 + rounds * (8 + 32 * degree); }
+size_t poly_commitment_bytes(size_t num_vars) { return 8 + 32 * ((size_t)1 << (num_vars / 2)); }
 size_t proof_bytes(const Strategy& S, const Dense& dense, const Gens& g) {
   const size_t alpha = (size_t)S.num_memories(), C = dense.C, log_s = log2_exact_or_ceil(dense.s);
   return 8 + 32 * ((size_t)1 << (g.nv_d / 2))                        // comm_derefs
-         + 8 + log_s * (8 + 32 * (size_t)S.sumcheck_poly_degree())  // primary sumcheck
+         + sumcheck_bytes(log_s, (size_t)S.sumcheck_poly_degree())  // primary sumcheck
          + 32 + 32 * alpha + dpl_bytes(g.nv_d)                      // claimed_evaluation, eval_derefs, proof_derefs
          + 4 * 32 * alpha + gpa_bytes(2 * alpha, dense.log_m) + gpa_bytes(2 * alpha, log_s)  // product layer
          + 32 * (3 * C + alpha) + dpl_bytes(g.nv_l) + dpl_bytes(g.nv_m) + dpl_bytes(g.nv_d);  // hash layer
-}
-
-std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
-                           const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,
-                           std::vector<fr_t>* challenges) {
-  Transcript transcript(transcript_label);
-  transcript.trace = challenges;
-  RandomTape tape(tape_label, tape_seed);
-  return prove(c, S, dense, r, g, transcript, tape, nullptr);
 }
 
 std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
@@ -1778,7 +1752,8 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     std::vector<fr_t> claims_rw, claims_if;
     for (size_t i = 0; i < alpha; i++) {
       fr_t hi = evaluate(0, 2 * i), hr = evaluate(1, 2 * i), hw = evaluate(1, 2 * i + 1), hf = evaluate(0, 2 * i + 1);
-      if (!fr_eq(fr_mul(hi, hw), fr_mul(hr, hf))) throw std::runtime_error("multiset hash check failed (memory_checking.rs:689)");
+      if (!fr_eq(fr_mul(hi, hw), fr_mul(hr, hf)))
+        throw LbError(LASSO_ERR_MULTISET, "multiset hash check failed (memory_checking.rs:689)");
       transcript.append_scalar("claim_hash_init", hi);
       transcript.append_scalar("claim_hash_read", hr);
       transcript.append_scalar("claim_hash_write", hw);
@@ -1866,14 +1841,11 @@ static bool rows_on_device(const Ctx* c, const uint64_t* Z, size_t rows, size_t 
 // memory and uploaded in one copy (1/G of the PCIe bytes); device rows are read by the ingest kernel at base rank and
 // stride G rows.  The verdict and the widest value are then agreed in one message to every process, so that every rank
 // fails together, or makes the same u32-mirror decision.
-Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err) {
+Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller) {
   SpanTimer sp(c, "DensePolynomial.new");
-  *err = 0;
   const size_t G = (size_t)c->world, gr = (size_t)c->rank;
-  if (device && len && !rows_on_device(c, Z, len, row_stride)) {
-    *err = 7;
-    return nullptr;
-  }
+  if (device && len && !rows_on_device(c, Z, len, row_stride))
+    throw LbError(LASSO_ERR_POINTER, "poly: the evaluations are not device memory of the context's GPU");
   std::unique_ptr<Poly> p(new Poly());
   p->ctx = c;
   p->len = next_pow2(std::max<size_t>(len, 1));  // new_padded (dense_mlpoly.rs:75-87): len itself when a power of two
@@ -1921,10 +1893,7 @@ Poly* poly_create(Ctx* c, const uint64_t* Z, size_t len, size_t row_stride, bool
     f[1] = 0;
     for (size_t r = 0; r < G; r++) f[1] = std::max(f[1], all[1 + r].v[0]);
   }
-  if (f[0]) {
-    *err = 8;
-    return nullptr;
-  }
+  if (f[0]) throw LbError(LASSO_ERR_VALUE, "poly: an evaluation is not a canonical Montgomery residue");
   p->bits = f[1];
   // integer values: the u32 mirror feeds commit_u32 / bound_u32 / multi_dot_u32, which give the same bytes as the
   // Montgomery forms (lasso_strategy_create_fr sets the same precedent)
@@ -2231,8 +2200,9 @@ void poly_read(Ctx* c, const Poly& p, uint64_t* out) {
   DBuf<fr_t> all;
   c->d2h(out, poly_whole(c, p, all), p.len * sizeof(fr_t));
 }
-int poly_read_device(Ctx* c, const Poly& p, uint64_t* dst, size_t row_stride, cudaStream_t caller) {
-  if (!rows_on_device(c, dst, p.len, row_stride)) return 7;
+void poly_read_device(Ctx* c, const Poly& p, uint64_t* dst, size_t row_stride, cudaStream_t caller) {
+  if (!rows_on_device(c, dst, p.len, row_stride))
+    throw LbError(LASSO_ERR_POINTER, "poly read: the destination is not device memory of the context's GPU");
   DBuf<fr_t> all;
   const fr_t* src = poly_whole(c, p, all);
   // the copy runs on the caller's stream after the polynomial is ready, and the library's later work (freeing the
@@ -2243,7 +2213,6 @@ int poly_read_device(Ctx* c, const Poly& p, uint64_t* dst, size_t row_stride, cu
                                   cudaMemcpyDeviceToDevice, caller));
   LB_CUDA_CHECK(cudaEventRecord(c->ev_caller, caller));
   LB_CUDA_CHECK(cudaStreamWaitEvent(c->st, c->ev_caller, 0));
-  return 0;
 }
 
 // ---------------------------------------------------------------------------------------------- caller sumchecks

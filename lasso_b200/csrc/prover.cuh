@@ -7,13 +7,21 @@
 #include <chrono>
 #include <map>
 #include <memory>
+#include <stdexcept>
 #include <vector>
 
+#include "../../include/lasso_b200.h"
 #include "host_transcript.hpp"
 #include "kernels.cuh"
 #include "msm.cuh"
 
 namespace lb {
+
+// A failure of the caller's input that the C boundary returns as its own LASSO_ERR_* code; any other exception is -1
+struct LbError : std::runtime_error {
+  int code;
+  LbError(int code, const std::string& msg) : std::runtime_error(msg), code(code) {}
+};
 
 struct Ctx {
   int device = 0;
@@ -326,23 +334,28 @@ void ctx_destroy(Ctx*);
 Gens* gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t c, size_t s, size_t num_memories,
                   size_t log_m);
 size_t gens_points_needed(size_t c, size_t s, size_t num_memories, size_t log_m);
-Dense* densify(Ctx*, const uint64_t* indices, size_t n_lookups, size_t C, size_t log_m, int* err);
-// *err: 3 an entry >= m, 4 bad shape or elem_bytes, 7 the matrix is not device memory of the context's GPU
+// Both throw LbError: LASSO_ERR_INDEX_RANGE for an entry >= m, LASSO_ERR_STRATEGY for a bad shape or elem_bytes,
+// LASSO_ERR_POINTER when the matrix is not device memory of the context's GPU.  Sharded: every rank throws together.
+Dense* densify(Ctx*, const uint64_t* indices, size_t n_lookups, size_t C, size_t log_m);
 Dense* densify_device(Ctx*, const void* indices, size_t elem_bytes, size_t n_lookups, size_t C, size_t row_stride,
-                      size_t col_stride, size_t log_m, cudaStream_t caller, int* err);
+                      size_t col_stride, size_t log_m, cudaStream_t caller);
 std::vector<uint8_t> commit(Ctx*, const Dense&, const Gens&);
 // SparsePolynomialEvaluationProof::prove (surge.rs:118-211) on the caller's transcript and tape, advanced in place.
 // Throws before the first transcript write when S or g do not fit the dense; the working memory is reserved in the
-// context's pool before it too.  *claimed_evaluation (may be null): the primary sumcheck's claim.
+// context's pool before it too.  *claimed_evaluation (may be null): the primary sumcheck's claim.  A failed multiset
+// check throws LbError(LASSO_ERR_MULTISET) after the transcript has moved.
 std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr_t>& r, const Gens&, Transcript&,
                            RandomTape&, fr_t* claimed_evaluation);
-// the same on Transcript::new(transcript_label) and RandomTape::new(tape_label) seeded with tape_seed; challenges (may
-// be null) receives every challenge drawn
-std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr_t>& r, const Gens&,
-                           const std::string& transcript_label, const std::string& tape_label, const fr_t& tape_seed,
-                           std::vector<fr_t>* challenges);
-// the size of prove's output, fixed by the shapes (S and g fit dense)
+// Serialised sizes, fixed by the shapes.  prove's output (S and g fit dense):
 size_t proof_bytes(const Strategy& S, const Dense&, const Gens&);
+// a PolyEvalProof at nv variables: L_vec and R_vec of nv - nv/2 points, delta, beta, z1, z2
+size_t dpl_bytes(size_t nv);
+// a BatchedGrandProductArgument over n circuits of v variables: layer j has j cubic rounds
+size_t gpa_bytes(size_t n, size_t v);
+// a SumcheckInstanceProof: a u64 count, then per round a u64 length and the degree coefficients except the linear one
+size_t sumcheck_bytes(size_t rounds, size_t degree);
+// a PolyCommitment at num_vars: a u64 count, then one point per row, 2^(num_vars/2) rows
+size_t poly_commitment_bytes(size_t num_vars);
 // The lookup outputs v[k] = combine_lookups(E_0[k], .., E_{alpha-1}[k]) for k < s as a new polynomial of log2(s)
 // variables, with a u32 mirror when every value is below 2^32.  Single-GPU contexts (the caller checks).
 Poly* dense_outputs(Ctx*, const Strategy& S, const Dense&);
@@ -361,10 +374,11 @@ inline bool poly_fits(size_t num_vars, int world) { return poly_R(num_vars) >= (
 // nullptr when n_points < R + 2
 Gens* poly_gens_create(Ctx*, const uint64_t* stream_affine, size_t n_points, size_t num_vars);
 // Z: len rows of 4 u64 Montgomery limbs, row_stride u64 apart; host memory, or device memory of the context's GPU
-// (device != 0, read in the order of `caller`).  *err: 8 an entry is not a canonical residue, 7 not device memory.
+// (device != 0, read in the order of `caller`).  Throws LbError: LASSO_ERR_VALUE for an entry that is not a canonical
+// residue, LASSO_ERR_POINTER for rows that are not device memory of the context's GPU.
 // Any len: zero-padded to next_pow2(max(len, 1)) evaluations (DensePolynomial::new_padded, dense_mlpoly.rs:75-87).
 // Sharded: every rank passes the whole polynomial and reads its rows; the verdict and the width are agreed by all ranks.
-Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller, int* err);
+Poly* poly_create(Ctx*, const uint64_t* Z, size_t len, size_t row_stride, bool device, cudaStream_t caller);
 std::vector<uint8_t> poly_commit(Ctx*, const Poly&, const Gens&);  // serialised PolyCommitment
 // the hiding PolyCommitment of the same size: row i is committed with blinds[i] on h (blinds.size() == L)
 std::vector<uint8_t> poly_commit_hiding(Ctx*, const Poly&, const Gens&, const std::vector<fr_t>& blinds);
@@ -395,9 +409,10 @@ Poly* poly_bind_bot(Ctx*, const Poly&, const std::vector<fr_t>& r);
 // split(idx) (dense_mlpoly.rs:101-107), idx a power of two, 2 idx <= len: the parent's bits and u32 mirror, halved
 void poly_split(Ctx*, const Poly&, size_t idx, Poly** lo, Poly** hi);
 // the len evaluations in natural order, 4 Montgomery limbs each: to host memory, or (poly_read_device) to device
-// memory of the context's GPU, row i at dst + i * row_stride, in the order of `caller`; 7: dst is not such memory
+// memory of the context's GPU, row i at dst + i * row_stride, in the order of `caller`; LbError(LASSO_ERR_POINTER) when
+// dst is not such memory
 void poly_read(Ctx*, const Poly&, uint64_t* out);
-int poly_read_device(Ctx*, const Poly&, uint64_t* dst, size_t row_stride, cudaStream_t caller);
+void poly_read_device(Ctx*, const Poly&, uint64_t* dst, size_t row_stride, cudaStream_t caller);
 
 // A combining function g(x_0..x_{n_inputs-1}) of SumcheckInstanceProof::prove_arbitrary: a checked program (capi.cu)
 // with its slots allocated, and the declared combined_degree.  Host only.

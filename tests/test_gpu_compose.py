@@ -246,6 +246,25 @@ def _raw_prove(ctx, S, dense, r, gens, t, tape, cap=1 << 22, proof_len=True, r_l
     return rc, n.value
 
 
+def _raw_prove_labels(ctx, S, dense, r, gens, seed, cap=1 << 22, label=b"example"):
+    """lasso_prove / lasso_prove_custom -> (error code, *proof_len)"""
+    import ctypes as C
+
+    from lasso_b200.api import _p, lib
+
+    out = np.zeros(max(cap, 1), dtype=np.uint8)
+    n = C.c_size_t(0)
+    r = np.ascontiguousarray(r, dtype=np.uint64).reshape(-1, 4)
+    seed = np.ascontiguousarray(seed, dtype=np.uint64)
+    tail = (dense._h, _p(r), C.c_size_t(r.shape[0]), gens._h, label, b"proof", _p(seed), _p(out), C.c_size_t(cap),
+            C.byref(n), None, C.c_size_t(0), None)
+    if isinstance(S, lb.CustomStrategy):
+        rc = lib().lasso_prove_custom(ctx._h, S._h, *tail)
+    else:
+        rc = lib().lasso_prove(ctx._h, S.kind, S.log_r, *tail)
+    return rc, n.value
+
+
 def test_errors_before_anything_moves(ctx):
     S, C_, log_m, _, _ = strategy(ctx, "xor")
     idx, dense, stream, gens, r, seed = setup(ctx, S, C_, log_m, 256, 4)
@@ -282,6 +301,27 @@ def test_errors_before_anything_moves(ctx):
             assert plen == need
         assert _next(t) == _next(lb.Transcript(b"example"))
         assert tape.random_scalar(b"x").tolist() == lb.RandomTape(b"proof", seed).random_scalar(b"x").tolist()
+    # the label path takes the same checks, built-in and custom: each error before any launch
+    for name in ("xor", "custom_u32"):
+        S_l, C_l, log_m_l, _, _ = strategy(ctx, name)
+        _, d_l, _, g_l, r_l, seed_l = setup(ctx, S_l, C_l, log_m_l, 256, 5)
+        need_l = len(lb.SparsePolynomialEvaluationProof.prove(ctx, S_l, d_l, r_l, g_l, tape_seed=seed_l).bytes)
+        n_other = lb.gens_points_needed(C_l, d_l.s * 2, S_l.num_memories, log_m_l)
+        other_l = lb.SparsePolyCommitmentGens.new(ctx, b"gens_sparse_poly", C_l, d_l.s * 2, S_l.num_memories, log_m_l,
+                                                  stream=ol.generators(n_other))
+        bad_r_l = r_l.copy()
+        bad_r_l[0] = ol.int_to_limbs(ol.L_FR)
+        for over, code in [(dict(gens=other_l), LASSO_ERR_GENS), (dict(r=bad_r_l), LASSO_ERR_VALUE),
+                           (dict(seed=ol.int_to_limbs(ol.L_FR)), LASSO_ERR_VALUE), (dict(label=None), LASSO_ERR_LENGTH),
+                           (dict(cap=need_l - 1), LASSO_ERR_LENGTH)]:
+            kw = dict(r=r_l, gens=g_l, seed=seed_l)
+            kw.update(over)
+            l0 = ctx.launches
+            rc, plen = _raw_prove_labels(ctx, S_l, d_l, **kw)
+            assert rc == code, (name, over, rc)
+            assert ctx.launches == l0
+            if over.get("cap"):
+                assert plen == need_l
     # LT with C = 8 is provable, with C = 9 not (its memories make 36 circuits)
     idx9 = np.zeros((16, 9), dtype=np.uint64)
     d9 = lb.DensifiedRepresentation.from_lookup_indices(ctx, idx9, 4)
@@ -298,6 +338,19 @@ def test_errors_before_anything_moves(ctx):
         dense.outputs(S_other)
     assert e.value.code == LASSO_ERR_STRATEGY
     del S_other
+    ctx2.close()
+
+
+def test_label_path_shares_generators_across_contexts(ctx):
+    """lasso_prove on a second context of the same GPU with the first context's generators, whose tables are only read
+    (the batched-throughput mode of bench.py): the first context's bytes"""
+    S, C_, log_m, _, _ = strategy(ctx, "xor")
+    idx, dense, stream, gens, r, seed = setup(ctx, S, C_, log_m, 256, 6)
+    want = lb.SparsePolynomialEvaluationProof.prove(ctx, S, dense, r, gens, tape_seed=seed).bytes
+    ctx2 = lb.Context(0)
+    d2 = lb.DensifiedRepresentation.from_lookup_indices(ctx2, idx, log_m)
+    assert lb.SparsePolynomialEvaluationProof.prove(ctx2, S, d2, r, gens, tape_seed=seed).bytes == want
+    del d2
     ctx2.close()
 
 
