@@ -293,8 +293,10 @@ int lasso_random_tape_random_vector(lasso_random_tape*, const char* label, size_
  * otherwise LASSO_ERR_LENGTH before any launch (lasso_poly_gens_create, lasso_poly_create[_device], lasso_poly_create_eq,
  * lasso_poly_create_comb).  Commitments make one all-gather of the row partials; evaluations add the ranks' partial
  * values in one message to every process; openings gather L.Z and run the Bulletproofs rounds replicated.
- * lasso_sumcheck_prove_cubic_batched is collective too.  lasso_sumcheck_prove, lasso_gp_circuit_create, lasso_gp_prove
- * and lasso_dense_outputs[_custom] are not available on a sharded context (LASSO_ERR_STRATEGY). */
+ * lasso_sumcheck_prove_cubic_batched is collective too.  lasso_sumcheck_prove, lasso_gp_circuit_create, lasso_gp_prove,
+ * lasso_dense_outputs[_custom] and the memory-checking calls (lasso_lookup_polys[_custom], lasso_dense_poly,
+ * lasso_memory_check_prove[_custom], lasso_memory_fingerprints) are not available on a sharded context: they return
+ * LASSO_ERR_STRATEGY before any work. */
 typedef struct lasso_poly_gens lasso_poly_gens;
 typedef struct lasso_poly lasso_poly;
 size_t lasso_poly_gens_points_needed(size_t num_vars); /* R + 2 */
@@ -433,6 +435,64 @@ int lasso_transcript_append_sparse_commitment(lasso_transcript*, const uint8_t* 
  * and on a sharded context; LASSO_ERR_LENGTH for a null output. */
 int lasso_dense_outputs(lasso_ctx*, int strategy, int log_R, const lasso_dense*, lasso_poly** out);
 int lasso_dense_outputs_custom(lasso_ctx*, const lasso_strategy*, const lasso_dense*, lasso_poly** out);
+
+/* ---------------------------------------------------------------- memory checking inside a caller's protocol
+ *
+ * The pieces of SparsePolynomialEvaluationProof::prove (lasso/surge.rs:119-211) around the primary sumcheck, so that a
+ * caller can run its own sumcheck over the lookup polynomials and still prove the memory check, and offline memory
+ * checking of a caller's own memory (Spark's eq(r_x) table read at addresses dim, say).  Single GPU only: on a sharded
+ * context each call returns LASSO_ERR_STRATEGY before any work.
+ *
+ * lasso_lookup_polys[_custom]: Subtables::new's lookup_polys (subtables/mod.rs:116-129), E_i[j] = T_sub(i)[dim_i[j]] for
+ * the alpha = num_memories memories in memory order, each a new polynomial of log2(s) variables with storage of its own.
+ * Their width is the strategy's table width, with the u32 mirror when that is <= 32, so that
+ * lasso_poly_create_merge(E) committed with the proof's derefs generators gives the proof's comm_derefs.  One table
+ * materialisation (built-in strategies) and one gather.  LASSO_ERR_STRATEGY as lasso_dense_outputs; LASSO_ERR_LENGTH
+ * for a null out or n_out != alpha. */
+int lasso_lookup_polys(lasso_ctx*, int strategy, int log_R, const lasso_dense*, lasso_poly** out, size_t n_out);
+int lasso_lookup_polys_custom(lasso_ctx*, const lasso_strategy*, const lasso_dense*, lasso_poly** out, size_t n_out);
+/* DensifiedRepresentation's dim_j, read_j or final_j (lasso/densified.rs:8-18) as a new polynomial: which takes
+ * lasso_dense_read's numbers (1 = dim, 2 = read, 3 = final), j < C (LASSO_ERR_LENGTH otherwise).  s evaluations (m for
+ * final), all integers, with the u32 mirror.  LASSO_ERR_STRATEGY for a null dense or a sharded context. */
+int lasso_dense_poly(lasso_ctx*, const lasso_dense*, int which, size_t j, lasso_poly** out);
+/* MemoryCheckingProof::prove (subtables/memory_checking.rs:56-83) at (gamma, tau) on the caller's transcript and tape,
+ * both advanced in place.  The reference's `subtables` argument is rebuilt from (strategy, dense): identical by
+ * construction, at the cost of one gather.  proof_out receives the ark-serialize (compressed) MemoryCheckingProof, the
+ * product layer then the hash layer, 4*32*alpha + gpa(2 alpha, log m) + gpa(2 alpha, log s) + 32 (3C + alpha) + three
+ * PolyEvalProofs at the generators' (nv_l, nv_m, nv_d); *proof_len receives that size, also when proof_cap is too small.
+ * Inside lasso_prove_transcript this is what follows challenge_vector("challenge_r_hash", 2) = (gamma, tau).
+ * Errors, each before any launch and before the transcript or the tape moves: LASSO_ERR_STRATEGY as lasso_prove;
+ * LASSO_ERR_LENGTH for a null transcript, tape, gamma, tau or proof_len, or proof_cap too small; LASSO_ERR_GENS for
+ * generators of another context or shape; LASSO_ERR_VALUE for a gamma or tau that is not a canonical residue.  The
+ * working memory is reserved in the context's pool before the first transcript write.  LASSO_ERR_MULTISET, as the
+ * reference's panic, can only be raised after the transcript has moved. */
+int lasso_memory_check_prove(lasso_ctx*, int strategy, int log_R, const lasso_dense*, const uint64_t gamma[4],
+                             const uint64_t tau[4], const lasso_gens*, lasso_transcript* transcript,
+                             lasso_random_tape* random_tape, uint8_t* proof_out, size_t proof_cap, size_t* proof_len);
+int lasso_memory_check_prove_custom(lasso_ctx*, const lasso_strategy*, const lasso_dense*, const uint64_t gamma[4],
+                                    const uint64_t tau[4], const lasso_gens*, lasso_transcript* transcript,
+                                    lasso_random_tape* random_tape, uint8_t* proof_out, size_t proof_cap,
+                                    size_t* proof_len);
+/* GrandProducts::new(eval_table, dim, dim_usize, read, final, (gamma, tau)) (subtables/memory_checking.rs:175-310)
+ * over a caller's memory, with dim doubling as dim_usize as in every reference caller: out receives four new
+ * full-width polynomials in the reference's field order, with hash(a, v, t) = t gamma^2 + v gamma + a - tau:
+ *   init[i] = hash(i, T[i], 0), final[i] = hash(i, T[i], final_ts[i])                    for i < M = table's length,
+ *   read[j] = hash(dim[j], T[dim[j]], read[j]), write[j] = hash(dim[j], T[dim[j]], read[j] + 1)   for j < s.
+ * read and write come from one pass that gathers T[dim[j]] (never stored); read and final_ts may be any field elements.
+ * Errors, each before any launch: LASSO_ERR_LENGTH when table and final_ts are not of one length M >= 2, dim and read
+ * not of one length s >= 2, or gamma, tau or out is null; LASSO_ERR_INDEX_RANGE when dim does not hold integers below M
+ * (its bit width, known without a device pass, exceeds log2 M); LASSO_ERR_VALUE for a gamma or tau that is not a
+ * canonical residue; LASSO_ERR_STRATEGY for a polynomial of another context or a sharded context.  Grand-product circuits
+ * over the results (lasso_gp_circuit_create) give the reference's GrandProducts. */
+int lasso_memory_fingerprints(lasso_ctx*, const lasso_poly* table, const lasso_poly* dim, const lasso_poly* read,
+                              const lasso_poly* final_ts, const uint64_t gamma[4], const uint64_t tau[4],
+                              lasso_poly* out[4]);
+/* CombinedTableCommitment::append_to_transcript (subtables/mod.rs:382-393) of PolyCommitment bytes (lasso_poly_commit's
+ * format): the begin / end subtable_evals_commitment messages around PolyCommitment::append_to_transcript under label.
+ * Host only.  LASSO_ERR_LENGTH for a null label or bytes that do not parse; LASSO_ERR_VALUE for a point that does not
+ * decompress; nothing is absorbed in either case. */
+int lasso_transcript_append_combined_table_commitment(lasso_transcript*, const char* label, const uint8_t* bytes,
+                                                      size_t len);
 
 /* ---------------------------------------------------------------- many polynomials per call
  *

@@ -170,6 +170,26 @@ extern "C" {
                                out: *mut *mut lasso_poly) -> c_int;
     pub fn lasso_dense_outputs_custom(ctx: *mut lasso_ctx, s: *const lasso_strategy, dense: *const lasso_dense,
                                       out: *mut *mut lasso_poly) -> c_int;
+    // memory checking inside a caller's protocol (single GPU; raw declarations only)
+    pub fn lasso_lookup_polys(ctx: *mut lasso_ctx, strategy: c_int, log_r: c_int, dense: *const lasso_dense,
+                              out: *mut *mut lasso_poly, n_out: usize) -> c_int;
+    pub fn lasso_lookup_polys_custom(ctx: *mut lasso_ctx, s: *const lasso_strategy, dense: *const lasso_dense,
+                                     out: *mut *mut lasso_poly, n_out: usize) -> c_int;
+    pub fn lasso_dense_poly(ctx: *mut lasso_ctx, dense: *const lasso_dense, which: c_int, j: usize,
+                            out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_memory_check_prove(ctx: *mut lasso_ctx, strategy: c_int, log_r: c_int, dense: *const lasso_dense,
+                                    gamma: *const u64, tau: *const u64, gens: *const lasso_gens,
+                                    transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
+                                    proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize) -> c_int;
+    pub fn lasso_memory_check_prove_custom(ctx: *mut lasso_ctx, s: *const lasso_strategy, dense: *const lasso_dense,
+                                           gamma: *const u64, tau: *const u64, gens: *const lasso_gens,
+                                           transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
+                                           proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize) -> c_int;
+    pub fn lasso_memory_fingerprints(ctx: *mut lasso_ctx, table: *const lasso_poly, dim: *const lasso_poly,
+                                     read: *const lasso_poly, final_ts: *const lasso_poly, gamma: *const u64,
+                                     tau: *const u64, out: *mut *mut lasso_poly) -> c_int;
+    pub fn lasso_transcript_append_combined_table_commitment(t: *mut lasso_transcript, label: *const c_char,
+                                                             bytes: *const u8, len: usize) -> c_int;
     // sumchecks over a caller's polynomials (raw declarations only; not compiled: no cargo was available)
     pub fn lasso_comb_create(n_inputs: c_int, program: *const i32, n_ops: c_int, constants: *const u64, n_constants: c_int,
                              degree: c_int, out: *mut *mut lasso_comb) -> c_int;

@@ -25,13 +25,22 @@ and, for a caller that composes Lasso into a larger protocol, its own dense poly
     GrandProductCircuit(ctx, poly).evaluate()                            src/subprotocols/grand_product.rs:38, 60
     BatchedGrandProductArgument.prove(ctx, circuits, transcript)         src/subprotocols/grand_product.rs:100
 
+and the memory check of a lookup proof, or of a caller's own memory, inside a caller's protocol (single GPU):
+
+    Subtables(ctx, strategy, dense).lookup_polys / .combined_poly / .commit   src/subtables/mod.rs:116, 177
+    DensifiedRepresentation.dim_poly(j) / .read_poly(j) / .final_poly(j)  src/lasso/densified.rs:8
+    MemoryCheckingProof.prove(ctx, strategy, dense, (gamma, tau), gens, transcript, random_tape)
+                                                                         src/subtables/memory_checking.rs:56
+    GrandProducts.new(ctx, eval_table, dim, read, final, (gamma, tau))   src/subtables/memory_checking.rs:175
+    Transcript.append_combined_table_commitment(commitment)              src/subtables/mod.rs:382
+
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, LassoError, MsmJob, PolyCommitmentGens, PolyEvalProof,
-    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, SumcheckInstanceProof, Transcript,
+    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, GrandProducts, LassoError, MemoryCheckingProof, MsmJob, PolyCommitmentGens, PolyEvalProof,
+    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Subtables, SumcheckInstanceProof, Transcript,
     bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,
     msm, poly_gens_points_needed, sample_generators, sumcheck_bind_round_arbitrary,

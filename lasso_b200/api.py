@@ -583,6 +583,24 @@ class DensifiedRepresentation:
         _chk(lib().lasso_commit(self.ctx._h, self._h, gens._h, _p(out), C.c_size_t(cap), C.byref(n)))
         return bytes(out[: n.value])
 
+    def _poly(self, which, j):
+        h = C.c_void_p()
+        _chk(lib().lasso_dense_poly(self.ctx._h, self._h, which, C.c_size_t(int(j)), C.byref(h)))
+        return DensePolynomial._wrap(self.ctx, h)
+
+    def dim_poly(self, j):
+        """dim_j (src/lasso/densified.rs:8-18) as a DensePolynomial of its own on ctx's GPU: the same values as
+        .dim[j], integer-valued (the u32 mirror).  Single GPU."""
+        return self._poly(1, j)
+
+    def read_poly(self, j):
+        """read_j, as dim_poly"""
+        return self._poly(2, j)
+
+    def final_poly(self, j):
+        """final_j (m evaluations), as dim_poly"""
+        return self._poly(3, j)
+
     def outputs(self, strategy):
         """The lookup outputs v[k] = combine_lookups(E_0[k], ..) for k < s (padded lookups included) as a
         DensePolynomial of log2(s) variables on the context's GPU.  Its MLE at r is the claimed evaluation of a proof
@@ -732,6 +750,12 @@ class Transcript:
         DensifiedRepresentation.commit's bytes"""
         b = bytes(commitment)
         _chk(lib().lasso_transcript_append_sparse_commitment(self._h, b, C.c_size_t(len(b))))
+
+    def append_combined_table_commitment(self, commitment, label=b"comm_poly_row_col_ops_val"):
+        """CombinedTableCommitment::append_to_transcript (src/subtables/mod.rs:382-393) of PolyCommitment bytes
+        (Subtables.commit, DensePolynomial.commit); label is the one surge.rs:139 passes"""
+        b = bytes(commitment)
+        _chk(lib().lasso_transcript_append_combined_table_commitment(self._h, _label(label), b, C.c_size_t(len(b))))
 
     def challenge_scalar(self, label):
         out = np.zeros(4, dtype=np.uint64)
@@ -1216,3 +1240,89 @@ class BatchedGrandProductArgument:
         _chk(lib().lasso_gp_prove(ctx._h, _handles(circuits), C.c_size_t(len(circuits)), transcript._h, _p(out),
                                   C.c_size_t(cap), C.byref(n), _p(r), _p(claims)))
         return cls(bytes(out[: n.value]), r[:v], claims[: len(circuits)])
+
+
+# ------------------------------------------------------------------ memory checking inside a caller's protocol
+def _strategy_call(strategy, builtin, custom):
+    """(function, leading arguments) of a built-in / custom strategy pair of C entry points"""
+    if isinstance(strategy, CustomStrategy):
+        if strategy._h is None:
+            raise LassoError(LASSO_ERR_STRATEGY, "the CustomStrategy was built without a context")
+        return custom, (strategy._h,)
+    return builtin, (strategy.kind, strategy.log_r)
+
+
+def _gamma_tau(hash_challenges):
+    gamma, tau = hash_challenges
+    return _limbs(gamma, 1, "gamma"), _limbs(tau, 1, "tau")
+
+
+class Subtables:
+    """Subtables::new (src/subtables/mod.rs:116-129) of a strategy over a DensifiedRepresentation, on ctx's GPU (single
+    GPU).  `.lookup_polys`: the num_memories polynomials E_i[j] = T_sub(i)[dim_i[j]] in memory order, each with its own
+    storage and the tables' width; `.combined_poly`: DensePolynomial.merge of them."""
+
+    def __init__(self, ctx, strategy, dense):
+        L = lib()
+        fn, head = _strategy_call(strategy, L.lasso_lookup_polys, L.lasso_lookup_polys_custom)
+        alpha = strategy.num_memories
+        hs = (C.c_void_p * max(alpha, 1))()
+        _chk(fn(ctx._h, *head, dense._h, hs, C.c_size_t(alpha)))
+        self.ctx = ctx
+        self.lookup_polys = [DensePolynomial._wrap(ctx, C.c_void_p(hs[i])) for i in range(alpha)]
+        self._combined = None
+
+    @property
+    def combined_poly(self):
+        if self._combined is None:
+            self._combined = DensePolynomial.merge(self.ctx, self.lookup_polys)
+        return self._combined
+
+    def commit(self, gens):
+        """Subtables::commit (src/subtables/mod.rs:177-184) -> the CombinedTableCommitment's bytes (those of its
+        PolyCommitment); gens: PolyCommitmentGens of combined_poly.num_vars, e.g. the proof's gens_derefs"""
+        return self.combined_poly.commit(gens)
+
+
+class MemoryCheckingProof:
+    """src/subtables/memory_checking.rs:26-147.  `.bytes` is the ark-serialize (compressed) proof: the product layer,
+    then the hash layer."""
+
+    def __init__(self, data):
+        self.bytes = data
+
+    @classmethod
+    def prove(cls, ctx, strategy, dense, hash_challenges, gens, transcript, random_tape):
+        """MemoryCheckingProof::prove(dense, (gamma, tau), subtables, gens, transcript, random_tape) on the caller's
+        transcript and tape, advanced in place; gens: the SparsePolyCommitmentGens of the lookup proof.  The subtables
+        are rebuilt from (strategy, dense).  Single GPU."""
+        L = lib()
+        fn, head = _strategy_call(strategy, L.lasso_memory_check_prove, L.lasso_memory_check_prove_custom)
+        gamma, tau = _gamma_tau(hash_challenges)
+        cap = 1 << 22
+        out = ctx._buf("proof", cap, np.uint8)
+        n = C.c_size_t(0)
+        _chk(fn(ctx._h, *head, dense._h, _p(gamma), _p(tau), gens._h, transcript._h, random_tape._h, _p(out),
+                C.c_size_t(cap), C.byref(n)))
+        return cls(bytes(out[: n.value]))
+
+
+class GrandProducts:
+    """GrandProducts::new(eval_table, dim, dim_usize, read, final, (gamma, tau)) (src/subtables/memory_checking.rs:
+    175-310) over a caller's memory: `.polys` are the fingerprint polynomials (init, read, write, final), and `.init`,
+    `.read`, `.write`, `.final` GrandProductCircuits over them.  dim doubles as dim_usize and must hold integers below
+    M = len(eval_table) (LassoError code 3 otherwise); read and final may be any field elements.  Single GPU."""
+
+    FIELDS = ("init", "read", "write", "final")
+
+    def __init__(self, ctx, polys):
+        self.ctx, self.polys = ctx, polys
+        for name, p in zip(self.FIELDS, polys):
+            setattr(self, name, GrandProductCircuit(ctx, p))
+
+    @classmethod
+    def new(cls, ctx, eval_table, dim, read, final, hash_challenges):
+        gamma, tau = _gamma_tau(hash_challenges)
+        hs = (C.c_void_p * 4)()
+        _chk(lib().lasso_memory_fingerprints(ctx._h, eval_table._h, dim._h, read._h, final._h, _p(gamma), _p(tau), hs))
+        return cls(ctx, [DensePolynomial._wrap(ctx, C.c_void_p(h)) for h in hs])

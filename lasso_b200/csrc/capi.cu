@@ -735,7 +735,23 @@ static int strategy_for(lasso_ctx* h, int strategy, int log_R, const lasso_strat
                " grand-product circuits exceed the batch limit of 32 (LT needs C <= 8)");
   return 0;
 }
+// The generators lasso_gens_create built for this (c, s, num_memories, log_m) (surge.rs:32-58), else LASSO_ERR_GENS.
 // shared_gens: generators of another single-GPU context on the same device will do (lasso_prove lets such contexts
+// share one set of read-only tables, many GB at 2^20 lookups); otherwise they must be the context's own
+static int gens_check(lasso_ctx* h, const Strategy& S, const Dense& dense, const lasso_gens* g, bool shared_gens,
+                      const char* what) {
+  const size_t alpha = (size_t)S.num_memories();
+  const Ctx* gc = g ? g->g->ctx : nullptr;
+  const bool shareable = shared_gens && gc && gc->device == h->c->device && gc->world == 1 && h->c->world == 1;
+  if (!g || (gc != h->c && !shareable))
+    return fail(LASSO_ERR_GENS, std::string(what) + ": null generators, or generators of another context");
+  const Gens& gg = *g->g;
+  if (gg.c != dense.C || next_pow2(gg.s) != dense.s || gg.num_memories != alpha || gg.log_m != dense.log_m ||
+      gg.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || gg.nv_l != dense.nv_l || gg.nv_m != dense.nv_m)
+    return fail(LASSO_ERR_GENS, std::string(what) + ": generators built for another (c, s, num_memories, log_m)");
+  return 0;
+}
+// shared_gens: as gens_check; generators of another single-GPU context on the same device will do (lasso_prove lets such contexts
 // share one set of read-only tables, many GB at 2^20 lookups); otherwise they must be the context's own
 static int prove_transcript(lasso_ctx* h, const Strategy& S, lasso_dense* d, const uint64_t* r, size_t r_len,
                             const lasso_gens* g, bool shared_gens, lasso_transcript* transcript, lasso_random_tape* tape,
@@ -744,16 +760,8 @@ static int prove_transcript(lasso_ctx* h, const Strategy& S, lasso_dense* d, con
   if (!transcript || !tape || !proof_len) return fail(LASSO_ERR_LENGTH, "prove: null transcript, random tape or proof_len");
   if (r_len != log2_exact_or_ceil(dense.s)) return fail(LASSO_ERR_LENGTH, "r.len() != log2(s)");  // surge.rs:131
   if (r_len && !r) return fail(LASSO_ERR_LENGTH, "prove: null point");
-  // the generators lasso_gens_create built for this (c, s, num_memories, log_m) (surge.rs:32-58)
-  const size_t alpha = (size_t)S.num_memories();
-  const Ctx* gc = g ? g->g->ctx : nullptr;
-  const bool shareable = shared_gens && gc && gc->device == h->c->device && gc->world == 1 && h->c->world == 1;
-  if (!g || (gc != h->c && !shareable))
-    return fail(LASSO_ERR_GENS, "prove: null generators, or generators of another context");
+  if (const int rc = gens_check(h, S, dense, g, shared_gens, "prove")) return rc;
   const Gens& gg = *g->g;
-  if (gg.c != dense.C || next_pow2(gg.s) != dense.s || gg.num_memories != alpha || gg.log_m != dense.log_m ||
-      gg.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || gg.nv_l != dense.nv_l || gg.nv_m != dense.nv_m)
-    return fail(LASSO_ERR_GENS, "prove: generators built for another (c, s, num_memories, log_m)");
   const size_t need = proof_bytes(S, dense, gg);
   if (const int rc = out_room("prove", need, proof_out, proof_cap, proof_len)) return rc;
   std::vector<fr_t> rv;
@@ -849,6 +857,111 @@ int lasso_dense_outputs_custom(lasso_ctx* h, const lasso_strategy* s, const lass
   if (out) *out = nullptr;
   if (!s) return fail(LASSO_ERR_STRATEGY, "outputs: null strategy");
   return dense_outputs_checked(h, 0, 0, s, d, out);
+  LB_CATCH
+}
+
+// ---- memory checking inside a caller's protocol (single GPU): Subtables::new, the densified polynomials,
+// MemoryCheckingProof::prove and GrandProducts::new over a caller's memory
+static int lookup_polys_checked(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
+                                lasso_poly** out, size_t n_out) {
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  Strategy S{};
+  if (const int rc = strategy_for(h, strategy, log_R, s, d, S)) return rc;
+  if (!out || n_out != (size_t)S.num_memories())
+    return fail(LASSO_ERR_LENGTH, "lookup polys: null output, or n_out != num_memories (" +
+                                      std::to_string(S.num_memories()) + ")");
+  for (size_t i = 0; i < n_out; i++) out[i] = nullptr;
+  const std::vector<Poly*> ps = lookup_polys(h->c, S, *d->d);
+  for (size_t i = 0; i < n_out; i++) out[i] = new lasso_poly{ps[i]};
+  return 0;
+}
+int lasso_lookup_polys(lasso_ctx* h, int strategy, int log_R, const lasso_dense* d, lasso_poly** out, size_t n_out) {
+  LB_TRY_CTX(h)
+  return lookup_polys_checked(h, strategy, log_R, nullptr, d, out, n_out);
+  LB_CATCH
+}
+int lasso_lookup_polys_custom(lasso_ctx* h, const lasso_strategy* s, const lasso_dense* d, lasso_poly** out,
+                              size_t n_out) {
+  LB_TRY_CTX(h)
+  if (!s) return fail(LASSO_ERR_STRATEGY, "lookup polys: null strategy");
+  return lookup_polys_checked(h, 0, 0, s, d, out, n_out);
+  LB_CATCH
+}
+int lasso_dense_poly(lasso_ctx* h, const lasso_dense* d, int which, size_t j, lasso_poly** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!d) return fail(LASSO_ERR_STRATEGY, "dense poly: null densified representation");
+  if (!out) return fail(LASSO_ERR_LENGTH, "dense poly: null output");
+  if (which < 1 || which > 3 || j >= d->d->C)
+    return fail(LASSO_ERR_LENGTH, "dense poly: which must be 1 (dim), 2 (read) or 3 (final), and j < C");
+  *out = new lasso_poly{dense_poly(h->c, *d->d, which, j)};
+  return 0;
+  LB_CATCH
+}
+static int memory_check_checked(lasso_ctx* h, int strategy, int log_R, const lasso_strategy* s, const lasso_dense* d,
+                                const uint64_t gamma[4], const uint64_t tau[4], const lasso_gens* g,
+                                lasso_transcript* transcript, lasso_random_tape* tape, uint8_t* proof_out,
+                                size_t proof_cap, size_t* proof_len) {
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  Strategy S{};
+  if (const int rc = strategy_for(h, strategy, log_R, s, d, S)) return rc;
+  const Dense& dense = *d->d;
+  if (!transcript || !tape || !proof_len || !gamma || !tau)
+    return fail(LASSO_ERR_LENGTH, "memory check: null transcript, random tape, gamma, tau or proof_len");
+  if (const int rc = gens_check(h, S, dense, g, false, "memory check")) return rc;
+  const size_t need = memory_check_bytes(S, dense, *g->g);
+  if (const int rc = out_room("memory check", need, proof_out, proof_cap, proof_len)) return rc;
+  std::vector<fr_t> gv, tv;
+  if (!load_scalars(gamma, 1, gv) || !load_scalars(tau, 1, tv))
+    return fail(LASSO_ERR_VALUE, "memory check: gamma or tau is not a canonical residue");
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return memory_check_prove(h->c, S, dense, gv[0], tv[0], *g->g, transcript->t, tape->t);
+  });
+  return out_copy("memory check", b, need, proof_out);
+}
+int lasso_memory_check_prove(lasso_ctx* h, int strategy, int log_R, const lasso_dense* d, const uint64_t gamma[4],
+                             const uint64_t tau[4], const lasso_gens* g, lasso_transcript* transcript,
+                             lasso_random_tape* random_tape, uint8_t* proof_out, size_t proof_cap, size_t* proof_len) {
+  LB_TRY_CTX(h)
+  return memory_check_checked(h, strategy, log_R, nullptr, d, gamma, tau, g, transcript, random_tape, proof_out,
+                              proof_cap, proof_len);
+  LB_CATCH
+}
+int lasso_memory_check_prove_custom(lasso_ctx* h, const lasso_strategy* s, const lasso_dense* d,
+                                    const uint64_t gamma[4], const uint64_t tau[4], const lasso_gens* g,
+                                    lasso_transcript* transcript, lasso_random_tape* random_tape, uint8_t* proof_out,
+                                    size_t proof_cap, size_t* proof_len) {
+  LB_TRY_CTX(h)
+  if (!s) return fail(LASSO_ERR_STRATEGY, "memory check: null strategy");
+  return memory_check_checked(h, 0, 0, s, d, gamma, tau, g, transcript, random_tape, proof_out, proof_cap, proof_len);
+  LB_CATCH
+}
+static int poly_array(lasso_ctx* h, const char* what, const lasso_poly* const* polys, size_t n, bool same_nv,
+                      std::vector<const Poly*>& ps);
+int lasso_memory_fingerprints(lasso_ctx* h, const lasso_poly* table, const lasso_poly* dim, const lasso_poly* read,
+                              const lasso_poly* final_ts, const uint64_t gamma[4], const uint64_t tau[4],
+                              lasso_poly* out[4]) {
+  LB_TRY_CTX(h)
+  if (out)
+    for (int k = 0; k < 4; k++) out[k] = nullptr;
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  const lasso_poly* in[4] = {table, dim, read, final_ts};
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "fingerprints", in, 4, false, ps)) return rc;
+  const Poly &T = *ps[0], &D = *ps[1], &R = *ps[2], &F = *ps[3];
+  if (T.len != F.len || T.len < 2) return fail(LASSO_ERR_LENGTH, "fingerprints: table and final_ts must be of one length M >= 2");
+  if (D.len != R.len || D.len < 2) return fail(LASSO_ERR_LENGTH, "fingerprints: dim and read must be of one length s >= 2");
+  if (!out || !gamma || !tau) return fail(LASSO_ERR_LENGTH, "fingerprints: null gamma, tau or output");
+  // dim.bits <= log2 M: every address is an integer below M, and dim has the u32 mirror the gather reads
+  if (D.bits > T.nv || !D.d_u32.p) return fail(LASSO_ERR_INDEX_RANGE, "fingerprints: dim must hold integers below M");
+  std::vector<fr_t> gv, tv;
+  if (!load_scalars(gamma, 1, gv) || !load_scalars(tau, 1, tv))
+    return fail(LASSO_ERR_VALUE, "fingerprints: gamma or tau is not a canonical residue");
+  Poly* o[4];
+  memory_fingerprints(h->c, T, D, R, F, gv[0], tv[0], o);
+  for (int k = 0; k < 4; k++) out[k] = new lasso_poly{o[k]};
+  return 0;
   LB_CATCH
 }
 
@@ -969,6 +1082,27 @@ int lasso_transcript_append_sparse_commitment(lasso_transcript* t, const uint8_t
     memcpy(&x, bytes + at + 8 * k, 8);
     t->t.append_u64(fields[k], x);
   }
+  return 0;
+  LB_CATCH
+}
+int lasso_transcript_append_combined_table_commitment(lasso_transcript* t, const char* label, const uint8_t* bytes,
+                                                      size_t len) {
+  LB_TRY_T(t)
+  if (!label) return fail(LASSO_ERR_LENGTH, "combined table commitment: null label");
+  uint64_t n = 0;
+  if (!bytes || len < 8) return fail(LASSO_ERR_LENGTH, "combined table commitment: shorter than its count");
+  memcpy(&n, bytes, 8);
+  if (n > (len - 8) / 32 || len != 8 + 32 * n)
+    return fail(LASSO_ERR_LENGTH, "combined table commitment: length != 8 + 32 * count");
+  for (uint64_t i = 0; i < n; i++)
+    if (!h64::decompresses(bytes + 8 + 32 * i))
+      return fail(LASSO_ERR_VALUE, "combined table commitment: a point does not decompress");
+  // CombinedTableCommitment::append_to_transcript (subtables/mod.rs:382-393)
+  t->t.append_message("subtable_evals_commitment", std::string("begin_subtable_evals_commitment"));
+  t->t.append_message(label, std::string("poly_commitment_begin"));
+  for (uint64_t i = 0; i < n; i++) t->t.append_point_compressed("poly_commitment_share", bytes + 8 + 32 * i);
+  t->t.append_message(label, std::string("poly_commitment_end"));
+  t->t.append_message("subtable_evals_commitment", std::string("end_subtable_evals_commitment"));
   return 0;
   LB_CATCH
 }

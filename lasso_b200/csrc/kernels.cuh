@@ -205,6 +205,11 @@ void launch_gp_fingerprints_mem(const fr_t* table, const fr_t* final_fr, size_t 
 void launch_gp_fingerprints_ops(const fr_t* dim_fr, const fr_t* E_fr, const fr_t* read_fr, size_t s,
                                 const fr_t& gamma, const fr_t& tau, fr_t* out_read, fr_t* out_write,
                                 cudaStream_t st);
+// read/write over a caller's memory in one pass: v = table[dim_u32[j]] gathered, t = read_u32[j] when read_u32 is
+// non-null, else read_fr[j]; write = read + gamma^2 (write ts = read ts + 1).  Single GPU.
+void launch_gp_fingerprints_gather(const fr_t* table, const uint32_t* dim_u32, const fr_t* read_fr,
+                                   const uint32_t* read_u32, size_t s, const fr_t& gamma, const fr_t& tau, fr_t* out_read,
+                                   fr_t* out_write, cudaStream_t st);
 // every product tree of one size N (grand_product.rs:20-58; contiguous layers, see poly_kernels.cu) + tagged publication of the two
 // top-layer elements of tree t as values 2*(slot0 + t) + {0, 1}
 struct TreePtrs {

@@ -1394,6 +1394,28 @@ void launch_gp_fingerprints_ops(const fr_t* dim_fr, const fr_t* E_fr, const fr_t
   launch(fp_ops_kernel, grid_for(s), kThreads, 0, st, dim_fr, E_fr, read_fr, s, gamma, fr_sqr(gamma), tau, out_read,
          out_write);
 }
+// GrandProducts::new over a caller's memory (memory_checking.rs:236-310, dim doubling as dim_usize): the address is read
+// as a u32 (4 B) and its value gathered from the table, which stays in L2 up to M = 2^20; the timestamp is a u32 when
+// the caller's read_ts has a mirror, else 32 B.  Neither E = T[dim] nor dim's field form is stored or read: 64 B of ~130
+// per op fewer than a gather into E followed by fp_ops_kernel.
+__global__ void __launch_bounds__(kThreads)
+    fp_ops_gather_kernel(const fr_t* table, const uint32_t* dim_u32, const fr_t* read_fr, const uint32_t* read_u32,
+                         size_t s, fr_t gamma, fr_t gamma2, fr_t tau, fr_t* out_read, fr_t* out_write) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < s; i += (size_t)gridDim.x * blockDim.x) {
+    const uint32_t a = __ldcs(dim_u32 + i);
+    const fr_t t = read_u32 ? fr_from_u64(__ldcs(read_u32 + i)) : ld_fr_stream(read_fr + i);
+    const fr_t av = fr_sub(fr_add(fr_mul(ld_fr(table + a), gamma), fr_from_u64(a)), tau);
+    const fr_t hr = fr_add(av, fr_mul(t, gamma2));
+    st_fr(out_read + i, hr);
+    st_fr(out_write + i, fr_add(hr, gamma2));  // write ts = read ts + 1
+  }
+}
+void launch_gp_fingerprints_gather(const fr_t* table, const uint32_t* dim_u32, const fr_t* read_fr,
+                                   const uint32_t* read_u32, size_t s, const fr_t& gamma, const fr_t& tau, fr_t* out_read,
+                                   fr_t* out_write, cudaStream_t st) {
+  launch(fp_ops_gather_kernel, grid_for(s), kThreads, 0, st, table, dim_u32, read_fr, read_u32, s, gamma, fr_sqr(gamma),
+         tau, out_read, out_write);
+}
 
 // grand_product.rs:20-58, all product trees of one size at once (single GPU).  A tree is one contiguous array: layer 0 (N elements),
 // then layer 1 (N/2), ...; layer k+1[i] = layer k[i] * layer k[i + len/2].  One launch per layer for every

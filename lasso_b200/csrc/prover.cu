@@ -1598,116 +1598,93 @@ size_t dpl_bytes(size_t nv) { return 2 * (8 + 32 * (nv - nv / 2)) + 4 * 32; }
 size_t gpa_bytes(size_t n, size_t v) { return 8 + v * (24 + 64 * n) + 52 * v * (v - 1); }
 size_t sumcheck_bytes(size_t rounds, size_t degree) { return 8 + rounds * (8 + 32 * degree); }
 size_t poly_commitment_bytes(size_t num_vars) { return 8 + 32 * ((size_t)1 << (num_vars / 2)); }
-size_t proof_bytes(const Strategy& S, const Dense& dense, const Gens& g) {
+// MemoryCheckingProof (memory_checking.rs:26-37): the product layer, then the hash layer
+size_t memory_check_bytes(const Strategy& S, const Dense& dense, const Gens& g) {
   const size_t alpha = (size_t)S.num_memories(), C = dense.C, log_s = log2_exact_or_ceil(dense.s);
+  return 4 * 32 * alpha + gpa_bytes(2 * alpha, dense.log_m) + gpa_bytes(2 * alpha, log_s)  // product layer
+         + 32 * (3 * C + alpha) + dpl_bytes(g.nv_l) + dpl_bytes(g.nv_m) + dpl_bytes(g.nv_d);  // hash layer
+}
+size_t proof_bytes(const Strategy& S, const Dense& dense, const Gens& g) {
+  const size_t alpha = (size_t)S.num_memories(), log_s = log2_exact_or_ceil(dense.s);
   return 8 + 32 * ((size_t)1 << (g.nv_d / 2))                        // comm_derefs
          + sumcheck_bytes(log_s, (size_t)S.sumcheck_poly_degree())  // primary sumcheck
          + 32 + 32 * alpha + dpl_bytes(g.nv_d)                      // claimed_evaluation, eval_derefs, proof_derefs
-         + 4 * 32 * alpha + gpa_bytes(2 * alpha, dense.log_m) + gpa_bytes(2 * alpha, log_s)  // product layer
-         + 32 * (3 * C + alpha) + dpl_bytes(g.nv_l) + dpl_bytes(g.nv_m) + dpl_bytes(g.nv_d);  // hash layer
+         + memory_check_bytes(S, dense, g);
 }
 
-std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
-                           Transcript& transcript, RandomTape& tape, fr_t* claimed_evaluation) {
-  SpanTimer sp_all(c, "SparsePoly.prove");
+// S and g were made for the dense: thrown before anything moves
+static void check_fit(const Strategy& S, const Dense& dense, const Gens& g) {
+  const size_t alpha = (size_t)S.num_memories();
+  if ((size_t)S.C != dense.C || (size_t)S.log_m != dense.log_m) throw std::runtime_error("strategy does not match the densified representation");
+  if (g.nv_d != log2_exact_or_ceil(next_pow2(alpha * dense.s)) || g.nv_l != dense.nv_l || g.nv_m != dense.nv_m)
+    throw std::runtime_error("generators were built for different (c, s, num_memories, log_m)");
+}
+// Reserves the proof's device memory, in elements of this rank, in the context's pool, which keeps freed memory, so
+// that a short device fails here, before the transcript or the tape has moved.  It is largest either in the primary
+// sumcheck (E, its u32 copy, the alpha + 1 working copies; with_primary only) or in the product layer (E, its u32 copy,
+// the eq table, four trees of 2N elements per memory, N = M for init / final and s for read / write), plus the built-in
+// tables and an opening's vectors (16 R + L + 4096, as combined_eval_prove reserves) at the widest of the three openings.
+static void reserve_working_memory(Ctx* c, const Strategy& S, const Dense& dense, const Gens& g, bool with_primary) {
+  const size_t G = (size_t)c->world, alpha = (size_t)S.num_memories(), s_loc = dense.s_loc, M_loc = dense.m_loc;
+  const size_t nd_loc = ((size_t)1 << g.nv_d) / G;
+  const size_t E_elems = nd_loc + nd_loc / 8 + 1;
+  const size_t primary = with_primary ? E_elems + (alpha + 1) * s_loc : 0;
+  const size_t product = E_elems + std::max(s_loc, M_loc) + 4 * alpha * (M_loc + s_loc) + 4 * alpha * 2 * G;
+  const size_t tables = S.kind == STRAT_CUSTOM ? 0 : (size_t)S.num_subtables() * dense.m * 9 / 8 + 1;
+  const size_t nv = std::max(g.nv_d, std::max(g.nv_l, g.nv_m)), R = poly_R(nv);
+  DBuf<fr_t> reserve(c, std::max(primary, product) + tables + 16 * R + ((size_t)1 << nv) / R + 4096);
+}
+// the bit width of the strategy's table entries: the windows of the lookup polynomials' commitment
+static unsigned table_bits(const Strategy& S) {
+  if (S.kind == STRAT_CUSTOM) return S.custom->tbits;
+  return S.kind == STRAT_LT ? 1 : (S.kind == STRAT_RANGE ? (unsigned)S.log_m : (unsigned)(S.log_m / 2));
+}
+
+// Subtables::new (subtables/mod.rs:116-129) on the device: the tables, and the lookup polynomials
+// E_i[j] = T_sub(i)[dim_i[j]] as combined_poly = E_0 | .. | E_{alpha-1} | 0-pad (this rank's shard of nd_loc elements),
+// with the same values as integers unless the tables are full width.  A custom strategy's tables were uploaded when it
+// was created and are read in place; the built-in ones are materialised (replicated, 2-6 MiB).
+struct LookupPolys {
+  DBuf<fr_t> tables_fr_buf;
+  DBuf<uint32_t> tables_u32_buf;
+  const fr_t* tables_fr = nullptr;
+  const uint32_t* tables_u32 = nullptr;
+  DBuf<fr_t> E;
+  DBuf<uint32_t> E_u32;
+  PolySrc src() const { return PolySrc(E_u32.p, E.p); }  // what the derefs commitment and openings read
+};
+static void lookup_polys_build(Ctx* c, const Strategy& S, const Dense& dense, size_t nd_loc, LookupPolys& L) {
+  const bool custom = S.kind == STRAT_CUSTOM;
+  const size_t M = dense.m, s_loc = dense.s_loc, alpha = (size_t)S.num_memories();
+  const int nsub = S.num_subtables();
+  L.tables_fr_buf.alloc(c, custom ? 0 : (size_t)nsub * M);
+  L.tables_u32_buf.alloc(c, custom ? 0 : (size_t)nsub * M);
+  L.tables_fr = custom ? S.custom->d_tables_fr : L.tables_fr_buf.p;
+  L.tables_u32 = custom ? S.custom->d_tables_u32 : L.tables_u32_buf.p;
+  const bool full_width = custom && S.custom->full_width();
+  L.E.alloc(c, nd_loc);
+  L.E_u32.alloc(c, full_width ? 0 : nd_loc);
+  SpanTimer sp(c, "Subtables.new");
+  if (!custom) launch_materialize_subtables(S, L.tables_fr_buf.p, L.tables_u32_buf.p, c->st);
+  launch_gather_lookup_polys(S, L.tables_fr, L.tables_u32, dense.nz(), s_loc, L.E.p, s_loc, L.E_u32.p, c->st);
+  if (nd_loc > alpha * s_loc) {
+    launch_fill_zero(L.E.p + alpha * s_loc, nd_loc - alpha * s_loc, c->st);
+    if (L.E_u32.p) LB_CUDA_CHECK(cudaMemsetAsync(L.E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
+  }
+}
+
+// MemoryCheckingProof::prove (memory_checking.rs:56-83) at (gamma, tau) over the lookup polynomials L of (S, dense),
+// appended to w.  eqtab: max(s_loc, M_loc) elements of scratch.  A failed multiset check throws
+// LbError(LASSO_ERR_MULTISET) after the transcript has moved.
+static void memory_check(Ctx* c, const Strategy& S, const Dense& dense, const LookupPolys& L, const Gens& g,
+                         const fr_t& gamma, const fr_t& tau, Transcript& transcript, RandomTape& tape, fr_t* eqtab,
+                         ByteWriter& w) {
   const int G = c->world, gr = c->rank;
   const size_t s = dense.s, C = dense.C, M = dense.m, alpha = (size_t)S.num_memories();
   const size_t s_loc = dense.s_loc, M_loc = dense.m_loc;
-  const size_t log_s = log2_exact_or_ceil(s);
-  if ((size_t)S.C != C || (size_t)S.log_m != dense.log_m) throw std::runtime_error("strategy does not match the densified representation");
-  if (g.nv_d != log2_exact_or_ceil(next_pow2(alpha * s)) || g.nv_l != dense.nv_l || g.nv_m != dense.nv_m)
-    throw std::runtime_error("generators were built for different (c, s, num_memories, log_m)");
-  const size_t nv_d = g.nv_d, nd_loc = ((size_t)1 << nv_d) / G;
-  {
-    // The proof's device memory, in elements of this rank, is largest either in the primary sumcheck (E, its u32 copy,
-    // the alpha + 1 working copies) or in the product layer (E, its u32 copy, the eq table, four trees of 2N elements per
-    // memory, N = M for init / final and s for read / write), plus the built-in tables and an opening's vectors
-    // (16 R + L + 4096, as combined_eval_prove reserves) at the widest of the three openings.  Reserving that much in
-    // the context's pool, which keeps freed memory, makes a short device fail here, before the transcript or the tape
-    // has moved.
-    const size_t E_elems = nd_loc + nd_loc / 8 + 1;
-    const size_t primary = E_elems + (alpha + 1) * s_loc;
-    const size_t product = E_elems + std::max(s_loc, M_loc) + 4 * alpha * (M_loc + s_loc) + 4 * alpha * 2 * (size_t)G;
-    const size_t tables = S.kind == STRAT_CUSTOM ? 0 : (size_t)S.num_subtables() * M * 9 / 8 + 1;
-    const size_t nv = std::max(nv_d, std::max(g.nv_l, g.nv_m)), R = poly_R(nv);
-    DBuf<fr_t> reserve(c, std::max(primary, product) + tables + 16 * R + ((size_t)1 << nv) / R + 4096);
-  }
-  transcript.append_protocol_name("Lasso SparsePolynomialEvaluationProof");
-
-  // ---- Subtables::new (subtables/mod.rs:116-129): materialise (replicated, 2-6 MiB), gather, merge
-  // a custom strategy's tables were uploaded when it was created: used in place
-  const bool custom = S.kind == STRAT_CUSTOM;
-  const int nsub = S.num_subtables();
-  DBuf<fr_t> tables_fr_buf(c, custom ? 0 : (size_t)nsub * M);
-  DBuf<uint32_t> tables_u32_buf(c, custom ? 0 : (size_t)nsub * M);
-  const fr_t* tables_fr = custom ? S.custom->d_tables_fr : tables_fr_buf.p;
-  const uint32_t* tables_u32 = custom ? S.custom->d_tables_u32 : tables_u32_buf.p;
-  const bool full_width = custom && S.custom->full_width();
-  DBuf<fr_t> E(c, nd_loc);          // combined_poly = E_0 | .. | E_{alpha-1} | 0-pad (this rank's shard)
-  DBuf<uint32_t> E_u32(c, full_width ? 0 : nd_loc);  // same values as integers for the small-scalar commit
-  const PolySrc E_src(E_u32.p, E.p);  // what the derefs commitment and openings read
-  {
-    SpanTimer sp(c, "Subtables.new");
-    if (!custom) {
-      launch_materialize_subtables(S, tables_fr_buf.p, tables_u32_buf.p, c->st);
-    }
-    launch_gather_lookup_polys(S, tables_fr, tables_u32, dense.nz(), s_loc, E.p, s_loc, E_u32.p, c->st);
-    if (nd_loc > alpha * s_loc) {
-      launch_fill_zero(E.p + alpha * s_loc, nd_loc - alpha * s_loc, c->st);
-      if (E_u32.p) LB_CUDA_CHECK(cudaMemsetAsync(E_u32.p + alpha * s_loc, 0, (nd_loc - alpha * s_loc) * 4, c->st));
-    }
-  }
-  ByteWriter w;
-  std::vector<uint8_t> comm_E;
-  // ---- comm_derefs (surge.rs:136-140, subtables/mod.rs:177-184, 382-393)
-  {
-    SpanTimer sp(c, "Subtables.commit");
-    unsigned tbits = custom ? S.custom->tbits
-                            : (S.kind == STRAT_LT ? 1 : (S.kind == STRAT_RANGE ? (unsigned)S.log_m : (unsigned)(S.log_m / 2)));
-    comm_E = commit_src(c, g, E_src, nv_d, tbits);
-    w.vec_pts(comm_E);
-  }
-  auto absorb_comm_E = [&]() {  // ~700 Keccak permutations (2^11 points): done while the device prepares the sumcheck
-    transcript.append_message("subtable_evals_commitment", std::string("begin_subtable_evals_commitment"));
-    transcript.append_message("comm_poly_row_col_ops_val", std::string("poly_commitment_begin"));
-    for (size_t i = 0; i < comm_E.size() / 32; i++)
-      transcript.append_point_compressed("poly_commitment_share", comm_E.data() + 32 * i);
-    transcript.append_message("comm_poly_row_col_ops_val", std::string("poly_commitment_end"));
-    transcript.append_message("subtable_evals_commitment", std::string("end_subtable_evals_commitment"));
-  };
-  // ---- primary sumcheck (surge.rs:142-172)
-  std::vector<fr_t> r_z;
-  {
-    DBuf<fr_t> Wk(c, (alpha + 1) * s_loc);  // clones of E_i + eq(r): the sumcheck binds them in place
-    LB_CUDA_CHECK(cudaMemcpyAsync(Wk.p, E.p, alpha * s_loc * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
-    eq_evals_shard(c, r, 0, log_s, Wk.p + alpha * s_loc);
-    launch_sumcheck_claim(S, Wk.p, s_loc, s_loc, c->d_partial, c->d_small, c->st);  // subtables/mod.rs:186-216
-    fr_t claimed_eval;
-    const Finalize fclaim = reduce_to_host_begin(c, c->d_small, 1);
-    absorb_comm_E();  // transcript order unchanged: the commitment, then the claim
-    c->fin_wait(fclaim, &claimed_eval, 1);
-    transcript.append_scalar("claim_eval_scalar_product", claimed_eval);
-    SumcheckProof primary = prove_arbitrary(c, S, Wk.p, s_loc, s_loc, transcript, r_z);
-    ser_sumcheck(w, primary);
-    w.fr(claimed_eval);
-    if (claimed_evaluation) *claimed_evaluation = claimed_eval;
-  }
-  // ---- eval_derefs = E_i(r_z) (surge.rs:175-176) and the combined opening (177-184)
-  DBuf<fr_t> eqtab(c, std::max(s_loc, M_loc));
-  std::vector<fr_t> eval_derefs(alpha);
-  {
-    SpanTimer sp(c, "CombinedEval.prove");
-    eq_evals_shard(c, r_z, 0, log_s, eqtab.p);
-    multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
-    reduce_to_host(c, c->d_small, (int)alpha, eval_derefs.data());
-    w.arr_fr(eval_derefs);
-    transcript.append_protocol_name("Lasso CombinedTableEvalProof");
-    ser_dpl(w, prove_joint(c, g, E_src, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
-                           "joint_claim_eval", r_z, transcript, tape));
-  }
-  // ---- memory checking (surge.rs:186-198)
-  std::vector<fr_t> r_hash = transcript.challenge_vector("challenge_r_hash", 2);
-  const fr_t gamma = r_hash[0], tau = r_hash[1];
+  const fr_t* tables_fr = L.tables_fr;
+  const fr_t* E = L.E.p;
+  const PolySrc E_src = L.src();
   transcript.append_protocol_name("Lasso MemoryCheckingProof");
   std::vector<fr_t> rand_mem, rand_ops;
   {
@@ -1729,7 +1706,7 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
       }
       launch_gp_fingerprints_mem(tables_fr + k * M, dense.fin(j), M_loc, G, gr, gamma, tau, init[i]->tree.p,
                                  fin[i]->tree.p, c->st);
-      launch_gp_fingerprints_ops(dense.dim(j), E.p + i * s_loc, dense.read(j), s_loc, gamma, tau, rd[i]->tree.p,
+      launch_gp_fingerprints_ops(dense.dim(j), E + i * s_loc, dense.read(j), s_loc, gamma, tau, rd[i]->tree.p,
                                  wr[i]->tree.p, c->st);
     }
     // all trees of a size at once + the top layers straight to the host
@@ -1784,9 +1761,9 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     SpanTimer sp(c, "HashLayer.prove");
     transcript.append_protocol_name("Lasso HashLayerProof");
     std::vector<fr_t> eval_derefs2(alpha), eval_dim(C), eval_read(C), eval_final(C);
-    eq_evals_shard(c, rand_ops, 0, rand_ops.size(), eqtab.p);
-    multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
-    launch_multi_dot_u32(dense.d_l_u32.p, s_loc, (int)(2 * C), eqtab.p, s_loc, c->d_partial + 65536, c->d_small + 64, c->st);
+    eq_evals_shard(c, rand_ops, 0, rand_ops.size(), eqtab);
+    multi_dot_src(E_src, s_loc, (int)alpha, eqtab, s_loc, c->d_partial, c->d_small, c->st);
+    launch_multi_dot_u32(dense.d_l_u32.p, s_loc, (int)(2 * C), eqtab, s_loc, c->d_partial + 65536, c->d_small + 64, c->st);
     {
       std::vector<fr_t> tmp(64 + 2 * C);
       reduce_to_host(c, c->d_small, (int)tmp.size(), tmp.data());
@@ -1798,10 +1775,10 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     }
     transcript.append_protocol_name("Lasso CombinedTableEvalProof");
     DotProductProofLogBytes proof_derefs =
-        prove_joint(c, g, E_src, nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
+        prove_joint(c, g, E_src, g.nv_d, eval_derefs2, true, "evals_ops_val", "challenge_combine_n_to_one",
                     "joint_claim_eval", rand_ops, transcript, tape);
-    eq_evals_shard(c, rand_mem, 0, rand_mem.size(), eqtab.p);
-    launch_multi_dot_u32(dense.d_m_u32.p, M_loc, (int)C, eqtab.p, M_loc, c->d_partial, c->d_small, c->st);
+    eq_evals_shard(c, rand_mem, 0, rand_mem.size(), eqtab);
+    launch_multi_dot_u32(dense.d_m_u32.p, M_loc, (int)C, eqtab, M_loc, c->d_partial, c->d_small, c->st);
     reduce_to_host(c, c->d_small, (int)C, eval_final.data());
     std::vector<fr_t> evals_ops = eval_dim;
     evals_ops.insert(evals_ops.end(), eval_read.begin(), eval_read.end());
@@ -1821,6 +1798,113 @@ std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::v
     ser_dpl(w, proof_mem);
     ser_dpl(w, proof_derefs);
   }
+}
+
+std::vector<uint8_t> prove(Ctx* c, const Strategy& S, Dense& dense, const std::vector<fr_t>& r, const Gens& g,
+                           Transcript& transcript, RandomTape& tape, fr_t* claimed_evaluation) {
+  SpanTimer sp_all(c, "SparsePoly.prove");
+  const int G = c->world;
+  const size_t s = dense.s, M_loc = dense.m_loc, alpha = (size_t)S.num_memories();
+  const size_t s_loc = dense.s_loc;
+  const size_t log_s = log2_exact_or_ceil(s);
+  check_fit(S, dense, g);
+  const size_t nv_d = g.nv_d, nd_loc = ((size_t)1 << nv_d) / G;
+  reserve_working_memory(c, S, dense, g, true);
+  transcript.append_protocol_name("Lasso SparsePolynomialEvaluationProof");
+
+  // ---- Subtables::new (subtables/mod.rs:116-129): materialise, gather, merge
+  LookupPolys L;
+  lookup_polys_build(c, S, dense, nd_loc, L);
+  const PolySrc E_src = L.src();
+  ByteWriter w;
+  std::vector<uint8_t> comm_E;
+  // ---- comm_derefs (surge.rs:136-140, subtables/mod.rs:177-184, 382-393)
+  {
+    SpanTimer sp(c, "Subtables.commit");
+    comm_E = commit_src(c, g, E_src, nv_d, table_bits(S));
+    w.vec_pts(comm_E);
+  }
+  auto absorb_comm_E = [&]() {  // ~700 Keccak permutations (2^11 points): done while the device prepares the sumcheck
+    transcript.append_message("subtable_evals_commitment", std::string("begin_subtable_evals_commitment"));
+    transcript.append_message("comm_poly_row_col_ops_val", std::string("poly_commitment_begin"));
+    for (size_t i = 0; i < comm_E.size() / 32; i++)
+      transcript.append_point_compressed("poly_commitment_share", comm_E.data() + 32 * i);
+    transcript.append_message("comm_poly_row_col_ops_val", std::string("poly_commitment_end"));
+    transcript.append_message("subtable_evals_commitment", std::string("end_subtable_evals_commitment"));
+  };
+  // ---- primary sumcheck (surge.rs:142-172)
+  std::vector<fr_t> r_z;
+  {
+    DBuf<fr_t> Wk(c, (alpha + 1) * s_loc);  // clones of E_i + eq(r): the sumcheck binds them in place
+    LB_CUDA_CHECK(cudaMemcpyAsync(Wk.p, L.E.p, alpha * s_loc * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+    eq_evals_shard(c, r, 0, log_s, Wk.p + alpha * s_loc);
+    launch_sumcheck_claim(S, Wk.p, s_loc, s_loc, c->d_partial, c->d_small, c->st);  // subtables/mod.rs:186-216
+    fr_t claimed_eval;
+    const Finalize fclaim = reduce_to_host_begin(c, c->d_small, 1);
+    absorb_comm_E();  // transcript order unchanged: the commitment, then the claim
+    c->fin_wait(fclaim, &claimed_eval, 1);
+    transcript.append_scalar("claim_eval_scalar_product", claimed_eval);
+    SumcheckProof primary = prove_arbitrary(c, S, Wk.p, s_loc, s_loc, transcript, r_z);
+    ser_sumcheck(w, primary);
+    w.fr(claimed_eval);
+    if (claimed_evaluation) *claimed_evaluation = claimed_eval;
+  }
+  // ---- eval_derefs = E_i(r_z) (surge.rs:175-176) and the combined opening (177-184)
+  DBuf<fr_t> eqtab(c, std::max(s_loc, M_loc));
+  std::vector<fr_t> eval_derefs(alpha);
+  {
+    SpanTimer sp(c, "CombinedEval.prove");
+    eq_evals_shard(c, r_z, 0, log_s, eqtab.p);
+    multi_dot_src(E_src, s_loc, (int)alpha, eqtab.p, s_loc, c->d_partial, c->d_small, c->st);
+    reduce_to_host(c, c->d_small, (int)alpha, eval_derefs.data());
+    w.arr_fr(eval_derefs);
+    transcript.append_protocol_name("Lasso CombinedTableEvalProof");
+    ser_dpl(w, prove_joint(c, g, E_src, nv_d, eval_derefs, true, "evals_ops_val", "challenge_combine_n_to_one",
+                           "joint_claim_eval", r_z, transcript, tape));
+  }
+  // ---- memory checking (surge.rs:186-198)
+  std::vector<fr_t> r_hash = transcript.challenge_vector("challenge_r_hash", 2);
+  memory_check(c, S, dense, L, g, r_hash[0], r_hash[1], transcript, tape, eqtab.p, w);
+  c->sync();
+  return w.b;
+}
+
+// Subtables::new's lookup_polys, single GPU: one gather of alpha x s elements, then a copy of each E_i into a
+// polynomial of its own with the tables' width (the u32 copy too, unless the tables are full width)
+std::vector<Poly*> lookup_polys(Ctx* c, const Strategy& S, const Dense& dense) {
+  const size_t s = dense.s, alpha = (size_t)S.num_memories();
+  LookupPolys L;
+  lookup_polys_build(c, S, dense, alpha * s, L);
+  std::vector<std::unique_ptr<Poly>> ps(alpha);
+  for (size_t i = 0; i < alpha; i++) {
+    ps[i].reset(new Poly());
+    Poly& p = *ps[i];
+    p.ctx = c;
+    p.len = p.len_loc = s;
+    p.nv = log2_exact_or_ceil(s);
+    p.bits = table_bits(S);
+    p.d_fr.alloc(c, s);
+    LB_CUDA_CHECK(cudaMemcpyAsync(p.d_fr.p, L.E.p + i * s, s * sizeof(fr_t), cudaMemcpyDeviceToDevice, c->st));
+    if (L.E_u32.p) {
+      p.d_u32.alloc(c, s);
+      LB_CUDA_CHECK(cudaMemcpyAsync(p.d_u32.p, L.E_u32.p + i * s, s * 4, cudaMemcpyDeviceToDevice, c->st));
+    }
+  }
+  std::vector<Poly*> out(alpha);
+  for (size_t i = 0; i < alpha; i++) out[i] = ps[i].release();
+  return out;
+}
+
+std::vector<uint8_t> memory_check_prove(Ctx* c, const Strategy& S, const Dense& dense, const fr_t& gamma,
+                                        const fr_t& tau, const Gens& g, Transcript& transcript, RandomTape& tape) {
+  SpanTimer sp_all(c, "MemoryChecking.prove");
+  check_fit(S, dense, g);
+  reserve_working_memory(c, S, dense, g, false);
+  LookupPolys L;  // the reference's `subtables` argument: identical by construction to the caller's
+  lookup_polys_build(c, S, dense, ((size_t)1 << g.nv_d) / (size_t)c->world, L);
+  DBuf<fr_t> eqtab(c, std::max(dense.s_loc, dense.m_loc));
+  ByteWriter w;
+  memory_check(c, S, dense, L, g, gamma, tau, transcript, tape, eqtab.p, w);
   c->sync();
   return w.b;
 }
@@ -2418,6 +2502,29 @@ CubicOut cubic_prove(Ctx* c, const Poly* const* A, const Poly* const* B, int n, 
   ser_sumcheck(w, proof);
   out.proof = std::move(w.b);
   return out;
+}
+
+// ---------------------------------------------------------------------------------------------- memory checking of a caller
+// dim_j, read_j or final_j of the dense (which = 1, 2, 3) as a polynomial of its own: the ingest of poly_create over the
+// dense's Montgomery array, which also finds the width and makes the u32 mirror
+Poly* dense_poly(Ctx* c, const Dense& d, int which, size_t j) {
+  const fr_t* src = which == 3 ? d.fin(j) : (which == 2 ? d.read(j) : d.dim(j));
+  return poly_create(c, reinterpret_cast<const uint64_t*>(src), which == 3 ? d.m : d.s, 4, true, c->st);
+}
+// GrandProducts::new (memory_checking.rs:175-310) over a caller's memory T with dim as dim_usize: init and final by the
+// prover's memory kernel (G = 1), read and write by one gather over dim's u32 mirror (poly_kernels.cu)
+void memory_fingerprints(Ctx* c, const Poly& T, const Poly& dim, const Poly& read, const Poly& fin, const fr_t& gamma,
+                         const fr_t& tau, Poly* out[4]) {
+  SpanTimer sp(c, "GrandProducts.new");
+  std::unique_ptr<Poly> init(poly_shell(c, T.nv, 253)), rd(poly_shell(c, dim.nv, 253)), wr(poly_shell(c, dim.nv, 253)),
+      fl(poly_shell(c, T.nv, 253));
+  launch_gp_fingerprints_mem(T.d_fr.p, fin.d_fr.p, T.len, 1, 0, gamma, tau, init->d_fr.p, fl->d_fr.p, c->st);
+  launch_gp_fingerprints_gather(T.d_fr.p, dim.d_u32.p, read.d_fr.p, read.d_u32.p, dim.len, gamma, tau, rd->d_fr.p,
+                                wr->d_fr.p, c->st);
+  out[0] = init.release();
+  out[1] = rd.release();
+  out[2] = wr.release();
+  out[3] = fl.release();
 }
 
 }  // namespace lb

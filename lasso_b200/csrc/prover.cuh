@@ -348,6 +348,8 @@ std::vector<uint8_t> prove(Ctx*, const Strategy& S, Dense&, const std::vector<fr
                            RandomTape&, fr_t* claimed_evaluation);
 // Serialised sizes, fixed by the shapes.  prove's output (S and g fit dense):
 size_t proof_bytes(const Strategy& S, const Dense&, const Gens&);
+// the MemoryCheckingProof that ends prove's output and memory_check_prove's (S and g fit dense)
+size_t memory_check_bytes(const Strategy& S, const Dense&, const Gens&);
 // a PolyEvalProof at nv variables: L_vec and R_vec of nv - nv/2 points, delta, beta, z1, z2
 size_t dpl_bytes(size_t nv);
 // a BatchedGrandProductArgument over n circuits of v variables: layer j has j cubic rounds
@@ -360,6 +362,24 @@ size_t poly_commitment_bytes(size_t num_vars);
 // variables, with a u32 mirror when every value is below 2^32.  Single-GPU contexts (the caller checks).
 Poly* dense_outputs(Ctx*, const Strategy& S, const Dense&);
 void sample_generators(const std::string& label, size_t count, uint64_t* out_affine);
+
+// Memory checking inside a caller's protocol (single GPU; the caller checks)
+// Subtables::new (subtables/mod.rs:116-129): the alpha lookup polynomials E_i[j] = T_sub(i)[dim_i[j]] in memory order,
+// each of log2(s) variables with storage of its own, bits = the tables' width, a u32 mirror when that is <= 32
+std::vector<Poly*> lookup_polys(Ctx*, const Strategy& S, const Dense&);
+// MemoryCheckingProof::prove (memory_checking.rs:56-83) at (gamma, tau) on the caller's transcript and tape, advanced in
+// place; the lookup polynomials are rebuilt from (S, dense).  Throws before the first transcript write when S or g do
+// not fit the dense, with the working memory reserved before it too; a failed multiset check throws
+// LbError(LASSO_ERR_MULTISET) after the transcript has moved.
+std::vector<uint8_t> memory_check_prove(Ctx*, const Strategy& S, const Dense&, const fr_t& gamma, const fr_t& tau,
+                                        const Gens&, Transcript&, RandomTape&);
+// dim_j, read_j or final_j (which = 1, 2, 3; j < C) as a new polynomial with its u32 mirror
+Poly* dense_poly(Ctx*, const Dense&, int which, size_t j);
+// GrandProducts::new (memory_checking.rs:175-310) with dim as dim_usize: out = init, read, write, final, full-width
+// polynomials with hash(a, v, t) = t gamma^2 + v gamma + a - tau.  T.len == fin.len >= 2, dim.len == read.len >= 2,
+// dim has a u32 mirror with every entry below T.len (the caller checks).
+void memory_fingerprints(Ctx*, const Poly& T, const Poly& dim, const Poly& read, const Poly& fin, const fr_t& gamma,
+                         const fr_t& tau, Poly* out[4]);
 
 // dense polynomials of a caller (prover.cu): PolyCommitmentGens, DensePolynomial::{new, commit, evaluate},
 // PolyEvalProof::prove.  On a sharded context the calls are collective: every rank calls them with the same arguments

@@ -632,4 +632,115 @@ size_t orcd_poly_new_padded(const uint64_t* Z, size_t len, uint64_t* out) {
   return p.len;
 }
 
+// ---- MemoryCheckingProof on a caller's transcript and tape (memory_checking.rs:26-147), built-in strategies.
+// indices: n x C; the densified representation, its commitment (comm_out, serialize_commitment's bytes) and the
+// combined-table commitment to the lookup polynomials (derefs_out, a PolyCommitment) are made as
+// SparsePolynomialEvaluationProof::prove makes them.  r == null: MemoryCheckingProof::prove at (gamma, tau) on the
+// transcript as it is.  r != null: gamma and tau are ignored, and the steps of surge.rs:129-186 run first on the
+// transcript and the tape (the proof's prefix, not returned), with (gamma, tau) = challenge_vector("challenge_r_hash", 2)
+// as surge.rs:188 draws them.  Returns the length of the serialised proof in out (0 on error); *comm_len and
+// *derefs_len receive the commitments' lengths.
+size_t orcd_memory_check_prove(int kind, size_t C, size_t log_m, size_t log_r, const uint64_t* indices, size_t n,
+                               const uint64_t* gamma, const uint64_t* tau, const uint64_t* r, const uint64_t* stream,
+                               size_t n_points, void* transcript, void* tape, uint8_t* out, size_t cap, uint8_t* comm_out,
+                               size_t comm_cap, size_t* comm_len, uint8_t* derefs_out, size_t derefs_cap,
+                               size_t* derefs_len) {
+  try {
+    const Strategy S{kind, C, log_m, log_r};
+    std::vector<std::vector<size_t>> idx(n, std::vector<size_t>(C));
+    for (size_t j = 0; j < n; j++)
+      for (size_t i = 0; i < C; i++) idx[j][i] = indices[j * C + i];
+    DensifiedRepresentation dense = DensifiedRepresentation::from_lookup_indices(idx, C, log_m);
+    if (n_points < SparsePolyCommitmentGens::needs_points(C, dense.s, S.num_memories(), log_m)) return 0;
+    SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, dense.s, S.num_memories(), log_m, ldstream(stream, n_points));
+    const std::vector<uint8_t> cb = serialize_commitment(densified_commit(dense, pg));
+    Subtables subtables(S, dense.dim_usize, dense.s);
+    const PolyCommitment comm_derefs = subtables.commit(pg.gens_derefs);
+    const std::vector<uint8_t> db = ser_commitment(comm_derefs);
+    Transcript& T = *(Transcript*)transcript;
+    RandomTape& tp = *(RandomTape*)tape;
+    Fr g = ldfr(gamma), t = ldfr(tau);
+    if (r) {  // surge.rs:129-188 with the oracle's own steps, as SparsePolynomialEvaluationProof::prove runs them
+      T.append_protocol_name("Lasso SparsePolynomialEvaluationProof");
+      append_combined_table_commitment(comm_derefs, "comm_poly_row_col_ops_val", T);
+      EqPolynomial eq(ldvec(r, ark_log2(dense.s)));
+      T.append_scalar("claim_eval_scalar_product", subtables.compute_sumcheck_claim(eq));
+      std::vector<DensePolynomial> combined;
+      for (auto& p : subtables.lookup_polys) combined.push_back(p.clone());
+      combined.emplace_back(eq.evals());
+      std::vector<Fr> r_z, final_evals, eval_derefs;
+      SumcheckInstanceProof::prove_arbitrary(
+          log_2(dense.s), combined, [&](const Fr* v) { return S.combine_lookups_eq(v); }, S.sumcheck_poly_degree(), T,
+          r_z, final_evals);
+      for (auto& p : subtables.lookup_polys) eval_derefs.push_back(p.evaluate(r_z));
+      CombinedTableEvalProof::prove(subtables.combined_poly, eval_derefs, r_z, pg.gens_derefs, T, tp);
+      const std::vector<Fr> r_hash = T.challenge_vector("challenge_r_hash", 2);
+      g = r_hash[0];
+      t = r_hash[1];
+    }
+    const MemoryCheckingProof mc = MemoryCheckingProof::prove(dense, g, t, subtables, pg, T, tp);
+    ByteWriter w;  // field order: memory_checking.rs:26-37, 655-660, 313-329
+    for (auto& e : mc.proof_prod_layer.grand_product_evals)
+      for (int k = 0; k < 4; k++) w.fr(e[k]);
+    ser(w, mc.proof_prod_layer.proof_mem);
+    ser(w, mc.proof_prod_layer.proof_ops);
+    const auto& hl = mc.proof_hash_layer;
+    w.arr_fr(hl.eval_dim);
+    w.arr_fr(hl.eval_read);
+    w.arr_fr(hl.eval_final);
+    w.arr_fr(hl.eval_derefs);
+    ser(w, hl.proof_ops.proof);
+    ser(w, hl.proof_mem.proof);
+    ser(w, hl.proof_derefs.proof_table_eval.proof);
+    if (w.b.size() > cap || cb.size() > comm_cap || db.size() > derefs_cap) return 0;
+    memcpy(out, w.b.data(), w.b.size());
+    memcpy(comm_out, cb.data(), cb.size());
+    memcpy(derefs_out, db.data(), db.size());
+    *comm_len = cb.size();
+    *derefs_len = db.size();
+    return w.b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_memory_check_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// MemoryCheckingProof::verify (memory_checking.rs:85-147) of serialised bytes at (gamma, tau) against the two
+// commitments orcd_memory_check_prove returns, on a caller's transcript: 0 accepted, 1 rejected, 2 the bytes do not
+// parse or the generator stream is too short
+int orcd_memory_check_verify(int kind, size_t C, size_t log_m, size_t log_r, const uint64_t* stream, size_t n_points,
+                             const uint8_t* comm, size_t comm_len, const uint8_t* derefs, size_t derefs_len,
+                             const uint8_t* proof, size_t proof_len, const uint64_t* gamma, const uint64_t* tau,
+                             void* transcript) {
+  const Strategy S{kind, C, log_m, log_r};
+  const size_t alpha = S.num_memories();
+  SparsePolynomialCommitment c;
+  if (!read_sparse_commitment(comm, comm_len, c)) return 2;
+  Reader rc{derefs, derefs_len};
+  PolyCommitment comm_derefs;
+  comm_derefs.C = rc.points();
+  if (!rc.ok || rc.at != derefs_len) return 2;
+  Reader rd{proof, proof_len};
+  MemoryCheckingProof mc;
+  auto& pl = mc.proof_prod_layer;
+  for (size_t i = 0; rd.ok && i < alpha; i++) {
+    std::array<Fr, 4> e;
+    for (int k = 0; k < 4; k++) e[k] = rd.fr();
+    pl.grand_product_evals.push_back(e);
+  }
+  pl.proof_mem = read_gpa(rd);
+  pl.proof_ops = read_gpa(rd);
+  auto& hl = mc.proof_hash_layer;
+  hl.eval_dim = read_frs(rd, C);
+  hl.eval_read = read_frs(rd, C);
+  hl.eval_final = read_frs(rd, C);
+  hl.eval_derefs = read_frs(rd, alpha);
+  hl.proof_ops.proof = read_dpl(rd);
+  hl.proof_mem.proof = read_dpl(rd);
+  hl.proof_derefs.proof_table_eval.proof = read_dpl(rd);
+  if (!rd.ok || rd.at != proof_len) return 2;
+  if (n_points < SparsePolyCommitmentGens::needs_points(C, c.s, alpha, log_m)) return 2;
+  SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, c.s, alpha, log_m, ldstream(stream, n_points));
+  return mc.verify(S, c, comm_derefs, pg, ldfr(gamma), ldfr(tau), c.s, *(Transcript*)transcript) ? 0 : 1;
+}
+
 }  // extern "C"
