@@ -593,6 +593,71 @@ int lasso_sumcheck_prove_cubic_batched(lasso_ctx*, const lasso_poly* const* A, c
 int lasso_poly_create_comb(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
                            lasso_poly** out);
 
+/* ---------------------------------------------------------------- zero-knowledge sumchecks
+ *
+ * The hiding form of lasso_sumcheck_prove, so that a caller's Spartan-style protocol over hiding commitments and
+ * openings (lasso_poly_commit_hiding, lasso_poly_eval_prove_hiding) puts no round polynomial in the clear.
+ *
+ * MultiCommitGens { n, G, h } (poly/commitments.rs:14-70) on the device: n points G (1 <= n <= 1024, LASSO_ERR_LENGTH
+ * otherwise) and h, in the 64-byte affine layout lasso_sample_generators writes; the points are not validated.  Both ways
+ * the reference builds them are explicit points of one stream s: MultiCommitGens::new(n, label) is G = s[0..n),
+ * h = s[n]; DotProductProofGens::new(n, label) (dot_product.rs:144-150) is gens_n = (s[0..n), s[n+1]) and
+ * gens_1 = ([s[n]], s[n+1]).  The object always builds the 8-bit digit-multiples table of its n + 1 points (393 KB per
+ * point, 0.4 GB at n = 1024), the one commitment path; LASSO_B200_NO_MULTIPLES does not apply to it.  LASSO_ERR_GENS for
+ * null points or output. */
+typedef struct lasso_mc_gens lasso_mc_gens;
+int lasso_mc_gens_create(lasso_ctx*, const uint64_t* G_affine, size_t n, const uint64_t h_affine[8], lasso_mc_gens** out);
+size_t lasso_mc_gens_n(const lasso_mc_gens*);
+void lasso_mc_gens_destroy(lasso_mc_gens*);
+/* Commitments::batch_commit (commitments.rs:84-93), and commit when gens.n == 1: out = <scalars, G> + blind h,
+ * compressed.  LASSO_ERR_GENS for generators of another context or n != gens.n; LASSO_ERR_LENGTH for a null input or
+ * output; LASSO_ERR_VALUE for a scalar or blind that is not a canonical residue. */
+int lasso_mc_commit(lasso_ctx*, const lasso_mc_gens*, const uint64_t* scalars, size_t n, const uint64_t blind[4],
+                    uint8_t out[32]);
+/* DotProductProof::prove (subprotocols/dot_product.rs:31-93) on the caller's transcript and tape, advanced in place:
+ * protocol name "dot product proof"; tape d_vec (n), r_delta, r_beta; transcript Cx, Cy, a, delta, beta, then
+ * challenge c.  proof_out: {delta, beta, z, z_delta, z_beta}, ark-serialize compressed, 136 + 32 n bytes (*proof_len
+ * receives the size, also when proof_cap is too small); Cx_out = <x, G_n> + blind_x h_n and Cy_out = y G_1 + blind_y
+ * h_1, the commitments the reference returns alongside.  As in the reference, y is not checked against <x, a>: a wrong y
+ * gives a proof the verifier rejects.  Two two-row MSMs over the gens' tables, one host wait.
+ * Errors, each before any launch and before the transcript or the tape moves: LASSO_ERR_GENS for null generators or
+ * generators of another context, gens_1.n != 1 or gens_n.n != n; LASSO_ERR_LENGTH for a null transcript, tape, input or
+ * output, or proof_cap too small; LASSO_ERR_VALUE for an x, a, y or blind that is not a canonical residue. */
+int lasso_dot_product_prove(lasso_ctx*, const lasso_mc_gens* gens_1, const lasso_mc_gens* gens_n, lasso_transcript*,
+                            lasso_random_tape*, const uint64_t* x, const uint64_t blind_x[4], const uint64_t* a, size_t n,
+                            const uint64_t y[4], const uint64_t blind_y[4], uint8_t* proof_out, size_t proof_cap,
+                            size_t* proof_len, uint8_t Cx_out[32], uint8_t Cy_out[32]);
+/* The sumcheck of lasso_sumcheck_prove (g of degree d over the caller's polynomials, num_rounds R) as a
+ * ZKSumcheckInstanceProof { comm_polys, comm_evals, proofs }, whose verifier is subprotocols/sumcheck.rs:331-447.
+ * The tape is drawn up front: random_vector("blinds_poly", R), random_vector("blinds_evals", R), then each round's
+ * DotProductProof draws.  Round j, with claim_0 = the claim and beta_0 = blind_claim, claim_j = eval_{j-1} and
+ * beta_j = blinds_evals[j-1] after it: the round polynomial's coefficients c are committed as comm_poly =
+ * <c, G_n> + blinds_poly[j] h_n and appended, r_j is drawn; comm_eval = poly(r_j) G_1 + blinds_evals[j] h_1; the
+ * transcript takes comm_claim_per_round (comm_claim in round 0, comm_evals[j-1] after it) and comm_eval and gives
+ * w = challenge_vector("combine_two_claims_to_one", 2); then DotProductProof::prove of x = c, a = w0 (2, 1, .., 1) +
+ * w1 (1, r_j, r_j^2, ..), y = w0 claim_j + w1 eval, blind_y = w0 beta_j + w1 blinds_evals[j].  The reference has no
+ * prover for this struct: this tape order is that of Spartan's prove_*_zk, recalled rather than checked against a
+ * source.
+ *  - proof_out: ark-serialize compressed, 24 + R (200 + 32 (d + 1)) bytes (*proof_len receives it, also when proof_cap
+ *    is too small); r_out: R challenges; final_evals_out: n_polys values, element 0 of every polynomial after the binds;
+ *  - claim_out (may be null): the first round polynomial at 0 plus at 1, as lasso_sumcheck_prove's;
+ *  - comm_claim_out (may be null): claim G_1 + blind_claim h_1, the commitment the verifier takes;
+ *  - blind_eval_out (may be null): blinds_evals[R-1], the blind of the last comm_eval, to link it to the caller's
+ *    openings.
+ * The polynomials are not modified.  Launches: those of lasso_sumcheck_prove, 2 ceil(R/2) for the deltas (two rounds per
+ * MSM, before the first round) and 6 per round (comm_poly; comm_eval, with comm_claim in round 0; Cy with beta): three
+ * host waits per round more than the plain call.
+ * Errors, each before any launch and before the transcript or the tape moves: those of lasso_sumcheck_prove
+ * (LASSO_ERR_STRATEGY on a sharded context); LASSO_ERR_GENS for null generators or generators of another context,
+ * gens_1.n != 1 or gens_n.n != d + 1 (sumcheck.rs:358); LASSO_ERR_LENGTH for a null tape, blind_claim, r_out or
+ * final_evals_out; LASSO_ERR_VALUE for a blind_claim that is not a canonical residue.  The working memory is allocated
+ * before the tape or the transcript moves. */
+int lasso_zk_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* const* polys, size_t n_polys,
+                            size_t num_rounds, const uint64_t blind_claim[4], const lasso_mc_gens* gens_1,
+                            const lasso_mc_gens* gens_n, lasso_transcript*, lasso_random_tape*, uint8_t* proof_out,
+                            size_t proof_cap, size_t* proof_len, uint64_t* r_out, uint64_t* final_evals_out,
+                            uint64_t claim_out[4], uint8_t comm_claim_out[32], uint64_t blind_eval_out[4]);
+
 /* ---------------------------------------------------------------- grand products over a caller's polynomials
  *
  * GrandProductCircuit::new (subprotocols/grand_product.rs:38-58) over a polynomial of the context with

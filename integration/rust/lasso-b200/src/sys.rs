@@ -46,6 +46,10 @@ pub struct lasso_comb {
 pub struct lasso_gp_circuit {
     _p: [u8; 0],
 }
+#[repr(C)]
+pub struct lasso_mc_gens {
+    _p: [u8; 0],
+}
 
 extern "C" {
     pub fn lasso_last_error() -> *const c_char;
@@ -198,6 +202,24 @@ extern "C" {
                                 num_rounds: usize, transcript: *mut lasso_transcript, proof_out: *mut u8, proof_cap: usize,
                                 proof_len: *mut usize, r_out: *mut u64, final_evals_out: *mut u64, claim_out: *mut u64)
                                 -> c_int;
+    pub fn lasso_mc_gens_create(ctx: *mut lasso_ctx, g_affine: *const u64, n: usize, h_affine: *const u64,
+                                out: *mut *mut lasso_mc_gens) -> c_int;
+    pub fn lasso_mc_gens_n(g: *const lasso_mc_gens) -> usize;
+    pub fn lasso_mc_gens_destroy(g: *mut lasso_mc_gens);
+    pub fn lasso_mc_commit(ctx: *mut lasso_ctx, gens: *const lasso_mc_gens, scalars: *const u64, n: usize, blind: *const u64,
+                           out: *mut u8) -> c_int;
+    pub fn lasso_dot_product_prove(ctx: *mut lasso_ctx, gens_1: *const lasso_mc_gens, gens_n: *const lasso_mc_gens,
+                                   transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape, x: *const u64,
+                                   blind_x: *const u64, a: *const u64, n: usize, y: *const u64, blind_y: *const u64,
+                                   proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize, cx_out: *mut u8,
+                                   cy_out: *mut u8) -> c_int;
+    pub fn lasso_zk_sumcheck_prove(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly,
+                                   n_polys: usize, num_rounds: usize, blind_claim: *const u64,
+                                   gens_1: *const lasso_mc_gens, gens_n: *const lasso_mc_gens,
+                                   transcript: *mut lasso_transcript, random_tape: *mut lasso_random_tape,
+                                   proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize, r_out: *mut u64,
+                                   final_evals_out: *mut u64, claim_out: *mut u64, comm_claim_out: *mut u8,
+                                   blind_eval_out: *mut u64) -> c_int;
     pub fn lasso_poly_create_comb(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly,
                                   n_polys: usize, out: *mut *mut lasso_poly) -> c_int;
     pub fn lasso_sumcheck_prove_cubic_batched(ctx: *mut lasso_ctx, a: *const *const lasso_poly, b: *const *const lasso_poly,

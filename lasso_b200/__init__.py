@@ -34,13 +34,22 @@ and the memory check of a lookup proof, or of a caller's own memory, inside a ca
     GrandProducts.new(ctx, eval_table, dim, read, final, (gamma, tau))   src/subtables/memory_checking.rs:175
     Transcript.append_combined_table_commitment(commitment)              src/subtables/mod.rs:382
 
+and zero-knowledge sumchecks over a caller's polynomials (single GPU; the commitments and dot-product proofs also sharded):
+
+    MultiCommitGens(ctx, G, h), MultiCommitGens.new(ctx, n, label), .commit(scalars, blind)   src/poly/commitments.rs:14, 84
+    DotProductProofGens.new(ctx, n, label).gens_n / .gens_1             src/subprotocols/dot_product.rs:144
+    DotProductProof.prove(ctx, gens_1, gens_n, transcript, random_tape, x, blind_x, a, y, blind_y)
+                                                                         src/subprotocols/dot_product.rs:31
+    ZKSumcheckInstanceProof.prove(ctx, comb, polys, num_rounds, blind_claim, gens_1, gens_n, transcript, random_tape)
+                                                                         src/subprotocols/sumcheck.rs:331 (its verifier)
+
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, GrandProductCircuit, GrandProducts, LassoError, MemoryCheckingProof, MsmJob, PolyCommitmentGens, PolyEvalProof,
-    RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Subtables, SumcheckInstanceProof, Transcript,
+    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, DotProductProof, DotProductProofGens, GrandProductCircuit, GrandProducts, LassoError, MemoryCheckingProof, MsmJob,
+    MultiCommitGens, PolyCommitmentGens, PolyEvalProof, RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Subtables, SumcheckInstanceProof, Transcript, ZKSumcheckInstanceProof,
     bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,
     msm, poly_gens_points_needed, sample_generators, sumcheck_bind_round_arbitrary,

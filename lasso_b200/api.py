@@ -1189,6 +1189,120 @@ class SumcheckInstanceProof:
         return cls(bytes(out[: ln.value]), r[:num_rounds], fin, claim.reshape(4).copy())
 
 
+# ------------------------------------------------------------------ zero-knowledge sumchecks
+class MultiCommitGens:
+    """src/poly/commitments.rs:14-70: n points G and h (64-byte affine, (n, 8) and (8,) uint64), 1 <= n <= 1024, on
+    ctx's GPU with the digit-multiples table of all n + 1 points.  Usable on a sharded context: no exchange."""
+
+    def __init__(self, ctx, G, h):
+        G, h = _fr(G, 8).reshape(-1, 8), _fr(h, 8).reshape(8)
+        self._h = None
+        hd = C.c_void_p()
+        _chk(lib().lasso_mc_gens_create(ctx._h, _p(G), C.c_size_t(G.shape[0]), _p(h), C.byref(hd)))
+        self.ctx, self._h, self.G, self.h, self.n = ctx, hd, G, h, G.shape[0]
+
+    @classmethod
+    def new(cls, ctx, n, label):
+        """MultiCommitGens::new(n, label) (commitments.rs:22-44): G = the first n points of the label's stream, h the
+        next"""
+        s = sample_generators(_label(label), int(n) + 1)
+        return cls(ctx, s[:n], s[n])
+
+    def commit(self, scalars, blind):
+        """Commitments::batch_commit (commitments.rs:84-93), commit when n == 1: <scalars, G> + blind h, 32 bytes
+        compressed"""
+        s = _limbs(scalars, self.n, "scalars")
+        b = _limbs(blind, 1, "the blind")
+        out = np.zeros(32, dtype=np.uint8)
+        _chk(lib().lasso_mc_commit(self.ctx._h, self._h, _p(s), C.c_size_t(self.n), _p(b), _p(out)))
+        return out.tobytes()
+
+    def __del__(self):
+        try:
+            if self._h and self.ctx._h:
+                lib().lasso_mc_gens_destroy(self._h)
+                self._h = None
+        except Exception:
+            pass
+
+
+class DotProductProofGens:
+    """src/subprotocols/dot_product.rs:138-150: MultiCommitGens::new(n + 1, label).split_at(n), i.e. gens_n =
+    (s[0..n), s[n+1]) and gens_1 = ([s[n]], s[n+1]) of the label's stream s"""
+
+    def __init__(self, n, gens_n, gens_1):
+        self.n, self.gens_n, self.gens_1 = n, gens_n, gens_1
+
+    @classmethod
+    def new(cls, ctx, n, label):
+        n = int(n)
+        s = sample_generators(_label(label), n + 2)
+        return cls(n, MultiCommitGens(ctx, s[:n], s[n + 1]), MultiCommitGens(ctx, s[n:n + 1], s[n + 1]))
+
+
+class DotProductProof:
+    """src/subprotocols/dot_product.rs:11-136"""
+
+    @staticmethod
+    def proof_len(n):
+        return 136 + 32 * int(n)
+
+    @staticmethod
+    def prove(ctx, gens_1, gens_n, transcript, random_tape, x, blind_x, a, y, blind_y):
+        """DotProductProof::prove on the caller's transcript and tape, advanced in place -> (proof bytes, Cx, Cy), the
+        commitments 32 bytes compressed.  y is not checked against <x, a>: a wrong one gives a proof the verifier
+        rejects."""
+        x = _limbs(x, what="x")
+        n = x.shape[0]
+        a = _limbs(a, n, "a")
+        bx, y, by = _limbs(blind_x, 1, "blind_x"), _limbs(y, 1, "y"), _limbs(blind_y, 1, "blind_y")
+        cap = DotProductProof.proof_len(n)
+        out = np.zeros(cap, dtype=np.uint8)
+        cx, cy = np.zeros(32, dtype=np.uint8), np.zeros(32, dtype=np.uint8)
+        ln = C.c_size_t(0)
+        _chk(lib().lasso_dot_product_prove(ctx._h, gens_1._h, gens_n._h, transcript._h, random_tape._h, _p(x), _p(bx),
+                                           _p(a), C.c_size_t(n), _p(y), _p(by), _p(out), C.c_size_t(cap), C.byref(ln),
+                                           _p(cx), _p(cy)))
+        return bytes(out[: ln.value]), cx.tobytes(), cy.tobytes()
+
+
+class ZKSumcheckInstanceProof:
+    """src/subprotocols/sumcheck.rs:330-447, proven on the GPU.  `.data` is the ark-serialize (compressed) proof, `.r`
+    the challenges, `.final_evals` every polynomial at r after the binds, `.claim` the sum over the hypercube,
+    `.comm_claim` its commitment claim G_1 + blind_claim h_1 (32 bytes), `.blind_eval` the blind of the last comm_eval."""
+
+    def __init__(self, data, r, final_evals, claim, comm_claim, blind_eval):
+        self.data, self.r, self.final_evals = data, r, final_evals
+        self.claim, self.comm_claim, self.blind_eval = claim, comm_claim, blind_eval
+
+    @staticmethod
+    def proof_len(num_rounds, degree):
+        return 24 + int(num_rounds) * (200 + 32 * (int(degree) + 1))
+
+    @classmethod
+    def prove(cls, ctx, comb, polys, num_rounds, blind_claim, gens_1, gens_n, transcript, random_tape):
+        """the sumcheck of SumcheckInstanceProof.prove_arbitrary, zero-knowledge, on the caller's transcript and tape,
+        advanced in place (include/lasso_b200.h lasso_zk_sumcheck_prove).  gens_1.n == 1, gens_n.n == comb.degree + 1.
+        num_rounds=None: num_vars.  Single GPU."""
+        polys = list(polys)
+        if num_rounds is None:
+            num_rounds = polys[0].num_vars if polys else 0
+        num_rounds = int(num_rounds)
+        bc = _limbs(blind_claim, 1, "blind_claim")
+        cap = cls.proof_len(max(num_rounds, 0), comb.degree)
+        out = np.zeros(cap, dtype=np.uint8)
+        r = np.zeros((max(num_rounds, 1), 4), dtype=np.uint64)
+        fin = np.zeros((max(len(polys), 1), 4), dtype=np.uint64)
+        claim, blind_eval = np.zeros(4, dtype=np.uint64), np.zeros(4, dtype=np.uint64)
+        cc = np.zeros(32, dtype=np.uint8)
+        n = C.c_size_t(0)
+        _chk(lib().lasso_zk_sumcheck_prove(ctx._h, comb._h, _handles(polys), C.c_size_t(len(polys)),
+                                           C.c_size_t(num_rounds), _p(bc), gens_1._h, gens_n._h, transcript._h,
+                                           random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin),
+                                           _p(claim), _p(cc), _p(blind_eval)))
+        return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim, cc.tobytes(), blind_eval)
+
+
 # ------------------------------------------------------------------ grand products over a caller's polynomials
 class GrandProductCircuit:
     """src/subprotocols/grand_product.rs:14-66 over a DensePolynomial of ctx with 1 <= num_vars <= 28: the layers above

@@ -50,6 +50,10 @@ struct lasso_poly {
 struct lasso_comb {
   Comb g;
 };
+// MultiCommitGens of the zero-knowledge sumcheck and dot-product proof
+struct lasso_mc_gens {
+  McGens* g;
+};
 // GrandProductCircuit over a caller's polynomial (layer 0, not owned); proving binds its layers, so it is proven once
 struct lasso_gp_circuit {
   Ctx* c;
@@ -1540,6 +1544,111 @@ int lasso_poly_create_comb(lasso_ctx* h, const lasso_comb* g, const lasso_poly* 
   if (const int rc = poly_size_check(h, ps[0]->nv)) return rc;
   if (!out) return fail(LASSO_ERR_LENGTH, "comb poly: null output");
   *out = new lasso_poly{poly_create_comb(h->c, g->g, ps.data(), (int)n_polys)};
+  return 0;
+  LB_CATCH
+}
+
+// ---- zero-knowledge sumchecks: MultiCommitGens, commitments, DotProductProof, ZKSumcheckInstanceProof
+// Every call but lasso_zk_sumcheck_prove runs on a sharded context too: each rank computes alone, with no exchange.
+int lasso_mc_gens_create(lasso_ctx* h, const uint64_t* G_affine, size_t n, const uint64_t h_affine[8],
+                         lasso_mc_gens** out) {
+  LB_TRY_CTX(h)
+  if (out) *out = nullptr;
+  if (!out || !G_affine || !h_affine) return fail(LASSO_ERR_GENS, "mc gens: null points or output");
+  if (n < 1 || n > kMcMaxN) return fail(LASSO_ERR_LENGTH, "mc gens: n must be in 1..1024");
+  *out = new lasso_mc_gens{mc_gens_create(h->c, G_affine, n, h_affine)};
+  return 0;
+  LB_CATCH
+}
+size_t lasso_mc_gens_n(const lasso_mc_gens* g) { return g ? g->g->n : 0; }
+void lasso_mc_gens_destroy(lasso_mc_gens* g) {
+  if (!g) return;
+  cudaSetDevice(g->g->ctx->device);
+  delete g->g;
+  delete g;
+}
+// gens of this context with n points (n == 0: any n)
+static int mc_gens_check(lasso_ctx* h, const char* what, const lasso_mc_gens* g, size_t n) {
+  if (!g || g->g->ctx != h->c) return fail(LASSO_ERR_GENS, std::string(what) + ": null generators, or of another context");
+  if (n && g->g->n != n)
+    return fail(LASSO_ERR_GENS, std::string(what) + ": generators of n = " + std::to_string(g->g->n) + ", expected " +
+                                    std::to_string(n));
+  return 0;
+}
+int lasso_mc_commit(lasso_ctx* h, const lasso_mc_gens* g, const uint64_t* scalars, size_t n, const uint64_t blind[4],
+                    uint8_t out[32]) {
+  LB_TRY_CTX(h)
+  if (const int rc = mc_gens_check(h, "mc commit", g, 0)) return rc;
+  if (n != g->g->n) return fail(LASSO_ERR_GENS, "mc commit: n != gens.n (commitments.rs:85)");
+  if (!scalars || !blind || !out) return fail(LASSO_ERR_LENGTH, "mc commit: null scalars, blind or output");
+  std::vector<fr_t> s, b;
+  if (!load_scalars(scalars, n, s) || !load_scalars(blind, 1, b))
+    return fail(LASSO_ERR_VALUE, "mc commit: a scalar or the blind is not a canonical residue");
+  timed(h->c->t_commit_ms, [&] {
+    mc_commit(h->c, *g->g, s, b[0], out);
+    return 0;
+  });
+  return 0;
+  LB_CATCH
+}
+int lasso_dot_product_prove(lasso_ctx* h, const lasso_mc_gens* gens_1, const lasso_mc_gens* gens_n,
+                            lasso_transcript* transcript, lasso_random_tape* tape, const uint64_t* x,
+                            const uint64_t blind_x[4], const uint64_t* a, size_t n, const uint64_t y[4],
+                            const uint64_t blind_y[4], uint8_t* proof_out, size_t proof_cap, size_t* proof_len,
+                            uint8_t Cx_out[32], uint8_t Cy_out[32]) {
+  LB_TRY_CTX(h)
+  if (const int rc = mc_gens_check(h, "dot product proof", gens_1, 1)) return rc;
+  if (const int rc = mc_gens_check(h, "dot product proof", gens_n, 0)) return rc;
+  if (gens_n->g->n != n) return fail(LASSO_ERR_GENS, "dot product proof: gens_n.n != a.len() (dot_product.rs:50)");
+  const size_t need = dot_product_bytes(n);
+  if (const int rc = out_room("dot product proof", need, proof_out, proof_cap, proof_len)) return rc;
+  if (!transcript || !tape || !x || !blind_x || !a || !y || !blind_y || !Cx_out || !Cy_out)
+    return fail(LASSO_ERR_LENGTH, "dot product proof: null transcript, random tape, input or output");
+  std::vector<fr_t> xv, av, bx, yv, by;
+  if (!load_scalars(x, n, xv) || !load_scalars(a, n, av) || !load_scalars(blind_x, 1, bx) || !load_scalars(y, 1, yv) ||
+      !load_scalars(blind_y, 1, by))
+    return fail(LASSO_ERR_VALUE, "dot product proof: x, a, y or a blind is not a canonical residue");
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return dot_product_prove(h->c, *gens_1->g, *gens_n->g, transcript->t, tape->t, xv, bx[0], av, yv[0], by[0], Cx_out,
+                             Cy_out);
+  });
+  return out_copy("dot product proof", b, need, proof_out);
+  LB_CATCH
+}
+int lasso_zk_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly* const* polys, size_t n_polys,
+                            size_t num_rounds, const uint64_t blind_claim[4], const lasso_mc_gens* gens_1,
+                            const lasso_mc_gens* gens_n, lasso_transcript* transcript, lasso_random_tape* tape,
+                            uint8_t* proof_out, size_t proof_cap, size_t* proof_len, uint64_t* r_out,
+                            uint64_t* final_evals_out, uint64_t claim_out[4], uint8_t comm_claim_out[32],
+                            uint64_t blind_eval_out[4]) {
+  LB_TRY_CTX(h)
+  if (poly_ctx_check(h)) return LASSO_ERR_STRATEGY;
+  if (!g) return fail(LASSO_ERR_STRATEGY, "zk sumcheck: null combining function");
+  if (!polys || n_polys != (size_t)g->g.n_inputs)
+    return fail(LASSO_ERR_STRATEGY, "zk sumcheck: " + std::to_string(n_polys) + " polynomials for a combining function of " +
+                                        std::to_string(g->g.n_inputs) + " inputs");
+  std::vector<const Poly*> ps;
+  if (const int rc = poly_array(h, "zk sumcheck", polys, n_polys, true, ps)) return rc;
+  if (num_rounds < 1 || num_rounds > ps[0]->nv) return fail(LASSO_ERR_LENGTH, "zk sumcheck: num_rounds must be in 1..num_vars");
+  if (const int rc = mc_gens_check(h, "zk sumcheck", gens_1, 1)) return rc;
+  // sumcheck.rs:358: gens_n.n == degree_bound + 1
+  if (const int rc = mc_gens_check(h, "zk sumcheck", gens_n, (size_t)g->g.degree + 1)) return rc;
+  const size_t need = zk_sumcheck_bytes(num_rounds, (size_t)g->g.degree);
+  if (const int rc = out_room("zk sumcheck", need, proof_out, proof_cap, proof_len)) return rc;
+  if (!transcript || !tape || !blind_claim || !r_out || !final_evals_out)
+    return fail(LASSO_ERR_LENGTH, "zk sumcheck: null transcript, random tape, blind_claim or output");
+  std::vector<fr_t> bc;
+  if (!load_scalars(blind_claim, 1, bc)) return fail(LASSO_ERR_VALUE, "zk sumcheck: blind_claim is not a canonical residue");
+  const ZkSumcheckOut o = timed(h->c->t_prove_ms, [&] {
+    return zk_sumcheck_prove(h->c, g->g, ps.data(), (int)n_polys, num_rounds, bc[0], *gens_1->g, *gens_n->g,
+                             transcript->t, tape->t);
+  });
+  if (const int rc = out_copy("zk sumcheck", o.proof, need, proof_out)) return rc;
+  for (size_t j = 0; j < num_rounds; j++) memcpy(r_out + 4 * j, o.r[j].v, 32);
+  for (size_t j = 0; j < n_polys; j++) memcpy(final_evals_out + 4 * j, o.final_evals[j].v, 32);
+  if (claim_out) memcpy(claim_out, o.claim.v, 32);
+  if (comm_claim_out) memcpy(comm_claim_out, o.comm_claim, 32);
+  if (blind_eval_out) memcpy(blind_eval_out, o.blind_eval.v, 32);
   return 0;
   LB_CATCH
 }

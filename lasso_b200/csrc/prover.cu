@@ -2330,13 +2330,15 @@ Poly* poly_create_comb(Ctx* c, const Comb& g, const Poly* const* polys, int k) {
   launch_comb_map(dev.pg, in, p->len_loc, p->d_fr.p, c->st);
   return p.release();
 }
-// prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first evaluates the
-// caller's buffers; each later one binds the previous challenge and evaluates, fused from q = 2^15 pairs up, else a
-// bind and an evaluation) and one kernel that binds the last challenge into element 0 of every input and publishes the
-// k final evaluations.  LASSO_B200_UNFUSED_SUMCHECK (read per call, for A/B runs in one process) never fuses.
-SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int k, size_t num_rounds,
-                           Transcript& transcript) {
-  SpanTimer sp(c, "Sumcheck.prove_arbitrary");
+// The rounds of prove_arbitrary over a caller's polynomials.  Launches per call: one round kernel per round (the first
+// evaluates the caller's buffers; each later one binds the previous challenge and evaluates, fused from q = 2^15 pairs
+// up, else a bind and an evaluation) and one kernel that binds the last challenge into element 0 of every input and
+// publishes the k final evaluations.  LASSO_B200_UNFUSED_SUMCHECK (read per call, for A/B runs in one process) never
+// fuses.  begin() runs once the working memory is allocated, before the first round; step(j, evals) turns round j's
+// d + 1 evaluations into its challenge.  Fills out.r and out.final_evals.
+template <class Begin, class Step>
+static void comb_rounds(Ctx* c, const Comb& g, const Poly* const* polys, int k, size_t num_rounds, SumcheckOut& out,
+                        Begin&& begin, Step&& step) {
   const size_t nv = polys[0]->nv, npts = (size_t)g.degree + 1;
   // every allocation before the first transcript write: a failure leaves the caller's transcript as it was
   DBuf<fr_t> ws;
@@ -2350,9 +2352,7 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
     if (ws.p) dst.p[j] = ws.p + ((size_t)j << (nv - 1));
   }
   const bool unfused = getenv("LASSO_B200_UNFUSED_SUMCHECK") != nullptr;
-  SumcheckOut out;
-  ByteWriter w;
-  w.u64(num_rounds);
+  begin();
   std::vector<fr_t> evals(npts);
   size_t len = polys[0]->len;  // the length of the arrays src points to
   fr_t r_prev = fr_zero();
@@ -2369,17 +2369,226 @@ SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int 
       len /= 2;
     }
     c->fin_wait(f, evals.data(), (int)npts);
-    if (j == 0) out.claim = fr_add(evals[0], evals[1]);
-    const std::vector<fr_t> coeffs = unipoly_from_evals(evals);
-    unipoly_append(coeffs, transcript);
-    r_prev = transcript.challenge_scalar("challenge_nextround");
+    r_prev = step(j, evals);
     out.r.push_back(r_prev);
-    w.vec_fr(unipoly_compress(coeffs));
   }
   out.final_evals.resize(k);
   const Finalize f = c->fin_begin();
   launch_final_comb(src, k, len / 2, r_prev, f, c->st);
   c->fin_wait(f, out.final_evals.data(), k);
+}
+SumcheckOut sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int k, size_t num_rounds,
+                           Transcript& transcript) {
+  SpanTimer sp(c, "Sumcheck.prove_arbitrary");
+  SumcheckOut out;
+  ByteWriter w;
+  w.u64(num_rounds);
+  comb_rounds(c, g, polys, k, num_rounds, out, [] {}, [&](size_t j, const std::vector<fr_t>& evals) {
+    if (j == 0) out.claim = fr_add(evals[0], evals[1]);
+    const std::vector<fr_t> coeffs = unipoly_from_evals(evals);
+    unipoly_append(coeffs, transcript);
+    const fr_t r_j = transcript.challenge_scalar("challenge_nextround");
+    w.vec_fr(unipoly_compress(coeffs));
+    return r_j;
+  });
+  out.proof = std::move(w.b);
+  return out;
+}
+
+// ---------------------------------------------------------------------------------------------- zero-knowledge sumchecks
+McGens* mc_gens_create(Ctx* c, const uint64_t* G_affine, size_t n, const uint64_t* h_affine) {
+  std::unique_ptr<McGens> g(new McGens());
+  g->ctx = c;
+  g->n = n;
+  const size_t np = n + 1;
+  DBuf<fq_t> bases(c, 2 * np);  // (x, y) per point, the layout of Gens::d_bases_ark
+  DBuf<pt_niels> table(c, (size_t)kMsmFullWindows * np);
+  LB_CUDA_CHECK(cudaMemcpyAsync(bases.p, G_affine, n * 64, cudaMemcpyHostToDevice, c->st));
+  LB_CUDA_CHECK(cudaMemcpyAsync(bases.p + 2 * n, h_affine, 64, cudaMemcpyHostToDevice, c->st));
+  launch_build_table(bases.p, np, table.p, np, kMsmFullWindows, c->st);
+  g->d_multiples.alloc(c, (size_t)kMsmFullWindows * np * 128);
+  launch_build_multiples(table.p, np, np, kMsmFullWindows, g->d_multiples.p, c->st);
+  c->sync();  // the sources are the caller's host memory
+  return g.release();
+}
+
+// Two-row MSMs over a McGens table (launch_msm_direct + msm_finish_quad_kernel, as the openings' (Cx, Cy)): each row is
+// n scalars on G_0..G_{n-1} and one on h.  The rows are staged as canonical integers in the pinned buffer, one slot per
+// message in flight; at most kPubRegions messages may be in flight (the publication ring), each waited for in order.
+struct McMsm {
+  Ctx* c;
+  size_t max_len;
+  DBuf<fr_t> scal;   // 2 x len: the launches run in stream order, so one device copy serves them all
+  DBuf<pt_ext> part;
+  unsigned slot = 0;
+  McMsm(Ctx* ctx, size_t max_n) : c(ctx), max_len(max_n + 1), scal(ctx, 2 * (max_n + 1)),
+                                  part(ctx, 2 * (size_t)msm_direct_chunks((int)(max_n + 1), 1)) {
+    if ((size_t)kPubRegions * 2 * max_len * 32 > c->h_pin_bytes) throw std::runtime_error("McMsm: staging too small");
+  }
+  // row0 = (v0[0..n), b0), row1 = (v1[0..n), b1) or zeros when v1 is null
+  PubDst launch(const McGens& g, const fr_t* v0, const fr_t& b0, const fr_t* v1 = nullptr, const fr_t& b1 = fr_zero()) {
+    const size_t len = g.n + 1;
+    uint8_t* st = c->h_pin + (size_t)(slot++ % kPubRegions) * 2 * max_len * 32;
+    memset(st, 0, 2 * len * 32);
+    for (size_t i = 0; i < g.n; i++) {
+      fr_to_bytes(v0[i], st + 32 * i);
+      if (v1) fr_to_bytes(v1[i], st + 32 * (len + i));
+    }
+    fr_to_bytes(b0, st + 32 * g.n);
+    if (v1) fr_to_bytes(b1, st + 32 * (len + g.n));
+    LB_CUDA_CHECK(cudaMemcpyAsync(scal.p, st, 2 * len * 32, cudaMemcpyHostToDevice, c->st));
+    const PubDst pd = c->pub_begin(false);
+    launch_msm_direct(g.d_multiples.p, len, (const uint32_t*)scal.p, (int)len, part.p, pd, c->st);
+    return pd;
+  }
+  // both points of the message, compressed (out1 may be null)
+  void wait(const PubDst& pd, uint8_t out0[32], uint8_t* out1 = nullptr) {
+    SpanTimer sp(c, "McMsm.wait");
+    uint32_t xyz[48];
+    uint8_t comp[64];
+    c->wait_points(pd, 2, xyz);
+    h64::compress_xyz_pair(xyz, xyz + 24, comp, comp + 32);
+    memcpy(out0, comp, 32);
+    if (out1) memcpy(out1, comp + 32, 32);
+  }
+};
+
+void mc_commit(Ctx* c, const McGens& g, const std::vector<fr_t>& scalars, const fr_t& blind, uint8_t out[32]) {
+  McMsm m(c, g.n);
+  m.wait(m.launch(g, scalars.data(), blind), out);
+}
+
+// DotProductProof (dot_product.rs:11-18), its tape draws (dot_product.rs:51-53) and its tail from the transcript's
+// Cx on (dot_product.rs:55-91): Cx, Cy, a, delta, beta, then c and the responses
+struct DotRand {
+  std::vector<fr_t> d;
+  fr_t r_delta, r_beta;
+};
+static DotRand dot_rand(RandomTape& tape, size_t n) {
+  DotRand r;
+  r.d = tape.random_vector("d_vec", n);
+  r.r_delta = tape.random_scalar("r_delta");
+  r.r_beta = tape.random_scalar("r_beta");
+  return r;
+}
+static fr_t dot(const std::vector<fr_t>& a, const std::vector<fr_t>& b) {
+  fr_t s = fr_zero();
+  for (size_t i = 0; i < a.size(); i++) s = fr_add(s, fr_mul(a[i], b[i]));
+  return s;
+}
+static void dot_finish(ByteWriter& w, Transcript& transcript, const uint8_t Cx[32], const uint8_t Cy[32],
+                       const std::vector<fr_t>& a, const uint8_t delta[32], const uint8_t beta[32],
+                       const std::vector<fr_t>& x, const fr_t& blind_x, const fr_t& blind_y, const DotRand& rd) {
+  transcript.append_point_compressed("Cx", Cx);
+  transcript.append_point_compressed("Cy", Cy);
+  transcript.append_scalars("a", a.data(), a.size());
+  transcript.append_point_compressed("delta", delta);
+  transcript.append_point_compressed("beta", beta);
+  const fr_t cc = transcript.challenge_scalar("c");
+  w.raw(delta, 32);
+  w.raw(beta, 32);
+  w.u64(x.size());
+  for (size_t i = 0; i < x.size(); i++) w.fr(fr_add(fr_mul(cc, x[i]), rd.d[i]));
+  w.fr(fr_add(fr_mul(cc, blind_x), rd.r_delta));
+  w.fr(fr_add(fr_mul(cc, blind_y), rd.r_beta));
+}
+
+// Two two-row MSMs, (Cx, delta) on gens_n and (Cy, beta) on gens_1, and one host wait before c
+std::vector<uint8_t> dot_product_prove(Ctx* c, const McGens& gens_1, const McGens& gens_n, Transcript& transcript,
+                                       RandomTape& tape, const std::vector<fr_t>& x, const fr_t& blind_x,
+                                       const std::vector<fr_t>& a, const fr_t& y, const fr_t& blind_y, uint8_t Cx[32],
+                                       uint8_t Cy[32]) {
+  SpanTimer sp(c, "DotProductProof.prove");
+  McMsm m(c, gens_n.n);
+  transcript.append_protocol_name("dot product proof");
+  const DotRand rd = dot_rand(tape, x.size());
+  const fr_t ad = dot(a, rd.d);
+  const PubDst pn = m.launch(gens_n, x.data(), blind_x, rd.d.data(), rd.r_delta);
+  const PubDst p1 = m.launch(gens_1, &y, blind_y, &ad, rd.r_beta);
+  uint8_t delta[32], beta[32];
+  m.wait(pn, Cx, delta);
+  m.wait(p1, Cy, beta);
+  ByteWriter w;
+  dot_finish(w, transcript, Cx, Cy, a, delta, beta, x, blind_x, blind_y, rd);
+  return std::move(w.b);
+}
+
+// Round j after its evaluations: comm_poly on gens_n -> r_j; comm_eval on gens_1 (with comm_claim in round 0) -> w;
+// (Cy, beta) on gens_1 -> the round's DotProductProof.  Three host waits per round; the R deltas are made before the
+// first round, two per launch.
+ZkSumcheckOut zk_sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys, int k, size_t num_rounds,
+                                const fr_t& blind_claim, const McGens& gens_1, const McGens& gens_n,
+                                Transcript& transcript, RandomTape& tape) {
+  SpanTimer sp(c, "ZKSumcheck.prove");
+  const size_t R = num_rounds, n = (size_t)g.degree + 1;
+  McMsm m(c, n);  // working memory before the tape or the transcript moves
+  ZkSumcheckOut out;
+  std::vector<fr_t> blinds_poly, blinds_evals;
+  std::vector<DotRand> rd;
+  std::vector<uint8_t> comm_polys(32 * R), comm_evals(32 * R), deltas(32 * R);
+  ByteWriter proofs;
+  proofs.u64(R);
+  fr_t claim_j, beta_j = blind_claim;  // the round's claim and the blind of its commitment
+  auto begin = [&] {
+    blinds_poly = tape.random_vector("blinds_poly", R);
+    blinds_evals = tape.random_vector("blinds_evals", R);
+    for (size_t j = 0; j < R; j++) rd.push_back(dot_rand(tape, n));
+    // delta_j = <d_vec_j, G_n> + r_delta_j h_n, two rounds per launch, kPubRegions launches in flight
+    std::vector<PubDst> pd;
+    for (size_t j = 0; j < R; j += 2) {
+      const bool two = j + 1 < R;
+      pd.push_back(m.launch(gens_n, rd[j].d.data(), rd[j].r_delta, two ? rd[j + 1].d.data() : nullptr,
+                            two ? rd[j + 1].r_delta : fr_zero()));
+      if (pd.size() == (size_t)kPubRegions || j + 2 >= R) {
+        const size_t j0 = j + 2 - 2 * pd.size();
+        for (size_t i = 0; i < pd.size(); i++)
+          m.wait(pd[i], &deltas[32 * (j0 + 2 * i)], j0 + 2 * i + 1 < R ? &deltas[32 * (j0 + 2 * i + 1)] : nullptr);
+        pd.clear();
+      }
+    }
+  };
+  auto step = [&](size_t j, const std::vector<fr_t>& evals) {
+    if (j == 0) claim_j = out.claim = fr_add(evals[0], evals[1]);
+    const std::vector<fr_t> coeffs = unipoly_from_evals(evals);
+    uint8_t* comm_poly = &comm_polys[32 * j];
+    m.wait(m.launch(gens_n, coeffs.data(), blinds_poly[j]), comm_poly);
+    transcript.append_point_compressed("comm_poly", comm_poly);
+    const fr_t r_j = transcript.challenge_scalar("challenge_nextround");
+    const fr_t eval = unipoly_evaluate(coeffs, r_j);
+    uint8_t* comm_eval = &comm_evals[32 * j];
+    if (j == 0)
+      m.wait(m.launch(gens_1, &out.claim, blind_claim, &eval, blinds_evals[0]), out.comm_claim, comm_eval);
+    else
+      m.wait(m.launch(gens_1, &eval, blinds_evals[j]), comm_eval);
+    transcript.append_point_compressed("comm_claim_per_round", j == 0 ? out.comm_claim : &comm_evals[32 * (j - 1)]);
+    transcript.append_point_compressed("comm_eval", comm_eval);
+    const std::vector<fr_t> w = transcript.challenge_vector("combine_two_claims_to_one", 2);
+    // a = w0 (2, 1, .., 1) + w1 (1, r_j, r_j^2, ..): the sum-check and the evaluation decommitments (sumcheck.rs:393-421)
+    std::vector<fr_t> a(n);
+    fr_t pw = fr_one();
+    for (size_t i = 0; i < n; i++) {
+      a[i] = fr_add(i == 0 ? fr_add(w[0], w[0]) : w[0], fr_mul(w[1], pw));
+      pw = fr_mul(pw, r_j);
+    }
+    const fr_t y = fr_add(fr_mul(w[0], claim_j), fr_mul(w[1], eval));
+    const fr_t blind_y = fr_add(fr_mul(w[0], beta_j), fr_mul(w[1], blinds_evals[j]));
+    transcript.append_protocol_name("dot product proof");
+    const fr_t ad = dot(a, rd[j].d);
+    uint8_t Cy[32], beta[32];
+    m.wait(m.launch(gens_1, &y, blind_y, &ad, rd[j].r_beta), Cy, beta);
+    dot_finish(proofs, transcript, comm_poly, Cy, a, &deltas[32 * j], beta, coeffs, blinds_poly[j], blind_y, rd[j]);
+    claim_j = eval;
+    beta_j = blinds_evals[j];
+    return r_j;
+  };
+  comb_rounds(c, g, polys, k, num_rounds, out, begin, step);
+  out.blind_eval = blinds_evals[R - 1];
+  ByteWriter w;
+  w.u64(R);
+  w.raw(comm_polys.data(), comm_polys.size());
+  w.u64(R);
+  w.raw(comm_evals.data(), comm_evals.size());
+  w.raw(proofs.b.data(), proofs.b.size());
   out.proof = std::move(w.b);
   return out;
 }

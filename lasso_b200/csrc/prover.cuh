@@ -464,6 +464,39 @@ struct CubicOut {
 CubicOut cubic_prove(Ctx*, const Poly* const* A, const Poly* const* B, int n, const Poly& C,
                      const std::vector<fr_t>& coeffs, const fr_t& claim, size_t num_rounds, Transcript&);
 
+// Zero-knowledge sumchecks (DESIGN §3.16)
+// MultiCommitGens { n, G, h } (poly/commitments.rs:14-70) on the device: the 8-bit digit-multiples table of its n + 1
+// points G_0..G_{n-1}, h (the layout of Gens::d_multiples), always built.  1 <= n <= kMcMaxN (the caller checks).
+static constexpr size_t kMcMaxN = 1024;
+struct McGens {
+  Ctx* ctx = nullptr;
+  size_t n = 0;
+  DBuf<pt_niels> d_multiples;  // kMsmFullWindows x (n + 1) x 128
+};
+// G_affine: n points, h_affine: one, 64-byte affine layout (sample_generators)
+McGens* mc_gens_create(Ctx*, const uint64_t* G_affine, size_t n, const uint64_t* h_affine);
+// Commitments::batch_commit (commitments.rs:84-93), commit when n == 1: <scalars, G> + blind h, compressed
+void mc_commit(Ctx*, const McGens&, const std::vector<fr_t>& scalars, const fr_t& blind, uint8_t out[32]);
+// a DotProductProof of n elements: delta, beta, z (u64 count + n), z_delta, z_beta
+inline size_t dot_product_bytes(size_t n) { return 136 + 32 * n; }
+// DotProductProof::prove (subprotocols/dot_product.rs:31-93) on the caller's transcript and tape; gens_1.n == 1,
+// gens_n.n == x.size() == a.size() (the caller checks).  Cx, Cy: the commitments the reference returns alongside.
+std::vector<uint8_t> dot_product_prove(Ctx*, const McGens& gens_1, const McGens& gens_n, Transcript&, RandomTape&,
+                                       const std::vector<fr_t>& x, const fr_t& blind_x, const std::vector<fr_t>& a,
+                                       const fr_t& y, const fr_t& blind_y, uint8_t Cx[32], uint8_t Cy[32]);
+// a ZKSumcheckInstanceProof of R rounds of degree d: comm_polys, comm_evals (u64 count + R points each), R proofs
+inline size_t zk_sumcheck_bytes(size_t rounds, size_t degree) { return 24 + rounds * (200 + 32 * (degree + 1)); }
+struct ZkSumcheckOut : SumcheckOut {
+  uint8_t comm_claim[32];  // claim G_1 + blind_claim h_1
+  fr_t blind_eval;         // the blind of the last comm_eval
+};
+// The prover of ZKSumcheckInstanceProof (verifier: subprotocols/sumcheck.rs:331-447) over the rounds of sumcheck_prove,
+// the tape drawn up front: blinds_poly (R), blinds_evals (R), then every round's d_vec / r_delta / r_beta.
+// gens_1.n == 1, gens_n.n == g.degree + 1, the rest as sumcheck_prove (the caller checks).
+ZkSumcheckOut zk_sumcheck_prove(Ctx*, const Comb& g, const Poly* const* polys, int k, size_t num_rounds,
+                                const fr_t& blind_claim, const McGens& gens_1, const McGens& gens_n, Transcript&,
+                                RandomTape&);
+
 // grand products over a caller's polynomials (single GPU)
 // GrandProductCircuit::new (grand_product.rs:38-58) with p as layer 0 (p.nv >= 1; p is only read and must outlive the
 // circuit); *product receives evaluate() (grand_product.rs:60-65)

@@ -5,8 +5,9 @@
 // DensePolynomial::commit / evaluate, PolyEvalProof::prove / verify_plain, ProofTranscript, RandomTape) but drives them
 // only inside its own round trips; this file puts C entry points on the same code that take and return what the
 // library takes and returns: serialised bytes, an explicit generator stream, and transcript / tape objects that live
-// across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof and the hiding forms
-// of DensePolynomial::commit / PolyEvalProof::prove (blinds on h), which oracle/ leaves out.
+// across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof, the hiding forms
+// of DensePolynomial::commit / PolyEvalProof::prove (blinds on h), and DotProductProof and ZKSumcheckInstanceProof with
+// a prover for the latter (DESIGN §3.16), which oracle/ leaves out.
 #include "sparse_bytes.hpp"
 
 using namespace oracle;
@@ -133,6 +134,198 @@ std::vector<uint8_t> ser_sumcheck(const SumcheckInstanceProof& p) {
     for (const Fr& f : c.coeffs_except_linear_term) put_fr(b, f);
   }
   return b;
+}
+
+// ---- zero-knowledge sumchecks: DotProductProof (subprotocols/dot_product.rs:11-136) and ZKSumcheckInstanceProof
+// (subprotocols/sumcheck.rs:331-447), restated over the MultiCommitGens / batch_commit / commit_scalar of oracle/
+MultiCommitGens ldgens(const uint64_t* G, size_t n, const uint64_t* h) {
+  const std::vector<Affine> s = ldstream(G, n);
+  MultiCommitGens g;
+  g.n = n;
+  for (const Affine& a : s) g.G.push_back(Point::from_affine(a));
+  g.h = Point::from_affine(ldstream(h, 1)[0]);
+  return g;
+}
+Fr dotp(const std::vector<Fr>& a, const std::vector<Fr>& b) {  // compute_dotproduct (dot_product.rs:26-29)
+  Fr s = Fr::zero();
+  for (size_t i = 0; i < a.size(); i++) s += a[i] * b[i];
+  return s;
+}
+struct DotProductProof {
+  Point delta, beta;
+  std::vector<Fr> z;
+  Fr z_delta, z_beta;
+};
+// dot_product.rs:31-93
+DotProductProof dot_prove(const MultiCommitGens& gens_1, const MultiCommitGens& gens_n, Transcript& transcript,
+                          RandomTape& tape, const std::vector<Fr>& x, const Fr& blind_x, const std::vector<Fr>& a,
+                          const Fr& y, const Fr& blind_y, Point& Cx, Point& Cy) {
+  transcript.append_protocol_name("dot product proof");
+  const size_t n = x.size();
+  if (a.size() != n || gens_n.n != n || gens_1.n != 1) throw std::runtime_error("dot_prove: lengths");
+  const std::vector<Fr> d_vec = tape.random_vector("d_vec", n);
+  const Fr r_delta = tape.random_scalar("r_delta");
+  const Fr r_beta = tape.random_scalar("r_beta");
+  Cx = batch_commit(x.data(), n, blind_x, gens_n);
+  transcript.append_point("Cx", Cx);
+  Cy = commit_scalar(y, blind_y, gens_1);
+  transcript.append_point("Cy", Cy);
+  transcript.append_scalars("a", a);
+  DotProductProof p;
+  p.delta = batch_commit(d_vec.data(), n, r_delta, gens_n);
+  transcript.append_point("delta", p.delta);
+  p.beta = commit_scalar(dotp(a, d_vec), r_beta, gens_1);
+  transcript.append_point("beta", p.beta);
+  const Fr c = transcript.challenge_scalar("c");
+  for (size_t i = 0; i < n; i++) p.z.push_back(c * x[i] + d_vec[i]);
+  p.z_delta = c * blind_x + r_delta;
+  p.z_beta = c * blind_y + r_beta;
+  return p;
+}
+// dot_product.rs:95-136
+bool dot_verify(const DotProductProof& p, const MultiCommitGens& gens_1, const MultiCommitGens& gens_n,
+                Transcript& transcript, const std::vector<Fr>& a, const Point& Cx, const Point& Cy) {
+  if (a.size() != gens_n.n || gens_1.n != 1 || p.z.size() != gens_n.n) return false;
+  transcript.append_protocol_name("dot product proof");
+  transcript.append_point("Cx", Cx);
+  transcript.append_point("Cy", Cy);
+  transcript.append_scalars("a", a);
+  transcript.append_point("delta", p.delta);
+  transcript.append_point("beta", p.beta);
+  const Fr c = transcript.challenge_scalar("c");
+  bool ok = Cx * c + p.delta == batch_commit(p.z.data(), p.z.size(), p.z_delta, gens_n);
+  ok &= Cy * c + p.beta == commit_scalar(dotp(p.z, a), p.z_beta, gens_1);
+  return ok;
+}
+void ser_dot(std::vector<uint8_t>& b, const DotProductProof& p) {
+  put_point(b, p.delta);
+  put_point(b, p.beta);
+  put_u64(b, p.z.size());
+  for (const Fr& f : p.z) put_fr(b, f);
+  put_fr(b, p.z_delta);
+  put_fr(b, p.z_beta);
+}
+DotProductProof read_dot(Reader& rd) {
+  DotProductProof p;
+  p.delta = rd.point();
+  p.beta = rd.point();
+  const uint64_t m = rd.u64();
+  if (m > (rd.n - rd.at) / 32) rd.ok = false;
+  for (uint64_t i = 0; rd.ok && i < m; i++) p.z.push_back(rd.fr());
+  p.z_delta = rd.fr();
+  p.z_beta = rd.fr();
+  return p;
+}
+struct ZKSumcheckInstanceProof {
+  std::vector<Point> comm_polys, comm_evals;
+  std::vector<DotProductProof> proofs;
+};
+std::vector<uint8_t> ser_zk(const ZKSumcheckInstanceProof& p) {
+  std::vector<uint8_t> b;
+  put_u64(b, p.comm_polys.size());
+  for (const Point& q : p.comm_polys) put_point(b, q);
+  put_u64(b, p.comm_evals.size());
+  for (const Point& q : p.comm_evals) put_point(b, q);
+  put_u64(b, p.proofs.size());
+  for (const DotProductProof& d : p.proofs) ser_dot(b, d);
+  return b;
+}
+// sumcheck.rs:347-446: false where the reference returns Err or fails an assertion; e = the last comm_eval
+bool zk_verify(const ZKSumcheckInstanceProof& p, const Point& comm_claim, size_t num_rounds, size_t degree_bound,
+               const MultiCommitGens& gens_1, const MultiCommitGens& gens_n, Transcript& transcript, Point& e,
+               std::vector<Fr>& r) {
+  if (gens_n.n != degree_bound + 1) return false;
+  if (p.comm_polys.size() != num_rounds || p.comm_evals.size() != num_rounds || p.proofs.size() < num_rounds) return false;
+  r.clear();
+  for (size_t i = 0; i < p.comm_polys.size(); i++) {
+    const Point& comm_poly = p.comm_polys[i];
+    transcript.append_point("comm_poly", comm_poly);
+    const Fr r_i = transcript.challenge_scalar("challenge_nextround");
+    const Point& comm_claim_per_round = i == 0 ? comm_claim : p.comm_evals[i - 1];
+    const Point& comm_eval = p.comm_evals[i];
+    transcript.append_point("comm_claim_per_round", comm_claim_per_round);
+    transcript.append_point("comm_eval", comm_eval);
+    const std::vector<Fr> w = transcript.challenge_vector("combine_two_claims_to_one", 2);
+    const Point comm_target = comm_claim_per_round * w[0] + comm_eval * w[1];
+    std::vector<Fr> a_sc(degree_bound + 1, Fr::one()), a_eval(degree_bound + 1, Fr::one()), a(degree_bound + 1);
+    a_sc[0] += Fr::one();
+    for (size_t j = 1; j < a_eval.size(); j++) a_eval[j] = a_eval[j - 1] * r_i;
+    for (size_t j = 0; j < a.size(); j++) a[j] = w[0] * a_sc[j] + w[1] * a_eval[j];
+    if (!dot_verify(p.proofs[i], gens_1, gens_n, transcript, a, p.comm_polys[i], comm_target)) return false;
+    r.push_back(r_i);
+  }
+  if (p.comm_evals.empty()) return false;  // the reference indexes comm_evals[len - 1]
+  e = p.comm_evals.back();
+  return true;
+}
+// The prover: the round polynomials of prove_arbitrary (oracle/lasso.hpp, restated: the transcript takes commitments
+// instead of the polynomials), the tape drawn up front as Spartan's prove_*_zk does (blinds_poly, blinds_evals, then
+// each round's DotProductProof draws), each round's transcript steps in the order of zk_verify above
+ZKSumcheckInstanceProof zk_prove(std::vector<DensePolynomial>& polys, const Program& g, size_t degree, size_t num_rounds,
+                                 const Fr& blind_claim, const MultiCommitGens& gens_1, const MultiCommitGens& gens_n,
+                                 Transcript& transcript, RandomTape& tape, std::vector<Fr>& r,
+                                 std::vector<Fr>& final_evals, Fr& claim, Point& comm_claim, Fr& blind_eval) {
+  const size_t alpha = polys.size(), n = degree + 1;
+  const std::vector<Fr> blinds_poly = tape.random_vector("blinds_poly", num_rounds);
+  const std::vector<Fr> blinds_evals = tape.random_vector("blinds_evals", num_rounds);
+  ZKSumcheckInstanceProof proof;
+  Fr claim_j, beta_j = blind_claim;
+  r.clear();
+  for (size_t round = 0; round < num_rounds; round++) {
+    std::vector<Fr> evals(n, Fr::zero());
+    const size_t half = polys[0].len / 2;
+#pragma omp parallel
+    {
+      std::vector<Fr> local(n, Fr::zero()), cur(alpha), nxt(alpha);
+#pragma omp for nowait
+      for (size_t i = 0; i < half; i++) {
+        for (size_t j = 0; j < alpha; j++) cur[j] = polys[j][i];
+        local[0] += g(cur.data());
+        for (size_t j = 0; j < alpha; j++) cur[j] = polys[j][half + i];
+        local[1] += g(cur.data());
+        for (size_t t = 2; t < n; t++) {
+          for (size_t j = 0; j < alpha; j++) nxt[j] = cur[j] + polys[j][half + i] - polys[j][i];
+          local[t] += g(nxt.data());
+          cur.swap(nxt);
+        }
+      }
+#pragma omp critical
+      for (size_t t = 0; t < n; t++) evals[t] += local[t];
+    }
+    if (round == 0) {
+      claim_j = claim = evals[0] + evals[1];
+      comm_claim = commit_scalar(claim, blind_claim, gens_1);
+    }
+    const UniPoly poly = UniPoly::from_evals(evals);
+    const Point comm_poly = batch_commit(poly.coeffs.data(), n, blinds_poly[round], gens_n);
+    transcript.append_point("comm_poly", comm_poly);
+    const Fr r_j = transcript.challenge_scalar("challenge_nextround");
+    r.push_back(r_j);
+    const Fr eval = poly.evaluate(r_j);
+    const Point comm_eval = commit_scalar(eval, blinds_evals[round], gens_1);
+    transcript.append_point("comm_claim_per_round", round == 0 ? comm_claim : proof.comm_evals.back());
+    transcript.append_point("comm_eval", comm_eval);
+    const std::vector<Fr> w = transcript.challenge_vector("combine_two_claims_to_one", 2);
+    std::vector<Fr> a(n);
+    Fr pw = Fr::one();
+    for (size_t j = 0; j < n; j++) {
+      a[j] = w[0] * (j == 0 ? Fr::one() + Fr::one() : Fr::one()) + w[1] * pw;
+      pw *= r_j;
+    }
+    const Fr blind_y = w[0] * beta_j + w[1] * blinds_evals[round];
+    Point Cx, Cy;
+    proof.proofs.push_back(dot_prove(gens_1, gens_n, transcript, tape, poly.coeffs, blinds_poly[round], a,
+                                     w[0] * claim_j + w[1] * eval, blind_y, Cx, Cy));
+    proof.comm_polys.push_back(comm_poly);
+    proof.comm_evals.push_back(comm_eval);
+    for (auto& p : polys) p.bound_poly_var_top(r_j);
+    claim_j = eval;
+    beta_j = blinds_evals[round];
+  }
+  final_evals.clear();
+  for (auto& p : polys) final_evals.push_back(p[0]);
+  blind_eval = blinds_evals[num_rounds - 1];
+  return proof;
 }
 
 }  // namespace
@@ -741,6 +934,108 @@ int orcd_memory_check_verify(int kind, size_t C, size_t log_m, size_t log_r, con
   if (n_points < SparsePolyCommitmentGens::needs_points(C, c.s, alpha, log_m)) return 2;
   SparsePolyCommitmentGens pg = SparsePolyCommitmentGens::make(C, c.s, alpha, log_m, ldstream(stream, n_points));
   return mc.verify(S, c, comm_derefs, pg, ldfr(gamma), ldfr(tau), c.s, *(Transcript*)transcript) ? 0 : 1;
+}
+
+// ---- zero-knowledge sumchecks.  A MultiCommitGens is (G: n affine points, h: one), 64 bytes per point.
+// Commitments::batch_commit (commitments.rs:84-93) -> out (32 bytes compressed)
+void orcd_mc_commit(const uint64_t* G, size_t n, const uint64_t* h, const uint64_t* scalars, const uint64_t* blind,
+                    uint8_t* out) {
+  const std::vector<Fr> s = ldvec(scalars, n);
+  batch_commit(s.data(), n, ldfr(blind), ldgens(G, n, h)).compress(out);
+}
+// DotProductProof::prove (dot_product.rs:31-93) on a caller's transcript and tape: returns the proof's length (0 on
+// error); Cx_out, Cy_out = the compressed commitments returned alongside
+size_t orcd_dot_prove(const uint64_t* G1, const uint64_t* h1, const uint64_t* Gn, size_t n, const uint64_t* hn,
+                      void* transcript, void* tape, const uint64_t* x, const uint64_t* blind_x, const uint64_t* a,
+                      const uint64_t* y, const uint64_t* blind_y, uint8_t* out, size_t cap, uint8_t* Cx_out,
+                      uint8_t* Cy_out) {
+  try {
+    Point Cx, Cy;
+    const DotProductProof p = dot_prove(ldgens(G1, 1, h1), ldgens(Gn, n, hn), *(Transcript*)transcript,
+                                        *(RandomTape*)tape, ldvec(x, n), ldfr(blind_x), ldvec(a, n), ldfr(y),
+                                        ldfr(blind_y), Cx, Cy);
+    std::vector<uint8_t> b;
+    ser_dot(b, p);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    Cx.compress(Cx_out);
+    Cy.compress(Cy_out);
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_dot_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// DotProductProof::verify (dot_product.rs:95-136) of serialised bytes: 0 accepted, 1 rejected, 2 the bytes or a
+// commitment do not parse
+int orcd_dot_verify(const uint64_t* G1, const uint64_t* h1, const uint64_t* Gn, size_t n, const uint64_t* hn,
+                    const uint8_t* proof, size_t proof_len, const uint64_t* a, const uint8_t* Cx, const uint8_t* Cy,
+                    void* transcript) {
+  Reader rd{proof, proof_len};
+  const DotProductProof p = read_dot(rd);
+  Point cx, cy;
+  if (!rd.ok || rd.at != proof_len || !ldpoint(Cx, cx) || !ldpoint(Cy, cy)) return 2;
+  return dot_verify(p, ldgens(G1, 1, h1), ldgens(Gn, n, hn), *(Transcript*)transcript, ldvec(a, n), cx, cy) ? 0 : 1;
+}
+// The ZK sumcheck prover of zk_prove on copies of polys (k x len Montgomery elements, row-major) with the program
+// interpreted on the host; gens_n has degree + 1 points.  out: the serialised ZKSumcheckInstanceProof (returns its
+// length, 0 on error); r_out: num_rounds challenges; final_out: k values; claim_out; comm_claim_out (32 bytes);
+// blind_eval_out.
+size_t orcd_zk_prove(const uint64_t* polys, size_t k, size_t len, size_t num_rounds, const int32_t* prog, size_t n_ops,
+                     const uint64_t* K, size_t n_k, size_t degree, const uint64_t* blind_claim, const uint64_t* G1,
+                     const uint64_t* h1, const uint64_t* Gn, const uint64_t* hn, void* transcript, void* tape,
+                     uint8_t* out, size_t cap, uint64_t* r_out, uint64_t* final_out, uint64_t* claim_out,
+                     uint8_t* comm_claim_out, uint64_t* blind_eval_out) {
+  try {
+    std::vector<DensePolynomial> ps;
+    for (size_t j = 0; j < k; j++) ps.emplace_back(ldvec(polys + 4 * len * j, len));
+    const Program g{k, std::vector<int32_t>(prog, prog + 3 * n_ops), ldvec(K, n_k)};
+    std::vector<Fr> r, final_evals;
+    Fr claim, blind_eval;
+    Point comm_claim;
+    const ZKSumcheckInstanceProof p =
+        zk_prove(ps, g, degree, num_rounds, ldfr(blind_claim), ldgens(G1, 1, h1), ldgens(Gn, degree + 1, hn),
+                 *(Transcript*)transcript, *(RandomTape*)tape, r, final_evals, claim, comm_claim, blind_eval);
+    const std::vector<uint8_t> b = ser_zk(p);
+    if (b.size() > cap) return 0;
+    memcpy(out, b.data(), b.size());
+    for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+    for (size_t j = 0; j < k; j++) stfr(final_out + 4 * j, final_evals[j]);
+    stfr(claim_out, claim);
+    comm_claim.compress(comm_claim_out);
+    stfr(blind_eval_out, blind_eval);
+    return b.size();
+  } catch (const std::exception& e) {
+    fprintf(stderr, "orcd_zk_prove: %s\n", e.what());
+    return 0;
+  }
+}
+// ZKSumcheckInstanceProof::verify (sumcheck.rs:347-446) of serialised bytes against a compressed comm_claim, gens_n of
+// degree_bound + 1 points: 0 accepted (e_out = the compressed last comm_eval, r_out = num_rounds challenges),
+// 1 rejected, 2 the bytes or comm_claim do not parse
+int orcd_zk_verify(const uint8_t* bytes, size_t nbytes, const uint8_t* comm_claim, size_t num_rounds, size_t degree_bound,
+                   const uint64_t* G1, const uint64_t* h1, const uint64_t* Gn, const uint64_t* hn, void* transcript,
+                   uint8_t* e_out, uint64_t* r_out) {
+  Reader rd{bytes, nbytes};
+  ZKSumcheckInstanceProof p;
+  for (auto* v : {&p.comm_polys, &p.comm_evals}) {
+    const uint64_t m = rd.u64();
+    if (m > nbytes / 32) rd.ok = false;
+    for (uint64_t i = 0; rd.ok && i < m; i++) v->push_back(rd.point());
+  }
+  const uint64_t m = rd.u64();
+  if (m > nbytes / 136) rd.ok = false;
+  for (uint64_t i = 0; rd.ok && i < m; i++) p.proofs.push_back(read_dot(rd));
+  Point cc;
+  if (!rd.ok || rd.at != nbytes || !ldpoint(comm_claim, cc)) return 2;
+  Point e;
+  std::vector<Fr> r;
+  if (!zk_verify(p, cc, num_rounds, degree_bound, ldgens(G1, 1, h1), ldgens(Gn, degree_bound + 1, hn),
+                 *(Transcript*)transcript, e, r))
+    return 1;
+  e.compress(e_out);
+  for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+  return 0;
 }
 
 }  // extern "C"
