@@ -658,6 +658,36 @@ int lasso_zk_sumcheck_prove(lasso_ctx*, const lasso_comb*, const lasso_poly* con
                             size_t proof_cap, size_t* proof_len, uint64_t* r_out, uint64_t* final_evals_out,
                             uint64_t claim_out[4], uint8_t comm_claim_out[32], uint64_t blind_eval_out[4]);
 
+/* ---------------------------------------------------------------- Σ-protocols of committed scalars
+ *
+ * The three proofs of subprotocols/zk.rs, which a Spartan-style protocol runs after its ZK sumcheck: knowledge of the
+ * value behind a commitment, one committed value the product of two others, two commitments to the same value.  Each
+ * runs on the caller's transcript and tape, advanced in place, as the reference's prove does; gens is a lasso_mc_gens
+ * with n == 1 (commitments.rs:79), in practice the gens_1 of the ZK sumcheck, and a commitment to v with blind s is
+ * v G + s h.  Proofs are ark-serialize compressed, of fixed size; the commitments are the points the reference returns
+ * alongside, 32 bytes compressed.  As in the reference, z is not checked against x y nor v1 against v2: a false
+ * statement gives a proof the verifier rejects.  Each call is one short MSM over the gens' table (2 launches) and one
+ * host wait.  On a sharded context every rank computes alone and returns the single-GPU bytes.
+ * Errors, each before any launch and before the transcript or the tape moves: LASSO_ERR_GENS for null generators,
+ * generators of another context or gens.n != 1; LASSO_ERR_LENGTH for a null transcript, tape, scalar or output;
+ * LASSO_ERR_VALUE for a value or blind that is not a canonical residue. */
+/* KnowledgeProof::prove (zk.rs:23-51): tape t1, t2; transcript "knowledge proof", C, alpha, then challenge c.
+ * proof_out: {alpha, z1, z2}, 96 bytes; C_out = x G + r h. */
+int lasso_knowledge_prove(lasso_ctx*, const lasso_mc_gens* gens, lasso_transcript*, lasso_random_tape*,
+                          const uint64_t x[4], const uint64_t r[4], uint8_t proof_out[96], uint8_t C_out[32]);
+/* EqualityProof::prove (zk.rs:89-121): tape r; transcript "equality proof", C1, C2, alpha, then challenge c.
+ * proof_out: {alpha, z}, 64 bytes; C1_out = v1 G + s1 h, C2_out = v2 G + s2 h. */
+int lasso_equality_prove(lasso_ctx*, const lasso_mc_gens* gens, lasso_transcript*, lasso_random_tape*,
+                         const uint64_t v1[4], const uint64_t s1[4], const uint64_t v2[4], const uint64_t s2[4],
+                         uint8_t proof_out[64], uint8_t C1_out[32], uint8_t C2_out[32]);
+/* ProductProof::prove (zk.rs:169-237): tape b1, .., b5; transcript "product proof", X, Y, Z, alpha, beta, delta, then
+ * challenge c.  proof_out: {alpha, beta, delta, z[5]}, 256 bytes (z as a fixed-size array: no length prefix);
+ * X_out = x G + rX h, Y_out = y G + rY h, Z_out = z G + rZ h. */
+int lasso_product_prove(lasso_ctx*, const lasso_mc_gens* gens, lasso_transcript*, lasso_random_tape*,
+                        const uint64_t x[4], const uint64_t rX[4], const uint64_t y[4], const uint64_t rY[4],
+                        const uint64_t z[4], const uint64_t rZ[4], uint8_t proof_out[256], uint8_t X_out[32],
+                        uint8_t Y_out[32], uint8_t Z_out[32]);
+
 /* ---------------------------------------------------------------- grand products over a caller's polynomials
  *
  * GrandProductCircuit::new (subprotocols/grand_product.rs:38-58) over a polynomial of the context with

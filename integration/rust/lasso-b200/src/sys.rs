@@ -220,6 +220,16 @@ extern "C" {
                                    proof_out: *mut u8, proof_cap: usize, proof_len: *mut usize, r_out: *mut u64,
                                    final_evals_out: *mut u64, claim_out: *mut u64, comm_claim_out: *mut u8,
                                    blind_eval_out: *mut u64) -> c_int;
+    pub fn lasso_knowledge_prove(ctx: *mut lasso_ctx, gens: *const lasso_mc_gens, transcript: *mut lasso_transcript,
+                                 random_tape: *mut lasso_random_tape, x: *const u64, r: *const u64, proof_out: *mut u8,
+                                 c_out: *mut u8) -> c_int;
+    pub fn lasso_equality_prove(ctx: *mut lasso_ctx, gens: *const lasso_mc_gens, transcript: *mut lasso_transcript,
+                                random_tape: *mut lasso_random_tape, v1: *const u64, s1: *const u64, v2: *const u64,
+                                s2: *const u64, proof_out: *mut u8, c1_out: *mut u8, c2_out: *mut u8) -> c_int;
+    pub fn lasso_product_prove(ctx: *mut lasso_ctx, gens: *const lasso_mc_gens, transcript: *mut lasso_transcript,
+                               random_tape: *mut lasso_random_tape, x: *const u64, r_x: *const u64, y: *const u64,
+                               r_y: *const u64, z: *const u64, r_z: *const u64, proof_out: *mut u8, x_out: *mut u8,
+                               y_out: *mut u8, z_out: *mut u8) -> c_int;
     pub fn lasso_poly_create_comb(ctx: *mut lasso_ctx, comb: *const lasso_comb, polys: *const *const lasso_poly,
                                   n_polys: usize, out: *mut *mut lasso_poly) -> c_int;
     pub fn lasso_sumcheck_prove_cubic_batched(ctx: *mut lasso_ctx, a: *const *const lasso_poly, b: *const *const lasso_poly,

@@ -43,13 +43,19 @@ and zero-knowledge sumchecks over a caller's polynomials (single GPU; the commit
     ZKSumcheckInstanceProof.prove(ctx, comb, polys, num_rounds, blind_claim, gens_1, gens_n, transcript, random_tape)
                                                                          src/subprotocols/sumcheck.rs:331 (its verifier)
 
+and the Σ-protocols over committed scalars that end such a protocol (gens: a MultiCommitGens with n == 1; also sharded):
+
+    KnowledgeProof.prove(ctx, gens, transcript, random_tape, x, r)       src/subprotocols/zk.rs:23
+    EqualityProof.prove(ctx, gens, transcript, random_tape, v1, s1, v2, s2)   src/subprotocols/zk.rs:89
+    ProductProof.prove(ctx, gens, transcript, random_tape, x, rX, y, rY, z, rZ)   src/subprotocols/zk.rs:169
+
 Everything runs through the C-ABI shared library (include/lasso_b200.h); there is no CPU fallback:
 importing works without a GPU, but creating a Context raises.
 """
 from .api import (  # noqa: F401
     AND, LT, OR, RANGE_CHECK, XOR,
-    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, DotProductProof, DotProductProofGens, GrandProductCircuit, GrandProducts, LassoError, MemoryCheckingProof, MsmJob,
-    MultiCommitGens, PolyCommitmentGens, PolyEvalProof, RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Subtables, SumcheckInstanceProof, Transcript, ZKSumcheckInstanceProof,
+    BatchedGrandProductArgument, Comb, CombinedTableEvalProof, Context, CustomStrategy, DensePolynomial, DensifiedRepresentation, DotProductProof, DotProductProofGens, EqualityProof, GrandProductCircuit, GrandProducts, KnowledgeProof, LassoError, MemoryCheckingProof, MsmJob,
+    MultiCommitGens, PolyCommitmentGens, PolyEvalProof, ProductProof, RandomTape, SparsePolyCommitmentGens, SparsePolynomialEvaluationProof, Strategy, Subtables, SumcheckInstanceProof, Transcript, ZKSumcheckInstanceProof,
     bind_bot, bind_top,
     commit_rows, eq_evals, fr_from_ints, gather_lookup_polys, gens_points_needed, lib, library_path, materialize_subtables,
     msm, poly_gens_points_needed, sample_generators, sumcheck_bind_round_arbitrary,

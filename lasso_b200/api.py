@@ -46,6 +46,15 @@ def lib():
         L.lasso_poly_num_vars.restype = C.c_size_t
         L.lasso_gp_circuit_num_vars.restype = C.c_size_t
         L.lasso_transcript_append_u64.argtypes = [C.c_void_p, C.c_char_p, C.c_uint64]
+        # the zero-knowledge calls, declared so that a pointer passed as a Python int keeps its 64 bits (an undeclared
+        # int argument goes over as a C int)
+        V, S = C.c_void_p, C.c_size_t
+        L.lasso_mc_commit.argtypes = [V, V, V, S, V, V]
+        L.lasso_dot_product_prove.argtypes = [V] * 8 + [S, V, V, V, S, V, V, V]
+        L.lasso_zk_sumcheck_prove.argtypes = [V, V, V, S, S] + [V] * 6 + [S] + [V] * 6
+        L.lasso_knowledge_prove.argtypes = [V] * 8
+        L.lasso_equality_prove.argtypes = [V] * 11
+        L.lasso_product_prove.argtypes = [V] * 14
         _lib = L
     return _lib
 
@@ -1301,6 +1310,57 @@ class ZKSumcheckInstanceProof:
                                            random_tape._h, _p(out), C.c_size_t(cap), C.byref(n), _p(r), _p(fin),
                                            _p(claim), _p(cc), _p(blind_eval)))
         return cls(bytes(out[: n.value]), r[:num_rounds], fin[: len(polys)], claim, cc.tobytes(), blind_eval)
+
+
+# ------------------------------------------------------------------ Σ-protocols of committed scalars
+def _sigma(fn, ctx, gens, transcript, random_tape, names, values, proof_len, n_points):
+    """one call of the Σ-provers: values are single Fr elements (uint64 limbs of shape (4,)) named for the errors ->
+    (proof bytes, n_points compressed commitments)"""
+    vals = [_limbs(v, 1, name) for name, v in zip(names, values)]
+    out = np.zeros(proof_len, dtype=np.uint8)
+    pts = [np.zeros(32, dtype=np.uint8) for _ in range(n_points)]
+    _chk(fn(ctx._h, gens._h, transcript._h, random_tape._h, *[_p(v) for v in vals], _p(out), *[_p(p) for p in pts]))
+    return (out.tobytes(),) + tuple(p.tobytes() for p in pts)
+
+
+class KnowledgeProof:
+    """src/subprotocols/zk.rs:11-76: knowledge of x and r behind C = x G + r h"""
+
+    proof_len = 96
+
+    @staticmethod
+    def prove(ctx, gens, transcript, random_tape, x, r):
+        """KnowledgeProof::prove on the caller's transcript and tape, advanced in place; gens: a MultiCommitGens with
+        n == 1 -> (proof bytes {alpha, z1, z2}, C)"""
+        return _sigma(lib().lasso_knowledge_prove, ctx, gens, transcript, random_tape, ("x", "r"), (x, r), 96, 1)
+
+
+class EqualityProof:
+    """src/subprotocols/zk.rs:78-154: C1 = v1 G + s1 h and C2 = v2 G + s2 h hide the same value"""
+
+    proof_len = 64
+
+    @staticmethod
+    def prove(ctx, gens, transcript, random_tape, v1, s1, v2, s2):
+        """EqualityProof::prove on the caller's transcript and tape, advanced in place; gens: a MultiCommitGens with
+        n == 1 -> (proof bytes {alpha, z}, C1, C2).  v1 is not checked against v2: a false statement gives a proof the
+        verifier rejects."""
+        return _sigma(lib().lasso_equality_prove, ctx, gens, transcript, random_tape, ("v1", "s1", "v2", "s2"),
+                      (v1, s1, v2, s2), 64, 2)
+
+
+class ProductProof:
+    """src/subprotocols/zk.rs:156-301: Z = z G + rZ h commits to the product of the values behind X and Y"""
+
+    proof_len = 256
+
+    @staticmethod
+    def prove(ctx, gens, transcript, random_tape, x, rX, y, rY, z, rZ):
+        """ProductProof::prove on the caller's transcript and tape, advanced in place; gens: a MultiCommitGens with
+        n == 1 -> (proof bytes {alpha, beta, delta, z[5]}, X, Y, Z).  z is not checked against x y: a false statement
+        gives a proof the verifier rejects."""
+        return _sigma(lib().lasso_product_prove, ctx, gens, transcript, random_tape, ("x", "rX", "y", "rY", "z", "rZ"),
+                      (x, rX, y, rY, z, rZ), 256, 3)
 
 
 # ------------------------------------------------------------------ grand products over a caller's polynomials

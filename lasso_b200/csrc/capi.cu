@@ -1653,6 +1653,66 @@ int lasso_zk_sumcheck_prove(lasso_ctx* h, const lasso_comb* g, const lasso_poly*
   LB_CATCH
 }
 
+// ---- Σ-protocols of committed scalars: KnowledgeProof, EqualityProof, ProductProof (subprotocols/zk.rs).  On a sharded
+// context every rank computes alone, with no exchange.
+// The shared checks, in the order of the other proofs: gens of this context with n == 1 (commitments.rs:79), then a null
+// transcript, tape, scalar or output, then every scalar a canonical residue (into v, in order).
+static int sigma_check(lasso_ctx* h, const char* what, const lasso_mc_gens* g, const void* transcript, const void* tape,
+                       std::initializer_list<const uint64_t*> in, std::initializer_list<const void*> outs,
+                       std::vector<fr_t>& v) {
+  if (const int rc = mc_gens_check(h, what, g, 1)) return rc;
+  bool null = !transcript || !tape;
+  for (const uint64_t* p : in) null |= !p;
+  for (const void* p : outs) null |= !p;
+  if (null) return fail(LASSO_ERR_LENGTH, std::string(what) + ": null transcript, random tape, scalar or output");
+  for (const uint64_t* p : in) {
+    std::vector<fr_t> s;
+    if (!load_scalars(p, 1, s)) return fail(LASSO_ERR_VALUE, std::string(what) + ": a value or blind is not a canonical residue");
+    v.push_back(s[0]);
+  }
+  return 0;
+}
+int lasso_knowledge_prove(lasso_ctx* h, const lasso_mc_gens* gens, lasso_transcript* transcript, lasso_random_tape* tape,
+                          const uint64_t x[4], const uint64_t r[4], uint8_t proof_out[96], uint8_t C_out[32]) {
+  LB_TRY_CTX(h)
+  std::vector<fr_t> v;
+  if (const int rc = sigma_check(h, "knowledge proof", gens, transcript, tape, {x, r}, {proof_out, C_out}, v)) return rc;
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return knowledge_prove(h->c, *gens->g, transcript->t, tape->t, v[0], v[1], C_out);
+  });
+  return out_copy("knowledge proof", b, kKnowledgeProofBytes, proof_out);
+  LB_CATCH
+}
+int lasso_equality_prove(lasso_ctx* h, const lasso_mc_gens* gens, lasso_transcript* transcript, lasso_random_tape* tape,
+                         const uint64_t v1[4], const uint64_t s1[4], const uint64_t v2[4], const uint64_t s2[4],
+                         uint8_t proof_out[64], uint8_t C1_out[32], uint8_t C2_out[32]) {
+  LB_TRY_CTX(h)
+  std::vector<fr_t> v;
+  if (const int rc =
+          sigma_check(h, "equality proof", gens, transcript, tape, {v1, s1, v2, s2}, {proof_out, C1_out, C2_out}, v))
+    return rc;
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return equality_prove(h->c, *gens->g, transcript->t, tape->t, v[0], v[1], v[2], v[3], C1_out, C2_out);
+  });
+  return out_copy("equality proof", b, kEqualityProofBytes, proof_out);
+  LB_CATCH
+}
+int lasso_product_prove(lasso_ctx* h, const lasso_mc_gens* gens, lasso_transcript* transcript, lasso_random_tape* tape,
+                        const uint64_t x[4], const uint64_t rX[4], const uint64_t y[4], const uint64_t rY[4],
+                        const uint64_t z[4], const uint64_t rZ[4], uint8_t proof_out[256], uint8_t X_out[32],
+                        uint8_t Y_out[32], uint8_t Z_out[32]) {
+  LB_TRY_CTX(h)
+  std::vector<fr_t> v;
+  if (const int rc = sigma_check(h, "product proof", gens, transcript, tape, {x, rX, y, rY, z, rZ},
+                                 {proof_out, X_out, Y_out, Z_out}, v))
+    return rc;
+  const std::vector<uint8_t> b = timed(h->c->t_prove_ms, [&] {
+    return product_prove(h->c, *gens->g, transcript->t, tape->t, v[0], v[1], v[2], v[3], v[4], v[5], X_out, Y_out, Z_out);
+  });
+  return out_copy("product proof", b, kProductProofBytes, proof_out);
+  LB_CATCH
+}
+
 // ---- grand products over a caller's polynomials
 int lasso_gp_circuit_create(lasso_ctx* h, const lasso_poly* p, lasso_gp_circuit** out) {
   LB_TRY_CTX(h)

@@ -180,6 +180,32 @@ inline void compress_xyz_pair(const uint32_t* xyz_a, const uint32_t* xyz_b, uint
     if ((top >> 62) != 0) dst[k][31] |= 0x80;
   }
 }
+// k <= 8 points (k x 24 words) at once (the rows of one short MSM): one inversion for all of them (Montgomery's trick)
+inline void compress_xyz_batch(const uint32_t* xyz, int k, uint8_t* out /* k x 32 */) {
+  fe pre[8], zi[8];  // pre[i] = Z_0 .. Z_{i-1}
+  fe acc = {{1, 0, 0, 0}};
+  for (int i = 0; i < k; i++) {
+    pre[i] = acc;
+    acc = mul(acc, from_limbs32(xyz + 24 * i + 16));
+  }
+  fe inv_acc = inv(acc);  // 1 / (Z_0 .. Z_{i})
+  for (int i = k - 1; i >= 0; i--) {
+    zi[i] = mul(inv_acc, pre[i]);
+    inv_acc = mul(inv_acc, from_limbs32(xyz + 24 * i + 16));
+  }
+  for (int i = 0; i < k; i++) {
+    const fe x = canonical(mul(from_limbs32(xyz + 24 * i), zi[i])), y = canonical(mul(from_limbs32(xyz + 24 * i + 8), zi[i]));
+    u128 c = 9;  // x > (q-1)/2  <=>  x + 9 >= 2^254
+    uint64_t top = 0;
+    for (int l = 0; l < 4; l++) {
+      c += x.v[l];
+      top = (uint64_t)c;
+      c >>= 64;
+    }
+    memcpy(out + 32 * i, y.v, 32);
+    if ((top >> 62) != 0) out[32 * i + 31] |= 0x80;
+  }
+}
 
 }  // namespace h64
 }  // namespace lb

@@ -37,6 +37,11 @@ int msm_direct_chunks(int len, int heavy_rows);
 // X, Y, Z; the host waits for the message and clears it (Ctx::wait_points)
 void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, pt_ext* partials, const PubDst& pub,
                        cudaStream_t st);
+// the same over nrows rows, 1 <= nrows <= kMsmDirectMaxRows: scalars = nrows x len, partials: nrows x
+// msm_direct_chunks(len, 1), elements 3*row + {0,1,2} of the message
+static constexpr int kMsmDirectMaxRows = 8;
+void launch_msm_direct_rows(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, int nrows, pt_ext* partials,
+                            const PubDst& pub, cudaStream_t st);
 // One Bulletproofs round (bullet.rs:73-134, unfolded generators) in ONE launch over the multiples table: scalars from
 // the (folded) a, b, w vectors, both rows L / R summed, tail terms c * Q + blind * h, publication of the two points.
 // a_in / b_in: 2m elements when fold != 0 (folded with u / uinv into a_out / b_out, m elements), else m;

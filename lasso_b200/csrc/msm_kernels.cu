@@ -869,7 +869,13 @@ int msm_direct_chunks(int len, int heavy_rows) {
 }
 void launch_msm_direct(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, pt_ext* partials, const PubDst& pub,
                        cudaStream_t st) {
-  const int nrows = 2, nchunks = msm_direct_chunks(len, 1);
+  launch_msm_direct_rows(M, npts, scalars, len, 2, partials, pub, st);
+}
+void launch_msm_direct_rows(const pt_niels* M, size_t npts, const uint32_t* scalars, int len, int nrows, pt_ext* partials,
+                            const PubDst& pub, cudaStream_t st) {
+  // msm_finish_quad_kernel: one CTA of 128 threads per row, its shared tree sized for 8 rows
+  if (nrows < 1 || nrows > kMsmDirectMaxRows) throw std::runtime_error("msm_direct: nrows must be in 1..8");
+  const int nchunks = msm_direct_chunks(len, 1);
   dim3 grid(nchunks, nrows);
   launch(msm_direct_kernel, grid, MSMD_T, 0, st, M, npts, scalars, len, partials);
   launch(msm_finish_quad_kernel, 1, 128 * nrows, 0, st, partials, nrows, nchunks, pub);

@@ -2412,42 +2412,57 @@ McGens* mc_gens_create(Ctx* c, const uint64_t* G_affine, size_t n, const uint64_
   return g.release();
 }
 
-// Two-row MSMs over a McGens table (launch_msm_direct + msm_finish_quad_kernel, as the openings' (Cx, Cy)): each row is
-// n scalars on G_0..G_{n-1} and one on h.  The rows are staged as canonical integers in the pinned buffer, one slot per
-// message in flight; at most kPubRegions messages may be in flight (the publication ring), each waited for in order.
+// Short MSMs of 1..8 rows over a McGens table (launch_msm_direct_rows + msm_finish_quad_kernel, as the openings'
+// (Cx, Cy)): each row is n scalars on G_0..G_{n-1} and one on h.  The rows are staged as canonical integers in the
+// pinned buffer, one slot per message in flight; at most kPubRegions messages may be in flight (the publication ring),
+// each waited for in order.
+struct McRow {
+  const fr_t* v;  // n scalars on G, or null for zeros
+  fr_t b;         // the scalar on h
+};
 struct McMsm {
   Ctx* c;
   size_t max_len;
-  DBuf<fr_t> scal;   // 2 x len: the launches run in stream order, so one device copy serves them all
+  DBuf<fr_t> scal;   // 8 x len: the launches run in stream order, so one device copy serves them all
   DBuf<pt_ext> part;
   unsigned slot = 0;
-  McMsm(Ctx* ctx, size_t max_n) : c(ctx), max_len(max_n + 1), scal(ctx, 2 * (max_n + 1)),
-                                  part(ctx, 2 * (size_t)msm_direct_chunks((int)(max_n + 1), 1)) {
-    if ((size_t)kPubRegions * 2 * max_len * 32 > c->h_pin_bytes) throw std::runtime_error("McMsm: staging too small");
+  McMsm(Ctx* ctx, size_t max_n) : c(ctx), max_len(max_n + 1), scal(ctx, kMsmDirectMaxRows * (max_n + 1)),
+                                  part(ctx, kMsmDirectMaxRows * (size_t)msm_direct_chunks((int)(max_n + 1), 1)) {
+    if ((size_t)kPubRegions * kMsmDirectMaxRows * max_len * 32 > c->h_pin_bytes)
+      throw std::runtime_error("McMsm: staging too small");
+  }
+  // one message of k rows, 1 <= k <= kMsmDirectMaxRows
+  PubDst launch_rows(const McGens& g, const McRow* rows, int k) {
+    const size_t len = g.n + 1;
+    uint8_t* st = c->h_pin + (size_t)(slot++ % kPubRegions) * kMsmDirectMaxRows * max_len * 32;
+    memset(st, 0, k * len * 32);
+    for (int r = 0; r < k; r++) {
+      uint8_t* row = st + r * len * 32;
+      if (rows[r].v)
+        for (size_t i = 0; i < g.n; i++) fr_to_bytes(rows[r].v[i], row + 32 * i);
+      fr_to_bytes(rows[r].b, row + 32 * g.n);
+    }
+    LB_CUDA_CHECK(cudaMemcpyAsync(scal.p, st, k * len * 32, cudaMemcpyHostToDevice, c->st));
+    const PubDst pd = c->pub_begin(false);
+    launch_msm_direct_rows(g.d_multiples.p, len, (const uint32_t*)scal.p, (int)len, k, part.p, pd, c->st);
+    return pd;
   }
   // row0 = (v0[0..n), b0), row1 = (v1[0..n), b1) or zeros when v1 is null
   PubDst launch(const McGens& g, const fr_t* v0, const fr_t& b0, const fr_t* v1 = nullptr, const fr_t& b1 = fr_zero()) {
-    const size_t len = g.n + 1;
-    uint8_t* st = c->h_pin + (size_t)(slot++ % kPubRegions) * 2 * max_len * 32;
-    memset(st, 0, 2 * len * 32);
-    for (size_t i = 0; i < g.n; i++) {
-      fr_to_bytes(v0[i], st + 32 * i);
-      if (v1) fr_to_bytes(v1[i], st + 32 * (len + i));
-    }
-    fr_to_bytes(b0, st + 32 * g.n);
-    if (v1) fr_to_bytes(b1, st + 32 * (len + g.n));
-    LB_CUDA_CHECK(cudaMemcpyAsync(scal.p, st, 2 * len * 32, cudaMemcpyHostToDevice, c->st));
-    const PubDst pd = c->pub_begin(false);
-    launch_msm_direct(g.d_multiples.p, len, (const uint32_t*)scal.p, (int)len, part.p, pd, c->st);
-    return pd;
+    const McRow rows[2] = {{v0, b0}, {v1, v1 ? b1 : fr_zero()}};
+    return launch_rows(g, rows, 2);
   }
-  // both points of the message, compressed (out1 may be null)
-  void wait(const PubDst& pd, uint8_t out0[32], uint8_t* out1 = nullptr) {
+  // the k points of the message, compressed, 32 bytes each; one Fq inversion for all of them
+  void wait_rows(const PubDst& pd, int k, uint8_t* out) {
     SpanTimer sp(c, "McMsm.wait");
-    uint32_t xyz[48];
+    uint32_t xyz[24 * kMsmDirectMaxRows];
+    c->wait_points(pd, k, xyz);
+    h64::compress_xyz_batch(xyz, k, out);
+  }
+  // both points of a two-row message (out1 may be null)
+  void wait(const PubDst& pd, uint8_t out0[32], uint8_t* out1 = nullptr) {
     uint8_t comp[64];
-    c->wait_points(pd, 2, xyz);
-    h64::compress_xyz_pair(xyz, xyz + 24, comp, comp + 32);
+    wait_rows(pd, 2, comp);
     memcpy(out0, comp, 32);
     if (out1) memcpy(out1, comp + 32, 32);
   }
@@ -2591,6 +2606,85 @@ ZkSumcheckOut zk_sumcheck_prove(Ctx* c, const Comb& g, const Poly* const* polys,
   w.raw(proofs.b.data(), proofs.b.size());
   out.proof = std::move(w.b);
   return out;
+}
+
+// ---- Σ-protocols of committed scalars (subprotocols/zk.rs).  Every point of these proofs is a row (a, b) -> a G + b h
+// on gens (n == 1) and all of them are known before the challenge: one k-row MSM, one host wait, then the k points go
+// on the transcript in row order under `labels` and c is drawn.  pts: k x 32 bytes.
+static fr_t sigma_points(McMsm& m, const McGens& g, Transcript& transcript, const McRow* rows, const char* const* labels,
+                         int k, uint8_t* pts) {
+  m.wait_rows(m.launch_rows(g, rows, k), k, pts);
+  for (int i = 0; i < k; i++) transcript.append_point_compressed(labels[i], pts + 32 * i);
+  return transcript.challenge_scalar("c");
+}
+
+// zk.rs:23-51: tape t1, t2; rows C = (x, r), alpha = (t1, t2)
+std::vector<uint8_t> knowledge_prove(Ctx* c, const McGens& g, Transcript& transcript, RandomTape& tape, const fr_t& x,
+                                     const fr_t& r, uint8_t C[32]) {
+  SpanTimer sp(c, "KnowledgeProof.prove");
+  McMsm m(c, 1);  // working memory before the tape or the transcript moves
+  transcript.append_protocol_name("knowledge proof");
+  const fr_t t1 = tape.random_scalar("t1");
+  const fr_t t2 = tape.random_scalar("t2");
+  const McRow rows[2] = {{&x, r}, {&t1, t2}};
+  static const char* const labels[2] = {"C", "alpha"};
+  uint8_t pts[64];
+  const fr_t cc = sigma_points(m, g, transcript, rows, labels, 2, pts);
+  memcpy(C, pts, 32);
+  ByteWriter w;
+  w.raw(pts + 32, 32);
+  w.fr(fr_add(fr_mul(x, cc), t1));
+  w.fr(fr_add(fr_mul(r, cc), t2));
+  return std::move(w.b);
+}
+
+// zk.rs:89-121: tape r; rows C1 = (v1, s1), C2 = (v2, s2), alpha = (0, r)
+std::vector<uint8_t> equality_prove(Ctx* c, const McGens& g, Transcript& transcript, RandomTape& tape, const fr_t& v1,
+                                    const fr_t& s1, const fr_t& v2, const fr_t& s2, uint8_t C1[32], uint8_t C2[32]) {
+  SpanTimer sp(c, "EqualityProof.prove");
+  McMsm m(c, 1);
+  transcript.append_protocol_name("equality proof");
+  const fr_t r = tape.random_scalar("r");
+  const McRow rows[3] = {{&v1, s1}, {&v2, s2}, {nullptr, r}};
+  static const char* const labels[3] = {"C1", "C2", "alpha"};
+  uint8_t pts[96];
+  const fr_t cc = sigma_points(m, g, transcript, rows, labels, 3, pts);
+  memcpy(C1, pts, 32);
+  memcpy(C2, pts + 32, 32);
+  ByteWriter w;
+  w.raw(pts + 64, 32);
+  w.fr(fr_add(fr_mul(cc, fr_sub(s1, s2)), r));
+  return std::move(w.b);
+}
+
+// zk.rs:169-237: tape b1..b5; rows X = (x, rX), Y = (y, rY), Z = (z, rZ), alpha = (b1, b2), beta = (b3, b4) and
+// delta = b3 X + b5 h, which is the row (b3 x, b3 rX + b5) since X = x G + rX h: the same group element, so the same
+// compressed bytes, with no base outside the table
+std::vector<uint8_t> product_prove(Ctx* c, const McGens& g, Transcript& transcript, RandomTape& tape, const fr_t& x,
+                                   const fr_t& rX, const fr_t& y, const fr_t& rY, const fr_t& z, const fr_t& rZ,
+                                   uint8_t X[32], uint8_t Y[32], uint8_t Z[32]) {
+  SpanTimer sp(c, "ProductProof.prove");
+  McMsm m(c, 1);
+  transcript.append_protocol_name("product proof");
+  fr_t b[5];
+  static const char* const blabels[5] = {"b1", "b2", "b3", "b4", "b5"};
+  for (int i = 0; i < 5; i++) b[i] = tape.random_scalar(blabels[i]);
+  const fr_t b3x = fr_mul(b[2], x);
+  const McRow rows[6] = {{&x, rX}, {&y, rY}, {&z, rZ}, {&b[0], b[1]}, {&b[2], b[3]}, {&b3x, fr_add(fr_mul(b[2], rX), b[4])}};
+  static const char* const labels[6] = {"X", "Y", "Z", "alpha", "beta", "delta"};
+  uint8_t pts[192];
+  const fr_t cc = sigma_points(m, g, transcript, rows, labels, 6, pts);
+  memcpy(X, pts, 32);
+  memcpy(Y, pts + 32, 32);
+  memcpy(Z, pts + 64, 32);
+  ByteWriter w;
+  w.raw(pts + 96, 96);  // alpha, beta, delta; z as [F; 5]: five scalars, no length
+  w.fr(fr_add(b[0], fr_mul(cc, x)));
+  w.fr(fr_add(b[1], fr_mul(cc, rX)));
+  w.fr(fr_add(b[2], fr_mul(cc, y)));
+  w.fr(fr_add(b[3], fr_mul(cc, rY)));
+  w.fr(fr_add(b[4], fr_mul(cc, fr_sub(rZ, fr_mul(rX, y)))));
+  return std::move(w.b);
 }
 
 // prove_cubic_batched over a caller's polynomials.  The pairs with a non-zero coefficient go through cubic_rounds on

@@ -497,6 +497,20 @@ ZkSumcheckOut zk_sumcheck_prove(Ctx*, const Comb& g, const Poly* const* polys, i
                                 const fr_t& blind_claim, const McGens& gens_1, const McGens& gens_n, Transcript&,
                                 RandomTape&);
 
+// Σ-protocols of committed scalars (subprotocols/zk.rs, DESIGN §3.17) on the caller's transcript and tape; gens.n == 1
+// (the caller checks).  Each is one short MSM of its 2, 3 or 6 rows and one host wait.  The proof bytes are
+// ark-serialize compressed; the commitments are the points the reference returns alongside.
+static constexpr size_t kKnowledgeProofBytes = 96;  // alpha, z1, z2
+static constexpr size_t kEqualityProofBytes = 64;   // alpha, z
+static constexpr size_t kProductProofBytes = 256;   // alpha, beta, delta, z[5]
+std::vector<uint8_t> knowledge_prove(Ctx*, const McGens&, Transcript&, RandomTape&, const fr_t& x, const fr_t& r,
+                                     uint8_t C[32]);
+std::vector<uint8_t> equality_prove(Ctx*, const McGens&, Transcript&, RandomTape&, const fr_t& v1, const fr_t& s1,
+                                    const fr_t& v2, const fr_t& s2, uint8_t C1[32], uint8_t C2[32]);
+std::vector<uint8_t> product_prove(Ctx*, const McGens&, Transcript&, RandomTape&, const fr_t& x, const fr_t& rX,
+                                   const fr_t& y, const fr_t& rY, const fr_t& z, const fr_t& rZ, uint8_t X[32],
+                                   uint8_t Y[32], uint8_t Z[32]);
+
 // grand products over a caller's polynomials (single GPU)
 // GrandProductCircuit::new (grand_product.rs:38-58) with p as layer 0 (p.nv >= 1; p is only read and must outlive the
 // circuit); *product receives evaluate() (grand_product.rs:60-65)

@@ -6,8 +6,9 @@
 // only inside its own round trips; this file puts C entry points on the same code that take and return what the
 // library takes and returns: serialised bytes, an explicit generator stream, and transcript / tape objects that live
 // across calls.  Nothing here is restated anew except the ark-serialize reading of a PolyEvalProof, the hiding forms
-// of DensePolynomial::commit / PolyEvalProof::prove (blinds on h), and DotProductProof and ZKSumcheckInstanceProof with
-// a prover for the latter (DESIGN §3.16), which oracle/ leaves out.
+// of DensePolynomial::commit / PolyEvalProof::prove (blinds on h), DotProductProof and ZKSumcheckInstanceProof with
+// a prover for the latter (DESIGN §3.16), and the Σ-protocols of subprotocols/zk.rs (DESIGN §3.17), which oracle/ leaves
+// out.
 #include "sparse_bytes.hpp"
 
 using namespace oracle;
@@ -326,6 +327,118 @@ ZKSumcheckInstanceProof zk_prove(std::vector<DensePolynomial>& polys, const Prog
   for (auto& p : polys) final_evals.push_back(p[0]);
   blind_eval = blinds_evals[num_rounds - 1];
   return proof;
+}
+
+// ---- Σ-protocols of committed scalars (subprotocols/zk.rs), restated over commit_scalar of oracle/.  gens has n == 1.
+// Proofs serialise as ark-serialize compressed: points, then scalars; ProductProof's z is [F; 5], a fixed-size array
+// written with no length prefix (recalled, not checked: no ark-serialize source is at hand).
+struct KnowledgeProof {
+  Point alpha;
+  Fr z1, z2;
+};
+// zk.rs:23-51
+KnowledgeProof knowledge_prove(const MultiCommitGens& g, Transcript& transcript, RandomTape& tape, const Fr& x,
+                               const Fr& r, Point& C) {
+  transcript.append_protocol_name("knowledge proof");
+  const Fr t1 = tape.random_scalar("t1");
+  const Fr t2 = tape.random_scalar("t2");
+  C = commit_scalar(x, r, g);
+  transcript.append_point("C", C);
+  KnowledgeProof p;
+  p.alpha = commit_scalar(t1, t2, g);
+  transcript.append_point("alpha", p.alpha);
+  const Fr c = transcript.challenge_scalar("c");
+  p.z1 = x * c + t1;
+  p.z2 = r * c + t2;
+  return p;
+}
+// zk.rs:53-75
+bool knowledge_verify(const KnowledgeProof& p, const MultiCommitGens& g, Transcript& transcript, const Point& C) {
+  transcript.append_protocol_name("knowledge proof");
+  transcript.append_point("C", C);
+  transcript.append_point("alpha", p.alpha);
+  const Fr c = transcript.challenge_scalar("c");
+  return commit_scalar(p.z1, p.z2, g) == C * c + p.alpha;
+}
+struct EqualityProof {
+  Point alpha;
+  Fr z;
+};
+// zk.rs:89-121
+EqualityProof equality_prove(const MultiCommitGens& g, Transcript& transcript, RandomTape& tape, const Fr& v1,
+                             const Fr& s1, const Fr& v2, const Fr& s2, Point& C1, Point& C2) {
+  transcript.append_protocol_name("equality proof");
+  const Fr r = tape.random_scalar("r");
+  C1 = commit_scalar(v1, s1, g);
+  transcript.append_point("C1", C1);
+  C2 = commit_scalar(v2, s2, g);
+  transcript.append_point("C2", C2);
+  EqualityProof p;
+  p.alpha = g.h * r;
+  transcript.append_point("alpha", p.alpha);
+  const Fr c = transcript.challenge_scalar("c");
+  p.z = c * (s1 - s2) + r;
+  return p;
+}
+// zk.rs:123-153
+bool equality_verify(const EqualityProof& p, const MultiCommitGens& g, Transcript& transcript, const Point& C1,
+                     const Point& C2) {
+  transcript.append_protocol_name("equality proof");
+  transcript.append_point("C1", C1);
+  transcript.append_point("C2", C2);
+  transcript.append_point("alpha", p.alpha);
+  const Fr c = transcript.challenge_scalar("c");
+  return g.h * p.z == (C1 + -C2) * c + p.alpha;
+}
+struct ProductProof {
+  Point alpha, beta, delta;
+  Fr z[5];
+};
+// zk.rs:169-237; delta = b3 X + b5 h over the variable base X, as the reference computes it
+ProductProof product_prove(const MultiCommitGens& g, Transcript& transcript, RandomTape& tape, const Fr& x, const Fr& rX,
+                           const Fr& y, const Fr& rY, const Fr& z, const Fr& rZ, Point& X, Point& Y, Point& Z) {
+  transcript.append_protocol_name("product proof");
+  const Fr b1 = tape.random_scalar("b1");
+  const Fr b2 = tape.random_scalar("b2");
+  const Fr b3 = tape.random_scalar("b3");
+  const Fr b4 = tape.random_scalar("b4");
+  const Fr b5 = tape.random_scalar("b5");
+  X = commit_scalar(x, rX, g);
+  transcript.append_point("X", X);
+  Y = commit_scalar(y, rY, g);
+  transcript.append_point("Y", Y);
+  Z = commit_scalar(z, rZ, g);
+  transcript.append_point("Z", Z);
+  ProductProof p;
+  p.alpha = commit_scalar(b1, b2, g);
+  transcript.append_point("alpha", p.alpha);
+  p.beta = commit_scalar(b3, b4, g);
+  transcript.append_point("beta", p.beta);
+  p.delta = X * b3 + g.h * b5;
+  transcript.append_point("delta", p.delta);
+  const Fr c = transcript.challenge_scalar("c");
+  p.z[0] = b1 + c * x;
+  p.z[1] = b2 + c * rX;
+  p.z[2] = b3 + c * y;
+  p.z[3] = b4 + c * rY;
+  p.z[4] = b5 + c * (rZ - rX * y);
+  return p;
+}
+// zk.rs:239-300 (check_equality: P + c X == z1 G + z2 h, the last one over the bases (X, h))
+bool product_verify(const ProductProof& p, const MultiCommitGens& g, Transcript& transcript, const Point& X,
+                    const Point& Y, const Point& Z) {
+  transcript.append_protocol_name("product proof");
+  transcript.append_point("X", X);
+  transcript.append_point("Y", Y);
+  transcript.append_point("Z", Z);
+  transcript.append_point("alpha", p.alpha);
+  transcript.append_point("beta", p.beta);
+  transcript.append_point("delta", p.delta);
+  const Fr c = transcript.challenge_scalar("c");
+  bool ok = p.alpha + X * c == commit_scalar(p.z[0], p.z[1], g);
+  ok &= p.beta + Y * c == commit_scalar(p.z[2], p.z[3], g);
+  ok &= p.delta + Z * c == X * p.z[2] + g.h * p.z[4];
+  return ok;
 }
 
 }  // namespace
@@ -1035,6 +1148,99 @@ int orcd_zk_verify(const uint8_t* bytes, size_t nbytes, const uint8_t* comm_clai
     return 1;
   e.compress(e_out);
   for (size_t j = 0; j < num_rounds; j++) stfr(r_out + 4 * j, r[j]);
+  return 0;
+}
+
+// ---- Σ-protocols of committed scalars (gens: G1 one affine point, h1 one).  The provers return the proof's length (0 on
+// error) and the compressed commitments the reference returns alongside; the verifiers return 0 accepted, 1 rejected,
+// 2 the bytes or a commitment do not parse.
+size_t orcd_knowledge_prove(const uint64_t* G1, const uint64_t* h1, void* transcript, void* tape, const uint64_t* x,
+                            const uint64_t* r, uint8_t* out, uint8_t* C_out) {
+  Point C;
+  const KnowledgeProof p =
+      knowledge_prove(ldgens(G1, 1, h1), *(Transcript*)transcript, *(RandomTape*)tape, ldfr(x), ldfr(r), C);
+  std::vector<uint8_t> b;
+  put_point(b, p.alpha);
+  put_fr(b, p.z1);
+  put_fr(b, p.z2);
+  memcpy(out, b.data(), b.size());
+  C.compress(C_out);
+  return b.size();
+}
+int orcd_knowledge_verify(const uint64_t* G1, const uint64_t* h1, const uint8_t* proof, size_t proof_len,
+                          const uint8_t* C, void* transcript) {
+  Reader rd{proof, proof_len};
+  KnowledgeProof p;
+  p.alpha = rd.point();
+  p.z1 = rd.fr();
+  p.z2 = rd.fr();
+  Point c;
+  if (!rd.ok || rd.at != proof_len || !ldpoint(C, c)) return 2;
+  return knowledge_verify(p, ldgens(G1, 1, h1), *(Transcript*)transcript, c) ? 0 : 1;
+}
+size_t orcd_equality_prove(const uint64_t* G1, const uint64_t* h1, void* transcript, void* tape, const uint64_t* v1,
+                           const uint64_t* s1, const uint64_t* v2, const uint64_t* s2, uint8_t* out, uint8_t* C1_out,
+                           uint8_t* C2_out) {
+  Point C1, C2;
+  const EqualityProof p = equality_prove(ldgens(G1, 1, h1), *(Transcript*)transcript, *(RandomTape*)tape, ldfr(v1),
+                                         ldfr(s1), ldfr(v2), ldfr(s2), C1, C2);
+  std::vector<uint8_t> b;
+  put_point(b, p.alpha);
+  put_fr(b, p.z);
+  memcpy(out, b.data(), b.size());
+  C1.compress(C1_out);
+  C2.compress(C2_out);
+  return b.size();
+}
+int orcd_equality_verify(const uint64_t* G1, const uint64_t* h1, const uint8_t* proof, size_t proof_len,
+                         const uint8_t* C1, const uint8_t* C2, void* transcript) {
+  Reader rd{proof, proof_len};
+  EqualityProof p;
+  p.alpha = rd.point();
+  p.z = rd.fr();
+  Point c1, c2;
+  if (!rd.ok || rd.at != proof_len || !ldpoint(C1, c1) || !ldpoint(C2, c2)) return 2;
+  return equality_verify(p, ldgens(G1, 1, h1), *(Transcript*)transcript, c1, c2) ? 0 : 1;
+}
+size_t orcd_product_prove(const uint64_t* G1, const uint64_t* h1, void* transcript, void* tape, const uint64_t* x,
+                          const uint64_t* rX, const uint64_t* y, const uint64_t* rY, const uint64_t* z,
+                          const uint64_t* rZ, uint8_t* out, uint8_t* X_out, uint8_t* Y_out, uint8_t* Z_out) {
+  Point X, Y, Z;
+  const ProductProof p = product_prove(ldgens(G1, 1, h1), *(Transcript*)transcript, *(RandomTape*)tape, ldfr(x), ldfr(rX),
+                                       ldfr(y), ldfr(rY), ldfr(z), ldfr(rZ), X, Y, Z);
+  std::vector<uint8_t> b;
+  put_point(b, p.alpha);
+  put_point(b, p.beta);
+  put_point(b, p.delta);
+  for (const Fr& f : p.z) put_fr(b, f);  // [F; 5]: no length prefix
+  memcpy(out, b.data(), b.size());
+  X.compress(X_out);
+  Y.compress(Y_out);
+  Z.compress(Z_out);
+  return b.size();
+}
+int orcd_product_verify(const uint64_t* G1, const uint64_t* h1, const uint8_t* proof, size_t proof_len, const uint8_t* X,
+                        const uint8_t* Y, const uint8_t* Z, void* transcript) {
+  Reader rd{proof, proof_len};
+  ProductProof p;
+  p.alpha = rd.point();
+  p.beta = rd.point();
+  p.delta = rd.point();
+  for (Fr& f : p.z) f = rd.fr();
+  Point x, y, z;
+  if (!rd.ok || rd.at != proof_len || !ldpoint(X, x) || !ldpoint(Y, y) || !ldpoint(Z, z)) return 2;
+  return product_verify(p, ldgens(G1, 1, h1), *(Transcript*)transcript, x, y, z) ? 0 : 1;
+}
+// sum_i scalars[i] points[i] of n compressed points -> out (compressed): a verifier's homomorphic combination of
+// commitments.  0, or 2 when a point does not decompress.
+int orcd_point_lincomb(const uint8_t* points, size_t n, const uint64_t* scalars, uint8_t* out) {
+  Point acc = Point::zero();
+  for (size_t i = 0; i < n; i++) {
+    Point p;
+    if (!ldpoint(points + 32 * i, p)) return 2;
+    acc += p * ldfr(scalars + 4 * i);
+  }
+  acc.compress(out);
   return 0;
 }
 
